@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — k-NN QPS of the nidx_vector HNSW search hot path on B200 (BASELINE.json configs[1]:
-"HNSW search 10M×768 cosine, ef=128 k=10, batch=1024 on 1×B200").
+"""bench.py — k-NN QPS of the nidx_vector HNSW search hot path on an H100 (BASELINE.json configs[1]:
+"HNSW search 10M×768 cosine, ef=128 k=10, batch=1024": 30.7 GB of vectors, which fits one 80 GB H100 with the graph).
 
 A step = one batch of `--batch` queries through OpenSegment::search (segment.rs:477-567 -> hnsw/search.rs:306-383)
-on one HBM-resident segment.  Contract (driver): `python bench.py --gpus N --steps K --warmup W [--impl reference]`
+on one HBM-resident segment.  `python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]`
 prints ONE JSON line on rank 0.  See DESIGN.md §measurement for what each key means.
 """
 from __future__ import annotations
@@ -51,9 +51,12 @@ def parse_args():
     ap.add_argument("--exchange", default="lib", choices=["lib", "torch"],
                     help="N>1: 'lib' = nidx_vec_search_sharded (search -> ncclAllGather -> Fssc merge inside the library, one stream, no host code "
                          "in between); 'torch' = round 1's torch.distributed all_gather + nidx_merge_topk")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the results of the last timed step (the arrays the caller receives: ids, scores, "
+                         "counts, ...) as DIR/<name>.npy in float64 (ids, counts) / float32 (scores), for comparing two builds output for output")
     ap.add_argument("--pipeline", action="store_true",
                     help="N>1: two batches in flight (exchange of batch i under the search of batch i+1) instead of search -> exchange -> merge back to "
-                         "back; measured 1.5 %% SLOWER at N=2 (profiles/r01c_bench_2M_n2_pipelined.json): the in-line exchange costs 0.02 ms of a 1.63 ms step")
+                         "back")
     return ap.parse_args()
 
 
@@ -137,7 +140,7 @@ def gen_queries(vecs, nq, seed, distance=0.05):
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed regions (B200_PROFILING.md) through NVML (the same
+    """SM clock / throttle reasons sampled DURING the timed regions through NVML (the same
     counters nvidia-smi prints; a 2 ms period needs the library, the CLI takes ~50 ms per call)."""
 
     def __init__(self, index):
@@ -209,8 +212,8 @@ class ClockSampler:
 
 
 def effective_cores() -> int:
-    """Host threads the CPU arm can really use: min(os.cpu_count(), the affinity mask, the cgroup CPU quota).  On this pool's
-    GPU boxes os.cpu_count() is 128 but cpu.max is 16 CPUs: 128 threads run 2.7x SLOWER than 16 (scripts/cpu_scaling_check.py)."""
+    """Host threads the CPU arm can really use: min(os.cpu_count(), the affinity mask, the cgroup CPU quota).  A container can see
+    far more CPUs than its quota grants, and oversubscribed threads run slower than the quota's count (scripts/cpu_scaling_check.py)."""
     n = os.cpu_count() or 1
     try:
         n = min(n, len(os.sched_getaffinity(0)))
@@ -354,6 +357,17 @@ def run_hybrid(args, rank, world, local_rank, dev, comm, seg, queries, k, ef, mu
     return out
 
 
+def dump_outputs(out_dir, result, sharded_lib):
+    """The last timed step's results as .npy files: ids / counts (int32 on the device) as float64 -- exact --, scores as float32.
+    One step is nq x k entries, far below 64 MB, so nothing is sampled."""
+    names = ("ids", "scores", "part", "counts") if sharded_lib else ("ids", "scores", "counts")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in zip(names, result):
+        a = t.cpu().numpy() if hasattr(t, "cpu") else np.asarray(t)
+        a = a.astype(np.float32) if a.dtype.kind == "f" else a.astype(np.float64)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def main():
     args = parse_args()
     import torch
@@ -429,7 +443,7 @@ def main():
             native = False
         og = export_graph_for_oracle(seg, O, n, m, m0)
         norms = O.norms(host_vecs, nthreads=cores)
-        sample = nq   # the whole batch: ~0.3 s of CPU work per step on the box's 16 usable cores
+        sample = nq   # the whole batch
         host_q = [q[:sample].cpu().numpy() for q in queries]
         for i in range(args.warmup):
             cpu_search_rate(O, host_vecs, og, host_q[i], k, ef, norms, cores, native)
@@ -473,15 +487,16 @@ def main():
         return seg.search(queries[i], k, ef=ef, method=_lib.NIDX_METHOD_HNSW, out=out)
 
     def run_steps(first, last):
+        res = None
         if not pipelined:
             for i in range(first, last):
-                step(i)
-            return
+                res = step(i)
+            return res
         for i in range(first, last):   # two batches in flight: the exchange of batch i overlaps the search of batch i + 1
             sharded.submit(queries[i], ef)
             if i > first:
                 sharded.collect()
-        sharded.collect()
+        return sharded.collect()
 
     # ---- warm-up + timed region: inputs resident in HBM (value) --------------------------------------
     # Everything with a host-side cost that differs between ranks (NVML initialisation: 8 processes contend for it on an
@@ -500,14 +515,16 @@ def main():
         torch.cuda.cudart().cudaProfilerStart()  # `ncu --profile-from-start off` captures exactly the timed region
         step_ev[0].record()
         if pipelined:
-            run_steps(args.warmup, n_batches)
+            last = run_steps(args.warmup, n_batches)
         else:
             for i in range(args.warmup, n_batches):
-                step(i)
+                last = step(i)
                 step_ev[i - args.warmup + 1].record()
         step_ev[-1].record()
         torch.cuda.synchronize()
         torch.cuda.cudart().cudaProfilerStop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, use_lib)
     ms_total = step_ev[0].elapsed_time(step_ev[-1])
     per_step = None if pipelined else [step_ev[i].elapsed_time(step_ev[i + 1]) for i in range(args.steps)]
     launches = L.nidx_launch_count() - launches0
@@ -538,7 +555,7 @@ def main():
         dist.barrier()
 
     # ---- the same steps with TWO batches in flight (N = 1) ----------------------------------------------
-    # A batch of 1024 queries runs as 592 + 432 CTAs (4 resident per SM): while the second wave drains, 27 % of the CTA slots are
+    # A batch of 1024 queries runs in more than one wave of CTAs (4 resident per SM): while the last wave drains, CTA slots are
     # empty.  The reference's searcher serves concurrent requests against one shared index (shard_search.rs:139-155); with the next
     # batch issued on a second stream its CTAs fill those slots.  Same K steps, inputs in HBM, events across both streams.
     two_streams = None
@@ -598,7 +615,7 @@ def main():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))   # H100 SXM data sheet: 3.35 TB/s of HBM3
     # The kernel's duration for the roofline comes from the TIMED REGION itself when it can: at N = 1 a step is memset + row norms
     # (~5 us) + hnsw_search_kernel, so the median per-step device time is an upper bound of the kernel's launch duration under the
     # very conditions the value was measured in (the separate accounting pass below the timed region runs after the CPU baseline
@@ -749,7 +766,7 @@ def main():
             import bench_extra as BX
 
             host_vecs = None
-            seg.close()                      # 33 GB of vectors + graph back to the allocator first
+            seg.close()                      # the vectors + graph back to the allocator first
             del seg
             torch.cuda.empty_cache()
             extra = BX.driver_extras(steps=max(3, min(args.steps, 10)), warmup=max(3, min(args.warmup, 5)))
@@ -778,7 +795,7 @@ def main():
                          "traffic_source": "profiles/ncu_traffic.json" if traffic else None, "kernel": "hnsw_search_kernel", "kernel_ms": kernel_ms_roof, "kernel_ms_accounting_pass": kernel_ms_accounting,
                          "kernel_ms_source": "min(median device time of the timed steps (upper bound: includes memset + row norms), mean kernel-only time of the accounting pass)" if not multi else "kernel-only events of the accounting pass",
                          "alg_bytes_per_launch": float(np.mean(alg_bytes)),
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "fallback"},
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks else "H100 SXM data sheet"},
             "cpu_baseline": cpu,
             "e2e": {"value": e2e_qps, "unit": "queries/s", "h2d_bytes_per_step": nq * d * 4, "d2h_bytes_per_step": nq * k * (12 if use_lib else 8) + nq * 4, **e2e_mode},
             "gpu_launches": int(launches),

@@ -6,7 +6,7 @@
          - "or_basic": nidx_paragraph semantics (OR of TermQuery(Basic), tf == 1)
          - "and_tf":   nidx_text semantics (conjunction, real tf) on 3-term queries
 
-bench.py (the driver's contract) stays the HNSW headline; this file produces the evidence kept under profiles/.
+bench.py (the driver's contract) stays the HNSW headline; this file produces the side measurements.
 """
 from __future__ import annotations
 
@@ -33,7 +33,7 @@ def peaks():
 
 
 def ncu_traffic(workload):
-    """DRAM bytes per launch of the committed ncu capture of this exact workload (profiles/ncu_traffic.json), or None."""
+    """DRAM bytes per launch of an ncu capture of this exact workload (profiles/ncu_traffic.json, when one is kept), or None."""
     try:
         return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json"))).get(workload, {}).get("dram_bytes_per_launch")
     except Exception:
@@ -83,12 +83,12 @@ def bench_scan(args):
         t0 = time.perf_counter()
         O.brute_force(host_v, host_q[: min(qq.shape[0], 256)], k, nthreads=effective_cores())
         cpu_dt = time.perf_counter() - t0
-        pk = float(peaks().get("hbm_gbs", 6650.0))
+        pk = float(peaks().get("hbm_gbs", 3350.0))
         ach = alg / (kms * 1e-3) / 1e9
         wl = f"nidx_vector brute-force cosine top-10, {n}x{d} f32, {label}"
         if qq.shape[0] >= 128:   # tensor-core filter: ONE TF32 pass over Q x N (2 N d Q flops); TF32 dense peak = half the measured bf16 peak
             tf = 2.0 * n * d * qq.shape[0] / (kms * 1e-3) / 1e12
-            tpk = float(peaks().get("bf16_tflops", 1590.0)) / 2
+            tpk = float(peaks().get("bf16_tflops", 989.0)) / 2
             roof = {"bound": "tensor", "achieved": tf, "peak": tpk, "unit": "TFLOP/s", "frac": tf / tpk, "kernel": "scan_tc_filter_kernel", "kernel_ms": kms,
                     "traffic": ncu_traffic(wl), "note": "2 N d Q flops of the single TF32 pass / the filter kernel's time; peak = MEASURED_PEAKS bf16_tflops / 2 "
                     "(TF32 runs at half the bf16 rate); the exact refine of the survivors is in ms_per_step, not here"}
@@ -129,7 +129,7 @@ def bench_build(args):
         gt = seg.search(q, 10, method=_lib.NIDX_METHOD_BRUTE)[0].cpu().numpy()
         rec = {ef: recall_at_k(seg.search(q, 10, ef=ef, method=_lib.NIDX_METHOD_HNSW)[0].cpu().numpy(), gt) for ef in (30, 128)}
         alg = c["similarities"] * (d * 4 + 4)
-        pk = float(peaks().get("hbm_gbs", 6650.0))
+        pk = float(peaks().get("hbm_gbs", 3350.0))
         lines.append({"metric": "HNSW build vectors/s", "value": n / dt, "unit": "vectors/s", "n_gpus": 1, "higher_is_better": True, "dtype": "f32", "data": "synthetic",
                       "config": {"workload": f"HNSW index build {n}x{d}, M={m} M0={m0} efC={efc}", "max_batch": 8192}, "seconds": dt,
                       "similarities": c["similarities"], "visited_overflows": c["overflows"], "recall_at_10": rec,
@@ -263,7 +263,7 @@ def bench_bm25(args):
         ok_counts = bool((cnt[:ns] == oc).all() and (tot[:ns] == otot).all())
         rel = float(np.max(np.abs(sc[:ns] - osc) / np.maximum(1.0, np.abs(osc))))
         same_ids = float(np.mean(docs[:ns] == od))
-        pk = float(peaks().get("hbm_gbs", 6650.0))
+        pk = float(peaks().get("hbm_gbs", 3350.0))
         ach = alg / (kms * 1e-3) / 1e9
         lines.append({"metric": "BM25 QPS", "value": nq / (ms * 1e-3), "unit": "queries/s", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
                       "ms_per_step": ms, "higher_is_better": True, "dtype": "f32 (u32 fixed-point accumulate)", "data": "synthetic",
@@ -305,7 +305,7 @@ def bench_rabitq(args):
     gt = seg.search(queries[0], k, method=_lib.NIDX_METHOD_BRUTE)[0].cpu().numpy()
     out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev), torch.empty((nq,), dtype=torch.int32, device=dev))
     lines = []
-    pk = float(peaks().get("hbm_gbs", 6650.0))
+    pk = float(peaks().get("hbm_gbs", 3350.0))
     for name, method, ef in (("quantised walk (RaBitQ query, 1000 layer-0 candidates, exact rerank)", _lib.NIDX_METHOD_HNSW_RABITQ, 0),
                              ("dense walk ef=128", _lib.NIDX_METHOD_HNSW, 128)):
         idx = [0]

@@ -1,4 +1,4 @@
-/* nidx_b200 — C ABI of the B200-native nidx search hot path (libnidx_b200.so).
+/* nidx_b200 — C ABI of the H100-native (sm_90a) nidx search hot path (libnidx_b200.so).
  *
  * This is the drop-in boundary: every entry point replaces one Rust interface of the reference
  * (cited per function) and is what a cgo/FFI/ctypes binding on the reference side binds

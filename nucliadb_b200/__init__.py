@@ -1,4 +1,4 @@
-"""nucliadb_b200 — B200-native (sm_100a) implementation of NucliaDB's nidx search hot path.
+"""nucliadb_b200 — H100-native (sm_90a) implementation of NucliaDB's nidx search hot path.
 
 Only what the hot path needs lives here (SURVEY.md §8): the CUDA kernels + C ABI (``csrc/``,
 ``libnidx_b200.so``) and a host-side mirror of the reference's plug-in interface

@@ -91,7 +91,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise ImportError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                          "(nvcc, sm_100a). nucliadb_b200 has no CPU fallback.")
+                          "(nvcc, sm_90a). nucliadb_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     L.nidx_last_error.restype = C.c_char_p
     L.nidx_launch_count.restype = C.c_uint64

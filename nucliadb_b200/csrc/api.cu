@@ -1143,7 +1143,7 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
             if (grid > 0x7FFFFFFFull) return fail(NIDX_EINVAL, "scan grid too large");
             if (q0 == 0) CU(cudaEventRecord(s->ev_k0, stream));
             if (tensor_scan) {
-                // large batch: the score matrix is a dense GEMM -> tcgen05 (3xTF32, f32 accumulate in TMEM)
+                // large batch: the score matrix is a dense GEMM -> wgmma (3xTF32, f32 accumulate in registers)
                 dim3 tgrid((unsigned)((s->n + TC_N - 1) / TC_N), (unsigned)((nqg + TC_M - 1) / TC_M));
                 scan_scores_tc_kernel<<<tgrid, TC_THREADS, TC_SMEM_BYTES, stream>>>(V, dq + (size_t)q0 * s->ld, w.qnorms.as<float>() + q0, nqg, w.scores.as<float>());
             } else {
@@ -1457,8 +1457,8 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
         int cache_rev = (int)std::min<size_t>(prune_max, budget / row_bytes);
         // prune of a full list: stage all mmax + 1 vectors and the pairwise table when they fit (<= ~200 KB)
         int full_rows = std::max(s->cfg.m0, M) + 1;
-        // NIDX_B200_PRUNE=table switches the prune to the staged pairwise-table variant (same result; measured
-        // slightly slower than the candidate-at-a-time loop at d = 768, M0 = 32: 4.94 s vs 4.71 s per 1M vectors)
+        // NIDX_B200_PRUNE=table switches the prune to the staged pairwise-table variant (same result as the
+        // candidate-at-a-time loop)
         const char* prune_env = getenv("NIDX_B200_PRUNE");
         bool preload = hb_smem_bytes(s->ld, full_rows, true) <= 200 * 1024 && prune_env && !strcmp(prune_env, "table");
         if (preload) cache_rev = full_rows;

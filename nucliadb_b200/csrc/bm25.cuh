@@ -1,4 +1,4 @@
-// nidx_b200 — K7: BM25 top-k over device-resident postings (sm_100a).
+// nidx_b200 — K7: BM25 top-k over device-resident postings (sm_90a).
 //
 // Replaces the tantivy collector call of the reference:
 //   nidx/nidx_text/src/reader.rs:432-435        TopDocs::with_limit(k+1).order_by_score() + Count
@@ -29,8 +29,8 @@
 // A tile that holds more postings than slots is redone with half the span; a single fine tile that still does not fit runs in
 // several rounds of slots (postings re-read in phase C): distinct documents <= BM_FINE = the accumulator's capacity, whatever
 // the posting count.
-// No atomicCAS, no probing: one atomicOr + one atomicAdd per posting (measured on B200: a warp-wide ATOMS per ~4 clk per SM,
-// scripts/ubench_smem.cu; an earlier hash-table accumulator spent 60 % of its instructions in divergent probe loops).
+// No atomicCAS, no probing: one atomicOr + one atomicAdd per posting (scripts/ubench_smem.cu measures the shared-memory atomic
+// rate; a hash-table accumulator would spend its instructions in divergent probe loops).
 // HBM traffic = the query's postings once (8 B each) + one skip entry per (term, tile).
 #pragma once
 #include "common.cuh"
@@ -39,8 +39,8 @@
 namespace nidx {
 
 // CTA shape: threads x posting slots per thread = 4096 slots per round; CTAs per SM (launch bounds).  512 x 8 x 2 (64 registers,
-// 32 warps per SM) measured against 256 x 16 x 3 (80 registers, 24 warps per SM) on 5 M documents: OR-50 338 k vs 335 k QPS,
-// AND-3 1.32 M vs 1.21 M; same outputs (make EXTRA="-DBM_THREADS_CFG=256 -DBM_PT_CFG=16 -DBM_MINB_CFG=3" builds the other one).
+// 32 warps per SM) by default; 256 x 16 x 3 (80 registers, 24 warps per SM) gives the same outputs
+// (make EXTRA="-DBM_THREADS_CFG=256 -DBM_PT_CFG=16 -DBM_MINB_CFG=3" builds it).
 #ifndef BM_THREADS_CFG
 #define BM_THREADS_CFG 512
 #define BM_PT_CFG 8

@@ -1,4 +1,4 @@
-// nidx_b200 — shared device helpers (sm_100a).
+// nidx_b200 — shared device helpers (sm_90a).
 //
 // The similarity arithmetic of nidx_vector (vector_types/dense_f32.rs:29-39 over simsimd) is done
 // in ONE fixed summation order everywhere ("lane-blocked", DESIGN.md §kernels): lane l of a warp

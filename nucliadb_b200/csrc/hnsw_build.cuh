@@ -1,4 +1,4 @@
-// nidx_b200 — K4: HNSW construction for nidx_vector (sm_100a).
+// nidx_b200 — K4: HNSW construction for nidx_vector (sm_90a).
 //
 // Reference: HnswBuilder (nidx/nidx_vector/src/hnsw/build.rs:36-166), driven by
 // create_indexes / merge_indexes (segment.rs:241-286, 137-197) with rayon + per-node RwLocks.

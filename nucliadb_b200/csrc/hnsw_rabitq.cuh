@@ -1,4 +1,4 @@
-// nidx_b200 — K5b: the HNSW walk with a RaBitQ query (sm_100a).  The reference's production path for Dot indexes that
+// nidx_b200 — K5b: the HNSW walk with a RaBitQ query (sm_90a).  The reference's production path for Dot indexes that
 // carry 1-bit codes:
 //   nidx/nidx_vector/src/segment.rs:506-513       the query becomes SearchVector::RabitQ when the store has vectors.quant
 //   nidx/nidx_vector/src/hnsw/search.rs:306-383   HnswSearcher::search: the walk ranks by the ESTIMATE (similarity_upper_bound().score,

@@ -1,4 +1,4 @@
-// nidx_b200 — K2/K3: HNSW search for nidx_vector (sm_100a).
+// nidx_b200 — K2/K3: HNSW search for nidx_vector (sm_90a).
 //
 // One CTA walks one query (or, in build mode, one node to insert) through the graph:
 //   HnswSearcher::layer_search      nidx/nidx_vector/src/hnsw/search.rs:242-304

@@ -1,4 +1,4 @@
-// nidx_b200 — K5: RaBitQ 1-bit quantisation for nidx_vector (sm_100a).  First slice of SURVEY §8f rank 1:
+// nidx_b200 — K5: RaBitQ 1-bit quantisation for nidx_vector (sm_90a).  First slice of SURVEY §8f rank 1:
 // encoding, the estimator and the quantised exact scan; the quantised HNSW walk is the next step.
 //
 //   nidx/nidx_vector/src/vector_types/rabitq.rs:75-106    EncodedVector::encode    -> rabitq_encode_kernel

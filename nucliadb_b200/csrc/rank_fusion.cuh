@@ -1,4 +1,4 @@
-// nidx_b200 — K9: rank fusion on the device (sm_100a).  SURVEY 8f rank 4: the step that follows a shard search in the reference
+// nidx_b200 — K9: rank fusion on the device (sm_90a).  SURVEY 8f rank 4: the step that follows a shard search in the reference
 // runs in Python on the host:
 //   nucliadb/src/nucliadb/search/search/rank_fusion.py:78-96    RankFusionAlgorithm.fuse (one non-empty source: no fusion)
 //   nucliadb/src/nucliadb/search/search/rank_fusion.py:143-186  ReciprocalRankFusion._fuse

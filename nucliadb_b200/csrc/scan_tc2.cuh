@@ -2,10 +2,9 @@
 //
 // brute_force_search (nidx/nidx_vector/src/segment.rs:569-623) evaluated for a batch of queries is a dense GEMM,
 // scores = Q · Vᵀ -- the one place on the nidx_vector path where the tensor cores apply.  The product is needed only to
-// find each query's top-k, so it is computed ONCE in TF32 (f32 operands straight from the stored rows, f32 accumulation in
-// tensor memory) as a filter with a rigorous error bound, never written to HBM, and only the few survivors are re-scored
-// with the lane-blocked f32 arithmetic of common.cuh.  Ids AND scores are therefore bit-identical to the small-batch kernel
-// and to the oracle (round 1's 3xTF32 kernel was 1e-6 off and materialised the [Q x N] matrix).
+// find each query's top-k, so it is computed ONCE in TF32 (f32 operands straight from the stored rows, f32 accumulation) as a
+// filter with a rigorous error bound, never written to HBM, and only the few survivors are re-scored with the lane-blocked f32
+// arithmetic of common.cuh.  Ids AND scores are therefore bit-identical to the small-batch kernel and to the oracle.
 //
 //   |tf32(q) . tf32(v) - q . v| <= 2^-9 |q| |v|  (each operand keeps 10 mantissa bits: relative error < 2^-10 per factor)
 //   eps = 2.2e-3 (cosine) or 2.2e-3 |q| max|v| (dot).  Let tau = the k-th largest APPROXIMATE score of a query over the
@@ -17,15 +16,14 @@
 //
 // scan_tc_filter_kernel: persistent CTAs; a CTA serves ONE 128-query block (slot s of grid / n_qblocks slots) and walks the
 // vector chunks s, s + slots, ...; the CTAs of one slot run together and share every chunk (L2 reuse).  Warp-specialised:
-//   warp 0   TMA producer: cp.async.bulk.tensor (128-byte swizzle) of a 128 x 32-float query tile and a 256 x 32-float
-//            vector tile per stage into a 4-stage mbarrier ring (48 KB per stage);
-//   warp 1   MMA issuer: one thread, tcgen05.mma.cta_group::1.kind::tf32, M = 128 (queries) x N = 256 (vectors) x K = 8,
-//            four per stage; tcgen05.commit releases the stage; accumulators double-buffered in TMEM (2 x 256 columns);
-//   warp 2   TMEM allocation;
-//   warps 4-11 epilogue: warp % 4 = TMEM lane quadrant, thread = query row; warps 4-7 read columns 0-127 of every tile, warps 8-11
-//            columns 128-255 (the read-out, not the tensor pipe, paces the kernel); tcgen05.ld 32 columns at a time, cosine scaling, eligibility bit,
-//            running top-L of the row in REGISTERS (unsorted + its minimum), fed through a per-row staging area in shared memory
-//            so that the (warp-wide) list update runs once per ~8-16 candidates of the busiest row, not once per column.
+//   warpgroup 0      TMA producer (one thread): cp.async.bulk.tensor (128-byte swizzle) of a 128 x 32-float query tile and a
+//                    128 x 32-float vector tile per stage into a 4-stage mbarrier ring (32 KB per stage);
+//   warpgroups 1, 2  consumers, 64 query rows each: wgmma.mma_async m64n128k8 tf32 from the stage (four per stage), f32
+//                    accumulators in registers; every consumer warp releases the stage when its MMAs have read it.  The
+//                    accumulators then go to a per-warpgroup score tile in shared memory and the same 128 threads run the
+//                    epilogue with thread = (query row, column half): cosine scaling, eligibility bit, running top-L of the
+//                    row's half in REGISTERS (unsorted + its minimum), fed through a per-row staging area in shared memory so
+//                    that the (warp-wide) list update runs once per ~8-16 candidates of the busiest row, not once per column.
 // scan_tc_refine_kernel: one CTA per query: overflow test, tau, survivors, exact re-scoring (one warp per survivor),
 //   min_score, top-k -- or the exact scan of the whole segment for an overflowed query.
 #pragma once
@@ -37,31 +35,54 @@
 
 namespace nidx {
 
-constexpr int TC2_M = 128;            // queries per block (UMMA M, TMEM lanes)
-constexpr int TC2_N = 256;            // vectors per tile (UMMA N)
+constexpr int TC2_M = 128;            // queries per block (two consumer warpgroups x wgmma M = 64)
+constexpr int TC2_N = 128;            // vectors per tile (wgmma N)
 constexpr int TC2_KB = 32;            // floats per k-block = one 128-byte swizzle row
 constexpr int TC2_STAGES = 4;
-constexpr int TC2_TILES = 8;          // vector tiles per chunk
+constexpr int TC2_TILES = 16;         // vector tiles per chunk
 constexpr int TC2_CHUNK = TC2_N * TC2_TILES;   // 2048 vectors
 constexpr int TC2_L = 24;             // candidates kept per (query, chunk)
 constexpr int TC2_KMAX = 16;          // the filter path serves k <= TC2_KMAX
-constexpr int TC2_EPI_WARPS = 8;      // epilogue warps: TMEM lane quadrant = warp % 4, column half of the tile = warp / 4
-constexpr int TC2_THREADS = (4 + TC2_EPI_WARPS) * 32;
+constexpr int TC2_CONSUMERS = 2;      // consumer warpgroups: query rows 64 c .. 64 c + 63
+constexpr int TC2_THREADS = (1 + TC2_CONSUMERS) * 128;
+constexpr int TC2_ROWS = TC2_M / TC2_CONSUMERS;   // query rows per consumer warpgroup
+constexpr int TC2_TILE_LD = TC2_N + 1;           // score tile row stride (floats): a warp reading one column of 32 rows hits 32 banks
 constexpr uint32_t TC2_A_BYTES = TC2_M * 128, TC2_B_BYTES = TC2_N * 128, TC2_STAGE_BYTES = TC2_A_BYTES + TC2_B_BYTES;
 constexpr int TC2_STAGE_ROWS = 12;    // staged candidates per (query row, column half) between two merges into the register list
-constexpr int TC2_LISTS = TC2_EPI_WARPS / 4;   // candidate lists per query row and CTA (one per column half)
-constexpr size_t TC2_SMEM_BYTES = 1024 /* alignment slack */ + (size_t)TC2_STAGES * TC2_STAGE_BYTES + 2 * TC2_N * 4 /* 1/|v| */ +
-                                  2 * (TC2_N / 32) * 4 /* eligibility */ + (size_t)TC2_STAGE_ROWS * TC2_M * TC2_LISTS * 8 /* staging */ + 256;
+constexpr int TC2_LISTS = 2;          // candidate lists per query row and CTA (one per column half of every tile)
+constexpr size_t TC2_SMEM_BYTES = 1024 /* alignment slack */ + (size_t)TC2_STAGES * TC2_STAGE_BYTES +
+                                  (size_t)TC2_CONSUMERS * TC2_ROWS * TC2_TILE_LD * 4 /* score tiles */ + TC2_CONSUMERS * TC2_N * 4 /* 1/|v| */ +
+                                  TC2_CONSUMERS * (TC2_N / 32) * 4 /* eligibility */ + (size_t)TC2_STAGE_ROWS * TC2_M * TC2_LISTS * 8 /* staging */ + 256;
+static_assert(TC2_SMEM_BYTES <= 227 * 1024, "the filter kernel's shared memory exceeds a Hopper block's 227 KB");
 constexpr float TC2_EPS = 2.2e-3f;
 constexpr int TC2_SURV_CAP = 512;     // survivors per query the refine kernel re-scores; more => exact scan
 
 __device__ __forceinline__ uint64_t tc2_desc(uint32_t smem_addr) {
-    // K-major, SWIZZLE_128B (cute::UMMA::make_umma_desc<Major::K>): start >> 4, LBO = 1, SBO = 8 rows x 128 B = 1024 B, version 1, layout 2
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+    // K-major, SWIZZLE_128B: LBO unused (16 B), SBO = 8 rows x 128 B = 1024 B
+    return wg_desc(smem_addr, 16, 1024, 1);
 }
-__device__ __forceinline__ uint32_t tc2_idesc() {
-    // c_format F32 = 1 [4,6), a/b_format TF32 = 2 [7,10) [10,13), K-major both, N >> 3 [17,23), M >> 4 [24,29)
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TC2_N >> 3) << 17) | ((uint32_t)(TC2_M >> 4) << 24);
+// d[64 x 128] (+)= A[64 x 8] · B[128 x 8]ᵀ: the m64n128k8 tf32 form of wg_mma_64x64_tf32 (same fragment layout, j = 0..15)
+__device__ __forceinline__ void wg_mma_64x128_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+__device__ __forceinline__ void wg_fence_regs64(float (&d)[64]) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i]) :: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* mbar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"((uint32_t)__cvta_generic_to_shared(mbar)), "r"(bytes) : "memory");
@@ -83,7 +104,7 @@ struct Tc2Args {
     unsigned int* work_counter;
 };
 
-// The (query block, chunk) sequence of a CTA -- the same in the three roles.  n_qblocks <= gridDim: CTA c serves block c % n_qblocks
+// The (query block, chunk) sequence of a CTA -- the same in both roles.  n_qblocks <= gridDim: CTA c serves block c % n_qblocks
 // as slot c / n_qblocks (CTAs beyond n_qblocks * slots idle); else one slot and CTA c serves blocks c, c + gridDim, ...
 struct Tc2Sched {
     int g0, gstride, slot, slots;
@@ -97,36 +118,28 @@ struct Tc2Sched {
 __global__ void __launch_bounds__(TC2_THREADS, 1) scan_tc_filter_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_v,
                                                                         VecDev V, Tc2Args a) {
     extern __shared__ unsigned char tc2_raw[];
-    __shared__ uint64_t full[TC2_STAGES], empty[TC2_STAGES], tmem_full[2], tmem_empty[2];
-    __shared__ uint32_t tmem_base_s;
+    __shared__ uint64_t full[TC2_STAGES], empty[TC2_STAGES];
     unsigned char* smem = reinterpret_cast<unsigned char*>(((uintptr_t)tc2_raw + 1023) & ~(uintptr_t)1023);   // SWIZZLE_128B tiles: 1024-byte aligned
     unsigned char* stages = smem;
-    float* inv_vn = reinterpret_cast<float*>(smem + (size_t)TC2_STAGES * TC2_STAGE_BYTES);     // [2][256]
-    uint32_t* elig = reinterpret_cast<uint32_t*>(inv_vn + 2 * TC2_N);                          // [2][8]
-    float* stg_sc = reinterpret_cast<float*>(elig + 2 * (TC2_N / 32));                         // [TC2_STAGE_ROWS][128] staged scores ...
+    float* tiles = reinterpret_cast<float*>(smem + (size_t)TC2_STAGES * TC2_STAGE_BYTES);         // [consumer][64][TC2_TILE_LD]
+    float* inv_vn = tiles + TC2_CONSUMERS * TC2_ROWS * TC2_TILE_LD;                                // [consumer][128]
+    uint32_t* elig = reinterpret_cast<uint32_t*>(inv_vn + TC2_CONSUMERS * TC2_N);                  // [consumer][4]
+    float* stg_sc = reinterpret_cast<float*>(elig + TC2_CONSUMERS * (TC2_N / 32));                 // [TC2_STAGE_ROWS][2 * 128] staged scores ...
     uint32_t* stg_id = reinterpret_cast<uint32_t*>(stg_sc + TC2_STAGE_ROWS * TC2_M * TC2_LISTS);   // ... and ids of the epilogue threads
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int warp = __shfl_sync(0xFFFFFFFFu, (int)threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
     const int n_kb = V.ld / TC2_KB;
     const Tc2Sched sch(a);
 
     if (threadIdx.x == 0) {
-        for (int s = 0; s < TC2_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        mbar_init(&tmem_full[0], 1); mbar_init(&tmem_full[1], 1);
-        mbar_init(&tmem_empty[0], TC2_EPI_WARPS); mbar_init(&tmem_empty[1], TC2_EPI_WARPS);   // one arrive per epilogue warp
+        for (int s = 0; s < TC2_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 4 * TC2_CONSUMERS); }   // one arrive per consumer warp
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 2) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"((uint32_t)__cvta_generic_to_shared(&tmem_base_s)), "n"(2 * TC2_N) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_d = tmem_base_s;
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ===== TMA producer =====
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");   // registers go to the consumers: 128 x 40 + 256 x 232 <= 64 K
+        if (threadIdx.x == 0) {
             uint32_t st = 0, ph = 0;
             for (int qb = sch.g0; qb < a.n_qblocks; qb += sch.gstride)
                 for (int ch = sch.slot; ch < a.n_chunks; ch += sch.slots)
@@ -143,41 +156,20 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) scan_tc_filter_kernel(const __
                         }
                     }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            const uint32_t idesc = tc2_idesc();
-            const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(stages);
-            uint32_t st = 0, ph = 0, tcount = 0;
-            for (int qb = sch.g0; qb < a.n_qblocks; qb += sch.gstride)
-                for (int ch = sch.slot; ch < a.n_chunks; ch += sch.slots)
-                    for (int t = 0; t < TC2_TILES; ++t) {
-                        int v0 = ch * TC2_CHUNK + t * TC2_N;
-                        if ((uint32_t)v0 >= V.n) break;
-                        uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-                        mbar_wait(&tmem_empty[acc], aph ^ 1);               // the epilogue has drained this accumulator
-                        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                        for (int kb = 0; kb < n_kb; ++kb) {
-                            mbar_wait(&full[st], ph);
-                            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                            uint32_t sa = sbase + st * TC2_STAGE_BYTES, sb = sa + TC2_A_BYTES;
-#pragma unroll
-                            for (int ks = 0; ks < TC2_KB / 8; ++ks)    // K = 8 tf32 = 32 bytes inside the 128-byte swizzle row
-                                tc_mma(tmem_d + acc * TC2_N, tc2_desc(sa + ks * 32), tc2_desc(sb + ks * 32), idesc, (kb | ks) != 0);
-                            tc_commit(&empty[st]);                          // frees the stage when these MMAs have read it
-                            if (++st == TC2_STAGES) { st = 0; ph ^= 1; }
-                        }
-                        tc_commit(&tmem_full[acc]);                         // accumulator complete
-                        ++tcount;
-                    }
-        }
-    } else if (warp >= 4) {
-        // ===== epilogue: thread = query row =====
-        const int row = (warp & 3) * 32 + lane;                 // TMEM lane = query row of the block
-        const int half = (warp - 4) >> 2;                       // which TC2_N / TC2_LISTS columns of every tile this warp reads
-        const int et = threadIdx.x - 128;                       // 0 .. 32 * TC2_EPI_WARPS - 1
+    } else {
+        // ===== consumers: MMA, then epilogue with thread = (query row, column half) =====
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+        const int c = (warp >> 2) - 1;                          // consumer warpgroup: query rows 64 c .. 64 c + 63
+        const int et = threadIdx.x - 128 * (c + 1);             // 0 .. 127
+        const int rl = et & (TC2_ROWS - 1), half = et >> 6;     // row of this warpgroup's 64, column half of every tile
+        const int row = c * TC2_ROWS + rl;                      // query row of the block
         const int srow = half * TC2_M + row;                    // this thread's column of the staging area
-        uint32_t tcount = 0;
+        float* tile = tiles + c * TC2_ROWS * TC2_TILE_LD;
+        float* ivn_c = inv_vn + c * TC2_N;
+        uint32_t* elig_c = elig + c * (TC2_N / 32);
+        const uint32_t bar_id = 1 + c;                          // named barrier of this warpgroup's 128 threads
+        const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(stages);
+        uint32_t st = 0, ph = 0;
         for (int qb = sch.g0; qb < a.n_qblocks; qb += sch.gstride) {
             int q = qb * TC2_M + row;
             float inv_qn = 1.0f;
@@ -218,40 +210,58 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) scan_tc_filter_kernel(const __
                 for (int t = 0; t < TC2_TILES; ++t) {
                     int v0 = ch * TC2_CHUNK + t * TC2_N;
                     if ((uint32_t)v0 >= V.n) break;
-                    uint32_t acc = tcount & 1, aph = (tcount >> 1) & 1;
-                    // per-tile column data: 1 / |v| (cosine) and the eligibility bits, by the 128 epilogue threads
-                    for (int j = et; j < TC2_N; j += 32 * TC2_EPI_WARPS) {
-                        uint32_t v = (uint32_t)v0 + j;
+                    // MMA: this warpgroup's 64 rows x 128 vectors over all k-blocks; a stage is released as soon as the MMAs
+                    // issued after it have been waited for (one wgmma group in flight behind the newest)
+                    float acc[64];
+                    wg_fence_regs64(acc);
+                    wg_fence();
+                    uint32_t prev = 0;
+                    for (int kb = 0; kb < n_kb; ++kb) {
+                        mbar_wait(&full[st], ph);
+                        uint32_t sa = sbase + st * TC2_STAGE_BYTES + (uint32_t)c * (TC2_ROWS * 128), sb = sbase + st * TC2_STAGE_BYTES + TC2_A_BYTES;
+#pragma unroll
+                        for (int ks = 0; ks < TC2_KB / 8; ++ks)    // K = 8 tf32 = 32 bytes inside the 128-byte swizzle row
+                            wg_mma_64x128_tf32(acc, tc2_desc(sa + ks * 32), tc2_desc(sb + ks * 32), (kb | ks) != 0);
+                        wg_commit();
+                        if (kb > 0) {
+                            wg_wait<1>();
+                            if (lane == 0) mbar_arrive(&empty[prev]);
+                        }
+                        prev = st;
+                        if (++st == TC2_STAGES) { st = 0; ph ^= 1; }
+                    }
+                    wg_wait<0>();
+                    wg_fence_regs64(acc);
+                    if (lane == 0) mbar_arrive(&empty[prev]);
+                    // the previous tile's epilogue is done with the score tile and the column data
+                    asm volatile("bar.sync %0, 128;" :: "r"(bar_id) : "memory");
+#pragma unroll
+                    for (int j = 0; j < TC2_N / 8; ++j)
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            tile[((warp & 3) * 16 + (lane >> 2) + 8 * (e >> 1)) * TC2_TILE_LD + 8 * j + 2 * (lane & 3) + (e & 1)] = acc[4 * j + e];
+                    // per-tile column data: 1 / |v| (cosine) and the eligibility bits
+                    {
+                        uint32_t v = (uint32_t)v0 + et;
                         float ivn = 1.0f;
                         if (V.sim == SIM_COSINE) { float vn = v < V.n ? __ldg(V.norms + v) : 0.0f; ivn = vn > 0.0f ? __frcp_rn(vn) : 0.0f; }
-                        inv_vn[acc * TC2_N + j] = ivn;
+                        ivn_c[et] = ivn;
                     }
                     if (et < TC2_N / 32) {
                         uint32_t w = 0xFFFFFFFFu;
                         uint32_t vb = (uint32_t)v0 + et * 32;
                         if (a.bits) w = vb < V.n ? reinterpret_cast<const uint32_t*>(a.bits)[vb >> 5] : 0u;
                         if (vb + 32 > V.n) w &= vb < V.n ? (0xFFFFFFFFu >> (32 - (V.n - vb))) : 0u;   // columns beyond the segment
-                        elig[acc * (TC2_N / 32) + et] = w;
+                        elig_c[et] = w;
                     }
-                    asm volatile("bar.sync 1, %0;" :: "n"(32 * TC2_EPI_WARPS) : "memory");
-                    mbar_wait(&tmem_full[acc], aph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+                    asm volatile("bar.sync %0, 128;" :: "r"(bar_id) : "memory");
                     for (int c0 = half * (TC2_N / TC2_LISTS); c0 < (half + 1) * (TC2_N / TC2_LISTS); c0 += 32) {
-                        uint32_t r[32];
-                        uint32_t taddr = tmem_d + ((uint32_t)((warp & 3) * 32) << 16) + acc * TC2_N + c0;
-                        asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                                     "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                                     : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                                       "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                                       "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                                       "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                                     : "r"(taddr));
-                        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-                        const uint32_t ew = q < a.nq ? elig[acc * (TC2_N / 32) + (c0 >> 5)] : 0u;
+                        const uint32_t ew = q < a.nq ? elig_c[c0 >> 5] : 0u;
+                        const float* trow = tile + rl * TC2_TILE_LD + c0;
 #pragma unroll
                         for (int j = 0; j < 32; ++j) {
-                            float sc = __uint_as_float(r[j]);
-                            if (V.sim == SIM_COSINE) sc = sc * inv_qn * inv_vn[acc * TC2_N + c0 + j];
+                            float sc = trow[j];
+                            if (V.sim == SIM_COSINE) sc = sc * inv_qn * ivn_c[c0 + j];
                             const bool pass = ((ew >> j) & 1u) && sc > thr;
                             if (pass) {                                   // predicated stores: the row's staging area, in column order
                                 stg_sc[n_st * (TC2_M * TC2_LISTS) + srow] = sc;
@@ -261,10 +271,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) scan_tc_filter_kernel(const __
                             if ((j & 3) == 3 && __any_sync(0xFFFFFFFFu, n_st > TC2_STAGE_ROWS - 4)) merge_staged();
                         }
                     }
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-                    ++tcount;
                 }
             merge_staged();
             if (q < a.nq) {
@@ -275,9 +281,6 @@ __global__ void __launch_bounds__(TC2_THREADS, 1) scan_tc_filter_kernel(const __
             }
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 2) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem_d), "n"(2 * TC2_N) : "memory");
 }
 
 // One CTA per query.  dynamic smem: ld floats (query) + cap keys (top-k buffer) + survivors.

@@ -1,4 +1,4 @@
-// nidx_b200 — K8: segments sharded over the GPUs of one node, behind the C ABI (sm_100a + NCCL over NVLink).
+// nidx_b200 — K8: segments sharded over the GPUs of one node, behind the C ABI (sm_90a + NCCL over NVLink).
 //
 // Replaces the reference's scatter-gather over shards / segments:
 //   nidx/src/searcher/grpc.rs:253-431            fan a request out to every shard's searcher, gather the responses

@@ -1,4 +1,4 @@
-// nidx_b200 — block-wide streaming top-k over 64-bit rank keys (sm_100a).
+// nidx_b200 — block-wide streaming top-k over 64-bit rank keys (sm_90a).
 //
 // Used by the exact scan (segment.rs:611-617: sort desc + take k), the BM25 collector
 // (TopDocs::with_limit(k).order_by_score, nidx_text/src/reader.rs:432) and the cross-segment merge

@@ -1,6 +1,6 @@
 """Multi-GPU search: one process per GPU, segments sharded across ranks, per-rank partial top-k
 exchanged with ``all_gather`` (NCCL over NVLink on the GPU box, gloo in the CPU tests) and merged by
-``parts_merge_kernel`` -- the B200-native form of the reference's gRPC scatter-gather + k-way merge
+``parts_merge_kernel`` -- the GPU-native form of the reference's gRPC scatter-gather + k-way merge
 (nidx/src/searcher/grpc.rs:253-431, shard_merge.rs:332-348 / 177-207).
 
 The exchange is [nq, k] (u32 id, f32 score) per rank = 8*nq*k bytes (80 KB at nq=1024, k=10): latency

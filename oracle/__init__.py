@@ -8,13 +8,14 @@ file:line each function follows).  Only ``tests/``, ``__graft_entry__.smoke()`` 
 
 Parity status: distances / brute force / HNSW are pinned to the reference's own known-answer tests
 (one-hot fixtures, tolerances; tests/test_oracle_*.py); BM25 is **parity unpinned** (tantivy is a
-third-party crate absent from /root/reference and no reference test asserts a BM25 value).
+third-party crate absent from the reference tree and no reference test asserts a BM25 value).
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -26,18 +27,27 @@ BM25_OR, BM25_AND = 0, 1
 _lib = None
 
 
+def _native_path() -> str:
+    # -march=native is built where it runs, at run time: into a per-user temporary directory, never into the source tree
+    return os.path.join(tempfile.gettempdir(), f"nidx_oracle_{os.getuid()}", "liboracle_native.so")
+
+
 def build(native: bool = False) -> str:
     """Compile the oracle (gcc only).  Returns the path of the shared object."""
-    target = "native" if native else "liboracle.so"
-    subprocess.run(["make", "-s", "-C", _HERE, target], check=True)
-    return os.path.join(_HERE, "liboracle_native.so" if native else "liboracle.so")
+    if native:
+        path = _native_path()
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        subprocess.run(["make", "-s", "-C", _HERE, "native", f"NATIVE_OUT={path}"], check=True)
+        return path
+    subprocess.run(["make", "-s", "-C", _HERE, "liboracle.so"], check=True)
+    return os.path.join(_HERE, "liboracle.so")
 
 
 def lib(native: bool = False):
     global _lib
     if _lib is not None and not native:
         return _lib
-    path = os.path.join(_HERE, "liboracle_native.so" if native else "liboracle.so")
+    path = _native_path() if native else os.path.join(_HERE, "liboracle.so")
     if not os.path.exists(path):
         build(native)
     L = C.CDLL(path)

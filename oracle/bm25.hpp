@@ -9,7 +9,7 @@
 //   nidx/nidx_tantivy/src/index_reader.rs:39-77 statistics are those of the UNION of all segments
 //   nidx/src/searcher/shard_merge.rs:227-231    order: bm25 desc, shard id, lower docaddr first
 //
-// The arithmetic lives in tantivy 0.26.1 (nidx/Cargo.lock:4894), which is NOT in /root/reference,
+// The arithmetic lives in tantivy 0.26.1 (nidx/Cargo.lock:4894), which is NOT in the reference tree,
 // and no reference test asserts a BM25 value (SURVEY F9, 8c) => parity unpinned.  Restated from
 // tantivy's published algorithm [recalled]:
 //   K1 = 1.2, B = 0.75

@@ -8,7 +8,7 @@
 //   nidx/nidx_vector/src/utils.rs:20-23                    normalize_vector
 //
 // The arithmetic itself lives in the third-party crate simsimd 6.5.16 (nidx/Cargo.lock:4552),
-// which is NOT in /root/reference.  Restated from its published algorithm [recalled]:
+// which is NOT in the reference tree.  Restated from its published algorithm [recalled]:
 //   dot:  ab = sum a_i*b_i                     (f32 lanes, backend-specific order)
 //   cos:  ab, a2, b2 accumulated together; distance =
 //           0                          if a2 == 0 && b2 == 0

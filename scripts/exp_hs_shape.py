@@ -1,5 +1,4 @@
-"""(Round-2 experiment; the NIDX_B200_HS_PAIR / NIDX_B200_HS_GRID switches it used were removed with the variants they selected: results under
-profiles/r02_exp_hs_*.jsonl.)  Experiment: HNSW search CTA shape (8 warps x 4 CTAs/SM vs 4 warps x 7 CTAs/SM) and batch size, one index, several configurations.
+"""(Round-2 experiment; the NIDX_B200_HS_PAIR / NIDX_B200_HS_GRID switches it used were removed with the variants they selected.)  Experiment: HNSW search CTA shape (8 warps x 4 CTAs/SM vs 4 warps x 7 CTAs/SM) and batch size, one index, several configurations.
     python scripts/exp_hs_shape.py [n_vectors]"""
 import json
 import os

@@ -1,19 +1,12 @@
-"""The constants the hot path takes from the reference, read from the reference's own Rust sources (build container only; skipped
-elsewhere) and compared with what the mirror, the oracle and the CUDA sources use."""
+"""The constants the hot path takes from the reference, as read from the reference's own Rust sources (nidx/nidx_vector/src) into
+tests/golden/reference_facts.json by tests/golden/make_reference_facts.py, compared with what the mirror, the oracle and the CUDA
+sources use."""
+import json
 import os
 import re
 
-import pytest
-
-REF = "/root/reference/nidx/nidx_vector/src"
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-pytestmark = pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not present")
-
-
-def rust_const(path, name):
-    m = re.search(rf"const\s+{name}\s*:\s*\w+\s*=\s*([0-9.]+)\s*;", open(os.path.join(REF, path)).read())
-    assert m, (path, name)
-    return float(m.group(1))
+FACTS = json.load(open(os.path.join(ROOT, "tests", "golden", "reference_facts.json")))["nidx_vector"]
 
 
 def test_hnsw_parameters():
@@ -21,12 +14,12 @@ def test_hnsw_parameters():
     from nucliadb_b200 import vector as V
 
     cfg = V.VectorConfig(dimension=8)
-    assert cfg.m == rust_const("hnsw/params.rs", "M") == rust_const("hnsw/params.rs", "M_MAX")
-    assert cfg.m0 == rust_const("hnsw/params.rs", "M_MAX_0")
-    assert cfg.ef_construction == rust_const("hnsw/params.rs", "EF_CONSTRUCTION")
-    assert cfg.ef_search == rust_const("hnsw/params.rs", "EF_SEARCH")
-    assert re.search(r"fn prune_m\(m: usize\) -> usize \{\s*m \* 95 / 100", open(os.path.join(REF, "hnsw/params.rs")).read())
-    assert "mmax * 95 / 100" in open(os.path.join(ROOT, "nucliadb_b200", "csrc", "hnsw_build.cuh")).read()
+    assert cfg.m == FACTS["M"] == FACTS["M_MAX"]
+    assert cfg.m0 == FACTS["M_MAX_0"]
+    assert cfg.ef_construction == FACTS["EF_CONSTRUCTION"]
+    assert cfg.ef_search == FACTS["EF_SEARCH"]
+    num, den = FACTS["prune_m"]
+    assert f"mmax * {num} / {den}" in open(os.path.join(ROOT, "nucliadb_b200", "csrc", "hnsw_build.cuh")).read()
     header = open(os.path.join(ROOT, "include", "nidx_b200.h")).read()
     for field, want in (("m;", 30), ("m0;", 60), ("ef_construction;", 100), ("ef_search;", 30)):
         assert re.search(rf"int32_t {re.escape(field)}[^\n]*0 => {want} \*/", header), field
@@ -34,7 +27,7 @@ def test_hnsw_parameters():
 
 def test_rabitq_constants():
     """vector_types/rabitq.rs:30-36: EPSILON, RERANKING_FACTOR, RERANKING_LIMIT in the kernels, the host code and the oracle."""
-    eps, fac, lim = rust_const("vector_types/rabitq.rs", "EPSILON"), rust_const("vector_types/rabitq.rs", "RERANKING_FACTOR"), rust_const("vector_types/rabitq.rs", "RERANKING_LIMIT")
+    eps, fac, lim = FACTS["EPSILON"], FACTS["RERANKING_FACTOR"], FACTS["RERANKING_LIMIT"]
     cu = open(os.path.join(ROOT, "nucliadb_b200", "csrc", "rabitq.cuh")).read()
     assert float(re.search(r"RABITQ_EPSILON = ([0-9.]+)f", cu).group(1)) == eps
     assert float(re.search(r"RABITQ_EPSILON = ([0-9.]+)f", open(os.path.join(ROOT, "oracle", "rabitq.hpp")).read()).group(1)) == eps
@@ -51,10 +44,8 @@ def test_cost_model_matches_the_reference_source():
 
     import oracle as O
 
-    seg = open(os.path.join(REF, "segment.rs")).read()
-    body = seg[seg.index("fn use_hnsw("):]
-    body = body[: body.index("\n}\n")]
-    assert "full_cost = 16;" in body and "RERANKING_FACTOR * 3 / 4" in body and "RERANKING_FACTOR / 2" in body and ".ln() - 2.0).powi(2)" in body
+    uh = FACTS["use_hnsw"]
+    assert uh == {"full_cost": 16, "search_mult": [3, 4], "rerank_div": 2, "ln_offset": 2.0, "power": 2}
 
     def f32(x):
         import numpy as np
@@ -87,6 +78,5 @@ def test_segment_file_names():
     ours = open(os.path.join(ROOT, "nucliadb_b200", "csrc", "segment_io.hpp")).read() + open(os.path.join(ROOT, "nucliadb_b200", "csrc", "api.cu")).read() + \
         open(os.path.join(ROOT, "nucliadb_b200", "paragraph_store.py")).read() + open(os.path.join(ROOT, "nucliadb_b200", "vector.py")).read()
     for name, (path, const) in want.items():
-        m = re.search(rf'const\s+{const}\s*:\s*&str\s*=\s*"([^"]+)"', open(os.path.join(REF, path)).read())
-        assert m and m.group(1) == name, (path, const)
+        assert FACTS["file_names"][f"{path}:{const}"] == name, (path, const)
         assert f'"/{name}"' in ours or f'"{name}"' in ours, name

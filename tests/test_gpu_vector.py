@@ -162,7 +162,7 @@ def test_parts_merge_matches_kmerge():
 
 @pytest.mark.parametrize("sim,d", [(_lib.NIDX_SIM_COSINE, 384), (_lib.NIDX_SIM_DOT, 128), (_lib.NIDX_SIM_COSINE, 768)])
 def test_tensor_core_filter_scan_is_bit_exact(sim, d, monkeypatch):
-    """Batches of >= 64 queries with k <= 16 take the tcgen05 TF32 FILTER + exact REFINE path (scan_tc2.cuh): ids and scores must
+    """Batches of >= 64 queries with k <= 16 take the wgmma TF32 FILTER + exact REFINE path (scan_tc2.cuh): ids and scores must
     equal the oracle's bit for bit -- the tensor cores only decide which vectors are re-scored -- with deletions, min_score, a
     ragged last tile and a ragged last query block; NIDX_B200_SCAN=exact (the CUDA-core kernels) gives the same arrays."""
     n = 20000 + 77
