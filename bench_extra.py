@@ -5,6 +5,7 @@
   bm25   configs[3]: BM25 5M docs / 50-term queries, top-100, postings in HBM
          - "or_basic": nidx_paragraph semantics (OR of TermQuery(Basic), tf == 1)
          - "and_tf":   nidx_text semantics (conjunction, real tf) on 3-term queries
+  facets the bm25 corpus + seeded labels: OR-50 top-100 with / without faceted=["/l"], and the all-documents facet count
 
 bench.py (the driver's contract) stays the HNSW headline; this file produces the side measurements.
 """
@@ -279,6 +280,111 @@ def bench_bm25(args):
     return lines
 
 
+def gpu_identity():
+    """The card's name and power limit, read in the same process as the measurement (a number is only worth something with them)."""
+    import subprocess
+
+    import torch
+
+    out = {"name": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"], capture_output=True, text=True, timeout=30)
+        out["power_limit_and_max_sm_clock"] = q.stdout.strip()
+    except Exception as e:  # noqa: BLE001
+        out["power_limit_and_max_sm_clock"] = f"unavailable: {e}"
+    return out
+
+
+def bench_facets(args):
+    """tantivy's FacetCollector on the BM25 corpus of `bm25` plus seeded labels: /l/s{00..99}/x{00..99} (a three-level hierarchy of
+    10 k leaf labels), 1..4 labels per document, Zipf over the leaves.  Reports OR-50 top-100 with and without faceted=["/l"] (the
+    same call, alternating), the all-documents count (empty body / only_faceted catalogue) against the HBM peak and the CPU
+    restatement (tests/facet_oracle.py, numpy, one process), and exact parity with it on a sample."""
+    import torch
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import facet_oracle as FO
+    from nucliadb_b200 import _lib
+    from nucliadb_b200.segment import TextSegment
+    from nucliadb_b200.text import fieldnorm_to_id
+
+    dev = torch.device("cuda", 0)
+    n_docs, n_terms, nq, k = args.docs, 1_000_000, 1024, 100
+    c = make_corpus(n_docs, n_terms, dev)
+    lut = np.asarray([fieldnorm_to_id(i) for i in range(int(c["lens"].max()) + 1)], dtype=np.uint8)
+    df = np.diff(c["term_off"].astype(np.int64)).astype(np.uint64)
+    ts = TextSegment.create(n_docs, n_terms, c["term_off"], c["post_doc"], c["post_tf"], lut[c["lens"]])
+    ts.set_stats(n_docs, c["total_tokens"], df)
+    # labels
+    rng = np.random.default_rng(12)
+    keys = sorted(f"l\0s{a:02d}\0x{b:02d}".encode() for a in range(100) for b in range(100))
+    zipf = 1.0 / np.arange(1, len(keys) + 1) ** 1.0
+    perm = rng.permutation(len(keys))   # popularity does not follow the key order
+    n_lab = rng.integers(1, 5, n_docs)
+    doc = np.repeat(np.arange(n_docs, dtype=np.int64), n_lab)
+    leaf = perm[np.searchsorted(np.cumsum(zipf / zipf.sum()), rng.random(len(doc))).clip(max=len(keys) - 1)]
+    pairs = np.unique(doc * len(keys) + leaf)
+    ords = (pairs % len(keys)).astype(np.uint32)
+    doc_off = np.zeros(n_docs + 1, dtype=np.uint64)
+    doc_off[1:] = np.cumsum(np.bincount(pairs // len(keys), minlength=n_docs))
+    ts.set_facets(keys, doc_off, ords)
+    alive_b = rng.random(n_docs) >= 0.01
+    alive = np.packbits(alive_b, bitorder="little")
+    alive = np.concatenate([alive, np.zeros(-len(alive) % 8, np.uint8)]).view(np.uint64)
+    ts.set_alive(alive)
+    request = [b"l"]
+    # OR-50 top-100, with and without the facets, alternating
+    rng_q = np.random.default_rng(11)
+    band = np.nonzero((df >= 1_000) & (df <= 100_000))[0]
+    queries = [rng_q.choice(band, 50, replace=False).astype(np.uint32) for _ in range(nq)]
+    qoff = torch.tensor(np.concatenate([[0], np.cumsum([len(x) for x in queries])]), dtype=torch.int32, device=dev)
+    qt = torch.tensor(np.concatenate(queries).astype(np.int64), dtype=torch.int32, device=dev)
+    out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
+           torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev))
+    plain_fn = lambda: ts.search(qt, qoff, k, mode=_lib.NIDX_BM25_OR, use_tf=False, out=out)
+    facet_fn = lambda: ts.search_faceted(qt, qoff, k, request, mode=_lib.NIDX_BM25_OR, use_tf=False)
+    plain_ms, facet_ms, plain_kms, facet_kms = [], [], [], []
+    for _ in range(5):
+        plain_ms.append(timed(plain_fn, args.steps, args.warmup)); plain_kms.append(ts.last_kernel_ms())
+        facet_ms.append(timed(facet_fn, args.steps, args.warmup)); facet_kms.append(ts.last_kernel_ms())
+    med = lambda x: float(np.median(x))
+    # parity on a sample: top-k / Count bit for bit against the search without facets, counts against the restatement
+    fd, fs, fc, ft, fcnt = facet_fn()
+    plain_fn()
+    torch.cuda.synchronize()
+    same_search = all(torch.equal(a, b) for a, b in zip(out, (fd, fs, fc, ft)))
+    bucket, b_req, _ = FO.plan(keys, request)
+    sample = 8
+    got = fcnt[:sample].cpu().numpy().astype(np.int64)
+    want = np.stack([FO.count(doc_off, ords, bucket, len(b_req), FO.matched(n_docs, c["term_off"], c["post_doc"], q.tolist(), False, alive)) for q in queries[:sample]])
+    # all documents
+    all_fn = lambda: ts.facet_count_all(request, device_out=True)
+    all_ms = timed(all_fn, args.steps, args.warmup)
+    all_kms = ts.last_kernel_ms()
+    dev_all = all_fn().cpu().numpy().astype(np.int64)
+    t0 = time.perf_counter()
+    cpu_all = FO.count(doc_off, ords, bucket, len(b_req), alive_b)
+    cpu_s = time.perf_counter() - t0
+    nbytes = 4 * (n_docs + 1) + 4 * len(ords) + 8 * len(alive)
+    pk = float(peaks().get("hbm_gbs", 3350.0))
+    ach = nbytes / (all_kms * 1e-3) / 1e9
+    return [{"metric": "facet overhead (OR-50 top-100, faceted=[\"/l\"])", "value": med(facet_ms) / med(plain_ms), "unit": "x (faceted / plain call)", "n_gpus": 1,
+             "steps": args.steps, "warmup": args.warmup, "gpu": gpu_identity(), "higher_is_better": False, "data": "synthetic",
+             "config": {"workload": f"BM25 {n_docs} docs / 50-term OR queries x {nq}, top-{k}, tf == 1", "facet_keys": len(keys), "facet_ords": int(len(ords)),
+                        "buckets": int(len(b_req)), "rounds": 5},
+             "plain": {"ms_per_call": med(plain_ms), "kernel_ms": med(plain_kms), "kernel": "bm25_kernel"},
+             "faceted": {"ms_per_call": med(facet_ms), "kernel_ms": med(facet_kms), "kernel": "bm25_facet_kernel"},
+             "kernel_ratio": med(facet_kms) / med(plain_kms),
+             "parity": {"search_identical_to_plain": bool(same_search), "counts_identical_to_oracle": bool(np.array_equal(got, want)), "sample": sample}},
+            {"metric": "facet count, all documents", "value": all_ms, "unit": "ms", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "gpu": gpu_identity(),
+             "higher_is_better": False, "data": "synthetic",
+             "config": {"workload": f"FacetCollector over {n_docs} alive-masked documents, faceted=[\"/l\"]", "facet_ords": int(len(ords)), "buckets": int(len(b_req))},
+             "roofline": {"bound": "hbm", "achieved": ach, "peak": pk, "unit": "GB/s", "frac": ach / pk, "kernel": "facet_count_all_kernel", "kernel_ms": all_kms,
+                          "alg_bytes": nbytes, "alg_bytes_note": "doc_off (4 B per document) + ords (4 B each) + alive bits, each read once"},
+             "parity": {"counts_identical_to_oracle": bool(np.array_equal(dev_all, cpu_all))},
+             "cpu_baseline": {"value": cpu_s * 1e3, "unit": "ms", "cores": 1, "kind": "numpy restatement (tests/facet_oracle.py), one process"}}]
+
+
 def bench_rabitq(args):
     """SURVEY 8f rank 1: the HNSW walk with a RaBitQ query on a Dot index (hnsw/search.rs:306-383: estimate-ranked walk, k * 100
     layer-0 results, exact rerank) -- what the reference runs on every Dot index that carries vectors.quant -- next to the dense
@@ -360,7 +466,7 @@ def driver_extras(steps=5, warmup=3):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("which", choices=["scan", "bm25", "build", "merge", "rabitq", "all"])
+    ap.add_argument("which", choices=["scan", "bm25", "build", "merge", "rabitq", "facets", "all"])
     ap.add_argument("--build-vectors", type=int, default=1_000_000)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
@@ -377,6 +483,8 @@ def main():
         lines += bench_merge(args)
     if args.which == "rabitq":
         lines += bench_rabitq(args)
+    if args.which == "facets":
+        lines += bench_facets(args)
     for line in lines:
         print(json.dumps(line))
 

@@ -265,9 +265,50 @@ int nidx_txt_search(nidx_txt_segment* seg, const uint32_t* query_terms, const ui
                     const nidx_txt_search_params* p, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total,
                     void* stream);
 
-/* Device time (CUDA events on the caller's stream) of bm25_kernel in the last nidx_txt_search on this segment (bench roofline);
- * not meaningful under concurrent searches. */
+/* Device time (CUDA events on the caller's stream) of bm25_kernel in the last nidx_txt_search on this segment (bench roofline),
+ * or of the facet kernel of the last nidx_txt_search_faceted / nidx_txt_facet_count_all; not meaningful under concurrent searches. */
 int nidx_txt_last_kernel_ms(nidx_txt_segment* seg, float* ms);
+
+/* ---- Facet counts: tantivy's FacetCollector next to Count and TopDocs
+ * (reference: the (Count, facet_collector, topdocs) tuples of nidx_text/src/reader.rs:388-450 and
+ *  nidx_paragraph/src/reader.rs:252-347; groups produced by produce_facets, nidx_text/src/reader.rs:43-62 and
+ *  nidx_paragraph/src/search_response.rs:48-77)
+ * A facet is given in tantivy's encoded form: the path's segments joined by 0x00 bytes, without the leading '/'
+ * ("/l/set/a" -> "l\0set\0a"); the root "/" is the empty string.  Facet order = memcmp order of the encoded bytes. */
+
+/* The segment's facet dictionary and every document's facets: n_facets keys, strictly ascending in facet order, key i =
+ * key_bytes[key_off[i] .. key_off[i + 1]); document d carries the ords doc_ords[doc_off[d] .. doc_off[d + 1]) (strictly
+ * ascending; doc_off has n_docs + 1 entries).  The keys stay on the host side of the library (a request is resolved by binary
+ * search: the descendants of a facet are one ord range), the ords live in HBM.  Segments of one index should be given the same
+ * dictionary, so that a bucket means the same child in every segment and per-segment counts add up as arrays.  Host pointers. */
+int nidx_txt_set_facets(nidx_txt_segment* seg, uint32_t n_facets, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
+                        const uint32_t* doc_ords);
+
+typedef struct nidx_txt_facet_request {   /* FacetCollector::add_facet for each facet: facet i = key_bytes[key_off[i] .. key_off[i + 1]) */
+    int32_t n;
+    const uint8_t* key_bytes;
+    const uint64_t* key_off;
+} nidx_txt_facet_request;
+
+/* The buckets of a request: one per direct child of a requested facet that the dictionary holds, requested facets taken in facet
+ * order (duplicates collapse), children in facet order.  out_bucket_req[b] = index of the request that bucket b belongs to,
+ * out_bucket_ord[b] = the first dictionary ord under its child (the child is that key cut after the requested facet's depth + 1).
+ * At most `cap` entries are written (n_facets is always enough); *out_n_buckets = the number of buckets.  A requested facet that
+ * is an ancestor of another is NIDX_EINVAL (tantivy asserts).  Host pointers; needs no device work. */
+int nidx_txt_facet_buckets(nidx_txt_segment* seg, const nidx_txt_facet_request* facets, uint32_t* out_bucket_req, uint32_t* out_bucket_ord,
+                           uint32_t cap, uint32_t* out_n_buckets);
+
+/* nidx_txt_search + the FacetCollector in the same pass: docs / scores / counts / totals are those of nidx_txt_search, and
+ * out_facet_counts[nq][n_buckets] (`mem`, u32) = for each bucket the number of matched documents (query match AND alive: the set
+ * out_total counts, whatever k, min_score or search-after) that carry its child or a descendant of it, once per document.
+ * A facet equal to the requested one counts nothing. */
+int nidx_txt_search_faceted(nidx_txt_segment* seg, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem,
+                            const nidx_txt_search_params* p, const nidx_txt_facet_request* facets, uint32_t* out_docs, float* out_scores,
+                            int32_t* out_counts, uint64_t* out_total, uint32_t* out_facet_counts, void* stream);
+
+/* The same counts over every alive document (the AllQuery of an empty body, nidx_text/src/search_query.rs:100-101: the
+ * only_faceted catalogue request): out_facet_counts[n_buckets] (`mem`, u32). */
+int nidx_txt_facet_count_all(nidx_txt_segment* seg, const nidx_txt_facet_request* facets, int mem, uint32_t* out_facet_counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Segments sharded over the GPUs of one node: one process (or thread) per GPU, one segment each

@@ -27,6 +27,7 @@ SYMBOLS = [
     "nidx_vec_search", "nidx_merge_topk", "nidx_vec_counters", "nidx_vec_counters_ex", "nidx_vec_last_kernel_ms",
     "nidx_vec_rabitq_encode", "nidx_vec_rabitq_codes", "nidx_vec_rabitq_estimate",
     "nidx_txt_create", "nidx_txt_set_stats", "nidx_txt_set_alive", "nidx_txt_close", "nidx_txt_search", "nidx_txt_last_kernel_ms",
+    "nidx_txt_set_facets", "nidx_txt_facet_buckets", "nidx_txt_search_faceted", "nidx_txt_facet_count_all",
     "nidx_shard_unique_id", "nidx_shard_init", "nidx_shard_destroy", "nidx_vec_set_paragraph_keys", "nidx_vec_search_sharded", "nidx_txt_search_sharded",
     "nidx_txt_set_doc_keys", "nidx_rank_fusion_rrf", "nidx_shard_search",
 ]
@@ -61,6 +62,10 @@ NIDX_F_LABEL, NIDX_F_KEYS, NIDX_F_AND, NIDX_F_OR, NIDX_F_NOT = 0, 1, 2, 3, 4
 class TxtSearchParams(C.Structure):
     _fields_ = [("k", C.c_int32), ("mode", C.c_int32), ("use_tf", C.c_int32), ("min_score", C.c_float), ("after_mode", C.c_int32),
                 ("after_score", C.c_float), ("after_docaddr", C.c_uint64), ("docaddr_base", C.c_uint64)]
+
+
+class TxtFacetRequest(C.Structure):
+    _fields_ = [("n", C.c_int32), ("key_bytes", C.c_void_p), ("key_off", C.c_void_p)]
 
 
 class RrfSource(C.Structure):

@@ -6,7 +6,7 @@ Reference:
                                                                    searcher_port, api_port
   nidx/nidx_protos/nidx.proto:9,20-21                             NidxApi.NewShard, NidxSearcher.Search
   nidx/src/searcher/shard_search.rs:60-241                        one SearchRequest -> prefilter -> vector / paragraph / document searches
-  nidx/src/searcher/shard_merge.rs:177-348                        merge of the per-shard responses
+  nidx/src/searcher/shard_merge.rs:177-348, 380-414               merge of the per-shard responses (merge_facets: facet counts)
   nidx/nidx_vector/src/indexer.rs:96-146                          Resource -> vector Elems (key = sentence id, labels = paragraph labels)
   nidx/nidx_text/src/resource_indexer.rs:22-91                    Resource.texts -> one document per field
   nidx/nidx_paragraph/src/resource_indexer.rs:33-131              Resource.paragraphs -> one document per paragraph (text[start:end])
@@ -83,6 +83,21 @@ def _doc_matches(e, doc: T.TextDoc) -> bool:
     if kind == "bool_or":
         return any(_doc_matches(o, doc) for o in e.bool_or.operands)
     return True
+
+
+def merge_facets(shards_facets) -> dict:
+    """shard_merge.rs:380-414: the counts of equal (group, tag) pairs of the shards' facet maps ({group: [(tag, total)]}) are
+    summed; the merged lists are not cut again.  The reference lists them in a HashMap's order; here count descending, then tag
+    in facet order."""
+    counts: dict = {}
+    for facets in shards_facets:
+        for group, values in facets.items():
+            for tag, total in values:
+                counts[(group, tag)] = counts.get((group, tag), 0) + int(total)
+    merged: dict = {}
+    for (group, tag), total in counts.items():
+        merged.setdefault(group, []).append((tag, total))
+    return {g: sorted(v, key=lambda t: (-t[1], T.facet_key(t[0]) or b"")) for g, v in merged.items()}
 
 
 class NidxBinding:
@@ -264,12 +279,14 @@ class NidxBinding:
                                          filter_operator=V.FilterOperator.Or if req.filter_operator == P.FILTER_OR else V.FilterOperator.And)
             out["vector"] = vi.searcher.search(vreq, prefilter).documents if vi.searcher is not None else []
         if req.document and shard.text_searcher is not None:
-            out["document"] = shard.text_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25)))
+            out["document"] = shard.text_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25),
+                                                                                 faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted)))
         if req.paragraph and shard.paragraph_searcher is not None:
             after = None
             if req.HasField("search_after"):
                 after = T.SearchAfter(score=req.search_after.score, tie_break="keep_after", docaddr=int(req.search_after.docaddr))
-            out["paragraph"] = shard.paragraph_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25), search_after=after))
+            out["paragraph"] = shard.paragraph_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25), search_after=after,
+                                                                                       faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted)))
         return out
 
     def _merge(self, req, parts):
@@ -293,6 +310,8 @@ class NidxBinding:
             target.total = sum(rs.total for _, rs in found)
             target.next_page = any(rs.next_page for _, rs in found) or len(rows) > k
             target.query = req.body
+            for group, values in merge_facets([{g: [(f.tag, f.total) for f in v] for g, v in rs.facets.items()} for _, rs in found]).items():
+                target.facets[group].facetresults.extend(P.FacetResult(tag=tag, total=total) for tag, total in values)
             for _, _, _, sid, r in rows[:k]:
                 o = target.results.add()
                 o.uuid, o.field = r.uuid, r.field

@@ -74,13 +74,13 @@ struct DevBuf {
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
-    DevBuf queries, qnorms, out_ids, out_scores, out_counts, scores, partial, filter, misc, sched;
+    DevBuf queries, qnorms, out_ids, out_scores, out_counts, scores, partial, filter, misc, sched, facets;
     cudaEvent_t done = nullptr;
     cudaStream_t last_stream = nullptr;
     bool busy = false;
     ~Workspace() {
         queries.release(); qnorms.release(); out_ids.release(); out_scores.release(); out_counts.release();
-        scores.release(); partial.release(); filter.release(); misc.release(); sched.release();
+        scores.release(); partial.release(); filter.release(); misc.release(); sched.release(); facets.release();
         if (done) cudaEventDestroy(done);
     }
 };
@@ -1764,6 +1764,11 @@ struct nidx_txt_segment {
     uint64_t own_tokens = 0;
     float max_weight = 0.0f;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around bm25_kernel of the last search (bench roofline)
+    // facets (nidx_txt_set_facets): the dictionary on the host in facet order, every document's ords (CSR) in HBM
+    std::vector<std::string> facet_keys;
+    uint32_t* d_fdoc_off = nullptr;   // [n_docs + 1]
+    uint32_t* d_ford = nullptr;       // [n_facet_ords]
+    uint64_t n_facet_ords = 0;
     WorkspacePool pool;
 };
 
@@ -1884,7 +1889,7 @@ void nidx_txt_close(nidx_txt_segment* t) {
     cudaSetDevice(t->device);
     cudaDeviceSynchronize();
     cudaFree(t->d_term_off); cudaFree(t->d_post); cudaFree(t->d_skip_row); cudaFree(t->d_skip); cudaFree(t->d_alive); cudaFree(t->d_weight);
-    cudaFree(t->d_norm_cache); cudaFree(t->d_error); cudaFree(t->d_doc_keys);
+    cudaFree(t->d_norm_cache); cudaFree(t->d_error); cudaFree(t->d_doc_keys); cudaFree(t->d_fdoc_off); cudaFree(t->d_ford);
     if (t->ev_k0) cudaEventDestroy(t->ev_k0);
     if (t->ev_k1) cudaEventDestroy(t->ev_k1);
     delete t;
@@ -1898,14 +1903,105 @@ int nidx_txt_last_kernel_ms(nidx_txt_segment* t, float* ms) {
     return 0;
 }
 
+int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
+                        const uint32_t* doc_ords) {
+    if (!t || !doc_off || (n_facets && (!key_bytes || !key_off))) return fail(NIDX_EINVAL, "null argument");
+    std::vector<std::string> keys(n_facets);
+    for (uint32_t i = 0; i < n_facets; ++i) {
+        keys[i].assign(reinterpret_cast<const char*>(key_bytes) + key_off[i], key_off[i + 1] - key_off[i]);
+        if (i && !(keys[i - 1] < keys[i])) return fail(NIDX_EINVAL, "facet keys must be strictly ascending (facet order)");
+    }
+    const uint64_t nnz = doc_off[t->n_docs];
+    if (nnz >= (1ull << 32)) return fail(NIDX_EINVAL, "at most 2^32-1 facet ords per segment");
+    if (nnz && !doc_ords) return fail(NIDX_EINVAL, "null argument");
+    std::vector<uint32_t> off(t->n_docs + 1);
+    for (uint32_t d = 0; d <= t->n_docs; ++d) {
+        if (d && doc_off[d] < doc_off[d - 1]) return fail(NIDX_EINVAL, "doc_off must be non-decreasing");
+        off[d] = (uint32_t)doc_off[d];
+    }
+    for (uint32_t d = 0; d < t->n_docs; ++d)
+        for (uint64_t i = doc_off[d]; i < doc_off[d + 1]; ++i)
+            if (doc_ords[i] >= n_facets || (i > doc_off[d] && doc_ords[i] <= doc_ords[i - 1]))
+                return fail(NIDX_EINVAL, "document %u: facet ords must be < n_facets and strictly ascending", d);
+    CU(cudaSetDevice(t->device));
+    cudaFree(t->d_fdoc_off); cudaFree(t->d_ford);
+    t->d_fdoc_off = nullptr; t->d_ford = nullptr;
+    t->facet_keys.clear(); t->n_facet_ords = 0;
+    CU(cudaMalloc(&t->d_fdoc_off, ((size_t)t->n_docs + 1) * 4));
+    CU(cudaMalloc(&t->d_ford, std::max<uint64_t>(nnz, 1) * 4));
+    CU(cudaMemcpy(t->d_fdoc_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (nnz) CU(cudaMemcpy(t->d_ford, doc_ords, nnz * 4, cudaMemcpyHostToDevice));
+    t->facet_keys = std::move(keys);
+    t->n_facet_ords = nnz;
+    return 0;
+}
+
 }  // extern "C"
 
-typedef void (*bm_kernel_t)(TxtDev, Bm25Args);
+// A facet request resolved against the segment's dictionary: bucket[ord] = the bucket of the requested facet's child the ord lies
+// under (NIL: none), and per bucket the request it belongs to and the first ord under its child (what names it).  Requests are
+// taken in facet order, so buckets ascend with the ord.
+struct FacetPlan {
+    std::vector<uint32_t> bucket, b_req, b_ord;
+};
 
-// The body of nidx_txt_search.  qhost / ohost as in vec_search_impl.
+static int facet_plan(const nidx_txt_segment* t, const nidx_txt_facet_request* r, FacetPlan& P) {
+    if (!r || r->n < 0 || (r->n && (!r->key_bytes || !r->key_off))) return fail(NIDX_EINVAL, "bad facet request");
+    if (!t->d_fdoc_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
+    std::vector<std::pair<std::string, int>> req;
+    for (int i = 0; i < r->n; ++i) req.emplace_back(std::string(reinterpret_cast<const char*>(r->key_bytes) + r->key_off[i], r->key_off[i + 1] - r->key_off[i]), i);
+    std::sort(req.begin(), req.end());
+    req.erase(std::unique(req.begin(), req.end(), [](const auto& x, const auto& y) { return x.first == y.first; }), req.end());   // duplicates collapse
+    // tantivy's FacetCollector::add_facet asserts that no requested facet is an ancestor of another: here an error.  In facet
+    // order an ancestor is immediately followed by one of its descendants (the root "" by anything).
+    for (size_t i = 0; i + 1 < req.size(); ++i) {
+        const std::string &a = req[i].first, &b = req[i + 1].first;
+        if (a.empty() || (b.size() > a.size() && b.compare(0, a.size(), a) == 0 && b[a.size()] == '\0'))
+            return fail(NIDX_EINVAL, "a requested facet is an ancestor of another requested facet");
+    }
+    const std::vector<std::string>& K = t->facet_keys;
+    P.bucket.assign(K.size(), NIDX_NIL);
+    P.b_req.clear(); P.b_ord.clear();
+    for (const auto& [f, idx] : req) {
+        const std::string prefix = f.empty() ? f : f + '\0';   // the root's children are the top-level facets
+        size_t o = std::lower_bound(K.begin(), K.end(), prefix) - K.begin();
+        std::string child;
+        for (; o < K.size() && K[o].compare(0, prefix.size(), prefix) == 0; ++o) {
+            if (K[o].size() == prefix.size()) continue;   // the root key "": the requested facet itself counts nothing
+            size_t end = K[o].find('\0', prefix.size());
+            std::string c = K[o].substr(0, end);
+            if (P.b_req.empty() || c != child) { child = c; P.b_req.push_back((uint32_t)idx); P.b_ord.push_back((uint32_t)o); }
+            P.bucket[o] = (uint32_t)P.b_req.size() - 1;
+        }
+    }
+    return 0;
+}
+
+// Uploads the plan's collapse table into the workspace and fills F (the counts go to d_out: [rows][n_buckets]).
+static int facet_args(const nidx_txt_segment* t, const FacetPlan& P, Workspace& w, uint32_t* d_out, cudaStream_t stream, FacetArgs& F) {
+    ENSURE(w.facets, std::max<size_t>(P.bucket.size(), 1) * 4);
+    if (!P.bucket.empty()) CU(cudaMemcpyAsync(w.facets.p, P.bucket.data(), P.bucket.size() * 4, cudaMemcpyHostToDevice, stream));
+    F.doc_off = t->d_fdoc_off; F.ords = t->d_ford; F.bucket = w.facets.as<uint32_t>();
+    F.n_buckets = (uint32_t)P.b_req.size();
+    F.smem = F.n_buckets <= FACET_SMEM_BUCKETS;
+    F.out = d_out;
+    return 0;
+}
+
+typedef void (*bm_kernel_t)(TxtDev, Bm25Args);
+typedef void (*bm_facet_kernel_t)(TxtDev, Bm25Args, FacetArgs);
+
+// The body of nidx_txt_search (facets == nullptr) and nidx_txt_search_faceted.  qhost / ohost as in vec_search_impl.
 static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, bool qhost, bool ohost,
-                           const nidx_txt_search_params* p, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total, cudaStream_t stream) {
+                           const nidx_txt_search_params* p, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total, cudaStream_t stream,
+                           const nidx_txt_facet_request* facets = nullptr, uint32_t* out_facet_counts = nullptr) {
     if (!t || !p || !query_off || !out_docs || !out_scores || !out_counts) return fail(NIDX_EINVAL, "null argument");
+    FacetPlan plan;
+    if (facets) {
+        if (!out_facet_counts) return fail(NIDX_EINVAL, "null argument");
+        int r = facet_plan(t, facets, plan);
+        if (r) return r;
+    }
     if (nq <= 0) return 0;
     int k = p->k;
     if (k <= 0 || k > 1024) return fail(NIDX_EINVAL, "k must be in 1..1024");
@@ -1956,12 +2052,32 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache; a.shift = shift;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
     a.out_keys = w.partial.as<uint64_t>(); a.out_total = d_total; a.error_flag = t->d_error;
-    bm_kernel_t kern = conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>);
-    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CU(cudaEventRecord(t->ev_k0, stream));
-    kern<<<nq, BM_THREADS, smem, stream>>>(T, a);
-    CU(cudaEventRecord(t->ev_k1, stream));
-    LAUNCHED();
+    if (!facets) {
+        bm_kernel_t kern = conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>);
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(cudaEventRecord(t->ev_k0, stream));
+        kern<<<nq, BM_THREADS, smem, stream>>>(T, a);
+        CU(cudaEventRecord(t->ev_k1, stream));
+        LAUNCHED();
+    } else {
+        const size_t nb = plan.b_req.size();
+        uint32_t* d_fc = out_facet_counts;
+        if (ohost) { ENSURE(w.scores, std::max<size_t>((size_t)nq * nb, 1) * 4); d_fc = w.scores.as<uint32_t>(); }
+        FacetArgs F;
+        int r = facet_args(t, plan, w, d_fc, stream, F);
+        if (r) return r;
+        if (F.smem && smem + nb * 4 > 220 * 1024) F.smem = 0;
+        if (!F.smem && nb) CU(cudaMemsetAsync(d_fc, 0, (size_t)nq * nb * 4, stream));
+        const size_t fsmem = smem + (F.smem ? nb * 4 : 0);
+        bm_facet_kernel_t kern = conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
+                                      : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>);
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+        CU(cudaEventRecord(t->ev_k0, stream));
+        kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F);
+        CU(cudaEventRecord(t->ev_k1, stream));
+        LAUNCHED();
+        if (ohost && nb) CU(cudaMemcpyAsync(out_facet_counts, d_fc, (size_t)nq * nb * 4, cudaMemcpyDeviceToHost, stream));
+    }
     bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
     LAUNCHED();
     CU(cudaGetLastError());
@@ -1984,6 +2100,60 @@ int nidx_txt_search(nidx_txt_segment* t, const uint32_t* query_terms, const uint
                     uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total, void* stream_) {
     bool host = mem == NIDX_MEM_HOST;
     return txt_search_impl(t, query_terms, query_off, nq, host, host, p, out_docs, out_scores, out_counts, out_total, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+int nidx_txt_facet_buckets(nidx_txt_segment* t, const nidx_txt_facet_request* facets, uint32_t* out_bucket_req, uint32_t* out_bucket_ord, uint32_t cap,
+                           uint32_t* out_n_buckets) {
+    if (!t || !out_n_buckets) return fail(NIDX_EINVAL, "null argument");
+    FacetPlan plan;
+    int r = facet_plan(t, facets, plan);
+    if (r) return r;
+    const size_t n = std::min<size_t>(plan.b_req.size(), cap);
+    if (n && (!out_bucket_req || !out_bucket_ord)) return fail(NIDX_EINVAL, "null argument");
+    if (n) { memcpy(out_bucket_req, plan.b_req.data(), n * 4); memcpy(out_bucket_ord, plan.b_ord.data(), n * 4); }
+    *out_n_buckets = (uint32_t)plan.b_req.size();
+    return 0;
+}
+
+int nidx_txt_search_faceted(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem, const nidx_txt_search_params* p,
+                            const nidx_txt_facet_request* facets, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total,
+                            uint32_t* out_facet_counts, void* stream_) {
+    if (!facets) return fail(NIDX_EINVAL, "null argument");
+    bool host = mem == NIDX_MEM_HOST;
+    return txt_search_impl(t, query_terms, query_off, nq, host, host, p, out_docs, out_scores, out_counts, out_total, reinterpret_cast<cudaStream_t>(stream_),
+                           facets, out_facet_counts);
+}
+
+int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* facets, int mem, uint32_t* out_facet_counts, void* stream_) {
+    if (!t || !out_facet_counts) return fail(NIDX_EINVAL, "null argument");
+    FacetPlan plan;
+    int r = facet_plan(t, facets, plan);
+    if (r) return r;
+    const size_t nb = plan.b_req.size();
+    if (!nb) return 0;
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(t->device));
+    WsGuard g(t->pool, stream);
+    Workspace& w = *g.w;
+    uint32_t* d_fc = out_facet_counts;
+    if (host) { ENSURE(w.scores, nb * 4); d_fc = w.scores.as<uint32_t>(); }
+    FacetArgs F;
+    r = facet_args(t, plan, w, d_fc, stream, F);
+    if (r) return r;
+    CU(cudaMemsetAsync(d_fc, 0, nb * 4, stream));
+    const int threads = 256;
+    const int blocks = std::max(1, std::min<int>(t->sm_count * (2048 / threads), (int)((t->n_docs + threads - 1) / threads)));
+    CU(cudaEventRecord(t->ev_k0, stream));
+    facet_count_all_kernel<<<blocks, threads, F.smem ? nb * 4 : 0, stream>>>(t->n_docs, t->d_alive, F);
+    CU(cudaEventRecord(t->ev_k1, stream));
+    LAUNCHED();
+    CU(cudaGetLastError());
+    if (host) {
+        CU(cudaMemcpyAsync(out_facet_counts, d_fc, nb * 4, cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+    }
+    return 0;
 }
 
 // ---- sharded search (shard.cuh) -------------------------------------------------------------------

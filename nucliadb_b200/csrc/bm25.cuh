@@ -112,6 +112,80 @@ __global__ void bm25_build_skip_kernel(const uint64_t* __restrict__ term_off, co
     }
 }
 
+// ---- facet counts (tantivy FacetCollector, nidx_text/src/reader.rs:388-450, nidx_paragraph/src/reader.rs:252-347) ----------
+// The segment's facets are a dictionary in facet order (host side) and every document's facet ords, ascending, in CSR form
+// (HBM).  A request maps every ord to the bucket of the requested facet's child it lies under, or NIL (the host's collapse
+// table); buckets ascend with the ord, so the repeats of one bucket among a document's ords are adjacent and a document adds one
+// to each of its buckets once.
+struct FacetArgs {
+    const uint32_t* doc_off;   // [n_docs + 1]
+    const uint32_t* ords;      // [doc_off[n_docs]]
+    const uint32_t* bucket;    // [n_facets] ord -> bucket or NIL
+    uint32_t n_buckets;
+    int smem;                  // 1: one CTA counts into shared memory and writes its row / adds its histogram; 0: global atomics
+    uint32_t* out;             // [nq][n_buckets]
+};
+constexpr uint32_t FACET_SMEM_BUCKETS = 4096;   // 16 KB of shared counters at most (bm25: beside the ~80 KB of a k <= 128 search)
+
+__device__ __forceinline__ void facet_doc(const FacetArgs& F, uint32_t doc, uint32_t* cnt) {
+    const uint32_t e = F.doc_off[doc + 1];
+    uint32_t prev = NIL;
+    for (uint32_t i = F.doc_off[doc]; i < e; ++i) {
+        uint32_t b = __ldg(F.bucket + __ldg(F.ords + i));
+        if (b != NIL && b != prev) { atomicAdd(cnt + b, 1u); prev = b; }
+    }
+}
+
+// FACET_BATCH documents at once (NIL = none): their offsets, then their ords step by step, are independent loads in flight
+// together -- a document alone is a chain of three dependent loads, and a pass over many documents is bound by its latency.
+constexpr int FACET_BATCH = 4;
+__device__ __forceinline__ void facet_docs(const FacetArgs& F, const uint32_t (&doc)[FACET_BATCH], uint32_t* cnt) {
+    uint32_t b[FACET_BATCH], e[FACET_BATCH], prev[FACET_BATCH];
+#pragma unroll
+    for (int j = 0; j < FACET_BATCH; ++j) {
+        b[j] = doc[j] != NIL ? __ldg(F.doc_off + doc[j]) : 0;
+        e[j] = doc[j] != NIL ? __ldg(F.doc_off + doc[j] + 1) : 0;
+        prev[j] = NIL;
+    }
+    for (bool more = true; more;) {
+        uint32_t bk[FACET_BATCH];
+        more = false;
+#pragma unroll
+        for (int j = 0; j < FACET_BATCH; ++j) bk[j] = b[j] < e[j] ? __ldg(F.ords + b[j]) : NIL;
+#pragma unroll
+        for (int j = 0; j < FACET_BATCH; ++j) bk[j] = bk[j] != NIL ? __ldg(F.bucket + bk[j]) : NIL;
+#pragma unroll
+        for (int j = 0; j < FACET_BATCH; ++j) {
+            if (b[j] < e[j]) { ++b[j]; more |= b[j] < e[j]; }
+            if (bk[j] != NIL && bk[j] != prev[j]) { atomicAdd(cnt + bk[j], 1u); prev[j] = bk[j]; }
+        }
+    }
+}
+
+// The matched-everything count (AllQuery: empty body / only_faceted catalogue): one pass over the CSR and the alive bits, a
+// histogram per block in shared memory (F.smem) added to F.out[0][*] at the end.
+__global__ void facet_count_all_kernel(uint32_t n_docs, const uint64_t* __restrict__ alive, FacetArgs F) {
+    extern __shared__ uint32_t hist[];
+    uint32_t* cnt = F.smem ? hist : F.out;
+    if (F.smem) for (uint32_t i = threadIdx.x; i < F.n_buckets; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const uint32_t stride = gridDim.x * blockDim.x;   // a thread takes FACET_BATCH documents `stride` apart: every load stays coalesced
+    for (uint32_t d0 = blockIdx.x * blockDim.x + threadIdx.x; d0 < n_docs; d0 += FACET_BATCH * stride) {
+        uint32_t dd[FACET_BATCH];
+#pragma unroll
+        for (int j = 0; j < FACET_BATCH; ++j) {
+            uint32_t d = d0 + j * stride;
+            dd[j] = d < n_docs && (!alive || ((alive[d >> 6] >> (d & 63)) & 1ull)) ? d : NIL;
+        }
+        facet_docs(F, dd, cnt);
+    }
+    if (F.smem) {
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < F.n_buckets; i += blockDim.x)
+            if (hist[i]) atomicAdd(F.out + i, hist[i]);
+    }
+}
+
 __host__ __device__ __forceinline__ size_t bm_smem_bytes(int cap, bool conj) {
     return (size_t)cap * 8 + 2 * BM_MAX_TERMS * 8 /* run start */ + BM_WORDS * 4 /* bitmap */ + BM_ACC * 4 /* acc */ + BM_ACC * 4 /* candidates */ +
            2 * BM_MAX_TERMS * 4 /* run length */ + BM_MAX_TERMS * 4 /* weights */ + 1024 /* norm / ratio table */ + BM_WORDS * 2 /* rank bases */ +
@@ -126,8 +200,10 @@ __device__ __forceinline__ uint2 ldg_post(const uint2* p) {
 }
 
 // CONJ: nidx_text (all terms must match).  TF: real term frequencies (else IndexRecordOption::Basic, tf == 1).
-template <bool CONJ, bool TF>
-__global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T, Bm25Args a) {
+// FACET: the FacetCollector runs beside Count on the same matched documents (bm25_facet_kernel); with FACET false every facet
+// statement compiles away and bm25_kernel is the search without facets.
+template <bool CONJ, bool TF, bool FACET>
+__device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, const FacetArgs& F) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int tk_count;
     __shared__ uint64_t tk_thr;
@@ -153,8 +229,13 @@ __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T,
     uint64_t* t_end = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;           // term_off[term + 1]
     uint64_t* t_cur = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;           // first posting not yet assigned to a tile
     uint64_t* t_skip = reinterpret_cast<uint64_t*>(p);                                 // offset of the term's skip row, ~0 = none
-
     const int q = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t* fcnt = nullptr;   // FACET: this query's bucket counts (shared memory past the term state, or its row of F.out)
+    if (FACET) {
+        fcnt = F.smem ? reinterpret_cast<uint32_t*>(t_skip + BM_MAX_TERMS) : F.out + (size_t)q * F.n_buckets;
+        if (F.smem) for (uint32_t i = threadIdx.x; i < F.n_buckets; i += BM_THREADS) fcnt[i] = 0;
+    }
+
     const uint32_t* terms = a.query_terms + a.query_off[q];
     int nt = (int)(a.query_off[q + 1] - a.query_off[q]);
     if (nt > BM_MAX_TERMS) nt = BM_MAX_TERMS;
@@ -273,6 +354,7 @@ __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T,
         bool match = true;
         if (T.alive) match = (T.alive[doc >> 6] >> (doc & 63)) & 1;
         if (CONJ && match) my_hits++;
+        if (FACET && CONJ && match) facet_doc(F, doc, fcnt);   // AND: every completed conjunction is a candidate
         if (match) {
             float score = __fdiv_rn((float)v, scale);
             bool after = true;   // is_after(): strictly lower score, or an equal score that the tie break keeps
@@ -449,6 +531,22 @@ __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T,
                     }
                 }
             }
+            if (FACET && !CONJ) {   // OR: the documents phase S counted (bitmap AND alive), FACET_BATCH at a time per thread
+                const uint32_t* al = T.alive ? reinterpret_cast<const uint32_t*>(T.alive) + (lo >> 5) : nullptr;
+                int w = (int)threadIdx.x - BM_THREADS;   // this thread's words: threadIdx.x, + BM_THREADS, ...
+                uint32_t v = 0;
+                for (;;) {
+                    uint32_t dd[FACET_BATCH];
+#pragma unroll
+                    for (int j = 0; j < FACET_BATCH; ++j) {
+                        while (v == 0 && w + BM_THREADS < nwords) { w += BM_THREADS; v = bitmap[w]; if (v && al) v &= al[w]; }
+                        dd[j] = v ? lo + 32u * (uint32_t)w + (uint32_t)(__ffs(v) - 1) : NIL;
+                        v &= v - 1;
+                    }
+                    if (dd[0] == NIL) break;
+                    facet_docs(F, dd, fcnt);
+                }
+            }
             __syncthreads();
             // ---- phase D: candidates -> top-k buffer; warp 0 resolves the next tile meanwhile ----
             // The branch below must be uniform: it is taken on the buffer fill recorded at the end of the previous tile
@@ -499,6 +597,19 @@ __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T,
     uint64_t* out = a.out_keys + (size_t)q * a.k;
     for (int i = threadIdx.x; i < a.k; i += blockDim.x) out[i] = i < c ? tk_buf[i] : 0;
     if (threadIdx.x == 0 && a.out_total) a.out_total[q] = s_hits;
+    // every tile ends with a barrier, so the shared counts are complete here
+    if (FACET && F.smem) for (uint32_t i = threadIdx.x; i < F.n_buckets; i += BM_THREADS) F.out[(size_t)q * F.n_buckets + i] = fcnt[i];
+}
+
+template <bool CONJ, bool TF>
+__global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T, Bm25Args a) {
+    bm25_body<CONJ, TF, false>(T, a, FacetArgs{});
+}
+
+// bm25_kernel + the FacetCollector: same top-k and Count, plus F.out[q][bucket] (shared counters: smem = bm_smem_bytes + 4 n_buckets)
+template <bool CONJ, bool TF>
+__global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_facet_kernel(TxtDev T, Bm25Args a, FacetArgs f) {
+    bm25_body<CONJ, TF, true>(T, a, f);
 }
 
 // keys -> (doc, score, count) with the min_score cut applied after top-k (reader.rs:302-305).

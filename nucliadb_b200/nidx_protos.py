@@ -5,6 +5,7 @@ hand (there is no protoc in this image): same packages, message names, field nam
 serialised by the reference's clients (``nidx_protos`` / ``nucliadb_protos``) decode, and the responses decode on their side.
 
     SearchRequest / SearchResponse                         nodereader.proto:388-437, 476-488
+    Faceted, FacetResult, FacetResults                     nodereader.proto:20-22, 40-46
     DocumentSearchResponse / DocumentResult / ResultScore  nodereader.proto:48-81
     ParagraphSearchResponse / ParagraphResult              nodereader.proto:83-124
     VectorSearchResponse / DocumentScored                  nodereader.proto:126-142
@@ -96,6 +97,12 @@ def _build():
                                             dependency=["nidx_protos/noderesources.proto"])
     e = fd.enum_type.add(name="FilterOperator")               # :333-336
     e.value.add(name="AND", number=0); e.value.add(name="OR", number=1)
+    m = fd.message_type.add(name="Faceted")                   # :20-22
+    _field(m, "labels", 1, "string", repeated=True)
+    m = fd.message_type.add(name="FacetResult")               # :40-43
+    _field(m, "tag", 1, "string"); _field(m, "total", 2, "int32")
+    m = fd.message_type.add(name="FacetResults")              # :44-46
+    _field(m, "facetresults", 1, ".nodereader.FacetResult", repeated=True)
     m = fd.message_type.add(name="ResultScore")               # :48-53
     _field(m, "bm25", 1, "float"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="DocumentResult")            # :55-64
@@ -104,7 +111,7 @@ def _build():
     _field(m, "labels", 5, "string", repeated=True); _field(m, "shard_id", 7, "bytes")
     m = fd.message_type.add(name="DocumentSearchResponse")    # :66-81
     _field(m, "total", 1, "int32"); _field(m, "results", 2, ".nodereader.DocumentResult", repeated=True); _field(m, "query", 6, "string")
-    _field(m, "next_page", 7, "bool")
+    _field(m, "next_page", 7, "bool"); _map(m, ".nodereader.DocumentSearchResponse", "facets", 3, "string", ".nodereader.FacetResults")
     m = fd.message_type.add(name="ParagraphResult")           # :83-104
     m.oneof_decl.add().name = "sort_value"
     _field(m, "uuid", 1, "string"); _field(m, "field", 3, "string"); _field(m, "start", 4, "uint64"); _field(m, "end", 5, "uint64")
@@ -114,6 +121,7 @@ def _build():
     m = fd.message_type.add(name="ParagraphSearchResponse")   # :106-124
     _field(m, "total", 1, "int32"); _field(m, "results", 2, ".nodereader.ParagraphResult", repeated=True); _field(m, "query", 6, "string")
     _field(m, "next_page", 7, "bool"); _field(m, "ematches", 9, "string", repeated=True)
+    _map(m, ".nodereader.ParagraphSearchResponse", "facets", 3, "string", ".nodereader.FacetResults")
     m = fd.message_type.add(name="DocumentVectorIdentifier")  # :126-128
     _field(m, "id", 1, "string")
     m = fd.message_type.add(name="DocumentScored")            # :130-135
@@ -138,7 +146,8 @@ def _build():
     m = fd.message_type.add(name="SearchAfter")               # :382-386
     _field(m, "score", 1, "float"); _field(m, "shard_id", 2, "bytes"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="SearchRequest")             # :388-437
-    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 3, "string"); _field(m, "result_per_page", 8, "int32")
+    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 3, "string"); _field(m, "faceted", 6, ".nodereader.Faceted")
+    _field(m, "result_per_page", 8, "int32")
     _field(m, "vector", 10, "float", repeated=True); _field(m, "paragraph", 12, "bool"); _field(m, "document", 13, "bool")
     _field(m, "with_duplicates", 14, "bool"); _field(m, "vectorset", 15, "string"); _field(m, "only_faceted", 16, "bool")
     _field(m, "min_score_semantic", 23, "float"); _field(m, "min_score_bm25", 25, "float")
@@ -186,6 +195,9 @@ def _cls(name):
 SearchRequest = _cls("nodereader.SearchRequest")
 SearchResponse = _cls("nodereader.SearchResponse")
 FilterExpression = _cls("nodereader.FilterExpression")
+Faceted = _cls("nodereader.Faceted")
+FacetResult = _cls("nodereader.FacetResult")
+FacetResults = _cls("nodereader.FacetResults")
 DocumentSearchResponse = _cls("nodereader.DocumentSearchResponse")
 ParagraphSearchResponse = _cls("nodereader.ParagraphSearchResponse")
 VectorSearchResponse = _cls("nodereader.VectorSearchResponse")

@@ -205,6 +205,19 @@ def merge_topk(ids, scores, device=0, part_stride=0, out=None):
     return out
 
 
+def _pack_keys(keys):
+    """[bytes] -> (concatenated bytes as uint8, uint64 offsets [n + 1])."""
+    off = np.zeros(len(keys) + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([len(k) for k in keys]) if len(keys) else []
+    return np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8).copy(), off
+
+
+def _facet_request(facets):
+    """-> (TxtFacetRequest, the arrays it points into: keep them alive for the call)."""
+    kb, ko = _pack_keys(list(facets))
+    return _lib.TxtFacetRequest(len(facets), ptr(kb), ptr(ko)), (kb, ko)
+
+
 class TextSegment:
     def __init__(self, handle, n_docs, n_terms, device):
         self._h, self.n_docs, self.n_terms, self.device = handle, n_docs, n_terms, device
@@ -257,6 +270,65 @@ class TextSegment:
         check(L.nidx_txt_search(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_HOST, C.byref(p), ptr(docs), ptr(scores), ptr(counts),
                                 ptr(total), None))
         return docs, scores, counts, total
+
+    # ---- facets (tantivy FacetCollector; keys in the encoded form of include/nidx_b200.h: segments joined by 0x00) -----------
+    def set_facets(self, keys, doc_off, doc_ords):
+        """keys: bytes, strictly ascending (facet order); document d carries doc_ords[doc_off[d]:doc_off[d + 1]] (ascending)."""
+        kb, ko = _pack_keys(keys)
+        doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+        doc_ords = np.ascontiguousarray(doc_ords, dtype=np.uint32)
+        check(_lib.load().nidx_txt_set_facets(self._h, C.c_uint32(len(keys)), ptr(kb), ptr(ko), ptr(doc_off), ptr(doc_ords)))
+
+    def facet_buckets(self, facets):
+        """facets: encoded facet keys -> (bucket_req, bucket_ord) uint32 arrays (include/nidx_b200.h nidx_txt_facet_buckets)."""
+        req, _keep = _facet_request(facets)
+        n = C.c_uint32()
+        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), None, None, C.c_uint32(0), C.byref(n)))
+        b_req, b_ord = np.empty(n.value, dtype=np.uint32), np.empty(n.value, dtype=np.uint32)
+        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), ptr(b_req), ptr(b_ord), C.c_uint32(n.value), C.byref(n)))
+        return b_req, b_ord
+
+    def search_faceted(self, query_terms, query_off, k, facets, mode=_lib.NIDX_BM25_OR, use_tf=True, min_score=0.0, after=None, docaddr_base=0):
+        """search() + per-query facet bucket counts in the same pass: (docs, scores, counts, total, facet_counts[nq][n_buckets]).
+        numpy -> host path, torch CUDA -> device path (as search())."""
+        L = _lib.load()
+        p = TxtSearchParams(k, mode, int(use_tf), min_score, 0, 0.0, 0, docaddr_base)
+        if after is not None:
+            p.after_score, p.after_mode, p.after_docaddr = float(after[0]), int(after[1]), int(after[2])
+        nb = len(self.facet_buckets(facets)[0])
+        req, _keep = _facet_request(facets)
+        if _is_torch(query_terms):
+            import torch
+
+            nq, dev = query_off.numel() - 1, query_terms.device
+            out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
+                   torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev),
+                   torch.empty((nq, nb), dtype=torch.int32, device=dev))
+            check(L.nidx_txt_search_faceted(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_DEVICE, C.byref(p), C.byref(req),
+                                            *[ptr(o) for o in out], _torch_stream(self.device)))
+            return out
+        query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
+        query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
+        nq = len(query_off) - 1
+        out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty(nq, dtype=np.int32), np.empty(nq, dtype=np.uint64),
+               np.zeros((nq, nb), dtype=np.uint32))
+        check(L.nidx_txt_search_faceted(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_HOST, C.byref(p), C.byref(req),
+                                        *[ptr(o) for o in out], None))
+        return out
+
+    def facet_count_all(self, facets, device_out=False):
+        """Bucket counts over every alive document (uint32 [n_buckets]; device_out: a torch CUDA int32 tensor, device path)."""
+        nb = len(self.facet_buckets(facets)[0])
+        req, _keep = _facet_request(facets)
+        if device_out:
+            import torch
+
+            out = torch.empty(nb, dtype=torch.int32, device=f"cuda:{self.device}")
+            check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), _lib.NIDX_MEM_DEVICE, ptr(out), _torch_stream(self.device)))
+            return out
+        out = np.zeros(nb, dtype=np.uint32)
+        check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), _lib.NIDX_MEM_HOST, ptr(out), None))
+        return out
 
     def set_doc_keys(self, keys: Optional[np.ndarray]):
         """Caller keys of the documents (paragraph ids) for rank fusion; None = the document number."""

@@ -12,7 +12,14 @@ Reference call shape (the scoring itself is tantivy's, restated in oracle/bm25.h
   (score desc, segment_ord asc, doc asc) with ``docaddr = (segment_ord << 32) + doc`` (reader.rs:310, Q13).
 
 Tokenisation mirrors tantivy's "default" analyzer (SimpleTokenizer + RemoveLongFilter(40) + LowerCaser)
-[recalled]; fuzzy fallback, facets, filters and stop words are query-preparation, outside the hot path.
+[recalled]; fuzzy fallback, filters and stop words are query-preparation, outside the hot path.
+
+Facets (tantivy's ``FacetCollector``, run beside ``Count`` and ``TopDocs``: nidx_text/src/reader.rs:388-450,
+nidx_paragraph/src/reader.rs:252-347) ARE on the hot path: a facet count visits every matched document, so it is counted inside
+the BM25 pass (``bm25_facet_kernel``), and over every alive document for an empty body (``facet_count_all_kernel``).  The index
+keeps ONE facet dictionary across its segments (like the term vocabulary), so per-segment bucket counts add up as arrays before the
+top-50 cut of ``FacetCounts::top_k`` (nidx_text/src/reader.rs:43-62).  Each group lists its children by count descending, ties in
+facet order (path segments compared bytewise); a group without a counted child is omitted.
 """
 from __future__ import annotations
 
@@ -67,6 +74,7 @@ class DocumentSearchRequest:  # nidx_text/src/request_types.rs:17-28
     result_per_page: int = 20
     min_score: float = 0.0
     only_faceted: bool = False
+    faceted: Sequence[str] = ()               # Faceted.labels: the facets to count children of (SearchRequest.faceted)
     search_after: Optional[SearchAfter] = None  # ParagraphSearchRequest.search_after (nidx_paragraph only)
 
 
@@ -78,11 +86,42 @@ class SearchAfter:  # nidx_paragraph/src/request_types.rs:20-31
 
 
 @dataclass
+class FacetResult:  # nodereader.proto:40-43
+    tag: str
+    total: int
+
+
+@dataclass
 class DocumentSearchResponse:
     results: list = field(default_factory=list)
     total: int = 0
     next_page: bool = False
     query: str = ""
+    facets: dict = field(default_factory=dict)   # request facet -> [FacetResult], top 50 (nodereader.proto:74, 115)
+
+
+FACET_TOP_K = 50   # FacetCounts::top_k(facet, 50): nidx_text/src/reader.rs:43-52, nidx_paragraph/src/search_response.rs:48-57
+
+
+def facet_key(path: str) -> Optional[bytes]:
+    """tantivy's encoded facet (segments joined by 0x00, no leading '/'; the root "/" is b""), or None when the string is not a
+    valid facet (Facet::from_text fails [recalled]: it must start with '/')."""
+    if not path.startswith("/"):
+        return None
+    return b"" if path == "/" else path[1:].encode("utf-8").replace(b"/", b"\0")
+
+
+def facet_path(key: bytes) -> str:
+    return "/" + key.replace(b"\0", b"/").decode("utf-8")
+
+
+def _facet_request(faceted: Sequence[str]):
+    """Faceted.labels -> the valid facets, duplicates collapsed, in request order (is_valid_facet / Facet::from_text(..).ok())."""
+    out = []
+    for f in faceted:
+        if facet_key(f) is not None and f not in out:
+            out.append(f)
+    return out
 
 
 @dataclass
@@ -126,7 +165,7 @@ class TextIndexSegment:
 
 
 class TextSearcher:
-    """nidx_text TextSearcher over one or more segments sharing one term dictionary."""
+    """nidx_text TextSearcher over one or more segments sharing one term dictionary (and one facet dictionary)."""
 
     conjunction = True   # QueryParser::set_conjunction_by_default (reader.rs:372-377)
     use_tf = True
@@ -142,6 +181,57 @@ class TextSearcher:
             df += s.doc_freq(n_terms)
         for s in self.segments:  # union statistics on every segment (index_reader.rs:39-77)
             s.upload(n_terms).set_stats(max(total_docs, 1), max(total_tokens, 1), df)
+        self.facet_keys: Optional[list] = None   # built on the first faceted request
+
+    def _ensure_facets(self):
+        """The index's facet dictionary (every valid label of every document, in facet order) and each segment's per-document
+        ords, uploaded once."""
+        if self.facet_keys is not None:
+            return
+        keys = sorted({k for s in self.segments for d in s.docs for k in map(facet_key, d.labels) if k is not None})
+        ord_of = {k: i for i, k in enumerate(keys)}
+        for s in self.segments:
+            rows = [sorted({ord_of[k] for k in map(facet_key, d.labels) if k is not None}) for d in s.docs]
+            off = np.zeros(len(rows) + 1, dtype=np.uint64)
+            off[1:] = np.cumsum([len(r) for r in rows])
+            s._gpu.set_facets(keys, off, np.asarray([o for r in rows for o in r], dtype=np.uint32))
+        self.facet_keys = keys
+
+    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict):
+        """Counts of the request's facets over the matched set of every segment, summed, then grouped and cut to the top 50.
+        With terms: the faceted BM25 search (returns its per-segment (docs, scores, counts, total) too); without: every alive
+        document (AllQuery)."""
+        from ._lib import NidxError
+
+        request = _facet_request(faceted)
+        self._ensure_facets()
+        keys = [facet_key(f) for f in request]
+        try:
+            b_req, b_ord = self.segments[0]._gpu.facet_buckets(keys)
+        except NidxError as e:
+            if e.code == -1:   # NIDX_EINVAL: one requested facet is an ancestor of another (tantivy asserts)
+                raise ValueError(str(e)) from e
+            raise
+        counts = np.zeros(len(b_req), dtype=np.int64)
+        hits = []
+        for ord_, seg in enumerate(self.segments):
+            if terms:
+                qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
+                docs, scores, cnt, total, fc = seg._gpu.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
+                hits.append((docs, scores, cnt, total))
+                counts += fc[0]
+            else:
+                counts += seg._gpu.facet_count_all(keys)
+        groups: dict = {}
+        for b, (r, o) in enumerate(zip(b_req, b_ord)):
+            if counts[b]:
+                depth = 0 if keys[r] == b"" else keys[r].count(b"\0") + 1
+                child = b"\0".join(self.facet_keys[o].split(b"\0")[: depth + 1])
+                groups.setdefault(int(r), []).append((-int(counts[b]), child))
+        facets = {}
+        for r in sorted(groups):
+            facets[request[r]] = [FacetResult(facet_path(c), -n) for n, c in sorted(groups[r])[:FACET_TOP_K]]
+        return facets, hits
 
     @classmethod
     def open(cls, docs_per_segment: Sequence[Sequence[TextDoc]], device=0):
@@ -159,18 +249,26 @@ class TextSearcher:
         terms = self._terms(request.body)
         k = request.result_per_page
         resp = DocumentSearchResponse(query=request.body)
+        after = None
+        if request.search_after is not None:
+            sa = request.search_after
+            after = (sa.score, {"drop": 1, "keep_after": 2, "keep": 3}[sa.tie_break], sa.docaddr)
+        params = dict(mode=_lib.NIDX_BM25_AND if self.conjunction else _lib.NIDX_BM25_OR, use_tf=self.use_tf, min_score=0.0, after=after)
+        hits = None
+        if _facet_request(request.faceted):
+            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params)
+        if request.only_faceted:   # only the facets: no results, total 0 (nidx_text/src/reader.rs:407-414, search_response.rs:111-124)
+            return DocumentSearchResponse(facets=resp.facets)
         if not terms or k <= 0:
             return resp
         qt = np.asarray(terms, dtype=np.uint32)
         qo = np.asarray([0, len(terms)], dtype=np.uint32)
         merged = []
         for ord_, seg in enumerate(self.segments):
-            after = None
-            if request.search_after is not None:
-                sa = request.search_after
-                after = (sa.score, {"drop": 1, "keep_after": 2, "keep": 3}[sa.tie_break], sa.docaddr)
-            docs, scores, counts, total = seg._gpu.search(qt, qo, k + 1, mode=_lib.NIDX_BM25_AND if self.conjunction else _lib.NIDX_BM25_OR,
-                                                          use_tf=self.use_tf, min_score=0.0, after=after, docaddr_base=ord_ << 32)
+            if hits is not None:   # the faceted pass already returned this segment's top-k and Count
+                docs, scores, counts, total = hits[ord_]
+            else:
+                docs, scores, counts, total = seg._gpu.search(qt, qo, k + 1, docaddr_base=ord_ << 32, **params)
             resp.total += int(total[0])
             merged += [(-float(scores[0, i]), ord_, int(docs[0, i])) for i in range(int(counts[0]))]
         merged.sort()  # score desc, then segment_ord, then doc: lower docaddr first
