@@ -206,6 +206,10 @@ int nidx_vec_counters(nidx_vec_segment* seg, uint64_t out[3]);
 /* The same with the quantised walk's: [0] exact similarities computed, [1] expansions, [2] visited-set overflows, [3] closest_up
  * overflows, [4] RaBitQ estimates, [5] exact similarities the sequential rerank_top needed (<= the share of [0] spent there). */
 int nidx_vec_counters_ex(nidx_vec_segment* seg, uint64_t out[6]);
+/* f32 vector rows the last HNSW search / build read to compute a similarity.  The walk screens neighbours on an fp16 copy of
+ * the vectors with a proven error bound and reads the f32 row only of those that can enter its list, so this is at most
+ * the similarity count of nidx_vec_counters (equal when the segment has no fp16 copy). */
+int nidx_vec_exact_rows(nidx_vec_segment* seg, uint64_t* out);
 
 /* RaBitQ 1-bit codes (vector_types/rabitq.rs; Dot similarity and dimension % 64 == 0 only, config.rs:170-173).
  * nidx_vec_rabitq_encode builds the reference's vectors.quant records ([f32 dot_quant_original][u32 sum_bits][dim/8 sign

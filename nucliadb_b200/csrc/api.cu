@@ -168,10 +168,17 @@ struct nidx_vec_segment {
     unsigned int* d_work_counter = nullptr;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around the dominant kernel of the last search (bench roofline)
     WorkspacePool pool;
+    // fp16 screening copy of the vectors for the HNSW walk (hs_half_kernel), made once by ensure_half_copy
+    __half* d_hvecs = nullptr;
+    float4* d_hrec = nullptr;
+    int ldh = 0;
+    bool half_decided = false;          // the copy was made, or was found not to fit (the walk then reads f32 rows only)
+    std::mutex half_mu;
 
     VecDev vdev() const {
         VecDev v;
         v.vecs = d_vecs; v.norms = d_norms; v.paragraph_of = d_par_of; v.n = (uint32_t)n; v.d = d; v.ld = ld; v.sim = cfg.similarity;
+        v.hvecs = nullptr; v.hrec = nullptr; v.ldh = 0;   // the HNSW walks attach the screening copy (attach_half_copy)
         return v;
     }
     GraphDev gdev() const {
@@ -229,6 +236,77 @@ __global__ void max_norm_kernel(const float* __restrict__ norms, uint64_t n, uns
     for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) m = fmaxf(m, norms[i]);
     for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, off));
     if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats order like their bit patterns
+}
+
+// The HNSW walk's fp16 screening copy (hs_screened_out in hnsw_search.cuh derives the bound), one warp per row:
+//   h = fp16(v * 2^e) with e = min(15 - exponent(max |v_i|), 126): max |v_i| * 2^e lies in [2^14, 2^15), so no element overflows
+//   fp16, and 2^-e is a normal f32 (tiny rows then use fp16 subnormals, which only widens rho);
+//   rec = {norms[i], 2^-e, err_q, err_abs}, err_q >= rho + g_m (2 |v| + rho), rho = |h * 2^-e - v|, err_abs >= 2^-149 (ld (1 + 2^-e) + 1).
+//   rho^2 and |v|^2 are f64 sums of squares of exact (or, for rho, correctly rounded f64) terms: each is within ld * 2^-52 of its
+//   value, which the factor 1 + 2^-20 covers along with the roundings of what follows; the f32 results are rounded up.  A row with
+//   a non-finite element gets err_q = +inf, so the walk always reads its f32 row.
+__global__ void hs_half_kernel(VecDev V, uint64_t n, int ldh, __half* __restrict__ hv, float4* __restrict__ rec) {
+    const int lane = threadIdx.x & 31;
+    const double slack = 1.0 + 0x1p-20, mu = dot_depth(V.ld) * 0x1p-24, gm = mu / (1.0 - mu);
+    for (uint64_t i = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 5; i < n; i += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+        const float* v = V.vecs + i * V.ld;
+        float m = 0.0f;
+        bool finite = true;
+        for (int k = lane; k < V.ld; k += 32) { float x = v[k]; finite = finite && isfinite(x); m = fmaxf(m, fabsf(x)); }
+        for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, off));
+        finite = __all_sync(0xFFFFFFFFu, finite);
+        int e = 0;
+        if (finite && m > 0.0f) { int ex; frexpf(m, &ex); e = min(15 - ex, 126); }
+        const float up = ldexpf(1.0f, e), down = ldexpf(1.0f, -e);
+        double r2 = 0.0, v2 = 0.0;
+        for (int k = lane; k < ldh; k += 32) {
+            float x = k < V.ld ? v[k] : 0.0f;
+            __half h = __float2half_rn(__fmul_rn(x, up));
+            hv[i * ldh + k] = h;
+            double dd = (double)__half2float(h) * (double)down - (double)x;
+            r2 = fma(dd, dd, r2);
+            v2 = fma((double)x, (double)x, v2);
+        }
+        for (int off = 16; off >= 1; off >>= 1) { r2 += __shfl_xor_sync(0xFFFFFFFFu, r2, off); v2 += __shfl_xor_sync(0xFFFFFFFFu, v2, off); }
+        if (lane == 0) {
+            double rho = sqrt(r2 * slack), vn = sqrt(v2 * slack);
+            double eq = (rho + gm * (2.0 * vn + rho)) * slack;
+            double ea = 0x1p-149 * ((double)V.ld * (1.0 + (double)down) + 1.0) * slack;
+            rec[i] = make_float4(V.norms[i], down, finite ? __double2float_ru(eq) : INFINITY, __double2float_ru(ea));
+        }
+    }
+}
+
+// Attach the screening copy to V for an HNSW walk, making it on the segment's first walk (build, extend or search) under the
+// segment's lock; the conversion has finished before any caller gets the pointers.  When the copy (ldh * 2 + 16 bytes per
+// vector) does not fit next to what HBM already holds with HS_HALF_MARGIN to spare, the segment keeps the f32-only walk.
+// NIDX_B200_HS_F16=0 forces the f32-only walk (the tests compare the two walks).
+constexpr size_t HS_HALF_MARGIN = (size_t)4 << 30;
+static int attach_half_copy(nidx_vec_segment* s, VecDev* V) {
+    const char* e = getenv("NIDX_B200_HS_F16");
+    if (e && !strcmp(e, "0")) return 0;
+    std::lock_guard<std::mutex> g(s->half_mu);
+    if (!s->half_decided && s->n) {
+        s->half_decided = true;
+        const int ldh = (s->ld + 7) / 8 * 8;
+        const size_t hbytes = (size_t)s->n * ldh * 2, rbytes = (size_t)s->n * 16;
+        size_t free_b = 0, total_b = 0;
+        CU(cudaMemGetInfo(&free_b, &total_b));
+        if (free_b < hbytes + rbytes + HS_HALF_MARGIN) return 0;
+        if (cudaMalloc(&s->d_hvecs, hbytes) != cudaSuccess || cudaMalloc(&s->d_hrec, rbytes) != cudaSuccess) {
+            (void)cudaGetLastError();   // out of memory is not an error here: the f32-only walk runs
+            cudaFree(s->d_hvecs); cudaFree(s->d_hrec);
+            s->d_hvecs = nullptr; s->d_hrec = nullptr;
+            return 0;
+        }
+        hs_half_kernel<<<s->sm_count * 8, 256>>>(s->vdev(), s->n, ldh, s->d_hvecs, s->d_hrec);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        CU(cudaDeviceSynchronize());
+        s->ldh = ldh;
+    }
+    if (s->ldh) { V->hvecs = s->d_hvecs; V->hrec = s->d_hrec; V->ldh = s->ldh; }
+    return 0;
 }
 
 // cuTensorMapEncodeTiled through the runtime's driver entry point (no link-time dependency on libcuda)
@@ -454,6 +532,7 @@ void nidx_vec_close(nidx_vec_segment* s) {
     free_graph(s);
     cudaFree(s->d_vecs); cudaFree(s->d_norms); cudaFree(s->d_par_of); cudaFree(s->d_par_first); cudaFree(s->d_alive);
     cudaFree(s->d_counters); cudaFree(s->d_work_counter); cudaFree(s->d_quant); cudaFree(s->d_par_keys); cudaFree(s->inv[0].d_post); cudaFree(s->inv[1].d_post);
+    cudaFree(s->d_hvecs); cudaFree(s->d_hrec);
     if (s->ev_k0) cudaEventDestroy(s->ev_k0);
     if (s->ev_k1) cudaEventDestroy(s->ev_k1);
     delete s;
@@ -550,6 +629,16 @@ int nidx_vec_counters(nidx_vec_segment* s, uint64_t out[3]) {
     unsigned long long* src = s->last_counters.load();
     CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
     out[0] = h[0]; out[1] = h[1]; out[2] = h[2] + h[3];
+    return 0;
+}
+
+int nidx_vec_exact_rows(nidx_vec_segment* s, uint64_t* out) {
+    if (!s || !out) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(s->cfg.device));
+    unsigned long long h[8];
+    unsigned long long* src = s->last_counters.load();
+    CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
+    *out = h[6];
     return 0;
 }
 
@@ -1228,6 +1317,8 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         size_t smem;
         int r = hnsw_search_smem(s, ef0, k, &list_cap, &cu_cap, &hash_bits, &smem);
         if (r) return r;
+        r = attach_half_copy(s, &V);
+        if (r) return r;
         SearchArgs a;
         memset(&a, 0, sizeof(a));
         a.mode = 0; a.nq = nq; a.queries = dq; a.qnorms = w.qnorms.as<float>(); a.k = k; a.ef0 = ef0; a.min_score = p->min_score;
@@ -1473,6 +1564,8 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
 
 
         VecDev V = s->vdev();
+        int hr = attach_half_copy(s, &V);
+        if (hr) return hr;
         GraphDev G = s->gdev();
         uint32_t begin = 0;
         for (size_t b = 0; b < ends.size(); ++b) {

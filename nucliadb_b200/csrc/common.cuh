@@ -6,6 +6,7 @@
 // accumulators per lane (one per component), lane value (ax+ay)+(az+aw), xor-butterfly 16,8,4,2,1.
 // All arithmetic uses the *_rn intrinsics so nvcc can neither contract nor reassociate it.
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -20,7 +21,15 @@ struct VecDev {
     const uint32_t* paragraph_of;  // [n] or nullptr (identity)
     uint32_t n;
     int d, ld, sim;
+    // The HNSW walk's screening copy (hs_half_kernel), or nullptr: the walk then reads every neighbour's f32 row.
+    const __half* hvecs;  // [n][ldh] fp16(v * 2^e_row), ldh = ld rounded up to 8 (16-byte rows), zero padded
+    const float4* hrec;   // [n] {norms[i], 2^-e_row, err_q, err_abs}: |screen dot - exact dot| <= |q| * err_q + err_abs
+    int ldh;
 };
+
+// Rounding depth of one product term in the lane-blocked dot (warp_dot / warp_dot_t / warp_dot_h): ceil(ngroups / 32) fused
+// multiply-adds in its lane's accumulator, two adds combining the four accumulators, five butterfly adds.
+__host__ __device__ __forceinline__ int dot_depth(int ld) { return (ld / 4 + 31) / 32 + 7; }
 
 struct GraphDev {
     uint32_t n;
@@ -152,6 +161,69 @@ __device__ __forceinline__ void warp_dot2_t(const float4* __restrict__ a0, const
         }
         r0 = butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
         r1 = butterfly_sum(__fadd_rn(__fadd_rn(cx, cy), __fadd_rn(cz, cw)));
+    }
+}
+
+__device__ __forceinline__ uint2 ldg_stream2(const uint2* p) {
+    uint2 r;
+    asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
+    return r;
+}
+
+// warp_dot_t's lane-blocked order over an fp16 row `a` ([ngroups] groups of four halves, 8-byte loads, widened to f32 in
+// registers -- exactly) against the f32 `b`: the same dot_depth(), so the same rounding-error bound as the f32 dot.
+template <int NG>
+__device__ __forceinline__ float warp_dot_h(const uint2* __restrict__ a, const float4* __restrict__ b, int ngroups, int lane) {
+    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
+    auto acc = [&](uint2 h, float4 vb) {
+        float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), hi = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+        ax = __fmaf_rn(lo.x, vb.x, ax);
+        ay = __fmaf_rn(lo.y, vb.y, ay);
+        az = __fmaf_rn(hi.x, vb.z, az);
+        aw = __fmaf_rn(hi.y, vb.w, aw);
+    };
+    if constexpr (NG == 0) {
+        for (int g = lane; g < ngroups; g += 32) acc(ldg_stream2(a + g), b[g]);
+    } else {
+        uint2 va[NG];
+#pragma unroll
+        for (int j = 0; j < NG; ++j) va[j] = ldg_stream2(a + j * 32 + lane);
+#pragma unroll
+        for (int j = 0; j < NG; ++j) acc(va[j], b[j * 32 + lane]);
+    }
+    return butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
+}
+
+// Two fp16 rows in flight (the 4-warp shape); each result is warp_dot_h's.
+template <int NG>
+__device__ __forceinline__ void warp_dot2_h(const uint2* __restrict__ a0, const uint2* __restrict__ a1, const float4* __restrict__ b, int ngroups, int lane,
+                                            float& r0, float& r1) {
+    if constexpr (NG == 0) {
+        r0 = warp_dot_h<0>(a0, b, ngroups, lane);
+        r1 = warp_dot_h<0>(a1, b, ngroups, lane);
+    } else {
+        uint2 va[NG], vc[NG];
+#pragma unroll
+        for (int j = 0; j < NG; ++j) va[j] = ldg_stream2(a0 + j * 32 + lane);
+#pragma unroll
+        for (int j = 0; j < NG; ++j) vc[j] = ldg_stream2(a1 + j * 32 + lane);
+        float s[2];
+#pragma unroll
+        for (int t = 0; t < 2; ++t) {
+            const uint2* v = t ? vc : va;
+            float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
+#pragma unroll
+            for (int j = 0; j < NG; ++j) {
+                float4 vb = b[j * 32 + lane];
+                float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v[j].x)), hi = __half22float2(*reinterpret_cast<const __half2*>(&v[j].y));
+                ax = __fmaf_rn(lo.x, vb.x, ax);
+                ay = __fmaf_rn(lo.y, vb.y, ay);
+                az = __fmaf_rn(hi.x, vb.z, az);
+                aw = __fmaf_rn(hi.y, vb.w, aw);
+            }
+            s[t] = butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
+        }
+        r0 = s[0]; r1 = s[1];
     }
 }
 

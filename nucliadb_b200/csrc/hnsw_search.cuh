@@ -78,8 +78,41 @@ struct SearchCtx {
     uint32_t hash_mask;
     int hash_bits, hash_limit;
     float qnorm;
+    float qbound;                    // >= |q| (hs_query_bound), for the screen's error bound
     unsigned long long n_dist, n_expand, n_overflow;
+    unsigned long long n_skip;       // similarities the screen settled without reading the f32 row
 };
+
+// An upper bound on |q| for the query in shared memory, the same in every thread: the squares are exact in f64 and the f64 sum
+// of ld of them is within ld * 2^-53 of its value, which the factor 1 + 2^-20 covers (ld < 2^30).
+__device__ inline float hs_query_bound(const float* q, int ld) {
+    double s = 0.0;
+    for (int i = threadIdx.x & 31; i < ld; i += 32) s = fma((double)q[i], (double)q[i], s);
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, off);
+    return __double2float_ru(__dsqrt_ru(__dmul_ru(s, 1.0 + 0x1p-20)));
+}
+
+// The screen of a neighbour y of the layer search, given ah = warp_dot_h of its fp16 row and r = its hrec record: true when the
+// exact key cannot exceed wkey, so the f32 row need not be read.
+//   Let a be the f32 dot warp_dot_t computes and p the real dot <v, q>.  Both dots round each product term at most
+//   m = dot_depth(ld) times, so |a - p| <= g_m * |v| |q| + ld * 2^-149 and |ah * 2^-e - <h', q>| <= g_m * |h'| |q| + ld * 2^-149 * 2^-e
+//   + 2^-150 (g_m = m u / (1 - m u), u = 2^-24; 2^-149 per fused multiply-add for subnormal results; the scaling by 2^-e is exact
+//   unless it underflows), with h' = h * 2^-e.  |<h', q> - p| <= rho |q|, rho = |h' - v| and |h'| <= |v| + rho.  Together:
+//   |ah * 2^-e - a| <= |q| (rho + g_m (2 |v| + rho)) + 2^-149 (ld (1 + 2^-e) + 1) = |q| * err_q + err_abs (hs_half_kernel rounds
+//   both up), and bnd below is rounded up again, so ab_up >= a.
+//   sim_from_parts never decreases as ab grows (for the three similarities, the ab == 0 and zero-norm cases of cosine included;
+//   ab_up >= +0 whenever a >= +0, so total_cmp's -0 < +0 cannot invert it) and make_key is monotone: key(a) <= key(ab_up) <= wkey.
+//   The bound needs every partial sum finite: bnd >= 2^-20 |v| |q| (g_m >= 8u), so bnd <= 2^100 keeps both dots' partial sums
+//   below 2^121.  A row with a non-finite element has err_q = +inf, a non-finite query gives a non-finite qbound, and an overflowed
+//   fp16 dot is non-finite: all of these fail the test and read the f32 row.
+__device__ __forceinline__ bool hs_screened_out(const VecDev& V, const SearchCtx& c, uint32_t y, float ah, float4 r, uint64_t wkey) {
+    float a = __fmul_rn(ah, r.y);
+    float bnd = __fmaf_ru(c.qbound, r.z, r.w);
+    if (!(fabsf(a) <= 0x1p120f && bnd <= 0x1p100f)) return false;
+    float s_up = sim_from_parts(V.sim, __fadd_ru(a, bnd), r.x, c.qnorm);
+    return make_key(s_up, y, 1) <= wkey;
+}
 
 __host__ __device__ __forceinline__ size_t hs_smem_bytes(int ld, int list_cap, int hash_bits) {
     return (size_t)ld * 4 + (size_t)list_cap * 16 + ((size_t)4 << hash_bits) + HS_MAX_ROW * 12 + HS_MAX_ROW * 8 + 16 + 64;
@@ -185,13 +218,20 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
         if (admit) { atomicAdd(c.s_nadmit, 1); atomicMax(c.s_maxtodo, (unsigned long long)key); }
         c.n_dist++;
     };
+    // Screen (layer search with a full list): a neighbour whose fp16 dot plus its error bound cannot beat wkey is rejected
+    // without reading its f32 row (hs_screened_out); the others take the exact path below unchanged.
+    const bool screen = !CU && wkey != 0 && V.hvecs != nullptr;
+    auto skip = [&](int j) { c.todo_key[j] = 0; c.n_dist++; c.n_skip++; };
+    const float4* qv = reinterpret_cast<const float4*>(c.qvec);
+    auto frow = [&](uint32_t y) { return reinterpret_cast<const float4*>(V.vecs + (size_t)y * V.ld); };
+    auto hrow = [&](uint32_t y) { return reinterpret_cast<const uint2*>(V.hvecs + (size_t)y * V.ldh); };
     // A warp's later rows (j + W, j + 2W, ...) are pulled into L2 while it works on its first one: their loads then cost an L2
     // hit instead of a second and third HBM round trip on the expansion's critical path (one prefetch per 128-byte line, a lane
-    // each; no registers held, unlike a second row in flight).
+    // each; no registers held, unlike a second row in flight).  Under the screen the row read first is the fp16 one.
     if (!PAIR) {
-        const int lines = (V.ld * 4 + 127) >> 7;
+        const int lines = screen ? (V.ldh * 2 + 127) >> 7 : (V.ld * 4 + 127) >> 7;
         for (int j = warp + W; j < ntodo; j += W) {
-            const char* rowp = reinterpret_cast<const char*>(V.vecs + (size_t)c.todo_id[j] * V.ld);
+            const char* rowp = screen ? reinterpret_cast<const char*>(hrow(c.todo_id[j])) : reinterpret_cast<const char*>(frow(c.todo_id[j]));
             for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(rowp + (size_t)l * 128));
         }
     }
@@ -200,18 +240,39 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
             uint32_t y0 = c.todo_id[j];
             bool two = j + W < ntodo;
             uint32_t y1 = two ? c.todo_id[j + W] : y0;
-            float n0 = V.sim != SIM_DOT ? __ldg(V.norms + y0) : 0.0f, n1 = (two && V.sim != SIM_DOT) ? __ldg(V.norms + y1) : 0.0f;
-            float ab0, ab1;
-            if (two) warp_dot2_t<NG>(reinterpret_cast<const float4*>(V.vecs + (size_t)y0 * V.ld), reinterpret_cast<const float4*>(V.vecs + (size_t)y1 * V.ld),
-                                     reinterpret_cast<const float4*>(c.qvec), ng, lane, ab0, ab1);
-            else { ab0 = warp_dot_t<NG>(reinterpret_cast<const float4*>(V.vecs + (size_t)y0 * V.ld), reinterpret_cast<const float4*>(c.qvec), ng, lane); ab1 = 0.0f; }
-            if (lane == 0) { finish(j, y0, ab0, n0); if (two) finish(j + W, y1, ab1, n1); }
+            bool x0 = true, x1 = two;   // the f32 row is read
+            float n0, n1;
+            if (screen) {
+                float4 r0 = __ldg(V.hrec + y0), r1 = __ldg(V.hrec + y1);
+                float h0, h1;
+                if (two) warp_dot2_h<NG>(hrow(y0), hrow(y1), qv, ng, lane, h0, h1);
+                else { h0 = warp_dot_h<NG>(hrow(y0), qv, ng, lane); h1 = 0.0f; }
+                x0 = !hs_screened_out(V, c, y0, h0, r0, wkey);
+                x1 = two && !hs_screened_out(V, c, y1, h1, r1, wkey);
+                n0 = r0.x; n1 = r1.x;
+            } else {
+                n0 = V.sim != SIM_DOT ? __ldg(V.norms + y0) : 0.0f; n1 = (two && V.sim != SIM_DOT) ? __ldg(V.norms + y1) : 0.0f;
+            }
+            float ab0 = 0.0f, ab1 = 0.0f;
+            if (x0 && x1) warp_dot2_t<NG>(frow(y0), frow(y1), qv, ng, lane, ab0, ab1);
+            else if (x0) ab0 = warp_dot_t<NG>(frow(y0), qv, ng, lane);
+            else if (x1) ab1 = warp_dot_t<NG>(frow(y1), qv, ng, lane);
+            if (lane == 0) {
+                if (x0) finish(j, y0, ab0, n0); else skip(j);
+                if (x1) finish(j + W, y1, ab1, n1); else if (two) skip(j + W);
+            }
         }
     } else {
         for (int j = warp; j < ntodo; j += W) {
             uint32_t y = c.todo_id[j];
-            float vnorm = V.sim != SIM_DOT ? __ldg(V.norms + y) : 0.0f;
-            float ab = warp_dot_t<NG>(reinterpret_cast<const float4*>(V.vecs + (size_t)y * V.ld), reinterpret_cast<const float4*>(c.qvec), ng, lane);
+            float vnorm;
+            if (screen) {
+                float4 r = __ldg(V.hrec + y);
+                float ah = warp_dot_h<NG>(hrow(y), qv, ng, lane);
+                if (hs_screened_out(V, c, y, ah, r, wkey)) { if (lane == 0) skip(j); continue; }
+                vnorm = r.x;
+            } else vnorm = V.sim != SIM_DOT ? __ldg(V.norms + y) : 0.0f;
+            float ab = warp_dot_t<NG>(frow(y), qv, ng, lane);
             if (lane == 0) finish(j, y, ab, vnorm);
         }
     }
@@ -408,7 +469,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_ker
     c.hash_bits = a.hash_bits;
     c.hash_mask = (1u << a.hash_bits) - 1;
     c.hash_limit = (int)((15u << a.hash_bits) >> 4) - HS_MAX_ROW;
-    c.n_dist = c.n_expand = c.n_overflow = 0;
+    c.n_dist = c.n_expand = c.n_overflow = c.n_skip = 0;
     int lane = threadIdx.x & 31;
     int ng = V.ld >> 2;
 
@@ -425,6 +486,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_ker
         else { self = a.nodes[q]; qsrc = V.vecs + (size_t)self * V.ld; c.qnorm = V.sim != SIM_DOT ? V.norms[self] : 0.0f; }
         for (int i = threadIdx.x; i < ng; i += blockDim.x) reinterpret_cast<float4*>(c.qvec)[i] = reinterpret_cast<const float4*>(qsrc)[i];
         __syncthreads();
+        if (V.hvecs) c.qbound = hs_query_bound(c.qvec, V.ld);
 
         // entry point: similarity + single-entry list (search.rs:256-261)
         if (threadIdx.x < 32) {
@@ -465,8 +527,8 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_ker
 
         if (a.mode == 0) hs_emit_results<NG, W, PAIR>(V, G, c, a, q);
     }
-    // counters: n_dist lives in lane 0 of every warp, the rest in thread 0
-    if (lane == 0 && c.n_dist) atomicAdd(&a.counters[0], c.n_dist);
+    // counters: n_dist and n_skip live in lane 0 of every warp, the rest in thread 0; [6] = f32 rows read for a similarity
+    if (lane == 0 && c.n_dist) { atomicAdd(&a.counters[0], c.n_dist); atomicAdd(&a.counters[6], c.n_dist - c.n_skip); }
     if (threadIdx.x == 0) {
         if (c.n_expand) atomicAdd(&a.counters[1], c.n_expand);
         if (c.n_overflow & 0xFFFFFFFFull) atomicAdd(&a.counters[2], c.n_overflow & 0xFFFFFFFFull);

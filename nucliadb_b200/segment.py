@@ -190,6 +190,12 @@ class VectorSegment:
         check(_lib.load().nidx_vec_counters(self._h, out))
         return dict(similarities=out[0], expansions=out[1], overflows=out[2])
 
+    def exact_rows(self) -> int:
+        """f32 rows the last HNSW search / build read (<= counters()["similarities"]; the rest were settled on the fp16 copy)."""
+        out = C.c_uint64()
+        check(_lib.load().nidx_vec_exact_rows(self._h, C.byref(out)))
+        return out.value
+
 
 def merge_topk(ids, scores, device=0, part_stride=0, out=None):
     """[n_parts, nq, k] torch CUDA tensors (each part sorted desc, NIL padded) -> merged (ids, scores, part).
