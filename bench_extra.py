@@ -6,6 +6,8 @@
          - "or_basic": nidx_paragraph semantics (OR of TermQuery(Basic), tf == 1)
          - "and_tf":   nidx_text semantics (conjunction, real tf) on 3-term queries
   facets the bm25 corpus + seeded labels: OR-50 top-100 with / without faceted=["/l"], and the all-documents facet count
+  order  the bm25 corpus + seeded created / modified seconds: OR-50 top-100 and AND-3 ordered by date against the same searches by
+         score, ordered + faceted=["/l"], and the catalogue listing (empty body, top-100 by date over every alive document)
 
 bench.py (the driver's contract) stays the HNSW headline; this file produces the side measurements.
 """
@@ -385,6 +387,101 @@ def bench_facets(args):
              "cpu_baseline": {"value": cpu_s * 1e3, "unit": "ms", "cores": 1, "kind": "numpy restatement (tests/facet_oracle.py), one process"}}]
 
 
+def bench_order(args):
+    """TopDocs::order_by_fast_field on the BM25 corpus of `bm25` with seeded dates: created spread over ten years at minute
+    granularity with 10 % of the documents on 20 shared dates (heavy ties) and 1 % undated, modified a month at most later, 1 % of
+    the documents deleted, 100 labels /l/s{00..99}.  Runs and its unordered twin alternate within one call; the listing's bytes are
+    the algorithmic ones (rank column 4 B + alive bit per document, plus the top-k out); parity with tests/order_oracle.py on a sample."""
+    import torch
+
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import order_oracle as OO
+    from nucliadb_b200 import _lib
+    from nucliadb_b200.segment import TextSegment
+    from nucliadb_b200.text import fieldnorm_to_id
+
+    dev = torch.device("cuda", 0)
+    n_docs, n_terms, nq, k = args.docs, 1_000_000, 1024, 100
+    c = make_corpus(n_docs, n_terms, dev)
+    lut = np.asarray([fieldnorm_to_id(i) for i in range(int(c["lens"].max()) + 1)], dtype=np.uint8)
+    df = np.diff(c["term_off"].astype(np.int64)).astype(np.uint64)
+    ts = TextSegment.create(n_docs, n_terms, c["term_off"], c["post_doc"], c["post_tf"], lut[c["lens"]])
+    ts.set_stats(n_docs, c["total_tokens"], df)
+    rng = np.random.default_rng(13)
+    keys = sorted(f"l\0s{a:02d}".encode() for a in range(100))
+    ords = rng.integers(0, len(keys), n_docs).astype(np.uint32)
+    ts.set_facets(keys, np.arange(n_docs + 1, dtype=np.uint64), ords)
+    created = (1_450_000_000 + rng.integers(0, 10 * 365 * 1440, n_docs) * 60).astype(np.int64)
+    tie = rng.random(n_docs) < 0.10
+    created[tie] = 1_600_000_000 + rng.integers(0, 20, int(tie.sum())) * 86_400
+    created[rng.random(n_docs) < 0.01] = OO.NONE
+    modified = np.where(created == OO.NONE, OO.NONE, created + rng.integers(0, 30 * 86_400, n_docs)).astype(np.int64)
+    t0 = time.perf_counter()
+    ts.set_dates(created, modified)
+    t_dates = time.perf_counter() - t0
+    alive_b = rng.random(n_docs) >= 0.01
+    alive = np.packbits(alive_b, bitorder="little")
+    alive = np.concatenate([alive, np.zeros(-len(alive) % 8, np.uint8)]).view(np.uint64)
+    ts.set_alive(alive)
+    rng_q = np.random.default_rng(11)
+    band = np.nonzero((df >= 1_000) & (df <= 100_000))[0]
+    med = lambda x: float(np.median(x))
+    gpu = gpu_identity()
+    lines = []
+    for name, nterms, mode, use_tf in (("OR-50", 50, _lib.NIDX_BM25_OR, False), ("AND-3", 3, _lib.NIDX_BM25_AND, True)):
+        queries = [rng_q.choice(band, nterms, replace=False).astype(np.uint32) for _ in range(nq)]
+        qoff = torch.tensor(np.concatenate([[0], np.cumsum([len(x) for x in queries])]), dtype=torch.int32, device=dev)
+        qt = torch.tensor(np.concatenate(queries).astype(np.int64), dtype=torch.int32, device=dev)
+        runs = {"by score": lambda: ts.search(qt, qoff, k, mode=mode, use_tf=use_tf),
+                "by date": lambda: ts.search_ordered(qt, qoff, k, _lib.NIDX_ORDER_CREATED, _lib.NIDX_ORDER_DESC, mode)}
+        if name == "OR-50":
+            runs["by score + faceted"] = lambda: ts.search_faceted(qt, qoff, k, [b"l"], mode=mode, use_tf=use_tf)
+            runs["by date + faceted"] = lambda: ts.search_ordered(qt, qoff, k, _lib.NIDX_ORDER_CREATED, _lib.NIDX_ORDER_DESC, mode, facets=[b"l"])
+        ms, kms = {r: [] for r in runs}, {r: [] for r in runs}
+        for _ in range(5):
+            for r, fn in runs.items():
+                ms[r].append(timed(fn, args.steps, args.warmup)); kms[r].append(ts.last_kernel_ms())
+        # parity on a sample: ids, dates, counts, totals against the restatement; total against the search by score
+        got = ts.search_ordered(qt, qoff, k, _lib.NIDX_ORDER_CREATED, _lib.NIDX_ORDER_DESC, mode)
+        plain = ts.search(qt, qoff, k, mode=mode, use_tf=use_tf)
+        torch.cuda.synchronize()
+        gd, gs, gc, gt = [x.cpu().numpy() for x in got]
+        ok = bool(np.array_equal(gt, plain[3].cpu().numpy()))
+        sample = 8
+        for i in range(sample):
+            d, s, tot = OO.search(n_docs, c["term_off"], c["post_doc"], queries[i].tolist(), mode == _lib.NIDX_BM25_AND, alive, created, k, OO.DESC)
+            ok &= int(gc[i]) == len(d) and int(gt[i]) == tot and np.array_equal(gd[i, :len(d)].astype(np.int64), d) and np.array_equal(gs[i, :len(d)], s)
+        lines.append({"metric": f"order by date ({name} top-{k})", "value": med(ms["by date"]) / med(ms["by score"]), "unit": "x (by date / by score call)",
+                      "n_gpus": 1, "steps": args.steps, "warmup": args.warmup, "gpu": gpu, "higher_is_better": False, "data": "synthetic",
+                      "config": {"workload": f"BM25 {n_docs} docs / {nterms}-term {'AND, tf' if use_tf else 'OR, tf == 1'} queries x {nq}, top-{k}, created DESC",
+                                 "rounds": 5, "set_dates_seconds": t_dates, "distinct_created": int(len(np.unique(created)))},
+                      "runs": {r: {"ms_per_call": med(ms[r]), "kernel_ms": med(kms[r])} for r in runs},
+                      "parity": {"identical_to_oracle_and_total_to_search": bool(ok), "sample": sample}})
+    # the catalogue listing
+    list_fn = lambda: ts.list_ordered(k, _lib.NIDX_ORDER_CREATED, _lib.NIDX_ORDER_DESC, device_out=True)
+    l_ms, l_kms = [], []
+    for _ in range(5):
+        l_ms.append(timed(list_fn, args.steps, args.warmup)); l_kms.append(ts.last_kernel_ms())
+    ok = True
+    for field, secs in ((_lib.NIDX_ORDER_CREATED, created), (_lib.NIDX_ORDER_MODIFIED, modified)):
+        for typ in (_lib.NIDX_ORDER_DESC, _lib.NIDX_ORDER_ASC):
+            docs, dates, count, total = ts.list_ordered(k, field, typ)
+            d, s, tot = OO.list_all(n_docs, alive, secs, k, typ)
+            ok &= count == len(d) and total == tot and np.array_equal(docs[:count].astype(np.int64), d) and np.array_equal(dates[:count], s)
+    nbytes = 4 * n_docs + n_docs // 8 + k * 12
+    pk = 3350.0
+    ach = nbytes / (med(l_kms) * 1e-3) / 1e9
+    lines.append({"metric": f"order by date, catalogue listing top-{k}", "value": med(l_ms), "unit": "ms", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
+                  "gpu": gpu, "higher_is_better": False, "data": "synthetic",
+                  "config": {"workload": f"empty body, created DESC, top-{k} over {n_docs} documents (1 % deleted)", "rounds": 5},
+                  "roofline": {"bound": "hbm", "achieved": ach, "peak": pk, "unit": "GB/s", "frac": ach / pk, "kernel": "date_topk_all_kernel + date_merge_kernel",
+                               "kernel_ms": med(l_kms), "alg_bytes": nbytes,
+                               "alg_bytes_note": "rank column (4 B per document) + alive bits, each read once, + the top-k out; peak = H100 SXM data sheet"},
+                  "parity": {"identical_to_oracle": bool(ok), "checked": "CREATED / MODIFIED x DESC / ASC"}})
+    ts.close()
+    return lines
+
+
 def bench_rabitq(args):
     """SURVEY 8f rank 1: the HNSW walk with a RaBitQ query on a Dot index (hnsw/search.rs:306-383: estimate-ranked walk, k * 100
     layer-0 results, exact rerank) -- what the reference runs on every Dot index that carries vectors.quant -- next to the dense
@@ -466,7 +563,7 @@ def driver_extras(steps=5, warmup=3):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("which", choices=["scan", "bm25", "build", "merge", "rabitq", "facets", "all"])
+    ap.add_argument("which", choices=["scan", "bm25", "build", "merge", "rabitq", "facets", "order", "all"])
     ap.add_argument("--build-vectors", type=int, default=1_000_000)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
@@ -485,6 +582,8 @@ def main():
         lines += bench_rabitq(args)
     if args.which == "facets":
         lines += bench_facets(args)
+    if args.which == "order":
+        lines += bench_order(args)
     for line in lines:
         print(json.dumps(line))
 

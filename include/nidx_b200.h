@@ -270,7 +270,8 @@ int nidx_txt_search(nidx_txt_segment* seg, const uint32_t* query_terms, const ui
                     void* stream);
 
 /* Device time (CUDA events on the caller's stream) of bm25_kernel in the last nidx_txt_search on this segment (bench roofline),
- * or of the facet kernel of the last nidx_txt_search_faceted / nidx_txt_facet_count_all; not meaningful under concurrent searches. */
+ * or of the facet kernel of the last nidx_txt_search_faceted / nidx_txt_facet_count_all, of the order kernel of the last
+ * nidx_txt_search_ordered, or of the two listing kernels of the last nidx_txt_list_ordered; not meaningful under concurrent searches. */
 int nidx_txt_last_kernel_ms(nidx_txt_segment* seg, float* ms);
 
 /* ---- Facet counts: tantivy's FacetCollector next to Count and TopDocs
@@ -313,6 +314,40 @@ int nidx_txt_search_faceted(nidx_txt_segment* seg, const uint32_t* query_terms, 
 /* The same counts over every alive document (the AllQuery of an empty body, nidx_text/src/search_query.rs:100-101: the
  * only_faceted catalogue request): out_facet_counts[n_buckets] (`mem`, u32). */
 int nidx_txt_facet_count_all(nidx_txt_segment* seg, const nidx_txt_facet_request* facets, int mem, uint32_t* out_facet_counts, void* stream);
+
+/* ---- Order by date: TopDocs::order_by_fast_field("created" | "modified", Desc | Asc) next to Count (and the FacetCollector)
+ * (reference: nidx_text/src/reader.rs:208-287, 415-431 and nidx_paragraph/src/reader.rs:229-243, 270-287, 310-327).
+ * Dates are seconds (the reference stores DateTime::from_timestamp_secs(ts.seconds) and returns {seconds, nanos: 0}:
+ * nidx_text/src/schema.rs:48-57).  Results are ordered by (date in the requested direction, then doc ascending); documents without
+ * a date come after every dated document in both directions.  The order is exact over the whole i64 range of seconds. */
+#define NIDX_DATE_NONE INT64_MIN   /* the document has no date */
+#define NIDX_ORDER_CREATED 0       /* OrderBy.OrderField (nodereader.proto) */
+#define NIDX_ORDER_MODIFIED 1
+#define NIDX_ORDER_DESC 0          /* OrderBy.OrderType */
+#define NIDX_ORDER_ASC 1
+
+typedef struct nidx_txt_order {
+    int32_t field;   /* NIDX_ORDER_CREATED | NIDX_ORDER_MODIFIED */
+    int32_t type;    /* NIDX_ORDER_DESC | NIDX_ORDER_ASC */
+} nidx_txt_order;
+
+/* Every document's created and modified seconds (n_docs each, NIDX_DATE_NONE = none; host pointers).  The seconds and, per field,
+ * each document's dense rank among the segment's distinct dates (built on the device) live in HBM. */
+int nidx_txt_set_dates(nidx_txt_segment* seg, const int64_t* created, const int64_t* modified);
+
+/* nidx_txt_search (facets == NULL) or nidx_txt_search_faceted with TopDocs ordered by date: the matched set, out_total and the facet
+ * counts are theirs; out_docs / out_dates [nq][p->k] (`mem`; dates in seconds, i64) follow the order above, out_counts[nq] entries
+ * are filled (NIDX_NIL / NIDX_DATE_NONE padded).  p->min_score and search-after are ignored, as in the reference (convert_int_order);
+ * p->use_tf does not matter.  A segment without dates (nidx_txt_set_dates) is NIDX_EINVAL. */
+int nidx_txt_search_ordered(nidx_txt_segment* seg, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem,
+                            const nidx_txt_search_params* p, const nidx_txt_order* order, const nidx_txt_facet_request* facets, uint32_t* out_docs,
+                            int64_t* out_dates, int32_t* out_counts, uint64_t* out_total, uint32_t* out_facet_counts, void* stream);
+
+/* The empty body with an order (AllQuery, nidx_text/src/search_query.rs:100-101: the catalogue listing): the top k (1..1024) of every
+ * alive document by the order above -> out_docs / out_dates [k], *out_count; *out_total = the alive documents (Count). `mem` applies
+ * to the outputs. */
+int nidx_txt_list_ordered(nidx_txt_segment* seg, const nidx_txt_order* order, int32_t k, int mem, uint32_t* out_docs, int64_t* out_dates,
+                          int32_t* out_count, uint64_t* out_total, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Segments sharded over the GPUs of one node: one process (or thread) per GPU, one segment each

@@ -16,6 +16,9 @@ NIDX_MEM_HOST, NIDX_MEM_DEVICE = 0, 1
 NIDX_SIM_DOT, NIDX_SIM_COSINE, NIDX_SIM_L2 = 0, 1, 2
 NIDX_METHOD_AUTO, NIDX_METHOD_HNSW, NIDX_METHOD_BRUTE, NIDX_METHOD_BRUTE_RABITQ, NIDX_METHOD_HNSW_RABITQ = 0, 1, 2, 3, 4
 NIDX_BM25_OR, NIDX_BM25_AND = 0, 1
+NIDX_ORDER_CREATED, NIDX_ORDER_MODIFIED = 0, 1   # OrderBy.OrderField
+NIDX_ORDER_DESC, NIDX_ORDER_ASC = 0, 1           # OrderBy.OrderType
+NIDX_DATE_NONE = -(1 << 63)                      # a document without a date
 NIL = 0xFFFFFFFF
 
 # every symbol include/nidx_b200.h declares (tests check the .so exports exactly these)
@@ -28,6 +31,7 @@ SYMBOLS = [
     "nidx_vec_rabitq_encode", "nidx_vec_rabitq_codes", "nidx_vec_rabitq_estimate",
     "nidx_txt_create", "nidx_txt_set_stats", "nidx_txt_set_alive", "nidx_txt_close", "nidx_txt_search", "nidx_txt_last_kernel_ms",
     "nidx_txt_set_facets", "nidx_txt_facet_buckets", "nidx_txt_search_faceted", "nidx_txt_facet_count_all",
+    "nidx_txt_set_dates", "nidx_txt_search_ordered", "nidx_txt_list_ordered",
     "nidx_shard_unique_id", "nidx_shard_init", "nidx_shard_destroy", "nidx_vec_set_paragraph_keys", "nidx_vec_search_sharded", "nidx_txt_search_sharded",
     "nidx_txt_set_doc_keys", "nidx_rank_fusion_rrf", "nidx_shard_search",
 ]
@@ -66,6 +70,10 @@ class TxtSearchParams(C.Structure):
 
 class TxtFacetRequest(C.Structure):
     _fields_ = [("n", C.c_int32), ("key_bytes", C.c_void_p), ("key_off", C.c_void_p)]
+
+
+class TxtOrder(C.Structure):
+    _fields_ = [("field", C.c_int32), ("type", C.c_int32)]
 
 
 class RrfSource(C.Structure):

@@ -7,6 +7,7 @@ Reference:
   nidx/nidx_protos/nidx.proto:9,20-21                             NidxApi.NewShard, NidxSearcher.Search
   nidx/src/searcher/shard_search.rs:60-241                        one SearchRequest -> prefilter -> vector / paragraph / document searches
   nidx/src/searcher/shard_merge.rs:177-348, 380-414               merge of the per-shard responses (merge_facets: facet counts)
+  nidx/src/searcher/shard_merge.rs:235-249, 313-328, 416-436      ... under SearchRequest.order: by date (merge_order_key)
   nidx/nidx_vector/src/indexer.rs:96-146                          Resource -> vector Elems (key = sentence id, labels = paragraph labels)
   nidx/nidx_text/src/resource_indexer.rs:22-91                    Resource.texts -> one document per field
   nidx/nidx_paragraph/src/resource_indexer.rs:33-131              Resource.paragraphs -> one document per paragraph (text[start:end])
@@ -98,6 +99,13 @@ def merge_facets(shards_facets) -> dict:
     for (group, tag), total in counts.items():
         merged.setdefault(group, []).append((tag, total))
     return {g: sorted(v, key=lambda t: (-t[1], T.facet_key(t[0]) or b"")) for g, v in merged.items()}
+
+
+def merge_order_key(seconds: Optional[int], order_type: int, shard_pos: int, rank: int):
+    """Cross-shard order of date-ordered results (sort_documents_fn / sort_paragraphs_fn with SortExpr::Date, shard_merge.rs:235-249,
+    313-328): the date in the requested direction, then the shard's position in the request, then the result's rank in its shard.
+    The reference's kmerge_by leaves equal dates unpinned; this is the rule here.  Results without a date come last."""
+    return T.date_sort_key(seconds, order_type) + (shard_pos, rank)
 
 
 class NidxBinding:
@@ -198,8 +206,13 @@ class NidxBinding:
             if elems:
                 vi.segments.append((V.VectorIndexer.index_elems(elems, vi.config), seq))
         # documents (nidx_text/src/resource_indexer.rs:22-91): one per field; paragraphs (nidx_paragraph): one per paragraph
+        # dates (IndexMetadata, seconds: nidx_text/src/schema.rs:48-57); a resource without metadata is indexed without dates
+        meta = res.metadata if res.HasField("metadata") else None
+        created = meta.created.seconds if meta is not None and meta.HasField("created") else None
+        modified = meta.modified.seconds if meta is not None and meta.HasField("modified") else None
         if not res.skip_texts:
-            docs = [T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, ti.text, tuple(list(res.labels) + list(ti.labels))) for fid, ti in res.texts.items()]
+            docs = [T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, ti.text, tuple(list(res.labels) + list(ti.labels)), created, modified)
+                    for fid, ti in res.texts.items()]
             if docs:
                 shard.text_segments.append((docs, seq))
         if not res.skip_paragraphs:
@@ -208,7 +221,7 @@ class NidxBinding:
                 text = res.texts[fid].text if fid in res.texts else ""
                 for pid, par in paragraphs.paragraphs.items():
                     labels = tuple(list(res.labels) + list(res.texts[fid].labels if fid in res.texts else ()) + list(par.labels))
-                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels))
+                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels, created, modified))
                     shard.paragraph_meta[(rid, "/" + fid if not fid.startswith("/") else fid, len(pdocs) - 1, seq)] = (pid, par)
             if pdocs:
                 shard.paragraph_segments.append((pdocs, seq))
@@ -263,6 +276,7 @@ class NidxBinding:
     def _search_shard(self, shard: _Shard, req):
         k = int(req.result_per_page)
         out = {}
+        order = T.OrderBy(sort_by=int(req.order.sort_by), type=int(req.order.type)) if req.HasField("order") else None
         # prefilter (shard_search.rs:108-137): field_filter on the documents -> the fields that may answer
         prefilter = V.PrefilterResult.all()
         if req.HasField("field_filter") and shard.text_searcher is not None:
@@ -280,13 +294,13 @@ class NidxBinding:
             out["vector"] = vi.searcher.search(vreq, prefilter).documents if vi.searcher is not None else []
         if req.document and shard.text_searcher is not None:
             out["document"] = shard.text_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25),
-                                                                                 faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted)))
+                                                                                 faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order))
         if req.paragraph and shard.paragraph_searcher is not None:
             after = None
             if req.HasField("search_after"):
                 after = T.SearchAfter(score=req.search_after.score, tie_break="keep_after", docaddr=int(req.search_after.docaddr))
             out["paragraph"] = shard.paragraph_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25), search_after=after,
-                                                                                       faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted)))
+                                                                                       faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order))
         return out
 
     def _merge(self, req, parts):
@@ -301,12 +315,18 @@ class NidxBinding:
             ds.labels.extend(d.labels)
             if d.metadata:
                 ds.metadata.CopyFrom(P.SentenceMetadata.FromString(d.metadata))
-        # documents / paragraphs: bm25 desc, then shard, then lower docaddr (shard_merge.rs:227-231)
+        # documents / paragraphs: bm25 desc, then shard, then lower docaddr (shard_merge.rs:227-231); under an order by date
+        # (merge_order_key), the sort value is the date
+        ordered = req.HasField("order")
         for kind, target in (("document", resp.document), ("paragraph", resp.paragraph)):
             found = [(sid, p[kind]) for sid, p in parts if kind in p]
             if not found:
                 continue
-            rows = sorted(((-r.score.bm25, i, r.score.docaddr, sid, r) for i, (sid, rs) in enumerate(found) for r in rs.results), key=lambda t: t[:3])
+            if ordered:
+                rows = sorted(((merge_order_key(r.date, int(req.order.type), i, j), i, 0, sid, r) for i, (sid, rs) in enumerate(found) for j, r in enumerate(rs.results)),
+                              key=lambda t: t[0])
+            else:
+                rows = sorted(((-r.score.bm25, i, r.score.docaddr, sid, r) for i, (sid, rs) in enumerate(found) for r in rs.results), key=lambda t: t[:3])
             target.total = sum(rs.total for _, rs in found)
             target.next_page = any(rs.next_page for _, rs in found) or len(rows) > k
             target.query = req.body
@@ -315,7 +335,10 @@ class NidxBinding:
             for _, _, _, sid, r in rows[:k]:
                 o = target.results.add()
                 o.uuid, o.field = r.uuid, r.field
-                o.score.bm25, o.score.docaddr = r.score.bm25, r.score.docaddr
+                if not ordered:
+                    o.score.bm25, o.score.docaddr = r.score.bm25, r.score.docaddr
+                elif r.date is not None:
+                    o.date.seconds, o.date.nanos = r.date, 0   # second precision: {seconds, nanos: 0} (nidx_text/src/schema.rs:48-57)
                 o.labels.extend(r.labels)
                 o.shard_id = sid.encode()
         return resp

@@ -2,6 +2,7 @@
 // what nidx_vector's OpenSegment / HnswBuilder and the tantivy collector call do on the CPU in the
 // reference is orchestrated here on one GPU.  No CPU fallback: every entry point needs a device.
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <atomic>
@@ -1862,6 +1863,10 @@ struct nidx_txt_segment {
     uint32_t* d_fdoc_off = nullptr;   // [n_docs + 1]
     uint32_t* d_ford = nullptr;       // [n_facet_ords]
     uint64_t n_facet_ords = 0;
+    // dates (nidx_txt_set_dates), per field (NIDX_ORDER_CREATED, NIDX_ORDER_MODIFIED): the seconds and every document's dense rank
+    int64_t* d_secs[2] = {nullptr, nullptr};     // [n_docs]
+    uint32_t* d_rank[2] = {nullptr, nullptr};    // [n_docs rounded up to 8], 0 = no date
+    uint32_t n_ranks[2] = {0, 0};
     WorkspacePool pool;
 };
 
@@ -1983,6 +1988,7 @@ void nidx_txt_close(nidx_txt_segment* t) {
     cudaDeviceSynchronize();
     cudaFree(t->d_term_off); cudaFree(t->d_post); cudaFree(t->d_skip_row); cudaFree(t->d_skip); cudaFree(t->d_alive); cudaFree(t->d_weight);
     cudaFree(t->d_norm_cache); cudaFree(t->d_error); cudaFree(t->d_doc_keys); cudaFree(t->d_fdoc_off); cudaFree(t->d_ford);
+    for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); }
     if (t->ev_k0) cudaEventDestroy(t->ev_k0);
     if (t->ev_k1) cudaEventDestroy(t->ev_k1);
     delete t;
@@ -2029,7 +2035,74 @@ int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* k
     return 0;
 }
 
+int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_t* modified) {
+    if (!t || !created || !modified) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->device));
+    for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); t->d_secs[f] = nullptr; t->d_rank[f] = nullptr; t->n_ranks[f] = 0; }
+    const uint32_t n = t->n_docs;
+    const size_t padded = std::max<size_t>(((size_t)n + 7) & ~(size_t)7, 8);
+    // ranks: sort (seconds, doc) on the device, flag the first document of every distinct date, inclusive prefix sum, scatter
+    int64_t* d_sorted = nullptr;
+    uint32_t *d_doc = nullptr, *d_doc_sorted = nullptr, *d_flag = nullptr, *d_incl = nullptr;
+    void* d_cub = nullptr;
+    int r = [&]() -> int {
+        size_t sort_bytes = 0, scan_bytes = 0;
+        if (n) {
+            CU(cudaMalloc(&d_sorted, (size_t)n * 8));
+            CU(cudaMalloc(&d_doc, (size_t)n * 4));
+            CU(cudaMalloc(&d_doc_sorted, (size_t)n * 4));
+            CU(cudaMalloc(&d_flag, (size_t)n * 4));
+            CU(cudaMalloc(&d_incl, (size_t)n * 4));
+            std::vector<uint32_t> iota(n);
+            for (uint32_t i = 0; i < n; ++i) iota[i] = i;
+            CU(cudaMemcpy(d_doc, iota.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+            CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const int64_t*)nullptr, d_sorted, d_doc, d_doc_sorted, (int)n));
+            CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, d_flag, d_incl, (int)n));
+            CU(cudaMalloc(&d_cub, std::max(sort_bytes, scan_bytes)));
+        }
+        const int blocks = std::max(1, std::min<int>(t->sm_count * 8, (int)((n + 255) / 256)));
+        for (int f = 0; f < 2; ++f) {
+            CU(cudaMalloc(&t->d_secs[f], std::max<size_t>(n, 1) * 8));
+            CU(cudaMalloc(&t->d_rank[f], padded * 4));
+            CU(cudaMemset(t->d_rank[f], 0, padded * 4));
+            if (!n) continue;
+            CU(cudaMemcpy(t->d_secs[f], f == 0 ? created : modified, (size_t)n * 8, cudaMemcpyHostToDevice));
+            size_t tmp = sort_bytes;
+            CU(cub::DeviceRadixSort::SortPairs(d_cub, tmp, (const int64_t*)t->d_secs[f], d_sorted, d_doc, d_doc_sorted, (int)n));
+            LAUNCHED();
+            date_flag_kernel<<<blocks, 256>>>(d_sorted, n, d_flag);
+            LAUNCHED();
+            tmp = scan_bytes;
+            CU(cub::DeviceScan::InclusiveSum(d_cub, tmp, d_flag, d_incl, (int)n));
+            LAUNCHED();
+            date_scatter_kernel<<<blocks, 256>>>(d_incl, d_doc_sorted, n, t->d_rank[f]);
+            LAUNCHED();
+            CU(cudaGetLastError());
+            CU(cudaMemcpy(&t->n_ranks[f], d_incl + n - 1, 4, cudaMemcpyDeviceToHost));
+        }
+        CU(cudaDeviceSynchronize());
+        return 0;
+    }();
+    cudaFree(d_sorted); cudaFree(d_doc); cudaFree(d_doc_sorted); cudaFree(d_flag); cudaFree(d_incl); cudaFree(d_cub);
+    if (r) {
+        for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); t->d_secs[f] = nullptr; t->d_rank[f] = nullptr; t->n_ranks[f] = 0; }
+    }
+    return r;
+}
+
 }  // extern "C"
+
+// An order resolved against the segment: the field's rank column and seconds.
+static int order_args(const nidx_txt_segment* t, const nidx_txt_order* order, OrderArgs& O) {
+    if (!order || (order->field != NIDX_ORDER_CREATED && order->field != NIDX_ORDER_MODIFIED) || (order->type != NIDX_ORDER_DESC && order->type != NIDX_ORDER_ASC))
+        return fail(NIDX_EINVAL, "bad order");
+    if (!t->d_rank[order->field]) return fail(NIDX_EINVAL, "the segment has no dates (nidx_txt_set_dates)");
+    O.rank = t->d_rank[order->field];
+    O.secs = t->d_secs[order->field];
+    O.n_ranks = t->n_ranks[order->field];
+    O.asc = order->type == NIDX_ORDER_ASC;
+    return 0;
+}
 
 // A facet request resolved against the segment's dictionary: bucket[ord] = the bucket of the requested facet's child the ord lies
 // under (NIL: none), and per bucket the request it belongs to and the first ord under its child (what names it).  Requests are
@@ -2083,16 +2156,25 @@ static int facet_args(const nidx_txt_segment* t, const FacetPlan& P, Workspace& 
 
 typedef void (*bm_kernel_t)(TxtDev, Bm25Args);
 typedef void (*bm_facet_kernel_t)(TxtDev, Bm25Args, FacetArgs);
+typedef void (*bm_order_kernel_t)(TxtDev, Bm25Args, OrderArgs);
+typedef void (*bm_order_facet_kernel_t)(TxtDev, Bm25Args, FacetArgs, OrderArgs);
 
-// The body of nidx_txt_search (facets == nullptr) and nidx_txt_search_faceted.  qhost / ohost as in vec_search_impl.
+// The body of nidx_txt_search (facets == nullptr), nidx_txt_search_faceted and nidx_txt_search_ordered (order != nullptr: dates to
+// out_dates instead of scores to out_scores).  qhost / ohost as in vec_search_impl.
 static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, bool qhost, bool ohost,
                            const nidx_txt_search_params* p, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total, cudaStream_t stream,
-                           const nidx_txt_facet_request* facets = nullptr, uint32_t* out_facet_counts = nullptr) {
-    if (!t || !p || !query_off || !out_docs || !out_scores || !out_counts) return fail(NIDX_EINVAL, "null argument");
+                           const nidx_txt_facet_request* facets = nullptr, uint32_t* out_facet_counts = nullptr, const nidx_txt_order* order = nullptr,
+                           int64_t* out_dates = nullptr) {
+    if (!t || !p || !query_off || !out_docs || !(order ? (void*)out_dates : (void*)out_scores) || !out_counts) return fail(NIDX_EINVAL, "null argument");
     FacetPlan plan;
     if (facets) {
         if (!out_facet_counts) return fail(NIDX_EINVAL, "null argument");
         int r = facet_plan(t, facets, plan);
+        if (r) return r;
+    }
+    OrderArgs O{};
+    if (order) {
+        int r = order_args(t, order, O);
         if (r) return r;
     }
     if (nq <= 0) return 0;
@@ -2132,11 +2214,12 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     unsigned long long* d_total = reinterpret_cast<unsigned long long*>(out_total);
     if (ohost) {
         ENSURE(w.out_ids, (size_t)nq * k * 4);
-        ENSURE(w.out_scores, (size_t)nq * k * 4);
+        ENSURE(w.out_scores, (size_t)nq * k * (order ? 8 : 4));
         ENSURE(w.out_counts, (size_t)nq * 4);
         d_docs = w.out_ids.as<uint32_t>(); d_sc = w.out_scores.as<float>(); d_cnt = w.out_counts.as<int>();
         d_total = w.misc.as<unsigned long long>();
     }
+    int64_t* d_dates = ohost ? w.out_scores.as<int64_t>() : out_dates;
     TxtDev T;
     T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
     T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
@@ -2145,7 +2228,15 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache; a.shift = shift;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
     a.out_keys = w.partial.as<uint64_t>(); a.out_total = d_total; a.error_flag = t->d_error;
-    if (!facets) {
+    if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after
+    if (order && !facets) {
+        bm_order_kernel_t kern = conj ? bm25_order_kernel<true> : bm25_order_kernel<false>;
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CU(cudaEventRecord(t->ev_k0, stream));
+        kern<<<nq, BM_THREADS, smem, stream>>>(T, a, O);
+        CU(cudaEventRecord(t->ev_k1, stream));
+        LAUNCHED();
+    } else if (!facets) {
         bm_kernel_t kern = conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>);
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         CU(cudaEventRecord(t->ev_k0, stream));
@@ -2162,21 +2253,31 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
         if (F.smem && smem + nb * 4 > 220 * 1024) F.smem = 0;
         if (!F.smem && nb) CU(cudaMemsetAsync(d_fc, 0, (size_t)nq * nb * 4, stream));
         const size_t fsmem = smem + (F.smem ? nb * 4 : 0);
-        bm_facet_kernel_t kern = conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
-                                      : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>);
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-        CU(cudaEventRecord(t->ev_k0, stream));
-        kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F);
-        CU(cudaEventRecord(t->ev_k1, stream));
+        if (order) {
+            bm_order_facet_kernel_t kern = conj ? bm25_order_facet_kernel<true> : bm25_order_facet_kernel<false>;
+            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+            CU(cudaEventRecord(t->ev_k0, stream));
+            kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F, O);
+            CU(cudaEventRecord(t->ev_k1, stream));
+        } else {
+            bm_facet_kernel_t kern = conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
+                                          : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>);
+            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+            CU(cudaEventRecord(t->ev_k0, stream));
+            kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F);
+            CU(cudaEventRecord(t->ev_k1, stream));
+        }
         LAUNCHED();
         if (ohost && nb) CU(cudaMemcpyAsync(out_facet_counts, d_fc, (size_t)nq * nb * 4, cudaMemcpyDeviceToHost, stream));
     }
-    bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
+    if (order) date_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, O.secs, d_docs, d_dates, d_cnt);
+    else bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
     LAUNCHED();
     CU(cudaGetLastError());
     if (ohost) {
         CU(cudaMemcpyAsync(out_docs, d_docs, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
+        if (order) CU(cudaMemcpyAsync(out_dates, d_dates, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, stream));
+        else CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
         CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
         if (out_total) CU(cudaMemcpyAsync(out_total, d_total, (size_t)nq * 8, cudaMemcpyDeviceToHost, stream));
         CU(cudaStreamSynchronize(stream));
@@ -2244,6 +2345,62 @@ int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* 
     CU(cudaGetLastError());
     if (host) {
         CU(cudaMemcpyAsync(out_facet_counts, d_fc, nb * 4, cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+    }
+    return 0;
+}
+
+int nidx_txt_search_ordered(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem, const nidx_txt_search_params* p,
+                            const nidx_txt_order* order, const nidx_txt_facet_request* facets, uint32_t* out_docs, int64_t* out_dates, int32_t* out_counts,
+                            uint64_t* out_total, uint32_t* out_facet_counts, void* stream_) {
+    if (!order) return fail(NIDX_EINVAL, "null argument");
+    bool host = mem == NIDX_MEM_HOST;
+    return txt_search_impl(t, query_terms, query_off, nq, host, host, p, out_docs, nullptr, out_counts, out_total, reinterpret_cast<cudaStream_t>(stream_),
+                           facets, out_facet_counts, order, out_dates);
+}
+
+int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int32_t k, int mem, uint32_t* out_docs, int64_t* out_dates, int32_t* out_count,
+                          uint64_t* out_total, void* stream_) {
+    if (!t || !out_docs || !out_dates || !out_count) return fail(NIDX_EINVAL, "null argument");
+    OrderArgs O;
+    int r = order_args(t, order, O);
+    if (r) return r;
+    if (k <= 0 || k > 1024) return fail(NIDX_EINVAL, "k must be in 1..1024");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(t->device));
+    WsGuard g(t->pool, stream);
+    Workspace& w = *g.w;
+    // per-CTA top-k over a grid-stride slice, then one merge (the scan_select / topk_merge pattern)
+    const int threads = 512;
+    const int blocks = std::max(1, std::min<int>(t->sm_count * 2, (int)(((size_t)t->n_docs + threads * DATE_PT - 1) / (threads * DATE_PT))));
+    const int cap = topk_cap(k, threads);
+    ENSURE(w.partial, (size_t)blocks * k * 8);
+    ENSURE(w.misc, 8);
+    uint32_t* d_docs = out_docs; int64_t* d_dates = out_dates; int* d_cnt = out_count;
+    unsigned long long* d_total = reinterpret_cast<unsigned long long*>(out_total);
+    if (host || !out_total) d_total = w.misc.as<unsigned long long>();
+    if (host) {
+        ENSURE(w.out_ids, (size_t)k * 4);
+        ENSURE(w.out_scores, (size_t)k * 8);
+        ENSURE(w.out_counts, 4);
+        d_docs = w.out_ids.as<uint32_t>(); d_dates = w.out_scores.as<int64_t>(); d_cnt = w.out_counts.as<int>();
+    }
+    CU(cudaFuncSetAttribute(date_topk_all_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    CU(cudaFuncSetAttribute(date_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    CU(cudaMemsetAsync(d_total, 0, 8, stream));
+    CU(cudaEventRecord(t->ev_k0, stream));
+    date_topk_all_kernel<<<blocks, threads, (size_t)cap * 8, stream>>>(t->n_docs, t->d_alive, O, k, cap, w.partial.as<uint64_t>(), d_total);
+    LAUNCHED();
+    date_merge_kernel<<<1, threads, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), blocks * k, k, cap, O.secs, d_docs, d_dates, d_cnt);
+    LAUNCHED();
+    CU(cudaEventRecord(t->ev_k1, stream));
+    CU(cudaGetLastError());
+    if (host) {
+        CU(cudaMemcpyAsync(out_docs, d_docs, (size_t)k * 4, cudaMemcpyDeviceToHost, stream));
+        CU(cudaMemcpyAsync(out_dates, d_dates, (size_t)k * 8, cudaMemcpyDeviceToHost, stream));
+        CU(cudaMemcpyAsync(out_count, d_cnt, 4, cudaMemcpyDeviceToHost, stream));
+        if (out_total) CU(cudaMemcpyAsync(out_total, d_total, 8, cudaMemcpyDeviceToHost, stream));
         CU(cudaStreamSynchronize(stream));
     }
     return 0;

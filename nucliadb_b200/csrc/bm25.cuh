@@ -186,6 +186,98 @@ __global__ void facet_count_all_kernel(uint32_t n_docs, const uint64_t* __restri
     }
 }
 
+// ---- order by date (TopDocs::order_by_fast_field("created" | "modified", Desc | Asc): nidx_text/src/reader.rs:208-224,
+// nidx_paragraph/src/reader.rs:229-243) ------------------------------------------------------------------------------------------
+// Every document of a segment holds the dense rank of its date among the segment's distinct dates (1..n_ranks, ascending seconds;
+// 0 = no date), built once by nidx_txt_set_dates.  The rank in the requested direction takes the score's place in the 64-bit key:
+//   key = dir_rank << 32 | (0x7FFFFFFF - doc) << 1,   dir_rank = rank (DESC) or n_ranks + 1 - rank (ASC), 0 without a date,
+// so the existing top-k orders by (date in the requested direction, doc ascending), undated documents last, and key_id() still
+// gives the document.  The order is exact over all of i64: the ranks come from a sort of the seconds themselves.
+struct OrderArgs {
+    const uint32_t* rank;      // [n_docs rounded up to 8] (padding 0)
+    const int64_t* secs;       // [n_docs] seconds, NIDX_DATE_NONE = no date
+    uint32_t n_ranks;
+    int asc;
+};
+constexpr int64_t DATE_NONE = INT64_MIN;
+
+__device__ __forceinline__ uint64_t order_key(uint32_t rank, uint32_t n_ranks, int asc, uint32_t doc) {
+    const uint32_t dr = rank == 0 ? 0u : (asc ? n_ranks + 1u - rank : rank);
+    return ((uint64_t)dr << 32) | (uint64_t)((0x7FFFFFFFu - doc) << 1);
+}
+__device__ __forceinline__ uint64_t order_key(const OrderArgs& O, uint32_t doc) { return order_key(__ldg(O.rank + doc), O.n_ranks, O.asc, doc); }
+
+// nidx_txt_set_dates: sorted (seconds, doc) pairs -> first-of-its-date flags (NIDX_DATE_NONE sorts first and is never flagged); their
+// inclusive prefix sum is the dense rank, scattered back to the documents.
+__global__ void date_flag_kernel(const int64_t* __restrict__ sorted, uint32_t n, uint32_t* __restrict__ flag) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+        flag[i] = sorted[i] != DATE_NONE && (i == 0 || sorted[i] != sorted[i - 1]);
+}
+__global__ void date_scatter_kernel(const uint32_t* __restrict__ incl, const uint32_t* __restrict__ doc_of, uint32_t n, uint32_t* __restrict__ rank) {
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) rank[doc_of[i]] = incl[i];
+}
+
+// The catalogue listing (empty body + order: AllQuery, nidx_text/src/search_query.rs:100-101): per CTA, the top-k by date key of
+// a grid-stride slice of the alive documents, written to partial[blockIdx.x][k]; the Count of AllQuery (alive documents) is added
+// to *total (zeroed by the caller).  A thread takes DATE_PT consecutive documents per round: two 16-byte rank loads and one byte of
+// alive bits, all in flight together.  dynamic smem: cap * 8.
+constexpr int DATE_PT = 8;
+__global__ void date_topk_all_kernel(uint32_t n_docs, const uint64_t* __restrict__ alive, OrderArgs O, int k, int cap, uint64_t* __restrict__ partial,
+                                     unsigned long long* __restrict__ total) {
+    extern __shared__ __align__(16) uint64_t tk_buf[];
+    __shared__ int tk_count;
+    __shared__ uint64_t tk_thr;
+    __shared__ unsigned long long s_hits;
+    BlockTopK tk;
+    if (threadIdx.x == 0) s_hits = 0;
+    tk.init(tk_buf, &tk_count, &tk_thr, k, cap);
+    unsigned int hits = 0;
+    const uint32_t step = gridDim.x * blockDim.x * DATE_PT;
+    for (uint32_t base = blockIdx.x * blockDim.x * DATE_PT; base < n_docs; base += step) {   // (uniform per CTA)
+        const uint32_t d0 = base + threadIdx.x * DATE_PT;
+        uint32_t r[DATE_PT];
+        uint32_t live = 0;
+        if (d0 < n_docs) {
+            const uint4 a = __ldg(reinterpret_cast<const uint4*>(O.rank + d0)), b = __ldg(reinterpret_cast<const uint4*>(O.rank + d0) + 1);
+            r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
+            live = alive ? __ldg(reinterpret_cast<const unsigned char*>(alive) + (d0 >> 3)) : 0xFFu;
+            if (n_docs - d0 < DATE_PT) live &= (1u << (n_docs - d0)) - 1u;
+            hits += __popc(live);
+        }
+#pragma unroll
+        for (int u = 0; u < DATE_PT; ++u) tk.offer((live >> u) & 1u ? order_key(r[u], O.n_ranks, O.asc, d0 + u) : 0);
+    }
+    for (int off = 16; off >= 1; off >>= 1) hits += __shfl_xor_sync(0xFFFFFFFFu, hits, off);
+    if ((threadIdx.x & 31) == 0 && hits) atomicAdd(&s_hits, (unsigned long long)hits);
+    int c = tk.finish();
+    uint64_t* out = partial + (size_t)blockIdx.x * k;
+    for (int i = threadIdx.x; i < k; i += blockDim.x) out[i] = i < c ? tk_buf[i] : 0;
+    if (threadIdx.x == 0 && s_hits) atomicAdd(total, s_hits);
+}
+
+// Per query: top-k of n_in date keys (0 = empty) -> (doc, seconds) and the count.  dynamic smem: cap * 8.
+__global__ void date_merge_kernel(const uint64_t* __restrict__ keys_in, int n_in, int k, int cap, const int64_t* __restrict__ secs, uint32_t* __restrict__ out_docs,
+                                  int64_t* __restrict__ out_dates, int* __restrict__ out_counts) {
+    extern __shared__ __align__(16) uint64_t tk_buf[];
+    __shared__ int tk_count;
+    __shared__ uint64_t tk_thr;
+    const int q = blockIdx.x;
+    BlockTopK tk;
+    tk.init(tk_buf, &tk_count, &tk_thr, k, cap);
+    const uint64_t* in = keys_in + (size_t)q * n_in;
+    for (int base = 0; base < n_in; base += blockDim.x) {
+        int i = base + threadIdx.x;
+        tk.offer(i < n_in ? in[i] : 0);
+    }
+    int c = tk.finish();
+    for (int i = threadIdx.x; i < k; i += blockDim.x) {
+        const uint32_t doc = i < c ? key_id(tk_buf[i]) : NIL;
+        out_docs[(size_t)q * k + i] = doc;
+        out_dates[(size_t)q * k + i] = i < c ? secs[doc] : DATE_NONE;
+    }
+    if (threadIdx.x == 0) out_counts[q] = c;
+}
+
 __host__ __device__ __forceinline__ size_t bm_smem_bytes(int cap, bool conj) {
     return (size_t)cap * 8 + 2 * BM_MAX_TERMS * 8 /* run start */ + BM_WORDS * 4 /* bitmap */ + BM_ACC * 4 /* acc */ + BM_ACC * 4 /* candidates */ +
            2 * BM_MAX_TERMS * 4 /* run length */ + BM_MAX_TERMS * 4 /* weights */ + 1024 /* norm / ratio table */ + BM_WORDS * 2 /* rank bases */ +
@@ -202,8 +294,12 @@ __device__ __forceinline__ uint2 ldg_post(const uint2* p) {
 // CONJ: nidx_text (all terms must match).  TF: real term frequencies (else IndexRecordOption::Basic, tf == 1).
 // FACET: the FacetCollector runs beside Count on the same matched documents (bm25_facet_kernel); with FACET false every facet
 // statement compiles away and bm25_kernel is the search without facets.
-template <bool CONJ, bool TF, bool FACET>
-__device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, const FacetArgs& F) {
+// ORDER: TopDocs orders by date instead of score (bm25_order_kernel): every matched document -- the set Count counts -- is offered
+// with its date key (OrderArgs) instead of a score key.  No score is computed: OR skips phase C and walks the tile bitmap AND alive
+// after phase S instead (phase O); AND keeps phase C's conjunction counters only.  min_score and search-after do not apply.  With
+// ORDER false every order statement compiles away.
+template <bool CONJ, bool TF, bool FACET, bool ORDER>
+__device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, const FacetArgs& F, const OrderArgs& O) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int tk_count;
     __shared__ uint64_t tk_thr;
@@ -355,7 +451,12 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
         if (T.alive) match = (T.alive[doc >> 6] >> (doc & 63)) & 1;
         if (CONJ && match) my_hits++;
         if (FACET && CONJ && match) facet_doc(F, doc, fcnt);   // AND: every completed conjunction is a candidate
-        if (match) {
+        if (ORDER) {
+            if (match) {
+                const uint64_t key = order_key(O, doc);
+                if (key > tk_thr) tk_buf[atomicAdd(&tk_count, 1)] = key;
+            }
+        } else if (match) {
             float score = __fdiv_rn((float)v, scale);
             bool after = true;   // is_after(): strictly lower score, or an equal score that the tie break keeps
             if (a.after_mode != 0) {
@@ -488,7 +589,8 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
             // base, the weight and the norm entry of different postings overlap); which adds crossed the threshold is kept in a
             // per-thread mask and the candidates are appended afterwards -- a warp vote per posting only where some lane has one
             // (rare once the top-k threshold is established).
-            for (int round = 0; round < nrounds; ++round) {
+            // ORDER: no scores; AND keeps the conjunction counters, OR has nothing to do here (phase O below).
+            for (int round = 0; round < (ORDER && !CONJ ? 0 : nrounds); ++round) {
                 if (!one_round) load_round(round);
                 uint32_t cmask = 0;
                 uint32_t cds[BM_PT];
@@ -499,19 +601,28 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
                         uint32_t off = pd[u].x - lo, tfn = pd[u].y;
                         uint32_t wd = bitmap[off >> 5];
                         uint32_t rank = (uint32_t)base[off >> 5] + __popc(wd & ((1u << (off & 31)) - 1u));
-                        float wgt = tw[(rpack[u >> 2] >> (8 * (u & 3))) & 0xFFu];
-                        float frac;
-                        if (TF) { float tff = (float)(tfn >> 8); frac = __fdiv_rn(tff, __fadd_rn(tff, ntab[tfn & 0xFFu])); }
-                        else frac = ntab[tfn & 0xFFu];
-                        uint32_t fx = (uint32_t)__float2uint_rn(__fmul_rn(wgt, frac));
-                        if (fx == 0) fx = 1;
-                        uint32_t oldv = atomicAdd(&acc[rank], fx);
                         bool crossed;
-                        if (CONJ) {
-                            uint32_t oldw = atomicAdd(&cnts[rank >> 2], 1u << (8 * (rank & 3)));   // byte counter (nt <= 128) inside its 32-bit word
-                            crossed = (int)(((oldw >> (8 * (rank & 3))) & 0xFFu) + 1) == nt;       // the posting that completes the conjunction hands the document on
+                        if (ORDER) {
+                            if (CONJ) {
+                                uint32_t oldw = atomicAdd(&cnts[rank >> 2], 1u << (8 * (rank & 3)));
+                                crossed = (int)(((oldw >> (8 * (rank & 3))) & 0xFFu) + 1) == nt;
+                            } else {
+                                crossed = false;
+                            }
                         } else {
-                            crossed = oldv < thr_fx && oldv + fx >= thr_fx;
+                            float wgt = tw[(rpack[u >> 2] >> (8 * (u & 3))) & 0xFFu];
+                            float frac;
+                            if (TF) { float tff = (float)(tfn >> 8); frac = __fdiv_rn(tff, __fadd_rn(tff, ntab[tfn & 0xFFu])); }
+                            else frac = ntab[tfn & 0xFFu];
+                            uint32_t fx = (uint32_t)__float2uint_rn(__fmul_rn(wgt, frac));
+                            if (fx == 0) fx = 1;
+                            uint32_t oldv = atomicAdd(&acc[rank], fx);
+                            if (CONJ) {
+                                uint32_t oldw = atomicAdd(&cnts[rank >> 2], 1u << (8 * (rank & 3)));   // byte counter (nt <= 128) inside its 32-bit word
+                                crossed = (int)(((oldw >> (8 * (rank & 3))) & 0xFFu) + 1) == nt;       // the posting that completes the conjunction hands the document on
+                            } else {
+                                crossed = oldv < thr_fx && oldv + fx >= thr_fx;
+                            }
                         }
                         cds[u] = (rank << 17) | off;
                         if (crossed) cmask |= 1u << u;
@@ -547,6 +658,18 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
                     facet_docs(F, dd, fcnt);
                 }
             }
+            if (ORDER && !CONJ) {   // phase O: every document phase S counted (bitmap AND alive) whose date key can still enter the top-k
+                const uint32_t* al = T.alive ? reinterpret_cast<const uint32_t*>(T.alive) + (lo >> 5) : nullptr;
+                for (int w = threadIdx.x; w < nwords; w += BM_THREADS) {
+                    uint32_t v = bitmap[w];
+                    if (v && al) v &= al[w];
+                    while (v) {
+                        const uint32_t off = 32u * (uint32_t)w + (uint32_t)(__ffs(v) - 1);
+                        v &= v - 1;
+                        if (order_key(O, lo + off) > tk_thr) cand[atomicAdd(&s_ncand, 1)] = off;   // a tile holds <= BM_ACC documents
+                    }
+                }
+            }
             __syncthreads();
             // ---- phase D: candidates -> top-k buffer; warp 0 resolves the next tile meanwhile ----
             // The branch below must be uniform: it is taken on the buffer fill recorded at the end of the previous tile
@@ -569,7 +692,7 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
             }
             __syncthreads();
             // ---- reset: bitmap words, used accumulators (and counters) ----
-            if (tk_thr != 0) {   // threshold in fixed point, conservative (float(v) is within 2^-24 of v)
+            if (!ORDER && tk_thr != 0) {   // threshold in fixed point, conservative (float(v) is within 2^-24 of v)
                 float ts = key_score(tk_thr);
                 float lowb = __fmul_rn(__fmul_rn(ts, scale), 0.9999990f);
                 thr_fx = lowb >= 1.0f ? (uint32_t)lowb : 1u;
@@ -577,7 +700,7 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
             const uint4 z4 = make_uint4(0, 0, 0, 0);
             const int nd4 = (s_ndistinct + 3) >> 2;
             for (int i = threadIdx.x; i < (nwords + 3) >> 2; i += BM_THREADS) reinterpret_cast<uint4*>(bitmap)[i] = z4;
-            for (int i = threadIdx.x; i < nd4; i += BM_THREADS) reinterpret_cast<uint4*>(acc)[i] = z4;
+            if (!ORDER) for (int i = threadIdx.x; i < nd4; i += BM_THREADS) reinterpret_cast<uint4*>(acc)[i] = z4;
             if (CONJ) for (int i = threadIdx.x; i < (nd4 + 3) >> 2; i += BM_THREADS) reinterpret_cast<uint4*>(cnts)[i] = z4;
             if (threadIdx.x == 0) { s_ncand = 0; s_tk_snapshot = tk_count; }
             if (f1 < n_fine) fill_omap(buf ^ 1);   // the next tile's octet map (its prefix was completed before the last barrier)
@@ -603,13 +726,42 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
 
 template <bool CONJ, bool TF>
 __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_kernel(TxtDev T, Bm25Args a) {
-    bm25_body<CONJ, TF, false>(T, a, FacetArgs{});
+    bm25_body<CONJ, TF, false, false>(T, a, FacetArgs{}, OrderArgs{});
 }
 
 // bm25_kernel + the FacetCollector: same top-k and Count, plus F.out[q][bucket] (shared counters: smem = bm_smem_bytes + 4 n_buckets)
 template <bool CONJ, bool TF>
 __global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_facet_kernel(TxtDev T, Bm25Args a, FacetArgs f) {
-    bm25_body<CONJ, TF, true>(T, a, f);
+    bm25_body<CONJ, TF, true, false>(T, a, f, OrderArgs{});
+}
+
+// bm25_kernel ordered by date (TopDocs::order_by_fast_field): same matched set and Count, keys from OrderArgs (no scores, so no TF)
+template <bool CONJ>
+__global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_order_kernel(TxtDev T, Bm25Args a, OrderArgs o) {
+    bm25_body<CONJ, false, false, true>(T, a, FacetArgs{}, o);
+}
+
+// bm25_order_kernel + the FacetCollector in the same pass
+template <bool CONJ>
+__global__ void __launch_bounds__(BM_THREADS, BM_MINB_CFG) bm25_order_facet_kernel(TxtDev T, Bm25Args a, FacetArgs f, OrderArgs o) {
+    bm25_body<CONJ, false, true, true>(T, a, f, o);
+}
+
+// date keys -> (doc, seconds, count); no min_score under an order (convert_int_order, nidx_text/src/reader.rs:226-287).
+__global__ void date_finish_kernel(const uint64_t* keys, int nq, int k, const int64_t* secs, uint32_t* out_docs, int64_t* out_dates, int* out_counts) {
+    int q = blockIdx.x;
+    __shared__ int s_count;
+    if (threadIdx.x == 0) s_count = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < k; i += blockDim.x) {
+        uint64_t key = keys[(size_t)q * k + i];
+        uint32_t doc = key != 0 ? key_id(key) : NIL;
+        out_docs[(size_t)q * k + i] = doc;
+        out_dates[(size_t)q * k + i] = key != 0 ? secs[doc] : DATE_NONE;
+        if (key != 0) atomicAdd(&s_count, 1);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) out_counts[q] = s_count;
 }
 
 // keys -> (doc, score, count) with the min_score cut applied after top-k (reader.rs:302-305).

@@ -6,16 +6,18 @@ serialised by the reference's clients (``nidx_protos`` / ``nucliadb_protos``) de
 
     SearchRequest / SearchResponse                         nodereader.proto:388-437, 476-488
     Faceted, FacetResult, FacetResults                     nodereader.proto:20-22, 40-46
+    OrderBy                                                nodereader.proto:24-38
     DocumentSearchResponse / DocumentResult / ResultScore  nodereader.proto:48-81
     ParagraphSearchResponse / ParagraphResult              nodereader.proto:83-124
     VectorSearchResponse / DocumentScored                  nodereader.proto:126-142
     FilterExpression, FilterOperator, SearchAfter          nodereader.proto:287-336, 382-386
     IndexMessage, TypeMessage                              nodewriter.proto:26-43
     Resource, IndexParagraph(s), VectorSentence, ...       noderesources.proto:8-180
+    IndexMetadata                                          noderesources.proto:17-20 (google.protobuf.Timestamp)
 """
 from __future__ import annotations
 
-from google.protobuf import descriptor_pb2, descriptor_pool, message_factory
+from google.protobuf import descriptor_pb2, descriptor_pool, message_factory, timestamp_pb2
 
 _F = descriptor_pb2.FieldDescriptorProto
 _T = {"string": _F.TYPE_STRING, "bytes": _F.TYPE_BYTES, "int32": _F.TYPE_INT32, "int64": _F.TYPE_INT64, "uint32": _F.TYPE_UINT32, "uint64": _F.TYPE_UINT64,
@@ -53,13 +55,19 @@ def _map(msg, pkg_path, name, number, key_type, value_type):
 
 def _build():
     pool = descriptor_pool.DescriptorPool()
+    ts = descriptor_pb2.FileDescriptorProto()   # google/protobuf/timestamp.proto, as the protobuf runtime ships it
+    timestamp_pb2.DESCRIPTOR.CopyToProto(ts)
+    pool.Add(ts)
 
     # ---- noderesources.proto ---------------------------------------------------------------------------------------------
-    fd = descriptor_pb2.FileDescriptorProto(name="nidx_protos/noderesources.proto", package="noderesources", syntax="proto3")
+    fd = descriptor_pb2.FileDescriptorProto(name="nidx_protos/noderesources.proto", package="noderesources", syntax="proto3",
+                                            dependency=["google/protobuf/timestamp.proto"])
     m = fd.message_type.add(name="TextInformation")           # :8-11
     _field(m, "text", 1, "string"); _field(m, "labels", 2, "string", repeated=True)
     m = fd.message_type.add(name="ResourceID")                # :36-39
     _field(m, "shard_id", 1, "string"); _field(m, "uuid", 2, "string")
+    m = fd.message_type.add(name="IndexMetadata")             # :17-20
+    _field(m, "modified", 1, ".google.protobuf.Timestamp"); _field(m, "created", 2, ".google.protobuf.Timestamp")
     m = fd.message_type.add(name="Position")                  # :53-67
     _field(m, "index", 1, "uint64"); _field(m, "start", 2, "uint64"); _field(m, "end", 3, "uint64"); _field(m, "page_number", 4, "uint64")
     _field(m, "start_seconds", 5, "uint32", repeated=True); _field(m, "end_seconds", 6, "uint32", repeated=True); _field(m, "in_page", 7, "bool")
@@ -81,7 +89,7 @@ def _build():
     m = fd.message_type.add(name="IndexParagraphs")           # :118-121
     _map(m, ".noderesources.IndexParagraphs", "paragraphs", 1, "string", ".noderesources.IndexParagraph")
     m = fd.message_type.add(name="Resource")                  # :123-180
-    _field(m, "resource", 1, ".noderesources.ResourceID")
+    _field(m, "resource", 1, ".noderesources.ResourceID"); _field(m, "metadata", 2, ".noderesources.IndexMetadata")
     _map(m, ".noderesources.Resource", "texts", 3, "string", ".noderesources.TextInformation")
     _field(m, "labels", 4, "string", repeated=True)
     _map(m, ".noderesources.Resource", "paragraphs", 6, "string", ".noderesources.IndexParagraphs")
@@ -94,7 +102,7 @@ def _build():
 
     # ---- nodereader.proto ------------------------------------------------------------------------------------------------
     fd = descriptor_pb2.FileDescriptorProto(name="nidx_protos/nodereader.proto", package="nodereader", syntax="proto3",
-                                            dependency=["nidx_protos/noderesources.proto"])
+                                            dependency=["nidx_protos/noderesources.proto", "google/protobuf/timestamp.proto"])
     e = fd.enum_type.add(name="FilterOperator")               # :333-336
     e.value.add(name="AND", number=0); e.value.add(name="OR", number=1)
     m = fd.message_type.add(name="Faceted")                   # :20-22
@@ -103,12 +111,16 @@ def _build():
     _field(m, "tag", 1, "string"); _field(m, "total", 2, "int32")
     m = fd.message_type.add(name="FacetResults")              # :44-46
     _field(m, "facetresults", 1, ".nodereader.FacetResult", repeated=True)
+    m = fd.message_type.add(name="OrderBy")                   # :24-38
+    e = m.enum_type.add(name="OrderType"); e.value.add(name="DESC", number=0); e.value.add(name="ASC", number=1)
+    e = m.enum_type.add(name="OrderField"); e.value.add(name="CREATED", number=0); e.value.add(name="MODIFIED", number=1)
+    _field(m, "type", 2, "enum:.nodereader.OrderBy.OrderType"); _field(m, "sort_by", 3, "enum:.nodereader.OrderBy.OrderField")
     m = fd.message_type.add(name="ResultScore")               # :48-53
     _field(m, "bm25", 1, "float"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="DocumentResult")            # :55-64
     m.oneof_decl.add().name = "sort_value"
     _field(m, "uuid", 1, "string"); _field(m, "score", 3, ".nodereader.ResultScore", oneof=0); _field(m, "field", 4, "string")
-    _field(m, "labels", 5, "string", repeated=True); _field(m, "shard_id", 7, "bytes")
+    _field(m, "labels", 5, "string", repeated=True); _field(m, "shard_id", 7, "bytes"); _field(m, "date", 6, ".google.protobuf.Timestamp", oneof=0)
     m = fd.message_type.add(name="DocumentSearchResponse")    # :66-81
     _field(m, "total", 1, "int32"); _field(m, "results", 2, ".nodereader.DocumentResult", repeated=True); _field(m, "query", 6, "string")
     _field(m, "next_page", 7, "bool"); _map(m, ".nodereader.DocumentSearchResponse", "facets", 3, "string", ".nodereader.FacetResults")
@@ -118,6 +130,7 @@ def _build():
     _field(m, "paragraph", 6, "string"); _field(m, "split", 7, "string"); _field(m, "index", 8, "uint64")
     _field(m, "score", 9, ".nodereader.ResultScore", oneof=0); _field(m, "matches", 10, "string", repeated=True)
     _field(m, "metadata", 11, ".noderesources.ParagraphMetadata"); _field(m, "labels", 12, "string", repeated=True); _field(m, "shard_id", 14, "bytes")
+    _field(m, "date", 13, ".google.protobuf.Timestamp", oneof=0)
     m = fd.message_type.add(name="ParagraphSearchResponse")   # :106-124
     _field(m, "total", 1, "int32"); _field(m, "results", 2, ".nodereader.ParagraphResult", repeated=True); _field(m, "query", 6, "string")
     _field(m, "next_page", 7, "bool"); _field(m, "ematches", 9, "string", repeated=True)
@@ -146,7 +159,8 @@ def _build():
     m = fd.message_type.add(name="SearchAfter")               # :382-386
     _field(m, "score", 1, "float"); _field(m, "shard_id", 2, "bytes"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="SearchRequest")             # :388-437
-    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 3, "string"); _field(m, "faceted", 6, ".nodereader.Faceted")
+    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 3, "string"); _field(m, "order", 5, ".nodereader.OrderBy")
+    _field(m, "faceted", 6, ".nodereader.Faceted")
     _field(m, "result_per_page", 8, "int32")
     _field(m, "vector", 10, "float", repeated=True); _field(m, "paragraph", 12, "bool"); _field(m, "document", 13, "bool")
     _field(m, "with_duplicates", 14, "bool"); _field(m, "vectorset", 15, "string"); _field(m, "only_faceted", 16, "bool")
@@ -196,6 +210,8 @@ SearchRequest = _cls("nodereader.SearchRequest")
 SearchResponse = _cls("nodereader.SearchResponse")
 FilterExpression = _cls("nodereader.FilterExpression")
 Faceted = _cls("nodereader.Faceted")
+OrderBy = _cls("nodereader.OrderBy")
+IndexMetadata = _cls("noderesources.IndexMetadata")
 FacetResult = _cls("nodereader.FacetResult")
 FacetResults = _cls("nodereader.FacetResults")
 DocumentSearchResponse = _cls("nodereader.DocumentSearchResponse")

@@ -336,6 +336,57 @@ class TextSegment:
         check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), _lib.NIDX_MEM_HOST, ptr(out), None))
         return out
 
+    # ---- order by date (TopDocs::order_by_fast_field; seconds, NIDX_DATE_NONE = no date) ----------------------------------------
+    def set_dates(self, created, modified):
+        """Every document's created / modified seconds (int64 [n_docs], _lib.NIDX_DATE_NONE = none)."""
+        created = np.ascontiguousarray(created, dtype=np.int64)
+        modified = np.ascontiguousarray(modified, dtype=np.int64)
+        assert len(created) == self.n_docs and len(modified) == self.n_docs
+        check(_lib.load().nidx_txt_set_dates(self._h, ptr(created), ptr(modified)))
+
+    def search_ordered(self, query_terms, query_off, k, field=_lib.NIDX_ORDER_CREATED, order=_lib.NIDX_ORDER_DESC, mode=_lib.NIDX_BM25_OR, facets=None):
+        """search() ordered by date: (docs, dates, counts, total) plus the facet counts [nq][n_buckets] when `facets` (encoded keys)
+        is given.  numpy -> host path, torch CUDA -> device path (as search())."""
+        L = _lib.load()
+        p = TxtSearchParams(k, mode, 0, 0.0, 0, 0.0, 0, 0)
+        o = _lib.TxtOrder(field, order)
+        req, _keep = _facet_request(facets) if facets is not None else (None, None)
+        nb = len(self.facet_buckets(facets)[0]) if facets is not None else 0
+        if _is_torch(query_terms):
+            import torch
+
+            nq, dev = query_off.numel() - 1, query_terms.device
+            out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.int64, device=dev),
+                   torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev),
+                   torch.empty((nq, nb), dtype=torch.int32, device=dev))
+            stream, mem = _torch_stream(self.device), _lib.NIDX_MEM_DEVICE
+        else:
+            query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
+            query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
+            nq = len(query_off) - 1
+            out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.int64), np.empty(nq, dtype=np.int32), np.empty(nq, dtype=np.uint64),
+                   np.zeros((nq, nb), dtype=np.uint32))
+            stream, mem = None, _lib.NIDX_MEM_HOST
+        check(L.nidx_txt_search_ordered(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), mem, C.byref(p), C.byref(o),
+                                        C.byref(req) if req is not None else None, ptr(out[0]), ptr(out[1]), ptr(out[2]), ptr(out[3]),
+                                        ptr(out[4]) if facets is not None else None, stream))
+        return out if facets is not None else out[:4]
+
+    def list_ordered(self, k, field=_lib.NIDX_ORDER_CREATED, order=_lib.NIDX_ORDER_DESC, device_out=False):
+        """The empty body ordered by date: the top k alive documents -> (docs [k], dates [k], count, total alive)."""
+        o = _lib.TxtOrder(field, order)
+        if device_out:
+            import torch
+
+            dev = f"cuda:{self.device}"
+            out = (torch.empty(k, dtype=torch.int32, device=dev), torch.empty(k, dtype=torch.int64, device=dev), torch.empty(1, dtype=torch.int32, device=dev),
+                   torch.empty(1, dtype=torch.int64, device=dev))
+            check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), C.c_int32(k), _lib.NIDX_MEM_DEVICE, *[ptr(x) for x in out], _torch_stream(self.device)))
+            return out
+        docs, dates, count, total = np.empty(k, dtype=np.uint32), np.empty(k, dtype=np.int64), np.zeros(1, dtype=np.int32), np.zeros(1, dtype=np.uint64)
+        check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), C.c_int32(k), _lib.NIDX_MEM_HOST, ptr(docs), ptr(dates), ptr(count), ptr(total), None))
+        return docs, dates, int(count[0]), int(total[0])
+
     def set_doc_keys(self, keys: Optional[np.ndarray]):
         """Caller keys of the documents (paragraph ids) for rank fusion; None = the document number."""
         k = None if keys is None else np.ascontiguousarray(keys, dtype=np.uint64)

@@ -20,6 +20,13 @@ the BM25 pass (``bm25_facet_kernel``), and over every alive document for an empt
 keeps ONE facet dictionary across its segments (like the term vocabulary), so per-segment bucket counts add up as arrays before the
 top-50 cut of ``FacetCounts::top_k`` (nidx_text/src/reader.rs:43-62).  Each group lists its children by count descending, ties in
 facet order (path segments compared bytewise); a group without a counted child is omitted.
+
+Order by date (``SearchRequest.order``: ``TopDocs::order_by_fast_field("created" | "modified")`` in place of ``order_by_score``,
+nidx_text/src/reader.rs:208-287, nidx_paragraph/src/reader.rs:229-243) is on the hot path too: every matched document is offered to
+the top-k with its date (``bm25_order_kernel``), and an empty body lists every alive document (``date_topk_all_kernel``).  Dates are
+seconds, results carry ``date`` instead of ``score``, ``min_score`` and search-after do not apply, and ``next_page = total > k``.
+Segments are merged by (date in the requested direction, undated documents last, segment ord, doc): the tie order and the place of
+undated documents are fixed here, not taken from the reference.
 """
 from __future__ import annotations
 
@@ -64,8 +71,15 @@ class ResultScore:  # nodereader.proto:48-53
 class DocumentResult:
     uuid: str
     field: str
-    score: ResultScore
+    score: Optional[ResultScore]
     labels: list
+    date: Optional[int] = None   # seconds: the sort value under an order (nodereader.proto DocumentResult.date), None without a date
+
+
+@dataclass
+class OrderBy:  # nodereader.proto OrderBy
+    sort_by: int = _lib.NIDX_ORDER_CREATED   # OrderField: CREATED 0, MODIFIED 1
+    type: int = _lib.NIDX_ORDER_DESC          # OrderType: DESC 0, ASC 1
 
 
 @dataclass
@@ -76,6 +90,7 @@ class DocumentSearchRequest:  # nidx_text/src/request_types.rs:17-28
     only_faceted: bool = False
     faceted: Sequence[str] = ()               # Faceted.labels: the facets to count children of (SearchRequest.faceted)
     search_after: Optional[SearchAfter] = None  # ParagraphSearchRequest.search_after (nidx_paragraph only)
+    order: Optional[OrderBy] = None            # SearchRequest.order: results by date instead of score
 
 
 @dataclass
@@ -130,6 +145,8 @@ class TextDoc:
     field: str
     text: str
     labels: Sequence[str] = ()
+    created: Optional[int] = None    # IndexMetadata.created / .modified, seconds
+    modified: Optional[int] = None
 
 
 class TextIndexSegment:
@@ -182,6 +199,7 @@ class TextSearcher:
         for s in self.segments:  # union statistics on every segment (index_reader.rs:39-77)
             s.upload(n_terms).set_stats(max(total_docs, 1), max(total_tokens, 1), df)
         self.facet_keys: Optional[list] = None   # built on the first faceted request
+        self._dates = False                        # uploaded on the first ordered request
 
     def _ensure_facets(self):
         """The index's facet dictionary (every valid label of every document, in facet order) and each segment's per-document
@@ -197,10 +215,20 @@ class TextSearcher:
             s._gpu.set_facets(keys, off, np.asarray([o for r in rows for o in r], dtype=np.uint32))
         self.facet_keys = keys
 
-    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict):
+    def _ensure_dates(self):
+        """Every segment's created / modified seconds, uploaded once."""
+        if self._dates:
+            return
+        none = _lib.NIDX_DATE_NONE
+        for s in self.segments:
+            s._gpu.set_dates(np.asarray([none if d.created is None else int(d.created) for d in s.docs], dtype=np.int64),
+                             np.asarray([none if d.modified is None else int(d.modified) for d in s.docs], dtype=np.int64))
+        self._dates = True
+
+    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None):
         """Counts of the request's facets over the matched set of every segment, summed, then grouped and cut to the top 50.
-        With terms: the faceted BM25 search (returns its per-segment (docs, scores, counts, total) too); without: every alive
-        document (AllQuery)."""
+        With terms: the faceted BM25 search, ordered by date when `order` is given (returns its per-segment (docs, scores or
+        dates, counts, total) too); without: every alive document (AllQuery)."""
         from ._lib import NidxError
 
         request = _facet_request(faceted)
@@ -217,7 +245,10 @@ class TextSearcher:
         for ord_, seg in enumerate(self.segments):
             if terms:
                 qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
-                docs, scores, cnt, total, fc = seg._gpu.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
+                if order is not None:
+                    docs, scores, cnt, total, fc = seg._gpu.search_ordered(qt, qo, k, order.sort_by, order.type, params["mode"], facets=keys)
+                else:
+                    docs, scores, cnt, total, fc = seg._gpu.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
                 hits.append((docs, scores, cnt, total))
                 counts += fc[0]
             else:
@@ -254,6 +285,8 @@ class TextSearcher:
             sa = request.search_after
             after = (sa.score, {"drop": 1, "keep_after": 2, "keep": 3}[sa.tie_break], sa.docaddr)
         params = dict(mode=_lib.NIDX_BM25_AND if self.conjunction else _lib.NIDX_BM25_OR, use_tf=self.use_tf, min_score=0.0, after=after)
+        if request.order is not None and not request.only_faceted:   # only_faceted comes first (nidx_text/src/reader.rs:405-414)
+            return self._search_ordered(request, terms, params)
         hits = None
         if _facet_request(request.faceted):
             resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params)
@@ -280,6 +313,42 @@ class TextSearcher:
             d = self.segments[ord_].docs[doc]
             resp.results.append(DocumentResult(d.uuid, d.field, ResultScore(score, (ord_ << 32) + doc), list(d.labels)))
         return resp
+
+
+    def _search_ordered(self, request: DocumentSearchRequest, terms, params: dict) -> DocumentSearchResponse:
+        """TopDocs(k + 1) ordered by date beside Count (and the FacetCollector) in one pass per segment; an empty body lists every
+        alive document.  convert_int_order (nidx_text/src/reader.rs:226-287): no min_score, next_page = total > k."""
+        order, k = request.order, request.result_per_page
+        resp = DocumentSearchResponse(query=request.body)
+        self._ensure_dates()
+        hits = None
+        if _facet_request(request.faceted):
+            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, order=order)
+        if k <= 0:
+            return resp
+        qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
+        rows = []
+        for ord_, seg in enumerate(self.segments):
+            if not terms:
+                docs, dates, count, total = seg._gpu.list_ordered(k + 1, order.sort_by, order.type)
+            else:
+                d2, t2, c2, tot2 = hits[ord_] if hits is not None else seg._gpu.search_ordered(qt, qo, k + 1, order.sort_by, order.type, params["mode"])
+                docs, dates, count, total = d2[0], t2[0], int(c2[0]), int(tot2[0])
+            resp.total += int(total)
+            rows += [(date_sort_key(int(dates[i]), order.type), ord_, int(docs[i]), int(dates[i])) for i in range(count)]
+        rows.sort()   # date in the requested direction (undated last), then segment ord, then doc
+        resp.next_page = resp.total > k
+        for _, ord_, doc, date in rows[:k]:
+            d = self.segments[ord_].docs[doc]
+            resp.results.append(DocumentResult(d.uuid, d.field, None, list(d.labels), None if date == _lib.NIDX_DATE_NONE else date))
+        return resp
+
+
+def date_sort_key(seconds: Optional[int], order_type: int):
+    """Sort key of a date under an order: the requested direction first, documents without a date (None or NIDX_DATE_NONE) last."""
+    if seconds is None or seconds == _lib.NIDX_DATE_NONE:
+        return (1, 0)
+    return (0, seconds if order_type == _lib.NIDX_ORDER_ASC else -seconds)
 
 
 class ParagraphSearcher(TextSearcher):
