@@ -1856,7 +1856,6 @@ struct nidx_txt_segment {
     uint64_t* d_doc_keys = nullptr;   // [n_docs] caller keys of the documents (paragraph ids) for rank fusion (nidx_txt_set_doc_keys)
     std::vector<uint64_t> own_df;
     uint64_t own_tokens = 0;
-    float max_weight = 0.0f;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around bm25_kernel of the last search (bench roofline)
     // facets (nidx_txt_set_facets): the dictionary on the host in facet order, every document's ords (CSR) in HBM
     std::vector<std::string> facet_keys;
@@ -1883,13 +1882,10 @@ static int txt_upload_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t t
     float cache[256];
     for (int i = 0; i < 256; ++i) cache[i] = K1 * (1.0f - B + B * (float)fieldnorm_id_to_value(i) / avg);
     std::vector<float> weight(t->n_terms);
-    float wmax = 0.0f;
     for (uint32_t i = 0; i < t->n_terms; ++i) {
         float x = ((float)(total_docs - df[i]) + 0.5f) / ((float)df[i] + 0.5f);
         weight[i] = logf(1.0f + x) * (1.0f + K1);
-        wmax = std::max(wmax, weight[i]);
     }
-    t->max_weight = wmax;
     CU(cudaMemcpy(t->d_norm_cache, cache, sizeof(cache), cudaMemcpyHostToDevice));
     if (t->n_terms) CU(cudaMemcpy(t->d_weight, weight.data(), (size_t)t->n_terms * 4, cudaMemcpyHostToDevice));
     return 0;
@@ -2199,11 +2195,6 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
         if (n_qt) CU(cudaMemcpyAsync(base + nq + 1, query_terms, (size_t)n_qt * 4, cudaMemcpyHostToDevice, stream));
         d_qo = base; d_qt = base + nq + 1;
     }
-    // fixed-point scale: the largest possible sum is max_terms * max term weight (tf factor < 1)
-    float bound = std::max(1.0f, t->max_weight * (float)std::max(max_terms, 1));
-    int shift = 24;
-    while (shift > 4 && bound * (float)(1u << shift) >= 4.0e9f) --shift;
-
     bool conj = p->mode == NIDX_BM25_AND;
     int cap = topk_cap(k, BM_THREADS);
     size_t smem = bm_smem_bytes(cap, conj);
@@ -2225,7 +2216,7 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
     Bm25Args a;
     a.query_terms = d_qt; a.query_off = d_qo; a.nq = nq; a.k = k; a.cap = cap;
-    a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache; a.shift = shift;
+    a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
     a.out_keys = w.partial.as<uint64_t>(); a.out_total = d_total; a.error_flag = t->d_error;
     if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after

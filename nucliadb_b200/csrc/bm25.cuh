@@ -22,8 +22,11 @@
 //      (ANDed with the alive bits);
 //   C  the same postings, from registers: score, atomicAdd into acc[rank].  Contributions are fixed point (2^-shift):
 //      the sum does not depend on the order, equal scores stay bit-equal and TopDocs' (score desc, doc asc) tie order is
-//      deterministic.  The thread whose add carries a document's sum across the current top-k threshold (OR) or completes
-//      the conjunction (AND) records it as a candidate: only documents that can still enter the top-k are looked at again;
+//      deterministic.  The shift is the query's own (largest s <= 24 with max(1, nt * max_t w_t) * 2^s < 4e9, so no sum can
+//      leave uint32): a query scores the same in any batch and on every segment that shares the index's statistics.
+//      tests/bm25_model.py restates the arithmetic bit for bit and bounds its error against float64.  The thread whose add
+//      carries a document's sum across the current top-k threshold (OR) or completes the conjunction (AND) records it as a
+//      candidate: only documents that can still enter the top-k are looked at again;
 //   D  candidates -> streaming top-k buffer (final sums, exact threshold test) while warp 0 resolves the next tile's
 //      slices (skip entries prefetched one tile ahead); then the bitmap, the used accumulators and the counters are cleared.
 // A tile that holds more postings than slots is redone with half the span; a single fine tile that still does not fit runs in
@@ -75,7 +78,6 @@ struct Bm25Args {
     int k, cap;                 // cap: top-k buffer entries (power of two >= 2k, >= k + BM_THREADS)
     const float* term_weight;   // [n_terms] idf * (1 + k1) from the collection statistics
     const float* norm_cache;    // [256] k1 * (1 - b + b * fieldnorm(id) / avg)
-    int shift;                  // fixed point: 2^-shift
     int after_mode;             // search-after (nidx_paragraph reader.rs:379-392): 0 none, 1 Drop, 2 KeepAfter, 3 Keep
     float after_score;
     uint64_t after_docaddr, docaddr_base;
@@ -303,7 +305,7 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int tk_count;
     __shared__ uint64_t tk_thr;
-    __shared__ int s_ncand, s_tk_snapshot, s_noct[2], s_ptile[2], s_minlen[2], s_ndistinct;
+    __shared__ int s_ncand, s_tk_snapshot, s_noct[2], s_ptile[2], s_minlen[2], s_ndistinct, s_shift;
     __shared__ uint32_t s_wsum[BM_WARPS];
     __shared__ unsigned long long s_hits;
     unsigned char* p = smem;
@@ -348,6 +350,7 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
     uint32_t t_pf[BM_TPL];
     bool missing = false;
     unsigned long long my_total = 0;
+    float wmax = 0.0f;   // the query's largest term weight (unknown terms weigh 0): it sets the query's fixed-point scale
 #pragma unroll
     for (int j = 0; j < BM_TPL; ++j) t_pf[j] = 0;
     if (warp == 0) {
@@ -359,7 +362,9 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
                 bool ok = t < T.n_terms;
                 uint64_t b = ok ? T.term_off[t] : 0, e = ok ? T.term_off[t + 1] : 0;
                 t_base[i] = b; t_end[i] = e; t_cur[i] = b;
-                tw[i] = ok ? a.term_weight[t] : 0.0f;   // scaled by 2^shift below (exact: a power of two), so a posting costs one multiply
+                const float w = ok ? a.term_weight[t] : 0.0f;
+                tw[i] = w;   // scaled by 2^shift below (exact: a power of two), so a posting costs one multiply
+                if (!ORDER) wmax = fmaxf(wmax, w);
                 uint32_t row = ok ? T.skip_row[t] : NIL;
                 t_skip[i] = row != NIL ? (uint64_t)row * (T.n_fine + 1) : ~0ull;
                 missing |= b == e;
@@ -367,11 +372,20 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
             }
         }
         for (int off = 16; off >= 1; off >>= 1) my_total += __shfl_xor_sync(0xFFFFFFFFu, my_total, off);
+        if (!ORDER) for (int off = 16; off >= 1; off >>= 1) wmax = fmaxf(wmax, __shfl_xor_sync(0xFFFFFFFFu, wmax, off));
     }
-    if (threadIdx.x == 0) { s_hits = 0; s_ncand = 0; s_tk_snapshot = 0; s_ptile[0] = (int)min(my_total, (unsigned long long)INT_MAX); }
+    if (threadIdx.x == 0) {
+        s_hits = 0; s_ncand = 0; s_tk_snapshot = 0; s_ptile[0] = (int)min(my_total, (unsigned long long)INT_MAX);
+        if (!ORDER) {   // fixed-point scale: a sum is at most nt * wmax * 2^s + nt / 2 (frac <= 1), kept below 4e9 < 2^32
+            const float bound = fmaxf(1.0f, __fmul_rn((float)nt, wmax));
+            int s = 24;
+            while (s > 4 && __fmul_rn(bound, (float)(1u << s)) >= 4.0e9f) --s;
+            s_shift = s;
+        }
+    }
     int any_missing = __syncthreads_or(missing);   // an AND query with a term without postings matches nothing
     const bool dead = (CONJ && any_missing) || nt == 0;
-    const float scale = (float)(1u << a.shift);
+    const float scale = ORDER ? 1.0f : (float)(1u << s_shift);
     if (threadIdx.x < nt) tw[threadIdx.x] = __fmul_rn(tw[threadIdx.x], scale);   // rn(rn(w * frac) * 2^s) == rn((w * 2^s) * frac)
     const uint32_t n_fine = dead ? 0 : T.n_fine;
     // tile span (fine tiles): the query's postings spread evenly would fill ~80 % of the slots per tile (octet padding takes some)

@@ -9,22 +9,26 @@ import oracle as O
 from conftest import make_queries, make_vectors
 
 
-def naive_bm25(docs, n_terms, query, mode, use_tf, k1=1.2, b=0.75):
-    """tantivy's Bm25Weight from its published formula, float64, document at a time.  docs: list of token-id lists."""
+def naive_bm25(docs, n_terms, query, mode, use_tf, k1=1.2, b=0.75, weights=None, norm=None):
+    """tantivy's Bm25Weight from its published formula, float64, document at a time.  docs: list of token-id lists.
+    weights[term] and norm[fieldnorm id], when given, replace idf * (1 + k1) and k1 * (1 - b + b * dl / avg): fed the f32 values a
+    scorer starts from (taken as exact), the float64 sum measures only that scorer's arithmetic after them."""
     n = len(docs)
     avg = sum(len(d) for d in docs) / n
-    df = [sum(1 for d in docs if t in d) for t in range(n_terms)]
+    df = [sum(1 for d in docs if t in d) for t in range(n_terms)] if weights is None else None
     out = []
     for i, d in enumerate(docs):
-        dl = O.fieldnorm_id_to_value(O.fieldnorm_to_id(len(d)))          # the 1-byte quantised length is what tantivy scores with
+        fid = O.fieldnorm_to_id(len(d))
+        dl = O.fieldnorm_id_to_value(fid)                                # the 1-byte quantised length is what tantivy scores with
         hits = [t for t in query if t < n_terms and t in d]
         if not hits or (mode == O.BM25_AND and len(hits) < len(query)):
             continue
         s = 0.0
         for t in hits:
             tf = d.count(t) if use_tf else 1
-            idf = math.log(1.0 + (n - df[t] + 0.5) / (df[t] + 0.5))
-            s += idf * (1.0 + k1) * tf / (tf + k1 * (1.0 - b + b * dl / avg))
+            w = math.log(1.0 + (n - df[t] + 0.5) / (df[t] + 0.5)) * (1.0 + k1) if weights is None else float(weights[t])
+            nrm = k1 * (1.0 - b + b * dl / avg) if norm is None else float(norm[fid])
+            s += w * tf / (tf + nrm)
         out.append((s, i))
     out.sort(key=lambda x: (-x[0], x[1]))
     return out
