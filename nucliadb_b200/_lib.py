@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# NIDX_B200_LIB names another build of the same library next to this file (kernel-shape experiments: scripts/exp_*.py)
+# NIDX_B200_LIB names another build of the same library next to this file (A/B runs of two builds)
 LIB_PATH = os.path.join(_HERE, os.path.basename(os.environ.get("NIDX_B200_LIB", "libnidx_b200.so")))
 
 NIDX_MEM_HOST, NIDX_MEM_DEVICE = 0, 1

@@ -23,7 +23,6 @@
 #include "rabitq.cuh"
 #include "rank_fusion.cuh"
 #include "scan.cu"
-#include "scan_tc.cuh"
 #include "scan_tc2.cuh"
 #include "segment_io.hpp"
 #include "shard.cuh"
@@ -783,20 +782,6 @@ static hs_kernel_t pick_search_kernel(int ld) {
     return hnsw_search_kernel<0>;
 }
 
-// the 4-warp shape (two rows per warp in flight, 7 CTAs per SM): see hnsw_search_kernel
-static hs_kernel_t pick_search_kernel_w4(int ld) {
-    if (ld % 128 == 0) switch (ld / 128) {
-        case 1: return hnsw_search_kernel<1, 4, true>;
-        case 2: return hnsw_search_kernel<2, 4, true>;
-        case 3: return hnsw_search_kernel<3, 4, true>;
-        case 4: return hnsw_search_kernel<4, 4, true>;
-        case 6: return hnsw_search_kernel<6, 4, true>;
-        case 8: return hnsw_search_kernel<8, 4, true>;
-        default: break;
-    }
-    return nullptr;
-}
-
 static hs_kernel_t pick_rabitq_walk_kernel_w4(int ld) {
     if (ld % 128 == 0) switch (ld / 128) {
         case 2: return hnsw_rabitq_kernel<2, 4>;
@@ -835,7 +820,9 @@ static scan_kernel_t pick_scan_kernel(int ld) {
     return scan_scores_kernel;
 }
 
-static int hnsw_search_smem(const nidx_vec_segment* s, int ef0, int k, int* list_cap, int* cu_cap, int* hash_bits, size_t* bytes) {
+// Shared-memory plans of the two walks, used by AUTO's choice and by the launch alike.  Each returns false when the plan does not
+// fit one CTA (the list and the visited set grow with ef and k).
+static bool hnsw_search_smem(const nidx_vec_segment* s, int ef0, int k, int* list_cap, int* cu_cap, int* hash_bits, size_t* bytes) {
     // closest_up_nodes pops at most k-1 candidates before it has k results when nothing is filtered
     // (search.rs:205-216), each adding at most one adjacency row of pending candidates.
     int cu = std::min(std::max(ef0 + k * s->s0, 2 * ef0), 4096);
@@ -846,8 +833,16 @@ static int hnsw_search_smem(const nidx_vec_segment* s, int ef0, int k, int* list
     slots = std::max(slots, next_pow2(4 * lc));
     *list_cap = lc; *cu_cap = cu; *hash_bits = ilog2(slots);
     *bytes = hs_smem_bytes(s->ld, lc, *hash_bits);
-    if (*bytes > 200 * 1024) return fail(NIDX_EINVAL, "HNSW search needs %zu bytes of shared memory (ef=%d, k=%d, dim=%d): too large", *bytes, ef0, k, s->d);
-    return 0;
+    return *bytes <= 200 * 1024;
+}
+
+static bool rq_walk_smem(const nidx_vec_segment* s, int k, int* last_k, int* cu_cap, int* list_cap, int* hash_bits, size_t* bytes) {
+    *last_k = (int)std::min<size_t>((size_t)k * 100, 2000);              // rabitq.rs:34-36 RERANKING_FACTOR / RERANKING_LIMIT
+    *cu_cap = std::min(std::max(k + k * s->s0, 2 * k), 4096);
+    *list_cap = std::max(*last_k, *cu_cap);
+    *hash_bits = ilog2(next_pow2(std::max(2048, 4 * *cu_cap)));
+    *bytes = rq_smem_bytes(s->ld, s->d, *list_cap, *hash_bits, k);
+    return *bytes <= 200 * 1024;
 }
 
 }  // extern "C"
@@ -1100,19 +1095,11 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
             // A walk keeps its list and visited set in shared memory: a very large top_k (the reference has no limit on it) does not
             // fit one CTA.  AUTO then takes the exhaustive scan -- exact results -- instead of failing the request.
             if (method == NIDX_METHOD_HNSW || method == NIDX_METHOD_HNSW_RABITQ) {
-                bool fits;
-                if (method == NIDX_METHOD_HNSW) {
-                    int ef = p->ef > 0 ? p->ef : s->cfg.ef_search;
-                    int cu = std::min(std::max(std::max(k, ef) + k * s->s0, 2 * std::max(k, ef)), 4096);
-                    int lcap = std::max(std::max(k, ef), cu);
-                    int slots = next_pow2(std::max(4096, (std::max(k, ef) * s->s0 * 3) / 2));
-                    slots = std::max(slots, next_pow2(4 * lcap));
-                    fits = hs_smem_bytes(s->ld, lcap, ilog2(slots)) <= 200 * 1024;
-                } else {
-                    int last_k = (int)std::min<size_t>((size_t)k * 100, 2000);
-                    int cu_cap = std::min(std::max(k + k * s->s0, 2 * k), 4096);
-                    fits = rq_smem_bytes(s->ld, s->d, std::max(last_k, cu_cap), ilog2(next_pow2(std::max(2048, 4 * cu_cap))), k) <= 200 * 1024;
-                }
+                int last_k, list_cap, cu_cap, hash_bits;
+                size_t bytes;
+                bool fits = method == NIDX_METHOD_HNSW
+                                ? hnsw_search_smem(s, std::max(k, p->ef > 0 ? p->ef : s->cfg.ef_search), k, &list_cap, &cu_cap, &hash_bits, &bytes)
+                                : rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &bytes);
                 if (!fits && k <= 1024) method = NIDX_METHOD_BRUTE;
             }
         }
@@ -1215,11 +1202,6 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         ENSURE(w.partial, (size_t)qgroup * n_chunks * k * 8);
         size_t smem_scan = (size_t)SCAN_QT * s->ld * 4;
         scan_kernel_t scan_kern = pick_scan_kernel(s->ld);
-        // Batches of >= 128 queries go to the tensor cores (scores within ~3e-7 of the lane-blocked order);
-        // NIDX_B200_SCAN=exact forces the bit-exact CUDA-core kernel, =tensor forces the tensor path.
-        const char* scan_env = getenv("NIDX_B200_SCAN");
-        bool tensor_scan = s->ld % TC_KB == 0 && scan_env && !strcmp(scan_env, "tensor3x");   // round 1's 3xTF32 score-matrix kernel: on request only
-        if (tensor_scan) CU(cudaFuncSetAttribute(scan_scores_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_BYTES));
         if (smem_scan > 48 * 1024) CU(cudaFuncSetAttribute(scan_kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_scan));
         if ((size_t)cap * 8 > 48 * 1024) {
             CU(cudaFuncSetAttribute(scan_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
@@ -1232,14 +1214,8 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
             uint64_t grid = n_vchunks * n_qtiles;
             if (grid > 0x7FFFFFFFull) return fail(NIDX_EINVAL, "scan grid too large");
             if (q0 == 0) CU(cudaEventRecord(s->ev_k0, stream));
-            if (tensor_scan) {
-                // large batch: the score matrix is a dense GEMM -> wgmma (3xTF32, f32 accumulate in registers)
-                dim3 tgrid((unsigned)((s->n + TC_N - 1) / TC_N), (unsigned)((nqg + TC_M - 1) / TC_M));
-                scan_scores_tc_kernel<<<tgrid, TC_THREADS, TC_SMEM_BYTES, stream>>>(V, dq + (size_t)q0 * s->ld, w.qnorms.as<float>() + q0, nqg, w.scores.as<float>());
-            } else {
-                scan_kern<<<(unsigned)grid, SCAN_WARPS * 32, smem_scan, stream>>>(V, dq + (size_t)q0 * s->ld, w.qnorms.as<float>() + q0, nqg, n_qtiles,
-                                                                                     w.scores.as<float>());
-            }
+            scan_kern<<<(unsigned)grid, SCAN_WARPS * 32, smem_scan, stream>>>(V, dq + (size_t)q0 * s->ld, w.qnorms.as<float>() + q0, nqg, n_qtiles,
+                                                                                 w.scores.as<float>());
             if (q0 == 0) CU(cudaEventRecord(s->ev_k1, stream));
             LAUNCHED();
             scan_select_kernel<<<dim3(n_chunks, nqg), 256, (size_t)cap * 8, stream>>>(w.scores.as<float>(), (uint32_t)s->n, s->n_par, s->d_par_first, nullptr, bits,
@@ -1262,16 +1238,12 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         RabitqQueryParams* params = reinterpret_cast<RabitqQueryParams*>(w.misc.as<unsigned char>() + ((plane_bytes + 15) / 16) * 16);
         rabitq_query_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(dq, s->ld, s->d, nq, planes, params);
         LAUNCHED();
-        int last_k = (int)std::min<size_t>((size_t)k * 100, 2000);              // rabitq.rs:34-36 RERANKING_FACTOR / RERANKING_LIMIT
-        int cu_cap = std::min(std::max(k + k * s->s0, 2 * k), 4096);
-        int list_cap = std::max(last_k, cu_cap);
-        int slots = next_pow2(std::max(2048, 4 * cu_cap));
-        int hash_bits = ilog2(slots);
+        int last_k, cu_cap, list_cap, hash_bits;
+        size_t smem;
+        if (!rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &smem))
+            return fail(NIDX_EINVAL, "quantised HNSW search needs %zu bytes of shared memory (k=%d, dim=%d): too large", smem, k, s->d);
         int gv_bits = 16;                                                       // 64 k slots: layer 0 visits ~10-20 k nodes at k = 10
         while ((1 << gv_bits) < 24 * last_k) ++gv_bits;
-        if (const char* e = getenv("NIDX_B200_RQ_VISITED_BITS")) { int b = atoi(e); if (b >= 12 && b <= 22) gv_bits = b; }
-        size_t smem = rq_smem_bytes(s->ld, s->d, list_cap, hash_bits, k);
-        if (smem > 200 * 1024) return fail(NIDX_EINVAL, "quantised HNSW search needs %zu bytes of shared memory (k=%d, dim=%d): too large", smem, k, s->d);
         // CTA shape: the walk is bound by the ~1 000 dependent hops of a query, so what counts is how many queries are resident.
         // 8 warps per query: 4 CTAs per SM; 4 warps: 7 per SM.  The 4-warp shape is taken when the batch does not fit one wave of the
         // 8-warp shape (NIDX_B200_RQ_W = 4 / 8 forces one).
@@ -1300,7 +1272,6 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = cu_cap;
         a.codes = s->d_quant; a.code_stride = s->quant_stride; a.planes = planes; a.qparams = params;
         a.gvisited = w.scores.as<uint32_t>(); a.gv_bits = gv_bits; a.last_k = last_k;
-        { const char* ep = getenv("NIDX_B200_RQ_PREFETCH"); a.rq_prefetch = ep ? atoi(ep) : 1; }
         ENSURE(w.sched, 128);
         a.work_counter = w.sched.as<unsigned int>();
         a.counters = reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64);   // per call, in the call's workspace
@@ -1316,9 +1287,9 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         int ef0 = std::max(k, ef);  // search.rs:338-345
         int list_cap, cu_cap, hash_bits;
         size_t smem;
-        int r = hnsw_search_smem(s, ef0, k, &list_cap, &cu_cap, &hash_bits, &smem);
-        if (r) return r;
-        r = attach_half_copy(s, &V);
+        if (!hnsw_search_smem(s, ef0, k, &list_cap, &cu_cap, &hash_bits, &smem))
+            return fail(NIDX_EINVAL, "HNSW search needs %zu bytes of shared memory (ef=%d, k=%d, dim=%d): too large", smem, ef0, k, s->d);
+        int r = attach_half_copy(s, &V);
         if (r) return r;
         SearchArgs a;
         memset(&a, 0, sizeof(a));
@@ -1333,26 +1304,12 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         CU(cudaMemsetAsync(a.work_counter, 0, 128, stream));
         s->last_counters.store(a.counters);
         hs_kernel_t kern = pick_search_kernel(s->ld);
-        int threads = HS_THREADS;
-        // Shape: 8 warps per query, 4 CTAs per SM -- or 4 warps with two rows in flight each, 7 CTAs per SM, when that lets the
-        // whole batch run as one wave (NIDX_B200_HS_W=4 / 8 forces a shape; the experiment's visited table is hs_w4_bits slots).
-        {
-            const char* e1 = getenv("NIDX_B200_HS_W");
-            const char* e2 = getenv("NIDX_B200_HS_W4_BITS");
-            const int force_w = e1 ? atoi(e1) : 0, w4_bits = e2 ? atoi(e2) : 0;
-            hs_kernel_t k4 = pick_search_kernel_w4(s->ld);
-            if (k4 && force_w == 4) {
-                int hb = w4_bits > 0 ? w4_bits : hash_bits;
-                size_t smem4 = hs_smem_bytes(s->ld, list_cap, hb);
-                kern = k4; threads = 128; smem = smem4; a.hash_bits = hb;
-            }
-        }
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int occ = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, HS_THREADS, smem));
         int grid = std::min(nq, std::max(1, occ) * s->sm_count);
         CU(cudaEventRecord(s->ev_k0, stream));
-        kern<<<grid, threads, smem, stream>>>(V, s->gdev(), a);
+        kern<<<grid, HS_THREADS, smem, stream>>>(V, s->gdev(), a);
         CU(cudaEventRecord(s->ev_k1, stream));
         LAUNCHED();
         CU(cudaGetLastError());
@@ -1547,14 +1504,7 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
         int cache_sel = (int)std::min<size_t>(M, budget / row_bytes);
         int prune_max = std::max(s->cfg.m0, M) * 95 / 100;
         int cache_rev = (int)std::min<size_t>(prune_max, budget / row_bytes);
-        // prune of a full list: stage all mmax + 1 vectors and the pairwise table when they fit (<= ~200 KB)
-        int full_rows = std::max(s->cfg.m0, M) + 1;
-        // NIDX_B200_PRUNE=table switches the prune to the staged pairwise-table variant (same result as the
-        // candidate-at-a-time loop)
-        const char* prune_env = getenv("NIDX_B200_PRUNE");
-        bool preload = hb_smem_bytes(s->ld, full_rows, true) <= 200 * 1024 && prune_env && !strcmp(prune_env, "table");
-        if (preload) cache_rev = full_rows;
-        size_t smem_sel = hb_smem_bytes(s->ld, cache_sel), smem_rev = hb_smem_bytes(s->ld, cache_rev, preload);
+        size_t smem_sel = hb_smem_bytes(s->ld, cache_sel), smem_rev = hb_smem_bytes(s->ld, cache_rev);
         CU(cudaFuncSetAttribute(select_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sel));
         CU(cudaFuncSetAttribute(reverse_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rev));
         int occ_rev = 0;
@@ -1592,7 +1542,7 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
             CU(cub::DeviceRadixSort::SortPairs(d_cub, tmp, d_rev_key, d_key_sorted, d_idx, d_idx_sorted, n_rev, 0, 40, stream));
             LAUNCHED();
             ReverseArgs ra;
-            ra.n_rev = n_rev; ra.key_sorted = d_key_sorted; ra.idx_sorted = d_idx_sorted; ra.rev_x = d_rev_x; ra.rev_sim = d_rev_sim; ra.cache_cap = cache_rev; ra.preload = preload ? 1 : 0;
+            ra.n_rev = n_rev; ra.key_sorted = d_key_sorted; ra.idx_sorted = d_idx_sorted; ra.rev_x = d_rev_x; ra.rev_sim = d_rev_sim; ra.cache_cap = cache_rev;
             ra.heads = d_heads; ra.n_heads = d_head_ctr; ra.work_counter = d_head_ctr + 1;
             CU(cudaMemsetAsync(d_head_ctr, 0, 8, stream));
             collect_heads_kernel<<<(n_rev + 255) / 256, 256, 0, stream>>>(d_key_sorted, n_rev, d_heads, d_head_ctr);

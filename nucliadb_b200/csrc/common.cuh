@@ -128,42 +128,6 @@ __device__ __forceinline__ float warp_dot_t(const float4* __restrict__ a, const 
     }
 }
 
-// Two rows in flight: both rows' loads are issued before either is consumed (twice the bytes in flight per warp).  Each row's
-// arithmetic is exactly warp_dot_t's, so the results are bit-identical to two separate calls.
-template <int NG>
-__device__ __forceinline__ void warp_dot2_t(const float4* __restrict__ a0, const float4* __restrict__ a1, const float4* __restrict__ b, int ngroups, int lane,
-                                            float& r0, float& r1) {
-    if constexpr (NG == 0) {
-        r0 = warp_dot(a0, b, ngroups, lane);
-        r1 = warp_dot(a1, b, ngroups, lane);
-    } else {
-        float4 va[NG], vc[NG];
-#pragma unroll
-        for (int j = 0; j < NG; ++j) va[j] = ldg_stream(a0 + j * 32 + lane);
-#pragma unroll
-        for (int j = 0; j < NG; ++j) vc[j] = ldg_stream(a1 + j * 32 + lane);
-        float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f, cx = 0.f, cy = 0.f, cz = 0.f, cw = 0.f;
-#pragma unroll
-        for (int j = 0; j < NG; ++j) {
-            float4 vb = b[j * 32 + lane];
-            ax = __fmaf_rn(va[j].x, vb.x, ax);
-            ay = __fmaf_rn(va[j].y, vb.y, ay);
-            az = __fmaf_rn(va[j].z, vb.z, az);
-            aw = __fmaf_rn(va[j].w, vb.w, aw);
-        }
-#pragma unroll
-        for (int j = 0; j < NG; ++j) {
-            float4 vb = b[j * 32 + lane];
-            cx = __fmaf_rn(vc[j].x, vb.x, cx);
-            cy = __fmaf_rn(vc[j].y, vb.y, cy);
-            cz = __fmaf_rn(vc[j].z, vb.z, cz);
-            cw = __fmaf_rn(vc[j].w, vb.w, cw);
-        }
-        r0 = butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
-        r1 = butterfly_sum(__fadd_rn(__fadd_rn(cx, cy), __fadd_rn(cz, cw)));
-    }
-}
-
 __device__ __forceinline__ uint2 ldg_stream2(const uint2* p) {
     uint2 r;
     asm volatile("ld.global.nc.L1::no_allocate.v2.u32 {%0, %1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
@@ -194,46 +158,9 @@ __device__ __forceinline__ float warp_dot_h(const uint2* __restrict__ a, const f
     return butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
 }
 
-// Two fp16 rows in flight (the 4-warp shape); each result is warp_dot_h's.
-template <int NG>
-__device__ __forceinline__ void warp_dot2_h(const uint2* __restrict__ a0, const uint2* __restrict__ a1, const float4* __restrict__ b, int ngroups, int lane,
-                                            float& r0, float& r1) {
-    if constexpr (NG == 0) {
-        r0 = warp_dot_h<0>(a0, b, ngroups, lane);
-        r1 = warp_dot_h<0>(a1, b, ngroups, lane);
-    } else {
-        uint2 va[NG], vc[NG];
-#pragma unroll
-        for (int j = 0; j < NG; ++j) va[j] = ldg_stream2(a0 + j * 32 + lane);
-#pragma unroll
-        for (int j = 0; j < NG; ++j) vc[j] = ldg_stream2(a1 + j * 32 + lane);
-        float s[2];
-#pragma unroll
-        for (int t = 0; t < 2; ++t) {
-            const uint2* v = t ? vc : va;
-            float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
-#pragma unroll
-            for (int j = 0; j < NG; ++j) {
-                float4 vb = b[j * 32 + lane];
-                float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&v[j].x)), hi = __half22float2(*reinterpret_cast<const __half2*>(&v[j].y));
-                ax = __fmaf_rn(lo.x, vb.x, ax);
-                ay = __fmaf_rn(lo.y, vb.y, ay);
-                az = __fmaf_rn(hi.x, vb.z, az);
-                aw = __fmaf_rn(hi.y, vb.w, aw);
-            }
-            s[t] = butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
-        }
-        r0 = s[0]; r1 = s[1];
-    }
-}
-
 __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) {
     unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(s), "l"(gmem_src));
-}
-__device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-    unsigned s = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(s), "l"(gmem_src));
 }
 __device__ __forceinline__ void cp_async_commit_wait_all() {
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_all;" ::: "memory");

@@ -19,20 +19,6 @@ namespace nidx {
 constexpr int HB_THREADS = 256;
 constexpr int HB_WARPS = HB_THREADS / 32;
 constexpr int HB_MAX_CAND = 256;  // efC <= 256 (candidates of one select), mmax + 1 <= 256
-constexpr int HB_PAIR_LD = HS_MAX_ROW + 1;  // a full adjacency row plus the pushed edge
-
-// lane-blocked dot of two rows that both live in shared memory (same arithmetic as warp_dot)
-__device__ __forceinline__ float warp_dot_ss(const float4* __restrict__ a, const float4* __restrict__ b, int ngroups, int lane) {
-    float ax = 0.f, ay = 0.f, az = 0.f, aw = 0.f;
-    for (int g = lane; g < ngroups; g += 32) {
-        float4 va = a[g], vb = b[g];
-        ax = __fmaf_rn(va.x, vb.x, ax);
-        ay = __fmaf_rn(va.y, vb.y, ay);
-        az = __fmaf_rn(va.z, vb.z, az);
-        aw = __fmaf_rn(va.w, vb.w, aw);
-    }
-    return butterfly_sum(__fadd_rn(__fadd_rn(ax, ay), __fadd_rn(az, aw)));
-}
 
 struct HeurSmem {
     uint32_t* cand_id;   // [HB_MAX_CAND]
@@ -40,16 +26,14 @@ struct HeurSmem {
     unsigned char* state;  // [HB_MAX_CAND] 0 = untouched, 1 = kept, 2 = discarded
     uint32_t* sel_id;    // [HB_MAX_CAND]
     float* sel_sim;      // [HB_MAX_CAND]
-    float* cache;        // [cache_cap][ld] kept vectors (PRELOAD: all candidate vectors)
-    float* pair;         // PRELOAD: [HB_PAIR_LD][HB_PAIR_LD] pairwise similarities
-    unsigned char* sel_src;  // PRELOAD: candidate index of each kept entry
+    float* cache;        // [cache_cap][ld] kept vectors
     int cache_cap;
     int* s_fail;
     int* s_nsel;
 };
 
-__host__ __device__ __forceinline__ size_t hb_smem_bytes(int ld, int cache_cap, bool preload = false) {
-    return (size_t)HB_MAX_CAND * (4 + 4 + 4 + 4 + 1 + 1) + 64 + (size_t)cache_cap * ld * 4 + (preload ? (size_t)HB_PAIR_LD * HB_PAIR_LD * 4 : 0);
+__host__ __device__ __forceinline__ size_t hb_smem_bytes(int ld, int cache_cap) {
+    return (size_t)HB_MAX_CAND * (4 + 4 + 4 + 4 + 1) + 64 + (size_t)cache_cap * ld * 4;
 }
 
 __device__ inline void hb_carve(HeurSmem& h, unsigned char* p, int ld, int cache_cap, int* s_ints) {
@@ -58,9 +42,7 @@ __device__ inline void hb_carve(HeurSmem& h, unsigned char* p, int ld, int cache
     h.cand_sim = reinterpret_cast<float*>(p); p += HB_MAX_CAND * 4;
     h.sel_id = reinterpret_cast<uint32_t*>(p); p += HB_MAX_CAND * 4;
     h.sel_sim = reinterpret_cast<float*>(p); p += HB_MAX_CAND * 4;
-    h.state = p; p += HB_MAX_CAND;
-    h.sel_src = p; p += HB_MAX_CAND;
-    h.pair = reinterpret_cast<float*>(p);   // only carved when the launch reserved it (preload)
+    h.state = p;
     h.cache_cap = cache_cap;
     h.s_fail = &s_ints[0];
     h.s_nsel = &s_ints[1];
@@ -68,11 +50,6 @@ __device__ inline void hb_carve(HeurSmem& h, unsigned char* p, int ld, int cache
 
 // build.rs:57-95.  Candidates (id, similarity to the new node) in h.cand_* [0, nc) in the given order.
 // Result in h.sel_* [0, return value).  All threads of the CTA call this.
-// PRELOAD (prune of a full adjacency list, nc <= mmax + 1): every candidate vector is staged in shared memory
-// once (h.cache row i = candidate i), all nc*(nc-1)/2 pairwise similarities are computed in parallel into
-// h.pair, and the sequential pick of build.rs:66-82 becomes a walk over that table by one warp -- same
-// comparisons, same result, without one HBM round trip and two barriers per candidate.
-template <bool PRELOAD>
 __device__ inline int select_neighbours_heuristic(const VecDev& V, HeurSmem& h, int nc, int k) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int ng = V.ld >> 2;
@@ -80,89 +57,6 @@ __device__ inline int select_neighbours_heuristic(const VecDev& V, HeurSmem& h, 
     if (threadIdx.x == 0) *h.s_nsel = 0;
     __syncthreads();
     int nsel = 0;
-    if (PRELOAD) {
-        for (int i = warp; i < nc; i += HB_WARPS) {   // one warp per candidate row: 3 KB coalesced, asynchronous (the rows of a warp overlap)
-            const float4* src = reinterpret_cast<const float4*>(V.vecs + (size_t)h.cand_id[i] * V.ld);
-            float4* dst = reinterpret_cast<float4*>(h.cache + (size_t)i * V.ld);
-            for (int g = lane; g < ng; g += 32) cp_async16(dst + g, src + g);
-        }
-        cp_async_commit_wait_all();
-        __syncthreads();
-        // All pairwise similarities, register tiled: a warp takes a 4 x 4 block of (i, j) pairs, loads the eight rows' float4 groups
-        // once per group and keeps the 16 pairs' four accumulators in registers -- a quarter of the shared-memory reads of one
-        // dot per pair (the phase is bound by shared-memory bandwidth: 33 x 32 / 2 pairs x 6 KB).  Per pair the arithmetic is
-        // exactly warp_dot_ss's (lane-blocked groups in increasing order, four FMA accumulators, the same butterfly): bit-identical.
-        {
-            const int nb = (nc + 3) >> 2;                 // blocks of four rows
-            const int nblk = nb * (nb + 1) / 2;           // block pairs (ib >= jb)
-            for (int bp = warp; bp < nblk; bp += HB_WARPS) {
-                int ib = (int)((sqrtf(1.0f + 8.0f * (float)bp) - 1.0f) * 0.5f);
-                while (ib * (ib + 1) / 2 > bp) --ib;
-                while ((ib + 1) * (ib + 2) / 2 <= bp) ++ib;
-                const int jb = bp - ib * (ib + 1) / 2;
-                float acc[4][4][4];
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c2 = 0; c2 < 4; ++c2) { acc[r][c2][0] = 0.f; acc[r][c2][1] = 0.f; acc[r][c2][2] = 0.f; acc[r][c2][3] = 0.f; }
-                const float4* rows_i[4];
-                const float4* rows_j[4];
-#pragma unroll
-                for (int r = 0; r < 4; ++r) {
-                    rows_i[r] = reinterpret_cast<const float4*>(h.cache + (size_t)min(ib * 4 + r, nc - 1) * V.ld);
-                    rows_j[r] = reinterpret_cast<const float4*>(h.cache + (size_t)min(jb * 4 + r, nc - 1) * V.ld);
-                }
-                for (int g = lane; g < ng; g += 32) {
-                    float4 va[4], vb[4];
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) { va[r] = rows_i[r][g]; vb[r] = rows_j[r][g]; }
-#pragma unroll
-                    for (int r = 0; r < 4; ++r)
-#pragma unroll
-                        for (int c2 = 0; c2 < 4; ++c2) {
-                            acc[r][c2][0] = __fmaf_rn(va[r].x, vb[c2].x, acc[r][c2][0]);
-                            acc[r][c2][1] = __fmaf_rn(va[r].y, vb[c2].y, acc[r][c2][1]);
-                            acc[r][c2][2] = __fmaf_rn(va[r].z, vb[c2].z, acc[r][c2][2]);
-                            acc[r][c2][3] = __fmaf_rn(va[r].w, vb[c2].w, acc[r][c2][3]);
-                        }
-                }
-#pragma unroll
-                for (int r = 0; r < 4; ++r)
-#pragma unroll
-                    for (int c2 = 0; c2 < 4; ++c2) {
-                        const int i = ib * 4 + r, j = jb * 4 + c2;
-                        float ab = butterfly_sum(__fadd_rn(__fadd_rn(acc[r][c2][0], acc[r][c2][1]), __fadd_rn(acc[r][c2][2], acc[r][c2][3])));
-                        if (lane == 0 && i < nc && j < i) {
-                            float sv = sim_from_parts(V.sim, ab, V.norms[h.cand_id[i]], V.norms[h.cand_id[j]]);
-                            h.pair[i * HB_PAIR_LD + j] = sv;
-                            h.pair[j * HB_PAIR_LD + i] = sv;
-                        }
-                    }
-            }
-        }
-        __syncthreads();
-        if (warp == 0) {   // 66-82 on the table: lanes test the kept set in parallel
-            int kept = 0;
-            for (int i = 0; i < nc && kept < k; ++i) {
-                float sim = h.cand_sim[i];
-                bool bad = false;
-                for (int j0 = 0; j0 < kept; j0 += 32) {
-                    int j = j0 + lane;
-                    bad = bad || (j < kept && !(sim > h.pair[i * HB_PAIR_LD + h.sel_src[j]]));
-                }
-                bad = __any_sync(0xFFFFFFFFu, bad);
-                if (lane == 0) {
-                    if (!bad) { h.sel_id[kept] = h.cand_id[i]; h.sel_sim[kept] = sim; h.sel_src[kept] = (unsigned char)i; h.state[i] = 1; }
-                    else h.state[i] = 2;
-                }
-                __syncwarp();
-                if (!bad) kept++;
-            }
-            if (lane == 0) *h.s_fail = kept;
-        }
-        __syncthreads();
-        nsel = *h.s_fail;
-    } else {
     // the candidates are visited one after the other and each costs a dependent read of its 3 KB row: keep the next few rows on
     // their way into L2 (a warp per row, a lane per 128-byte line)
     constexpr int AHEAD = 4;
@@ -197,7 +91,6 @@ __device__ inline int select_neighbours_heuristic(const VecDev& V, HeurSmem& h, 
             h.state[i] = 2;
         }
         __syncthreads();
-    }
     }
     if (nsel < k) {  // 84-92 keepPrunedConnections: best discarded first, then sort the whole list desc
         int need = k - nsel;
@@ -260,7 +153,7 @@ __global__ void __launch_bounds__(HB_THREADS) select_link_kernel(VecDev V, Graph
     const uint64_t* f = a.found + ((size_t)slot * HS_MAX_LAYERS + layer) * a.efC;
     for (int i = threadIdx.x; i < nc; i += blockDim.x) { h.cand_id[i] = key_id(f[i]); h.cand_sim[i] = key_score(f[i]); }
     __syncthreads();
-    int nsel = select_neighbours_heuristic<false>(V, h, nc, a.M);
+    int nsel = select_neighbours_heuristic(V, h, nc, a.M);
     uint32_t* row = G.row(x, layer);
     float* wrow = G.wrow(x, layer);
     int stride = G.stride(layer);
@@ -283,7 +176,6 @@ struct ReverseArgs {
     const uint32_t* rev_x;
     const float* rev_sim;
     int cache_cap;
-    int preload;   // 1: the whole list (mmax + 1 vectors) fits in shared memory -> table-driven prune
     const uint32_t* heads;         // compacted segment heads (indices into key_sorted)
     const unsigned int* n_heads;
     unsigned int* work_counter;
@@ -304,8 +196,10 @@ __global__ void collect_heads_kernel(const uint64_t* __restrict__ key_sorted, in
     }
 }
 
-// build.rs:111-118: persistent CTAs pull (layer, neighbour) segments from the compacted head list.
-__global__ void __launch_bounds__(HB_THREADS) reverse_link_kernel(VecDev V, GraphDev G, ReverseArgs a) {
+// build.rs:111-118: persistent CTAs pull (layer, neighbour) segments from the compacted head list.  The minimum of one CTA per
+// SM keeps ptxas from trimming the kernel to 48 registers for occupancy (with spills, 5 % slower on an H100): the ~100 KB vector
+// cache already allows only two CTAs per SM at d = 768.
+__global__ void __launch_bounds__(HB_THREADS, 1) reverse_link_kernel(VecDev V, GraphDev G, ReverseArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_ints[4];
     __shared__ unsigned int s_work;
@@ -338,8 +232,7 @@ __global__ void __launch_bounds__(HB_THREADS) reverse_link_kernel(VecDev V, Grap
             if (len > mmax) {  // 115-117
                 for (int j = threadIdx.x; j < len; j += blockDim.x) { h.cand_id[j] = h.sel_id[j]; h.cand_sim[j] = h.sel_sim[j]; }
                 __syncthreads();
-                len = a.preload ? select_neighbours_heuristic<true>(V, h, len, mmax * 95 / 100)   // params.rs:29-31 prune_m
-                                : select_neighbours_heuristic<false>(V, h, len, mmax * 95 / 100);
+                len = select_neighbours_heuristic(V, h, len, mmax * 95 / 100);   // params.rs:29-31 prune_m
             }
         }
         __syncthreads();

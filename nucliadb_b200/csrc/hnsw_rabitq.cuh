@@ -228,7 +228,7 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
     }
     if (warp == W - 1) {
         cp_async_commit_wait_all();
-        if (GLOBAL_VIS && a.rq_prefetch) {
+        if (GLOBAL_VIS) {
             // The predicted next node's adjacency row is in shared memory now: pull its neighbours' codes and visited-table slots
             // into L2 while this hop's merge runs (3.6 KB + 32 lines per hop; wasted when the prediction fails).
             __syncwarp();

@@ -60,7 +60,6 @@ struct SearchArgs {
     uint32_t* gvisited;               // [grid][1 << gv_bits] layer-0 visited table in global memory (L2)
     int gv_bits;
     int last_k;                       // min(k * RERANKING_FACTOR, RERANKING_LIMIT)
-    int rq_prefetch;                  // pull the predicted next node's neighbour codes / visited slots into L2
 };
 
 struct SearchCtx {
@@ -156,7 +155,7 @@ __device__ inline void hs_reseed(SearchCtx& c) {
 // into the other half of a double buffer; the row's HBM latency then overlaps this expansion's vector loads.
 // LEAN (the layer search's hot loop): the list length arrives in a register and s_best_next alternates between two slots, so that
 // hs_merge needs no barrier after thread 0 has published the new length -- three barriers per expansion instead of four.
-template <bool CU, int NG, int W = HS_WARPS, bool PAIR = false, bool LEAN = false>
+template <bool CU, int NG, int W = HS_WARPS, bool LEAN = false>
 __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& c, uint32_t node, int layer, int ef, float min_score, int best, int len_in = -1) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int stride = G.stride(layer);
@@ -228,53 +227,22 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
     // A warp's later rows (j + W, j + 2W, ...) are pulled into L2 while it works on its first one: their loads then cost an L2
     // hit instead of a second and third HBM round trip on the expansion's critical path (one prefetch per 128-byte line, a lane
     // each; no registers held, unlike a second row in flight).  Under the screen the row read first is the fp16 one.
-    if (!PAIR) {
-        const int lines = screen ? (V.ldh * 2 + 127) >> 7 : (V.ld * 4 + 127) >> 7;
-        for (int j = warp + W; j < ntodo; j += W) {
-            const char* rowp = screen ? reinterpret_cast<const char*>(hrow(c.todo_id[j])) : reinterpret_cast<const char*>(frow(c.todo_id[j]));
-            for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(rowp + (size_t)l * 128));
-        }
+    const int lines = screen ? (V.ldh * 2 + 127) >> 7 : (V.ld * 4 + 127) >> 7;
+    for (int j = warp + W; j < ntodo; j += W) {
+        const char* rowp = screen ? reinterpret_cast<const char*>(hrow(c.todo_id[j])) : reinterpret_cast<const char*>(frow(c.todo_id[j]));
+        for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(rowp + (size_t)l * 128));
     }
-    if constexpr (PAIR) {   // two rows in flight per warp (fewer warps per query, more queries per SM)
-        for (int j = warp; j < ntodo; j += 2 * W) {
-            uint32_t y0 = c.todo_id[j];
-            bool two = j + W < ntodo;
-            uint32_t y1 = two ? c.todo_id[j + W] : y0;
-            bool x0 = true, x1 = two;   // the f32 row is read
-            float n0, n1;
-            if (screen) {
-                float4 r0 = __ldg(V.hrec + y0), r1 = __ldg(V.hrec + y1);
-                float h0, h1;
-                if (two) warp_dot2_h<NG>(hrow(y0), hrow(y1), qv, ng, lane, h0, h1);
-                else { h0 = warp_dot_h<NG>(hrow(y0), qv, ng, lane); h1 = 0.0f; }
-                x0 = !hs_screened_out(V, c, y0, h0, r0, wkey);
-                x1 = two && !hs_screened_out(V, c, y1, h1, r1, wkey);
-                n0 = r0.x; n1 = r1.x;
-            } else {
-                n0 = V.sim != SIM_DOT ? __ldg(V.norms + y0) : 0.0f; n1 = (two && V.sim != SIM_DOT) ? __ldg(V.norms + y1) : 0.0f;
-            }
-            float ab0 = 0.0f, ab1 = 0.0f;
-            if (x0 && x1) warp_dot2_t<NG>(frow(y0), frow(y1), qv, ng, lane, ab0, ab1);
-            else if (x0) ab0 = warp_dot_t<NG>(frow(y0), qv, ng, lane);
-            else if (x1) ab1 = warp_dot_t<NG>(frow(y1), qv, ng, lane);
-            if (lane == 0) {
-                if (x0) finish(j, y0, ab0, n0); else skip(j);
-                if (x1) finish(j + W, y1, ab1, n1); else if (two) skip(j + W);
-            }
-        }
-    } else {
-        for (int j = warp; j < ntodo; j += W) {
-            uint32_t y = c.todo_id[j];
-            float vnorm;
-            if (screen) {
-                float4 r = __ldg(V.hrec + y);
-                float ah = warp_dot_h<NG>(hrow(y), qv, ng, lane);
-                if (hs_screened_out(V, c, y, ah, r, wkey)) { if (lane == 0) skip(j); continue; }
-                vnorm = r.x;
-            } else vnorm = V.sim != SIM_DOT ? __ldg(V.norms + y) : 0.0f;
-            float ab = warp_dot_t<NG>(frow(y), qv, ng, lane);
-            if (lane == 0) finish(j, y, ab, vnorm);
-        }
+    for (int j = warp; j < ntodo; j += W) {
+        uint32_t y = c.todo_id[j];
+        float vnorm;
+        if (screen) {
+            float4 r = __ldg(V.hrec + y);
+            float ah = warp_dot_h<NG>(hrow(y), qv, ng, lane);
+            if (hs_screened_out(V, c, y, ah, r, wkey)) { if (lane == 0) skip(j); continue; }
+            vnorm = r.x;
+        } else vnorm = V.sim != SIM_DOT ? __ldg(V.norms + y) : 0.0f;
+        float ab = warp_dot_t<NG>(frow(y), qv, ng, lane);
+        if (lane == 0) finish(j, y, ab, vnorm);
     }
     if (warp == W - 1) cp_async_commit_wait_all();
     c.hop++;
@@ -341,12 +309,12 @@ __device__ inline void hs_merge(SearchCtx& c, int cap, int best, int* len_io = n
 }
 
 // hnsw/search.rs:242-304 on the list held in shared memory.
-template <int NG, int W = HS_WARPS, bool PAIR = false>
+template <int NG, int W = HS_WARPS>
 __device__ inline void hs_layer_search(const VecDev& V, const GraphDev& G, SearchCtx& c, int layer, int ef) {
     int best = *c.s_best, len = *c.s_len;     // published by hs_reseed (behind its barrier); from here on in registers
     while (best < len) {
         uint64_t ckey = c.A[best];
-        hs_expand<false, NG, W, PAIR, true>(V, G, c, key_id(ckey), layer, ef, 0.0f, best, len);
+        hs_expand<false, NG, W, true>(V, G, c, key_id(ckey), layer, ef, 0.0f, best, len);
         hs_merge<false, true>(c, ef, best, &len, &best);
     }
     c.s_best_next = c.s_bn;                    // (callers that use the shared copies come after a barrier)
@@ -381,7 +349,7 @@ __device__ inline bool hs_passes(const VecDev& V, const SearchArgs& a, uint32_t 
 }
 
 // hnsw/search.rs:188-240.  Results go straight to out_ids/out_scores (already descending).
-template <int NG, int W = HS_WARPS, bool PAIR = false>
+template <int NG, int W = HS_WARPS>
 __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, uint32_t* out_ids, float* out_scores) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     hs_reseed(c);
@@ -404,7 +372,7 @@ __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCt
         __syncthreads();
         nacc += *c.s_flag;
         if (nacc == a.k) break;  // 214
-        hs_expand<true, NG, W, PAIR>(V, G, c, node, 0, 0, a.min_score, 0);
+        hs_expand<true, NG, W>(V, G, c, node, 0, 0, a.min_score, 0);
         hs_merge<true>(c, a.cu_cap, 0);
     }
     return nacc;
@@ -412,11 +380,11 @@ __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCt
 
 // The tail of HnswSearcher::search for query q: closest_up_nodes on the list in c.A (search.rs:369-375), the final stable sort
 // (search.rs:381) and the NIL padding of the outputs.
-template <int NG, int W = HS_WARPS, bool PAIR = false>
+template <int NG, int W = HS_WARPS>
 __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, unsigned int q) {
     uint32_t* oi = a.out_ids + (size_t)q * a.k;
     float* os = a.out_scores + (size_t)q * a.k;
-    int nacc = hs_closest_up<NG, W, PAIR>(V, G, c, a, oi, os);
+    int nacc = hs_closest_up<NG, W>(V, G, c, a, oi, os);
     __syncthreads();
     // search.rs:381 `filtered_result.sort_by(|a, b| b.1.total_cmp(&a.1))`: stable, descending.
     // (closest_up_nodes can accept a late-found neighbour that outranks earlier results.)
@@ -441,11 +409,9 @@ __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, Searc
     if (threadIdx.x == 0) a.out_counts[q] = nacc;
 }
 
-// W warps per CTA.  W = 8: one row per warp in flight, 4 CTAs per SM (592 queries resident).  W = 4 (PAIR): two rows per warp in
-// flight, 7 CTAs per SM -- 1036 queries resident, so a batch of 1024 runs as ONE wave instead of 592 + 432 (the second wave of
-// the 8-warp shape leaves 27 % of the CTA slots empty while it runs).
-template <int NG, int W = HS_WARPS, bool PAIR = false>
-__global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_kernel(VecDev V, GraphDev G, SearchArgs a) {
+// HS_WARPS = 8 warps per CTA, one row per warp in flight, 4 CTAs per SM (528 queries resident on 132 SMs).
+template <int NG>
+__global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, GraphDev G, SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
     __shared__ int s_ints[8];
     __shared__ unsigned int s_work;
@@ -506,7 +472,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_ker
             if (a.mode == 0) ef = layer == 0 ? a.ef0 : 1;
             else ef = layer <= top ? a.efC : 1;
             hs_reseed(c);
-            hs_layer_search<NG, W, PAIR>(V, G, c, layer, ef);
+            hs_layer_search<NG>(V, G, c, layer, ef);
             __syncthreads();
             if (a.mode == 1 && layer <= top && layer < HS_MAX_LAYERS) {
                 int len = *c.s_len;
@@ -525,7 +491,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_search_ker
         if (a.mode == 1 && threadIdx.x == 0)
             for (int layer = (int)G.entry_layer + 1; layer <= top && layer < HS_MAX_LAYERS; ++layer) a.found_count[(size_t)q * HS_MAX_LAYERS + layer] = 0;
 
-        if (a.mode == 0) hs_emit_results<NG, W, PAIR>(V, G, c, a, q);
+        if (a.mode == 0) hs_emit_results<NG>(V, G, c, a, q);
     }
     // counters: n_dist and n_skip live in lane 0 of every warp, the rest in thread 0; [6] = f32 rows read for a similarity
     if (lane == 0 && c.n_dist) { atomicAdd(&a.counters[0], c.n_dist); atomicAdd(&a.counters[6], c.n_dist - c.n_skip); }

@@ -30,7 +30,6 @@
 #include <cuda.h>
 
 #include "common.cuh"
-#include "scan_tc.cuh"
 #include "topk.cuh"
 
 namespace nidx {
@@ -57,11 +56,31 @@ static_assert(TC2_SMEM_BYTES <= 227 * 1024, "the filter kernel's shared memory e
 constexpr float TC2_EPS = 2.2e-3f;
 constexpr int TC2_SURV_CAP = 512;     // survivors per query the refine kernel re-scores; more => exact scan
 
+// wgmma shared-memory matrix descriptor: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46), layout [62,64)
+// (0 = no swizzle, 1 = 128-byte swizzle)
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)((lbo_bytes & 0x3FFFFu) >> 4) << 16) | ((uint64_t)((sbo_bytes & 0x3FFFFu) >> 4) << 32) |
+           ((uint64_t)layout << 62);
+}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" :: "n"(N) : "memory"); }
+__device__ __forceinline__ void mbar_init(uint64_t* mbar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"((uint32_t)__cvta_generic_to_shared(mbar)), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* mbar, uint32_t parity) {
+    uint32_t addr = (uint32_t)__cvta_generic_to_shared(mbar);
+    asm volatile("{\n\t.reg .pred p;\n\tWAIT_%=:\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t@p bra DONE_%=;\n\tbra WAIT_%=;\n\tDONE_%=:\n\t}"
+                 :: "r"(addr), "r"(parity) : "memory");
+}
+
 __device__ __forceinline__ uint64_t tc2_desc(uint32_t smem_addr) {
     // K-major, SWIZZLE_128B: LBO unused (16 B), SBO = 8 rows x 128 B = 1024 B
     return wg_desc(smem_addr, 16, 1024, 1);
 }
-// d[64 x 128] (+)= A[64 x 8] · B[128 x 8]ᵀ: the m64n128k8 tf32 form of wg_mma_64x64_tf32 (same fragment layout, j = 0..15)
+// d[64 x 128] (+)= A[64 x 8] · B[128 x 8]ᵀ, tf32 operands from shared memory, f32 accumulator fragment d[64] per thread:
+// d[4j + e] (j = 0..15) holds row (warp % 4) * 16 + lane / 4 + 8 * (e / 2), column 8j + 2 (lane % 4) + e % 2.
 __device__ __forceinline__ void wg_mma_64x128_tf32(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"

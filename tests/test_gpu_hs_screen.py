@@ -44,11 +44,9 @@ def _same(a, b):
     assert np.array_equal(a[1].view(np.uint32), b[1].view(np.uint32))   # bitwise
 
 
-@pytest.mark.parametrize("shape", ["8", "4"])
 @pytest.mark.parametrize("sim", SIMS)
 @pytest.mark.parametrize("d", [128, 100])
-def test_screened_walk_is_the_f32_walk_and_the_oracle(sim, d, shape, monkeypatch):
-    monkeypatch.setenv("NIDX_B200_HS_W", shape)
+def test_screened_walk_is_the_f32_walk_and_the_oracle(sim, d, monkeypatch):
     v, q = _data(sim, 8000, d, seed=21 + d + sim)
     seg = VectorSegment.create(v, d, similarity=sim, m=16, m0=32, ef_construction=64)
     monkeypatch.setenv("NIDX_B200_HS_F16", "0")

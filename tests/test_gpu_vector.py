@@ -47,11 +47,7 @@ def test_brute_force_min_score_and_alive():
     assert all(alive[i] for i in ids[ids != 0xFFFFFFFF])
 
 
-@pytest.mark.parametrize("shape", ["8", "4"])
-def test_hnsw_search_matches_oracle_on_oracle_graph(small_data, shape, monkeypatch):
-    """Both CTA shapes of hnsw_search_kernel (8 warps per query, the default; 4 warps with two rows in flight each) walk exactly
-    like the oracle."""
-    monkeypatch.setenv("NIDX_B200_HS_W", shape)
+def test_hnsw_search_matches_oracle_on_oracle_graph(small_data):
     v, q = small_data
     g = O.hnsw_build(v, M=16, M0=32, efC=100, max_batch=64, nthreads=8)
     seg = _seg(v, _lib.NIDX_SIM_COSINE, m=16, m0=32, ef_construction=100)
@@ -255,17 +251,6 @@ def test_tiny_segments(n):
     hi, hs, hc = seg.search(q, 5, ef=8, method=_lib.NIDX_METHOD_HNSW)
     gi, gs, gc, _ = O.hnsw_search(v, og, q, 5, 8)
     assert (hc == gc).all() and (hi == gi).all() and np.array_equal(hs, gs)
-
-
-@pytest.mark.parametrize("prune", ["table", "seq"])
-def test_prune_variants_build_the_same_graph(prune, monkeypatch):
-    monkeypatch.setenv("NIDX_B200_PRUNE", prune)
-    v = make_vectors(3000, 64, seed=14)
-    seg = _seg(v, _lib.NIDX_SIM_COSINE, m=8, m0=16, ef_construction=40)
-    seg.build_hnsw(seed=2, max_batch=128)
-    g = seg.get_graph()
-    og = O.hnsw_build(v, M=8, M0=16, efC=40, seed=2, max_batch=128, nthreads=8)
-    assert (g["adj0"] == og.adj0).all() and np.array_equal(g["w0"], og.w0)
 
 
 def test_zero_vectors_and_large_k(small_data):
