@@ -199,7 +199,7 @@ int nidx_vec_search_formula(nidx_vec_segment* seg, const float* queries, int32_t
 int nidx_merge_topk(int32_t device, const uint32_t* ids, const float* scores, int32_t n_parts, int64_t part_stride, int32_t nq, int32_t k,
                     uint32_t* out_ids, float* out_scores, int32_t* out_part, void* stream);
 
-/* Counters of the last HNSW search / build on this segment (for the roofline accounting,
+/* Counters of the last HNSW search / build on this segment (0 after an exhaustive f32 scan; for the roofline accounting,
  * SURVEY 8d): [0] similarity evaluations, [1] node expansions, [2] visited-set overflows.  Every search call counts into its
  * own workspace, so concurrent searches never mix their counts; "last" = the call that was issued last. */
 int nidx_vec_counters(nidx_vec_segment* seg, uint64_t out[3]);
@@ -210,6 +210,10 @@ int nidx_vec_counters_ex(nidx_vec_segment* seg, uint64_t out[6]);
  * the vectors with a proven error bound and reads the f32 row only of those that can enter its list, so this is at most
  * the similarity count of nidx_vec_counters (equal when the segment has no fp16 copy). */
 int nidx_vec_exact_rows(nidx_vec_segment* seg, uint64_t* out);
+/* The tensor-core filter of the last exhaustive scan (batches of >= 64 queries, k <= 16): [0] vectors re-scored exactly as
+ * survivors of the filter, [1] queries scanned exactly in full instead (a list that may have overflowed, too many survivors, or
+ * a query outside the filter's error bound).  Both are 0 when the scan did not use the filter. */
+int nidx_vec_scan_counters(nidx_vec_segment* seg, uint64_t out[2]);
 
 /* RaBitQ 1-bit codes (vector_types/rabitq.rs; Dot similarity and dimension % 64 == 0 only, config.rs:170-173).
  * nidx_vec_rabitq_encode builds the reference's vectors.quant records ([f32 dot_quant_original][u32 sum_bits][dim/8 sign

@@ -7,6 +7,7 @@
 #include <algorithm>
 #include <atomic>
 #include <cmath>
+#include <cfloat>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -157,6 +158,7 @@ struct nidx_vec_segment {
     uint64_t* d_upper_off = nullptr;
     uint32_t* d_adjU = nullptr; float* d_wU = nullptr;
     float max_norm = 0.0f;              // max |v| (error bound of the tensor-core filter for Dot)
+    bool tc_rows_ok = false;            // every row meets the filter's bound (max_norm_kernel): else batches take the exact scan
     CUtensorMap map_v;                  // TMA descriptor of the vector block (scan_tc2.cuh), built on first use
     bool map_v_ready = false;
     std::mutex map_mu;
@@ -231,11 +233,21 @@ static int alloc_graph(nidx_vec_segment* s, const uint8_t* level) {
     return 0;
 }
 
-__global__ void max_norm_kernel(const float* __restrict__ norms, uint64_t n, unsigned int* __restrict__ out_bits) {
+// out[0] = bits of max |v|; out[1] = 1 if some row is outside the tensor-core filter's bound (scan_tc2.cuh): a non-finite norm, or
+// (cosine) a row with a non-zero element whose norm is below TC2_MIN_NORM.  Rows are read only for such tiny norms.
+__global__ void max_norm_kernel(VecDev V, uint64_t n, unsigned int* __restrict__ out) {
     float m = 0.0f;
-    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) m = fmaxf(m, norms[i]);
+    bool bad = false;
+    for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const float nv = V.norms[i];
+        m = fmaxf(m, nv);
+        if (!(nv <= FLT_MAX)) bad = true;
+        else if (V.sim == SIM_COSINE && nv < TC2_MIN_NORM)
+            for (int j = 0; j < V.ld && !bad; ++j) bad = V.vecs[i * V.ld + j] != 0.0f;
+    }
     for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xFFFFFFFFu, m, off));
-    if ((threadIdx.x & 31) == 0) atomicMax(out_bits, __float_as_uint(m));   // non-negative floats order like their bit patterns
+    if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));   // non-negative floats order like their bit patterns
+    if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(out + 1, 1u);
 }
 
 // The HNSW walk's fp16 screening copy (hs_screened_out in hnsw_search.cuh derives the bound), one warp per row:
@@ -394,16 +406,17 @@ static int finish_create(nidx_vec_segment* s, const uint32_t* paragraph_of_host)
             CU(cudaMemcpy(s->d_par_first, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
         }
     }
-    if (n) {   // max |v| for the Dot error bound of the tensor-core filter
+    if (n) {   // max |v| for the Dot error bound of the tensor-core filter, and whether every row meets the bound
         unsigned int* d_bits = nullptr;
-        CU(cudaMalloc(&d_bits, 4));
-        CU(cudaMemset(d_bits, 0, 4));
-        max_norm_kernel<<<std::min<uint64_t>((n + 255) / 256, (uint64_t)s->sm_count * 8), 256>>>(s->d_norms, n, d_bits);
+        CU(cudaMalloc(&d_bits, 8));
+        CU(cudaMemset(d_bits, 0, 8));
+        max_norm_kernel<<<std::min<uint64_t>((n + 255) / 256, (uint64_t)s->sm_count * 8), 256>>>(s->vdev(), n, d_bits);
         LAUNCHED();
-        unsigned int hb = 0;
-        CU(cudaMemcpy(&hb, d_bits, 4, cudaMemcpyDeviceToHost));
+        unsigned int hb[2] = {0, 0};
+        CU(cudaMemcpy(hb, d_bits, 8, cudaMemcpyDeviceToHost));
         cudaFree(d_bits);
-        memcpy(&s->max_norm, &hb, 4);
+        memcpy(&s->max_norm, &hb[0], 4);
+        s->tc_rows_ok = hb[1] == 0;
     }
     CU(cudaMalloc(&s->d_counters, 8 * sizeof(unsigned long long)));
     CU(cudaMemset(s->d_counters, 0, 8 * sizeof(unsigned long long)));
@@ -639,6 +652,16 @@ int nidx_vec_exact_rows(nidx_vec_segment* s, uint64_t* out) {
     unsigned long long* src = s->last_counters.load();
     CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
     *out = h[6];
+    return 0;
+}
+
+int nidx_vec_scan_counters(nidx_vec_segment* s, uint64_t out[2]) {
+    if (!s || !out) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(s->cfg.device));
+    unsigned long long h[8];
+    unsigned long long* src = s->last_counters.load();
+    CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
+    out[0] = h[6]; out[1] = h[7];
     return 0;
 }
 
@@ -991,8 +1014,9 @@ static int filter_formula_device(nidx_vec_segment* s, Workspace& w, const nidx_f
 
 // The tensor-core filter + refine path serves large batches of small-k queries on single-vector segments whose rows are whole
 // 128-byte swizzle rows.  NIDX_B200_SCAN=exact forces the CUDA-core kernels (same results, bit for bit), =tensor forces the filter.
+// Rows outside the filter's error bound (a non-finite norm, a tiny cosine row) keep the whole segment on the CUDA-core kernels.
 static bool use_tc_filter(const nidx_vec_segment* s, int nq, int k) {
-    if (k > TC2_KMAX || s->ld % TC2_KB != 0 || s->d_par_first || s->n < (uint64_t)TC2_N || s->cfg.similarity == NIDX_SIM_L2) return false;
+    if (k > TC2_KMAX || s->ld % TC2_KB != 0 || s->d_par_first || s->n < (uint64_t)TC2_N || s->cfg.similarity == NIDX_SIM_L2 || !s->tc_rows_ok) return false;
     const char* e = getenv("NIDX_B200_SCAN");
     if (e && !strcmp(e, "exact")) return false;
     if (e && !strcmp(e, "tensor")) return true;
@@ -1190,6 +1214,9 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         CU(cudaGetLastError());
     } else if (method == NIDX_METHOD_BRUTE) {
         if (k > 1024) return fail(NIDX_EINVAL, "brute-force k above 1024 not supported");
+        ENSURE(w.sched, 128);   // zero counters for this call: nidx_vec_scan_counters then reports that the filter did not run
+        CU(cudaMemsetAsync(w.sched.p, 0, 128, stream));
+        s->last_counters.store(reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64));
         int cap = topk_cap(k, 256);
         int n_chunks = (int)std::min<uint64_t>(std::max<uint64_t>(1, ((uint64_t)s->sm_count * 4 + nq - 1) / nq), (s->n_par + 4095) / 4096);
         n_chunks = std::max(n_chunks, 1);

@@ -131,7 +131,8 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
     c.s_nadmit = cnt;
     c.s_maxtodo = &s_maxtodo[cur];
     const int len = *c.s_len;
-    const uint64_t wkey = len >= ef ? c.A[len - 1] : 0;
+    const bool full = len >= ef;
+    const float wscore = full ? key_score(c.A[len - 1]) : 0.0f;
     const int visited = *c.s_hash_count;       // stable during the expansion (thread 0 updates it after the barrier)
     if (threadIdx.x == 0) *c.s_best_next = INT_MAX;   // hs_merge's atomicMin target: reset before the barrier below
     const int nchunks = a.code_stride >> 4;
@@ -217,7 +218,7 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
             float est, err;
             rq_finish(r, idot, w[0][0].x, w[0][0].y, est, err);       // chunk 0 starts with the code's header (dot_quant_original, sum_bits)
             uint64_t key = make_key(est, y, 1);
-            if (key > wkey) {                                             // layer_search (search.rs:286): better than the worst of a full list
+            if (!full || est > wscore) {                                  // layer_search (search.rs:286): a SCORE above the worst of a full list (a tie is refused whatever the ids)
                 c.todo_key[atomicAdd(&cnt[0], 1)] = key;
                 atomicMax(c.s_maxtodo, (unsigned long long)key);
             }

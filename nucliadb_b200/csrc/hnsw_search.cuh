@@ -212,7 +212,7 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
     auto finish = [&](int j, uint32_t y, float ab, float vnorm) {
         float s = sim_from_parts(V.sim, ab, vnorm, c.qnorm);
         uint64_t key = make_key(s, y, 1);
-        bool admit = CU ? (s >= min_score) : (key > wkey);
+        bool admit = CU ? (s >= min_score) : (wkey == 0 || s > key_score(wkey));   // search.rs:286 compares scores: a tie with the worst is refused
         c.todo_key[j] = admit ? key : 0;
         if (admit) { atomicAdd(c.s_nadmit, 1); atomicMax(c.s_maxtodo, (unsigned long long)key); }
         c.n_dist++;

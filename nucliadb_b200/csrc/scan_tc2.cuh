@@ -6,8 +6,24 @@
 // filter with a rigorous error bound, never written to HBM, and only the few survivors are re-scored with the lane-blocked f32
 // arithmetic of common.cuh.  Ids AND scores are therefore bit-identical to the small-batch kernel and to the oracle.
 //
-//   |tf32(q) . tf32(v) - q . v| <= 2^-9 |q| |v|  (each operand keeps 10 mantissa bits: relative error < 2^-10 per factor)
-//   eps = 2.2e-3 (cosine) or 2.2e-3 |q| max|v| (dot).  Let tau = the k-th largest APPROXIMATE score of a query over the
+// The bound, for ld = the padded row length (the tensor cores' internal summation order and rounding are not documented, so the
+// accumulation is taken as the worst case: a sequential f32 sum rounded toward zero, unit 2^-23; products of tf32 operands are
+// exact in f32).  With S = sum |q_i v_i| <= |q| |v|:
+//   operands   |tf32(q_i) tf32(v_i) - q_i v_i| <= (2^-9 + 2^-20) |q_i v_i|   (truncation to 10 mantissa bits: < 2^-10 per factor)
+//   accumulate <= (ld - 1) 2^-23 / (1 - ld 2^-23) (1 + 2^-10)^2 S              (any summation tree of ld terms)
+//   exact dot  <= dot_depth(ld) 2^-24 S <= 2^-18 S                             (the lane-blocked f32 score it is compared with)
+//   cosine     the epilogue's four rn roundings (frcp_rn of both norms, two products) and the exact score's (division, two
+//              subtractions) add < 2^-21; stored norms are within 2^-22 of |q|, |v|
+//   subnormal  all of the above holds for normal f32 values only.  With |q|, |v| (cosine: every non-zero row) or |q|, max|v| (dot)
+//              >= TC2_MIN_NORM = 2^-40, an operand, product or partial sum that is subnormal -- or flushed to zero, which the PTX
+//              ISA leaves open for tf32 -- errs by < 2^-126 absolute, ld 2^-126 (1 + |q| + |v|) in all, < 2^-33 of |q| |v| at ld <= 4096
+// Up to ld = 4096 all but the operand term stay below 65 2^-23, so |approx - exact| <= eps(ld) S with
+//   eps(ld) = max(2.2e-3, 2^-9 + 2^-20 + (ld + 64) 2^-23)   (tc2_eps: 2.2e-3 up to ld = 1999, 2.45e-3 at 4096)
+// as a cosine score, or eps(ld) |q| max|v| as a dot product.  tests/test_scan_filter_bound.py checks it against a model of the
+// filter, and shows that 2.2e-3 alone fails at d = 4096.  Outside the bound the query or the segment takes the exact scan:
+// a segment with a non-finite norm or (cosine) a non-zero row with |v| < TC2_MIN_NORM (api.cu, max_norm_kernel); a query with
+// |q| or max|v| below TC2_MIN_NORM, |q| max|v| above 2^126 or not finite (so no tf32 sum or exact dot overflows), or a non-finite tau.
+//   Let tau = the k-th largest APPROXIMATE score of a query over the
 //   eligible vectors: every member of the true top-k has approx >= tau - 2 eps.  Each CTA keeps, per query row, the best
 //   TC2_L approximate scores of ITS share of the vectors (a list in registers); the k best approximations overall are in
 //   those lists (at most k - 1 entries of a share rank above any of them, and L >= k), so tau is known exactly from the
@@ -54,7 +70,10 @@ constexpr size_t TC2_SMEM_BYTES = 1024 /* alignment slack */ + (size_t)TC2_STAGE
                                   TC2_CONSUMERS * (TC2_N / 32) * 4 /* eligibility */ + (size_t)TC2_STAGE_ROWS * TC2_M * TC2_LISTS * 8 /* staging */ + 256;
 static_assert(TC2_SMEM_BYTES <= 227 * 1024, "the filter kernel's shared memory exceeds a Hopper block's 227 KB");
 constexpr float TC2_EPS = 2.2e-3f;
+constexpr float TC2_MIN_NORM = 0x1p-40f;   // far from the subnormal range: see the header comment
 constexpr int TC2_SURV_CAP = 512;     // survivors per query the refine kernel re-scores; more => exact scan
+// eps(ld) of the header comment
+__host__ __device__ __forceinline__ float tc2_eps(int ld) { return fmaxf(TC2_EPS, 0x1p-9f + 0x1p-20f + (float)(ld + 64) * 0x1p-23f); }
 
 // wgmma shared-memory matrix descriptor: start >> 4 [0,14), LBO >> 4 [16,30), SBO >> 4 [32,46), layout [62,64)
 // (0 = no swizzle, 1 = 128-byte swizzle)
@@ -322,15 +341,19 @@ __global__ void __launch_bounds__(256) scan_tc_refine_kernel(VecDev V, const flo
     for (int i = threadIdx.x; i < ng; i += blockDim.x) reinterpret_cast<float4*>(qv)[i] = reinterpret_cast<const float4*>(queries + (size_t)q * V.ld)[i];
     const float qn = V.sim == SIM_COSINE ? qnorms[q] : 0.0f;
     // eps of this query: cosine scores are scale free; a dot product scales with both norms
-    float eps = TC2_EPS;
+    float eps = tc2_eps(V.ld), qabs = qn;
     if (V.sim != SIM_COSINE) {
         float s = 0.0f;
         for (int i = lane; i < V.d; i += 32) { float x = queries[(size_t)q * V.ld + i]; s += x * x; }
         for (int off = 16; off >= 1; off >>= 1) s += __shfl_xor_sync(0xFFFFFFFFu, s, off);
-        eps = TC2_EPS * sqrtf(s) * max_vnorm;
+        qabs = sqrtf(s);
+        eps *= qabs * max_vnorm;
     }
     const float margin = 2.0f * eps;
-    if (threadIdx.x == 0) { s_overflow = (V.sim == SIM_COSINE && !(qn > 0.0f)) ? 1 : 0; s_nsurv = 0; }
+    // a query outside the bound (header comment) is scanned exactly: NaN / inf elements, a tiny query or segment (subnormal
+    // products), or sums that may overflow
+    const bool out_of_bound = !(qabs >= TC2_MIN_NORM) || !(max_vnorm >= TC2_MIN_NORM) || !(qabs * max_vnorm <= 0x1p126f);
+    if (threadIdx.x == 0) { s_overflow = out_of_bound ? 1 : 0; s_nsurv = 0; }
     BlockTopK tk;
     tk.init(tk_buf, &tk_count, &tk_thr, k, cap);
     const float* cs = cand_score + (size_t)q * n_lists * TC2_L;
@@ -345,6 +368,7 @@ __global__ void __launch_bounds__(256) scan_tc_refine_kernel(VecDev V, const flo
     }
     int c = tk.finish();
     const float tau = c >= k ? key_score(tk_buf[k - 1]) : -INFINITY;
+    if (threadIdx.x == 0 && (tau == INFINITY || isnan(tau - margin))) s_overflow = 1;
     __syncthreads();
     // 2. overflow test per list: full (no NIL entry), and its smallest entry still within the margin of tau
     for (int l = threadIdx.x; l < n_lists; l += blockDim.x) {

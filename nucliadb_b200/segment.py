@@ -196,6 +196,13 @@ class VectorSegment:
         check(_lib.load().nidx_vec_exact_rows(self._h, C.byref(out)))
         return out.value
 
+    def scan_counters(self):
+        """The last exhaustive scan's tensor-core filter: vectors re-scored as survivors, and queries scanned in full instead
+        (both 0 when the scan did not use the filter)."""
+        out = (C.c_uint64 * 2)()
+        check(_lib.load().nidx_vec_scan_counters(self._h, out))
+        return dict(survivors=out[0], full_scans=out[1])
+
 
 def merge_topk(ids, scores, device=0, part_stride=0, out=None):
     """[n_parts, nq, k] torch CUDA tensors (each part sorted desc, NIL padded) -> merged (ids, scores, part).

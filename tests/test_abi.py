@@ -44,6 +44,8 @@ def test_no_device_fails_loudly():
     v = np.zeros((4, 8), dtype=np.float32)
     rc = L.nidx_vec_create(C.byref(cfg), _lib.ptr(v), C.c_uint64(4), C.c_int32(8), _lib.NIDX_MEM_HOST, None, C.byref(h))
     assert rc == -2 and b"no CUDA device" in L.nidx_last_error()
+    out = (C.c_uint64 * 2)()
+    assert L.nidx_vec_scan_counters(None, out) != 0 and b"null" in L.nidx_last_error()
     with pytest.raises(_lib.NidxError):
         _lib.require_device()
     from nucliadb_b200.segment import VectorSegment

@@ -45,7 +45,7 @@ def _same(a, b):
 
 
 @pytest.mark.parametrize("sim", SIMS)
-@pytest.mark.parametrize("d", [128, 100])
+@pytest.mark.parametrize("d", [128, 100, 512, 1024, 1536, 4096])
 def test_screened_walk_is_the_f32_walk_and_the_oracle(sim, d, monkeypatch):
     v, q = _data(sim, 8000, d, seed=21 + d + sim)
     seg = VectorSegment.create(v, d, similarity=sim, m=16, m0=32, ef_construction=64)

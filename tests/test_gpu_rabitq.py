@@ -11,7 +11,7 @@ from nucliadb_b200.segment import VectorSegment
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("d", [64, 256, 768])
+@pytest.mark.parametrize("d", [64, 256, 768, 1984, 2048, 4096])
 def test_codes_and_estimates_are_bit_identical(d):
     v = make_vectors(3000, d, seed=51)
     v[5, :7] = 0.0                      # zeros quantise to the negative side (v > 0.0 is false)
@@ -69,7 +69,7 @@ def _oracle_graph(seg, n, m, m0):
 
 
 @pytest.mark.parametrize("shape", ["8", "4"])
-@pytest.mark.parametrize("d,n", [(128, 20000), (768, 6000)])
+@pytest.mark.parametrize("d,n", [(128, 20000), (768, 6000), (1984, 3000), (2048, 3000), (4096, 3000)])
 def test_quantised_walk_matches_oracle(d, n, shape, monkeypatch):
     """hnsw/search.rs:306-383 with a RaBitQ query: ids, scores and the number of estimates / expansions equal the oracle's
     restatement on the same graph (oracle.hnsw_search_rabitq), with and without deletions, duplicates suppression and min_score --

@@ -15,7 +15,7 @@ def _seg(v, sim, **kw):
 
 
 @pytest.mark.parametrize("sim", [_lib.NIDX_SIM_COSINE, _lib.NIDX_SIM_DOT])
-@pytest.mark.parametrize("d", [128, 100, 384])
+@pytest.mark.parametrize("d", [128, 100, 384, 512, 1024, 1536, 2048, 3072, 4096])
 def test_brute_force_matches_oracle(sim, d):
     v = make_vectors(5000, d, seed=5)
     if sim == _lib.NIDX_SIM_DOT:
@@ -156,7 +156,9 @@ def test_parts_merge_matches_kmerge():
     assert (got2[0].cpu().numpy() == want_ids).all() and (got2[2].cpu().numpy() == want_part).all()
 
 
-@pytest.mark.parametrize("sim,d", [(_lib.NIDX_SIM_COSINE, 384), (_lib.NIDX_SIM_DOT, 128), (_lib.NIDX_SIM_COSINE, 768)])
+@pytest.mark.parametrize("sim,d", [(_lib.NIDX_SIM_COSINE, 384), (_lib.NIDX_SIM_DOT, 128), (_lib.NIDX_SIM_COSINE, 768), (_lib.NIDX_SIM_COSINE, 512),
+                                   (_lib.NIDX_SIM_DOT, 1024), (_lib.NIDX_SIM_COSINE, 1536), (_lib.NIDX_SIM_DOT, 2048), (_lib.NIDX_SIM_COSINE, 3072),
+                                   (_lib.NIDX_SIM_DOT, 4096)])
 def test_tensor_core_filter_scan_is_bit_exact(sim, d, monkeypatch):
     """Batches of >= 64 queries with k <= 16 take the wgmma TF32 FILTER + exact REFINE path (scan_tc2.cuh): ids and scores must
     equal the oracle's bit for bit -- the tensor cores only decide which vectors are re-scored -- with deletions, min_score, a
@@ -172,6 +174,8 @@ def test_tensor_core_filter_scan_is_bit_exact(sim, d, monkeypatch):
         monkeypatch.setenv("NIDX_B200_SCAN", "tensor")
         ids, sc, cnt = seg.search(q, k, min_score=ms, method=_lib.NIDX_METHOD_BRUTE)
         assert (cnt == oc).all() and (ids == oi).all() and np.array_equal(sc, os_)
+        c = seg.scan_counters()
+        assert c["survivors"] > 0 and c["full_scans"] < len(q)    # the filter served the batch
         monkeypatch.setenv("NIDX_B200_SCAN", "exact")
         ids2, sc2, cnt2 = seg.search(q, k, min_score=ms, method=_lib.NIDX_METHOD_BRUTE)
         assert (ids2 == ids).all() and np.array_equal(sc2, sc) and (cnt2 == cnt).all()
