@@ -191,13 +191,20 @@ int nidx_vec_filter(nidx_vec_segment* seg, const nidx_filter_node* nodes, int32_
 int nidx_vec_search_formula(nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem, const nidx_vec_search_params* p,
                             const nidx_filter_node* nodes, int32_t n_nodes, uint32_t* out_ids, float* out_scores, int32_t* out_counts, void* stream);
 
-/* Searcher::_search's cross-segment / cross-shard top-k (searcher.rs:241-290 Fssc without the string
- * keys, shard_merge.rs:332-348): merge n_parts partial results [n_parts][nq][k] (score desc) into
- * [nq][k]; out_part[nq][k] receives the index of the part each winner came from.  part_stride = elements
- * between consecutive parts in ids / scores (0 = nq*k, i.e. dense), so an all-gather buffer can be merged in place.
- * Device pointers. */
+/* The text merge: n_parts partial results [n_parts][nq][k] (score desc, NIDX_NIL padded) of the segments of ONE
+ * document-partitioned index -> [nq][k] ranked (score desc, part asc, position asc).  Inside one index the parts are segments in
+ * docaddr order, so this is merge_document_responses' order (bm25 desc, docaddr asc; shard_merge.rs:211-231) for them.  It is NOT
+ * the vector merge: use nidx_merge_vector_parts for vector shards.  out_part[nq][k] receives the index of the part each winner
+ * came from.  part_stride = elements between consecutive parts in ids / scores (0 = nq*k, i.e. dense), so an all-gather buffer can
+ * be merged in place.  k <= 1024.  Device pointers. */
 int nidx_merge_topk(int32_t device, const uint32_t* ids, const float* scores, int32_t n_parts, int64_t part_stride, int32_t nq, int32_t k,
                     uint32_t* out_ids, float* out_scores, int32_t* out_part, void* stream);
+/* merge_vector_responses (shard_merge.rs:332-348) with nidx_merge_topk's arguments: kmerge_by(|a, b| a.score >= b.score), take(k),
+ * exactly as itertools 0.14 runs it, over the parts in the order given (the reference's `responses` vector).  A part ends at its
+ * first NIDX_NIL.  Equal scores (f32 ==, so -0 == +0) are NOT resolved lower part first: itertools' heap decides which equal head
+ * leads (e.g. 2 parts of scores (1, 1, 0.5) -> (part, position) = (1,0) (0,0) (1,1) (0,1) ...).  n_parts * k < 2^31.  Device pointers. */
+int nidx_merge_vector_parts(int32_t device, const uint32_t* ids, const float* scores, int32_t n_parts, int64_t part_stride, int32_t nq, int32_t k,
+                            uint32_t* out_ids, float* out_scores, int32_t* out_part, void* stream);
 
 /* Counters of the last HNSW search / build on this segment (0 after an exhaustive f32 scan; for the roofline accounting,
  * SURVEY 8d): [0] similarity evaluations, [1] node expansions, [2] visited-set overflows.  Every search call counts into its
@@ -373,8 +380,10 @@ void nidx_shard_destroy(nidx_shard_comm* comm);
 int nidx_vec_set_paragraph_keys(nidx_vec_segment* seg, const uint64_t* keys);
 
 /* OpenSegment::search on this rank's segment + exchange + merge, identical results on every rank.  Collective: every rank calls
- * it with the same queries, nq, k and dedup, in the same order (one call at a time per communicator).
- *   dedup = 0: the parts are shards -- merge_vector_responses (kmerge by score, shard_merge.rs:332-348);
+ * it with the same queries, nq, k and dedup, in the same order (one call at a time per communicator).  It is
+ * nidx_vec_shard_record (rank = this rank), an all-gather of the records in rank order, then nidx_shard_merge.
+ *   dedup = 0: the parts are shards -- merge_vector_responses (kmerge_by(score >=), shard_merge.rs:332-348), parts in rank
+ *              order standing for the reference's `responses` order; ties as nidx_merge_vector_parts;
  *   dedup = 1: the parts are segments of ONE index -- Fssc (searcher.rs:150-199): one entry per paragraph key, and with
  *              p->with_duplicates == 0 byte-identical vectors are suppressed across segments (by a 64-bit hash of the bytes).
  * out_ids are vector addresses local to the part in out_part[nq][k] (-1 = none); out_counts[nq] may be NULL.
@@ -382,6 +391,26 @@ int nidx_vec_set_paragraph_keys(nidx_vec_segment* seg, const uint64_t* keys);
 int nidx_vec_search_sharded(nidx_shard_comm* comm, nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem,
                             const nidx_vec_search_params* p, int32_t dedup, uint32_t* out_ids, float* out_scores, int32_t* out_part, int32_t* out_counts,
                             void* stream);
+
+/* The two halves of nidx_vec_search_sharded without the exchange, for a host that gathers the records by other means (or one GPU
+ * holding several parts).  A record of nq queries at k = p->k is, in 32-bit words:
+ *     [ids nq*k u32][scores nq*k f32]                                    dedup = 0   (2 * nq * k words)
+ *     [ids nq*k u32][scores nq*k f32][par_key nq*k u64][vec_key nq*k u64] dedup = 1   (6 * nq * k words)
+ * ids / scores are nidx_vec_search's (vector addresses local to the segment, score desc, NIDX_NIL padded).  par_key = the
+ * paragraph key of nidx_vec_set_paragraph_keys, or (rank << 32) | paragraph address without keys; vec_key = a 64-bit hash of the
+ * vector's bytes when p->with_duplicates == 0, else one constant for every vector (the merge does not read it then); both 0 for
+ * NIDX_NIL entries.
+ * nidx_vec_shard_record: search `seg` into out_record (device memory on the segment's GPU).  `mem` applies to the queries (and
+ * p->filter_bits); asynchronous on `stream`. */
+int nidx_vec_shard_record(nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem, const nidx_vec_search_params* p, int32_t rank,
+                          int32_t dedup, uint32_t* out_record, void* stream);
+/* nidx_shard_merge: merge n_parts records laid end to end (device memory, part i at records + i * record words) with the rule of
+ * nidx_vec_search_sharded for `dedup` (with_duplicates: Fssc's flag; ignored for dedup = 0) -> out_ids / out_scores /
+ * out_part [nq][k], out_counts[nq] (out_part, out_counts may be NULL).  The de-duplicating merge keeps 16 k + 8 n_parts k bytes per
+ * query in shared memory and refuses more than 96 KiB (NIDX_EINVAL).  `mem` applies to the outputs; NIDX_MEM_HOST returns when they
+ * are in place, NIDX_MEM_DEVICE is asynchronous on `stream`. */
+int nidx_shard_merge(int32_t device, const uint32_t* records, int32_t n_parts, int32_t nq, int32_t k, int32_t dedup, int32_t with_duplicates, int mem,
+                     uint32_t* out_ids, float* out_scores, int32_t* out_part, int32_t* out_counts, void* stream);
 /* BM25 over a document-partitioned index (every part scores with the statistics of the whole index, nidx_txt_set_stats):
  * merge_document_responses' order (bm25 desc, part asc, doc asc; shard_merge.rs:227-231); out_total = Count over all parts. */
 int nidx_txt_search_sharded(nidx_shard_comm* comm, nidx_txt_segment* seg, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem,

@@ -27,12 +27,13 @@ SYMBOLS = [
     "nidx_vec_create", "nidx_vec_open", "nidx_vec_save", "nidx_vec_close", "nidx_vec_len", "nidx_vec_device_vectors",
     "nidx_use_hnsw", "nidx_hnsw_levels", "nidx_normalize_vectors", "nidx_vec_build_hnsw", "nidx_vec_extend_hnsw", "nidx_vec_graph_dims", "nidx_vec_set_graph", "nidx_vec_get_graph", "nidx_vec_set_alive",
     "nidx_vec_set_inverted_index", "nidx_vec_filter", "nidx_vec_search_formula",
-    "nidx_vec_search", "nidx_merge_topk", "nidx_vec_counters", "nidx_vec_counters_ex", "nidx_vec_exact_rows", "nidx_vec_scan_counters", "nidx_vec_last_kernel_ms",
+    "nidx_vec_search", "nidx_merge_topk", "nidx_merge_vector_parts", "nidx_vec_counters", "nidx_vec_counters_ex", "nidx_vec_exact_rows", "nidx_vec_scan_counters", "nidx_vec_last_kernel_ms",
     "nidx_vec_rabitq_encode", "nidx_vec_rabitq_codes", "nidx_vec_rabitq_estimate",
     "nidx_txt_create", "nidx_txt_set_stats", "nidx_txt_set_alive", "nidx_txt_close", "nidx_txt_search", "nidx_txt_last_kernel_ms",
     "nidx_txt_set_facets", "nidx_txt_facet_buckets", "nidx_txt_search_faceted", "nidx_txt_facet_count_all",
     "nidx_txt_set_dates", "nidx_txt_search_ordered", "nidx_txt_list_ordered",
-    "nidx_shard_unique_id", "nidx_shard_init", "nidx_shard_destroy", "nidx_vec_set_paragraph_keys", "nidx_vec_search_sharded", "nidx_txt_search_sharded",
+    "nidx_shard_unique_id", "nidx_shard_init", "nidx_shard_destroy", "nidx_vec_set_paragraph_keys", "nidx_vec_search_sharded",
+    "nidx_vec_shard_record", "nidx_shard_merge", "nidx_txt_search_sharded",
     "nidx_txt_set_doc_keys", "nidx_rank_fusion_rrf", "nidx_shard_search",
 ]
 

@@ -19,6 +19,7 @@ than the local file store, relations / JSON / graph / suggest are outside the ho
 """
 from __future__ import annotations
 
+import itertools
 import os
 import threading
 import uuid as _uuid
@@ -31,6 +32,7 @@ import numpy as np
 from . import nidx_protos as P
 from . import text as T
 from . import vector as V
+from .shard_merge import bm25_order_key, kmerge_by
 
 
 @dataclass
@@ -307,16 +309,18 @@ class NidxBinding:
         k = int(req.result_per_page)
         resp = P.SearchResponse()
         resp.shard_ids.extend(sid for sid, _ in parts)
-        # vectors: kmerge_by(score >=), take(k) (shard_merge.rs:332-348)
-        vec = sorted(((-d.score, i, j, d) for i, (_, p) in enumerate(parts) for j, d in enumerate(p.get("vector", []))), key=lambda t: t[:3])[:k]
-        for _, _, _, d in vec:
+        # vectors: kmerge_by(score >=), take(k) (shard_merge.rs:332-348), shards in request order standing for the reference's
+        # `responses` order; equal scores come out in the order itertools' heap gives them, not first shard first
+        merged = kmerge_by([p.get("vector", []) for _, p in parts], lambda a, b: a.score >= b.score)
+        vec = [d for _, d in itertools.islice(merged, max(k, 0))]
+        for d in vec:
             ds = resp.vector.documents.add()
             ds.doc_id.id, ds.score = d.doc_id, d.score
             ds.labels.extend(d.labels)
             if d.metadata:
                 ds.metadata.CopyFrom(P.SentenceMetadata.FromString(d.metadata))
-        # documents / paragraphs: bm25 desc, then shard, then lower docaddr (shard_merge.rs:227-231); under an order by date
-        # (merge_order_key), the sort value is the date
+        # documents / paragraphs: bm25 desc (total_cmp), then shard_id bytes descending, then lower docaddr (shard_merge.rs:211-231,
+        # 289-309); the bytes are those written to `shard_id` below.  Under an order by date (merge_order_key), the sort value is the date
         ordered = req.HasField("order")
         for kind, target in (("document", resp.document), ("paragraph", resp.paragraph)):
             found = [(sid, p[kind]) for sid, p in parts if kind in p]
@@ -326,7 +330,8 @@ class NidxBinding:
                 rows = sorted(((merge_order_key(r.date, int(req.order.type), i, j), i, 0, sid, r) for i, (sid, rs) in enumerate(found) for j, r in enumerate(rs.results)),
                               key=lambda t: t[0])
             else:
-                rows = sorted(((-r.score.bm25, i, r.score.docaddr, sid, r) for i, (sid, rs) in enumerate(found) for r in rs.results), key=lambda t: t[:3])
+                rows = sorted(((bm25_order_key(r.score.bm25, sid.encode(), r.score.docaddr), i, 0, sid, r) for i, (sid, rs) in enumerate(found) for r in rs.results),
+                              key=lambda t: t[0])
             target.total = sum(rs.total for _, rs in found)
             target.next_page = any(rs.next_page for _, rs in found) or len(rows) > k
             target.query = req.body

@@ -1425,6 +1425,34 @@ int nidx_merge_topk(int32_t device, const uint32_t* ids, const float* scores, in
     return 0;
 }
 
+// kmerge_parts_kernel: one thread per query, n_parts heap entries (u32) per thread in shared memory
+static int launch_kmerge(const uint32_t* ids, const float* scores, int n_parts, size_t part_stride, int nq, int k, uint32_t* out_ids, float* out_scores,
+                         int* out_part, int* out_counts, cudaStream_t stream) {
+    if ((long long)n_parts * k >= (1ll << 31)) return fail(NIDX_EINVAL, "n_parts * k must stay below 2^31");
+    size_t per = (size_t)n_parts * 4;
+    if (per > 96 * 1024) return fail(NIDX_EINVAL, "%d parts are too many for the vector merge", n_parts);
+    int threads = (int)std::max<size_t>(1, std::min<size_t>(128, (size_t)(48 * 1024) / per));
+    threads = std::min(threads, nq);
+    size_t smem = per * threads;
+    if (smem > 48 * 1024) CU(cudaFuncSetAttribute(kmerge_parts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kmerge_parts_kernel<<<(nq + threads - 1) / threads, threads, smem, stream>>>(ids, scores, n_parts, part_stride, nq, k, out_ids, out_scores, out_part,
+                                                                                 out_counts);
+    LAUNCHED();
+    return 0;
+}
+
+int nidx_merge_vector_parts(int32_t device, const uint32_t* ids, const float* scores, int32_t n_parts, int64_t part_stride, int32_t nq, int32_t k,
+                            uint32_t* out_ids, float* out_scores, int32_t* out_part, void* stream_) {
+    int r = check_device(device);
+    if (r) return r;
+    if (!ids || !scores || !out_ids || !out_scores || n_parts <= 0 || nq <= 0 || k <= 0) return fail(NIDX_EINVAL, "bad argument");
+    r = launch_kmerge(ids, scores, n_parts, part_stride > 0 ? (size_t)part_stride : (size_t)nq * k, nq, k, out_ids, out_scores, out_part, nullptr,
+                      reinterpret_cast<cudaStream_t>(stream_));
+    if (r) return r;
+    CU(cudaGetLastError());
+    return 0;
+}
+
 // ---- build ------------------------------------------------------------------------------------
 // Level RNG: build.rs:40,97-101.  rand 0.10 SmallRng = xoshiro256++ seeded by SplitMix64 [recalled].
 static void host_assign_levels(uint64_t n, int M, uint64_t seed, uint8_t* level) {
@@ -2432,37 +2460,42 @@ int nidx_vec_set_paragraph_keys(nidx_vec_segment* s, const uint64_t* keys) {
     return 0;
 }
 
-// common tail: all-gather the local part, merge, deliver
-static int shard_exchange_and_merge(nidx_shard_comm* c, int nq, int k, bool dedup, int with_duplicates, bool ohost, uint32_t* out_ids, float* out_scores,
-                                    int32_t* out_part, int32_t* out_counts, cudaStream_t stream) {
-    NcclApi& N = nccl_api();
-    size_t words = shard_part_words(nq, k, dedup);
-    uint32_t* local = c->local.as<uint32_t>();
-    uint32_t* gathered = c->gathered.as<uint32_t>();
-    NC(N.AllGather(local, gathered, words * 4, NCCL_INT8, c->comm, stream));
-    LAUNCHED();
-    // outputs: device pointers, or staged behind the gathered parts when the caller's are host pointers
+// How the parts of a sharded search are merged (step 3)
+enum class PartsRule {
+    text,     // documents of one index: (score desc, part asc, position asc), parts_merge_kernel + shard_count_kernel
+    kmerge,   // vector shards: merge_vector_responses, kmerge_by(score >=) (kmerge_parts_kernel)
+    fssc,     // vector segments of one index: Fssc with the paragraph / vector keys of the records (shard_fssc_kernel)
+};
+
+// Step 3: merge n_parts records laid end to end (shard_part_words each) into [nq][k] ids / scores / part + counts.  Outputs are
+// device pointers, or (ohost) host pointers staged through `stage` (nq * k * 12 + nq * 4 bytes of device memory) and copied back
+// asynchronously on `stream`.
+static int shard_merge_impl(const uint32_t* gathered, int n_parts, int nq, int k, PartsRule rule, int with_duplicates, bool ohost, uint32_t* stage,
+                            uint32_t* out_ids, float* out_scores, int32_t* out_part, int32_t* out_counts, cudaStream_t stream) {
+    size_t words = shard_part_words(nq, k, rule == PartsRule::fssc);
     uint32_t* d_ids = out_ids; float* d_sc = out_scores; int* d_part = out_part; int* d_cnt = out_counts;
     if (ohost) {
-        uint32_t* stage = gathered + (size_t)c->world * words;
         d_ids = stage; d_sc = reinterpret_cast<float*>(stage + (size_t)nq * k); d_part = reinterpret_cast<int*>(stage + 2 * (size_t)nq * k);
         d_cnt = reinterpret_cast<int*>(stage + 3 * (size_t)nq * k);
     }
-    if (dedup) {
-        size_t per = (size_t)k * 16 + (size_t)c->world * k * 8;
+    const float* gathered_scores = reinterpret_cast<const float*>(gathered + (size_t)nq * k);
+    if (rule == PartsRule::fssc) {
+        size_t per = (size_t)k * 16 + (size_t)n_parts * k * 8;
         int threads = (int)std::max<size_t>(1, std::min<size_t>(64, (size_t)(96 * 1024) / per));
-        if (per > 96 * 1024) return fail(NIDX_EINVAL, "k = %d is too large for the de-duplicating merge over %d parts", k, c->world);
+        if (per > 96 * 1024) return fail(NIDX_EINVAL, "k = %d is too large for the de-duplicating merge over %d parts", k, n_parts);
         threads = std::min(threads, nq);
         size_t smem = per * threads;
         if (smem > 48 * 1024) CU(cudaFuncSetAttribute(shard_fssc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        shard_fssc_kernel<<<(nq + threads - 1) / threads, threads, smem, stream>>>(gathered, c->world, words, nq, k, with_duplicates, d_ids, d_sc, d_part, d_cnt);
+        shard_fssc_kernel<<<(nq + threads - 1) / threads, threads, smem, stream>>>(gathered, n_parts, words, nq, k, with_duplicates, d_ids, d_sc, d_part, d_cnt);
         LAUNCHED();
+    } else if (rule == PartsRule::kmerge) {
+        int r = launch_kmerge(gathered, gathered_scores, n_parts, words, nq, k, d_ids, d_sc, d_part, d_cnt, stream);
+        if (r) return r;
     } else {
-        if (k > 1024 || (long long)c->world * k >= (1ll << 31)) return fail(NIDX_EINVAL, "k above 1024 not supported");
+        if (k > 1024 || (long long)n_parts * k >= (1ll << 31)) return fail(NIDX_EINVAL, "k above 1024 not supported");
         int cap = topk_cap(k, 256);
         if ((size_t)cap * 8 > 48 * 1024) CU(cudaFuncSetAttribute(parts_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
-        parts_merge_kernel<<<nq, 256, (size_t)cap * 8, stream>>>(gathered, reinterpret_cast<const float*>(gathered + (size_t)nq * k), c->world, words, nq, k, cap, d_ids,
-                                                                  d_sc, d_part);
+        parts_merge_kernel<<<nq, 256, (size_t)cap * 8, stream>>>(gathered, gathered_scores, n_parts, words, nq, k, cap, d_ids, d_sc, d_part);
         LAUNCHED();
         if (d_cnt) {
             shard_count_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(d_ids, nq, k, d_cnt);
@@ -2476,6 +2509,67 @@ static int shard_exchange_and_merge(nidx_shard_comm* c, int nq, int k, bool dedu
         if (out_part) CU(cudaMemcpyAsync(out_part, d_part, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
         if (out_counts) CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
     }
+    return 0;
+}
+
+// common tail: all-gather the local part, merge, deliver (outputs staged behind the gathered parts when they are host pointers)
+static int shard_exchange_and_merge(nidx_shard_comm* c, int nq, int k, PartsRule rule, int with_duplicates, bool ohost, uint32_t* out_ids, float* out_scores,
+                                    int32_t* out_part, int32_t* out_counts, cudaStream_t stream) {
+    NcclApi& N = nccl_api();
+    size_t words = shard_part_words(nq, k, rule == PartsRule::fssc);
+    uint32_t* local = c->local.as<uint32_t>();
+    uint32_t* gathered = c->gathered.as<uint32_t>();
+    NC(N.AllGather(local, gathered, words * 4, NCCL_INT8, c->comm, stream));
+    LAUNCHED();
+    return shard_merge_impl(gathered, c->world, nq, k, rule, with_duplicates, ohost, gathered + (size_t)c->world * words, out_ids, out_scores, out_part,
+                            out_counts, stream);
+}
+
+// Step 1: this part's segment searched into its exchange record (queries from the caller's memory, results straight into the
+// record), plus the de-duplication keys.  `counts` = nq ints of device scratch, or NULL.
+static int shard_record_impl(nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, bool qhost, const nidx_vec_search_params* p, int32_t rank,
+                             bool dedup, uint32_t* record, int32_t* counts, cudaStream_t stream) {
+    int k = p->k;
+    int r = vec_search_impl(seg, queries, nq, ldq, qhost, false, p, record, reinterpret_cast<float*>(record + (size_t)nq * k), counts, stream);
+    if (r) return r;
+    if (dedup) {
+        int n_res = nq * k;
+        shard_keys_kernel<<<(n_res * 32 + 255) / 256, 256, 0, stream>>>(seg->vdev(), record, n_res, seg->d_par_keys, (uint32_t)rank, p->with_duplicates ? 0 : 1,
+                                                                       reinterpret_cast<uint64_t*>(record + 2 * (size_t)nq * k),
+                                                                       reinterpret_cast<uint64_t*>(record + 4 * (size_t)nq * k));
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    return 0;
+}
+
+int nidx_vec_shard_record(nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem, const nidx_vec_search_params* p, int32_t rank,
+                          int32_t dedup, uint32_t* out_record, void* stream_) {
+    if (!seg || !p || !out_record) return fail(NIDX_EINVAL, "null argument");
+    if (nq <= 0) return 0;
+    if (p->k <= 0) return fail(NIDX_EINVAL, "k must be positive");
+    if (rank < 0) return fail(NIDX_EINVAL, "rank must not be negative");
+    CU(cudaSetDevice(seg->cfg.device));
+    return shard_record_impl(seg, queries, nq, ldq, mem == NIDX_MEM_HOST, p, rank, dedup != 0, out_record, nullptr, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+int nidx_shard_merge(int32_t device, const uint32_t* records, int32_t n_parts, int32_t nq, int32_t k, int32_t dedup, int32_t with_duplicates, int mem,
+                     uint32_t* out_ids, float* out_scores, int32_t* out_part, int32_t* out_counts, void* stream_) {
+    int r = check_device(device);
+    if (r) return r;
+    if (!records || !out_ids || !out_scores || n_parts <= 0 || k <= 0) return fail(NIDX_EINVAL, "bad argument");
+    if (nq <= 0) return 0;
+    CU(cudaSetDevice(device));
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    PartsRule rule = dedup ? PartsRule::fssc : PartsRule::kmerge;
+    if (mem != NIDX_MEM_HOST) return shard_merge_impl(records, n_parts, nq, k, rule, with_duplicates, false, nullptr, out_ids, out_scores, out_part, out_counts, stream);
+    DevBuf stage;
+    r = stage.ensure((size_t)nq * k * 12 + (size_t)nq * 4);
+    if (!r) r = shard_merge_impl(records, n_parts, nq, k, rule, with_duplicates, true, stage.as<uint32_t>(), out_ids, out_scores, out_part, out_counts, stream);
+    cudaError_t e = cudaStreamSynchronize(stream);
+    stage.release();
+    if (r) return r;
+    if (e != cudaSuccess) return fail(NIDX_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
     return 0;
 }
 
@@ -2494,19 +2588,12 @@ int nidx_vec_search_sharded(nidx_shard_comm* c, nidx_vec_segment* seg, const flo
     ENSURE(c->local, words * 4 + (size_t)nq * 4);
     ENSURE(c->gathered, (size_t)c->world * words * 4 + (size_t)nq * k * 12 + (size_t)nq * 4 + 64);
     uint32_t* local = c->local.as<uint32_t>();
-    int* local_cnt = reinterpret_cast<int*>(local + words);
-    // 1. this rank's segment: queries from the caller's memory, results straight into the exchange record
-    int r = vec_search_impl(seg, queries, nq, ldq, host, false, p, local, reinterpret_cast<float*>(local + (size_t)nq * k), local_cnt, stream);
+    // 1. this rank's segment into the exchange record
+    int r = shard_record_impl(seg, queries, nq, ldq, host, p, c->rank, dedup != 0, local, reinterpret_cast<int*>(local + words), stream);
     if (r) return r;
-    if (dedup) {
-        int n_res = nq * k;
-        shard_keys_kernel<<<(n_res * 32 + 255) / 256, 256, 0, stream>>>(seg->vdev(), local, n_res, seg->d_par_keys, (uint32_t)c->rank, p->with_duplicates ? 0 : 1,
-                                                                       reinterpret_cast<uint64_t*>(local + 2 * (size_t)nq * k),
-                                                                       reinterpret_cast<uint64_t*>(local + 4 * (size_t)nq * k));
-        LAUNCHED();
-    }
     // 2. + 3. exchange and merge
-    r = shard_exchange_and_merge(c, nq, k, dedup != 0, p->with_duplicates, host, out_ids, out_scores, out_part, out_counts, stream);
+    r = shard_exchange_and_merge(c, nq, k, dedup ? PartsRule::fssc : PartsRule::kmerge, p->with_duplicates, host, out_ids, out_scores, out_part, out_counts,
+                                 stream);
     if (r) return r;
     if (host) CU(cudaStreamSynchronize(stream));
     return 0;
@@ -2537,7 +2624,7 @@ int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uin
     if (r) return r;
     NC(N.AllReduce(d_total, d_total, (size_t)nq, NCCL_UINT64, NCCL_SUM, c->comm, stream));   // Count collector over all parts
     LAUNCHED();
-    r = shard_exchange_and_merge(c, nq, k, false, 1, host, out_docs, out_scores, out_part, out_counts, stream);
+    r = shard_exchange_and_merge(c, nq, k, PartsRule::text, 1, host, out_docs, out_scores, out_part, out_counts, stream);
     if (r) return r;
     if (host) {
         if (out_total) CU(cudaMemcpyAsync(out_total, d_total, (size_t)nq * 8, cudaMemcpyDeviceToHost, stream));

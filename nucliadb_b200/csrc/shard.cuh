@@ -58,7 +58,8 @@ inline NcclApi& nccl_api() {
     return api;
 }
 
-// ---- exchange record of one rank: [ids nq*k u32][scores nq*k f32] (+ [par_key nq*k u64][vec_key nq*k u64] with de-dup) --------
+// ---- exchange record of one part: [ids nq*k u32][scores nq*k f32] (+ [par_key nq*k u64][vec_key nq*k u64] with de-dup), in u32 words
+// (nidx_vec_shard_record writes one, nidx_shard_merge merges n_parts of them laid end to end) ------------------------------------
 __host__ __device__ __forceinline__ size_t shard_part_words(int nq, int k, bool dedup) { return (size_t)nq * k * (dedup ? 6 : 2); }
 
 // 64-bit keys of the local results for the cross-segment de-duplication: par_key = the caller's paragraph key (the hash of the
@@ -91,7 +92,9 @@ __global__ void shard_keys_kernel(VecDev V, const uint32_t* __restrict__ ids, in
 // part by part (the reference's segment loop), each part in its own order (score descending).
 //   add(): with_duplicates == false and the vector was seen -> skip; full -> the lowest-scored entry that scores below the
 //   candidate is evicted; the candidate is inserted unless its paragraph key is already present (HashSet::insert keeps the
-//   old element).  Result sorted by score descending, stable over the collection's order (insertion order here).
+//   old element), so an eviction followed by a present key shrinks the collection.  Among entries tied for the lowest score the
+//   first in insertion order is evicted (the reference takes whichever its HashSet iterates first, which is not fixed).  Result
+//   sorted by score descending, stable over the collection's order (insertion order here).
 __global__ void shard_fssc_kernel(const uint32_t* __restrict__ gathered, int n_parts, size_t part_words, int nq, int k, int with_duplicates,
                                   uint32_t* __restrict__ out_ids, float* __restrict__ out_scores, int* __restrict__ out_part, int* __restrict__ out_counts) {
     extern __shared__ __align__(16) unsigned char fs_smem[];
@@ -156,6 +159,57 @@ __global__ void shard_fssc_kernel(const uint32_t* __restrict__ gathered, int n_p
         }
     }
     if (out_counts) out_counts[q] = nb;
+}
+
+// merge_vector_responses (shard_merge.rs:332-348): kmerge_by(|a, b| a.score >= b.score).take(k) over the parts, taken in the order
+// given (the reference's `responses` vector).  itertools 0.14's KMergeBy restated: a binary heap, ordered by `less_than`, of the
+// non-empty parts' iterators in part order, built by heapify; every next() yields the head of heap[0], advances that part or, when it
+// is exhausted, swap_remove(0)s it, then sift_down(0) (the branchless form: the right child is taken when less_than(right, left)).
+// The predicate holds both ways for equal scores, so ties do NOT come out lower part first: the heap's shape decides which equal
+// head leads.  A part ends at its first NIL.  IEEE f32 >=: -0 and +0 are equal, a NaN is never >=.  One thread per query; its heap
+// (part * k + position of each part's head) lives in shared memory, entry i of thread t at [i * blockDim.x + t].
+__global__ void kmerge_parts_kernel(const uint32_t* __restrict__ ids, const float* __restrict__ scores, int n_parts, size_t part_stride, int nq, int k,
+                                    uint32_t* __restrict__ out_ids, float* __restrict__ out_scores, int* __restrict__ out_part, int* __restrict__ out_counts) {
+    extern __shared__ __align__(16) uint32_t km_heap[];
+    int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= nq) return;
+    uint32_t* heap = km_heap + threadIdx.x;
+    const size_t W = blockDim.x;
+    auto src = [&](uint32_t slot) { return (size_t)(slot / (uint32_t)k) * part_stride + (size_t)q * k + slot % (uint32_t)k; };
+    auto less = [&](uint32_t a, uint32_t b) { return scores[src(a)] >= scores[src(b)]; };
+    auto swap = [&](int a, int b) { uint32_t t = heap[a * W]; heap[a * W] = heap[b * W]; heap[b * W] = t; };
+    auto sift_down = [&](int pos, int len) {
+        int child = 2 * pos + 1;
+        while (child + 1 < len) {
+            child += less(heap[(child + 1) * W], heap[child * W]) ? 1 : 0;
+            if (!less(heap[child * W], heap[pos * W])) return;
+            swap(pos, child);
+            pos = child;
+            child = 2 * pos + 1;
+        }
+        if (child + 1 == len && less(heap[child * W], heap[pos * W])) swap(pos, child);
+    };
+    int len = 0;
+    for (int part = 0; part < n_parts; ++part)
+        if (ids[(size_t)part * part_stride + (size_t)q * k] != NIL) heap[(size_t)(len++) * W] = (uint32_t)part * (uint32_t)k;
+    for (int i = len / 2 - 1; i >= 0; --i) sift_down(i, len);
+    int c = 0;
+    for (; c < k && len > 0; ++c) {
+        uint32_t top = heap[0];
+        size_t s = src(top), dst = (size_t)q * k + c;
+        out_ids[dst] = ids[s];
+        out_scores[dst] = scores[s];
+        if (out_part) out_part[dst] = (int)(top / (uint32_t)k);
+        if (top % (uint32_t)k + 1 < (uint32_t)k && ids[s + 1] != NIL) heap[0] = top + 1;
+        else heap[0] = heap[(size_t)(--len) * W];
+        sift_down(0, len);
+    }
+    for (int i = c; i < k; ++i) {
+        size_t dst = (size_t)q * k + i;
+        out_ids[dst] = NIL; out_scores[dst] = 0.0f;
+        if (out_part) out_part[dst] = -1;
+    }
+    if (out_counts) out_counts[q] = c;
 }
 
 __global__ void shard_count_kernel(const uint32_t* __restrict__ ids, int nq, int k, int* __restrict__ out_counts) {

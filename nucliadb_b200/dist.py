@@ -1,7 +1,11 @@
 """Multi-GPU search: one process per GPU, segments sharded across ranks, per-rank partial top-k
-exchanged with ``all_gather`` (NCCL over NVLink on the GPU box, gloo in the CPU tests) and merged by
-``parts_merge_kernel`` -- the GPU-native form of the reference's gRPC scatter-gather + k-way merge
-(nidx/src/searcher/grpc.rs:253-431, shard_merge.rs:332-348 / 177-207).
+exchanged with ``all_gather`` (NCCL over NVLink on the GPU box, gloo in the CPU tests) and merged on the device
+-- the GPU-native form of the reference's gRPC scatter-gather + k-way merge (nidx/src/searcher/grpc.rs:253-431,
+shard_merge.rs:332-348 / 177-231).  Vectors merge by ``kmerge_parts_kernel`` (merge_vector_responses' kmerge_by(score >=)),
+text by ``parts_merge_kernel`` ((score desc, part asc, position asc): the parts are segments of one index).  Parts are
+taken in rank order, which stands for the order of the reference's ``responses`` vector; the reference itself groups
+responses by node (grpc.rs:253-285), so it fixes no order across nodes: what the merge pins is kmerge_by's output for a
+given order.
 
 The exchange is [nq, k] (u32 id, f32 score) per rank = 8*nq*k bytes (80 KB at nq=1024, k=10): latency
 bound, so it is one collective per batch, not per query.
@@ -33,7 +37,7 @@ def global_ids(local_ids, part, vectors_per_rank: int):
 class ShardedSearcher:
     """One rank's view of a segment-sharded index.  Buffers are allocated once: the local result is written
     straight into this rank's slot of the exchange buffer ([2, nq, k]: ids, score bits), ONE all_gather moves
-    every rank's slot, and parts_merge_kernel merges the gathered buffer in place (part_stride = 2*nq*k).
+    every rank's slot, and kmerge_parts_kernel merges the gathered buffer in place (part_stride = 2*nq*k).
 
     ``search`` does the three steps back to back.  ``submit`` / ``collect`` pipeline them over `depth` buffer sets:
     the all_gather of batch i runs on the process group's own stream while batch i+1 is being searched on the
@@ -71,10 +75,10 @@ class ShardedSearcher:
     def _merge_device(self, slot):
         import torch
 
-        from .segment import merge_topk
+        from .segment import merge_vector_parts
 
         g = slot["gathered"]
-        return merge_topk(g[:, 0], g[:, 1].view(torch.float32), device=self.device, part_stride=2 * self.nq * self.k, out=slot["out"])
+        return merge_vector_parts(g[:, 0], g[:, 1].view(torch.float32), device=self.device, part_stride=2 * self.nq * self.k, out=slot["out"])
 
     # -- pipeline -----------------------------------------------------------------------------------------------
     def submit(self, queries, ef, **kw):
@@ -106,6 +110,61 @@ class ShardedSearcher:
         return self.collect()
 
 
+def shard_record(segment, queries, k, rank=0, dedup=False, ef=0, min_score=-1.0, with_duplicates=True, method=None, filter_bits=None, out=None):
+    """nidx_vec_shard_record: search `segment` into one exchange record -> a torch int32 tensor of 2*nq*k words ([ids][score
+    bits]; 6*nq*k with dedup: + [par_key u64][vec_key u64]) on the segment's GPU, asynchronous on the current stream.  numpy
+    queries / filter bits are host memory, torch CUDA tensors device memory."""
+    import ctypes as C
+
+    import numpy as np
+    import torch
+
+    from . import _lib
+    from .segment import _is_torch, _torch_stream
+
+    dev = segment.cfg.device
+    p = _lib.VecSearchParams(k, ef, min_score, int(with_duplicates), _lib.NIDX_METHOD_AUTO if method is None else method, None, 0)
+    if _is_torch(queries):
+        mem = _lib.NIDX_MEM_DEVICE
+        if filter_bits is not None:
+            p.filter_bits = filter_bits.data_ptr()
+    else:
+        mem = _lib.NIDX_MEM_HOST
+        queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
+        if filter_bits is not None:
+            filter_bits = np.ascontiguousarray(filter_bits, dtype=np.uint64)
+            p.filter_bits = filter_bits.ctypes.data
+    nq, ldq = queries.shape
+    if out is None:
+        out = torch.empty(nq * k * (6 if dedup else 2), dtype=torch.int32, device=torch.device("cuda", dev))
+    _lib.check(_lib.load().nidx_vec_shard_record(segment._h, _lib.ptr(queries), C.c_int32(nq), C.c_int32(ldq), mem, C.byref(p), C.c_int32(rank),
+                                                 C.c_int32(int(dedup)), _lib.ptr(out), _torch_stream(dev)))
+    return out
+
+
+def shard_merge(records, n_parts, nq, k, dedup=False, with_duplicates=True, device=0, host=False):
+    """nidx_shard_merge over n_parts records laid end to end in one torch CUDA tensor -> (ids local to their part, scores, part,
+    counts): torch tensors on the device (asynchronous on the current stream), or numpy arrays with host=True."""
+    import ctypes as C
+
+    import numpy as np
+    import torch
+
+    from . import _lib
+    from .segment import _torch_stream
+
+    if host:
+        out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty((nq, k), dtype=np.int32), np.empty(nq, dtype=np.int32))
+    else:
+        dev = records.device
+        out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
+               torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int32, device=dev))
+    _lib.check(_lib.load().nidx_shard_merge(C.c_int32(device), _lib.ptr(records), C.c_int32(n_parts), C.c_int32(nq), C.c_int32(k), C.c_int32(int(dedup)),
+                                            C.c_int32(int(with_duplicates)), _lib.NIDX_MEM_HOST if host else _lib.NIDX_MEM_DEVICE,
+                                            _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]), _torch_stream(device)))
+    return out
+
+
 def docaddr(local_docs, part):
     """nidx_paragraph reader.rs:310 / nidx_text reader.rs: docaddr = (segment_ord << 32) + doc; NIL stays -1."""
     import torch
@@ -118,9 +177,18 @@ class ShardedTextSearcher(ShardedSearcher):
     """BM25 over a doc-partitioned index: every rank holds the postings of its own documents (one tantivy segment per rank in
     the reference's terms) scored with the statistics of the WHOLE index (`TextSegment.set_stats`; tantivy computes N, df and
     the average length over the union of segments, nidx_tantivy/src/index_reader.rs:39-77).  Per batch: local top-k + local
-    `Count` -> one all_gather of the [2, nq, k] (doc, score bits) partials + one all_reduce of the [nq] counts -> the same
-    merge kernel as the vector path, which ranks (score desc, part asc, position asc) = merge_document_responses' comparator
-    (bm25 desc, shard, lower docaddr first; shard_merge.rs:227-231) because every part arrives sorted (score desc, doc asc)."""
+    `Count` -> one all_gather of the [2, nq, k] (doc, score bits) partials + one all_reduce of the [nq] counts -> the text
+    merge (nidx_merge_topk), which ranks (score desc, part asc, position asc).  The parts are segments of one index, so part
+    ascending is docaddr ascending (docaddr = segment << 32 | doc) and this is merge_document_responses' order within one
+    shard (bm25 desc, lower docaddr first; shard_merge.rs:211-231) because every part arrives sorted (score desc, doc asc)."""
+
+    def _merge_device(self, slot):
+        import torch
+
+        from .segment import merge_topk
+
+        g = slot["gathered"]
+        return merge_topk(g[:, 0], g[:, 1].view(torch.float32), device=self.device, part_stride=2 * self.nq * self.k, out=slot["out"])
 
     def __init__(self, segment, nq, k, device, group=None, depth=2, local_search=None, merge=None):
         import torch

@@ -204,18 +204,29 @@ class VectorSegment:
         return dict(survivors=out[0], full_scans=out[1])
 
 
-def merge_topk(ids, scores, device=0, part_stride=0, out=None):
-    """[n_parts, nq, k] torch CUDA tensors (each part sorted desc, NIL padded) -> merged (ids, scores, part).
-    ids / scores may be strided views of one all-gather buffer: part_stride = elements between parts."""
+def _merge_parts(entry, ids, scores, device, part_stride, out):
     import torch
 
     n_parts, nq, k = ids.shape
     if out is None:
         out = (torch.empty((nq, k), dtype=ids.dtype, device=ids.device), torch.empty((nq, k), dtype=torch.float32, device=ids.device),
                torch.empty((nq, k), dtype=torch.int32, device=ids.device))
-    check(_lib.load().nidx_merge_topk(C.c_int32(device), ptr(ids), ptr(scores), C.c_int32(n_parts), C.c_int64(part_stride), C.c_int32(nq), C.c_int32(k),
+    check(getattr(_lib.load(), entry)(C.c_int32(device), ptr(ids), ptr(scores), C.c_int32(n_parts), C.c_int64(part_stride), C.c_int32(nq), C.c_int32(k),
                                       ptr(out[0]), ptr(out[1]), ptr(out[2]), _torch_stream(device)))
     return out
+
+
+def merge_topk(ids, scores, device=0, part_stride=0, out=None):
+    """The text merge (nidx_merge_topk): [n_parts, nq, k] torch CUDA tensors (each part sorted desc, NIL padded) -> merged
+    (ids, scores, part) ranked (score desc, part asc, position asc).  ids / scores may be strided views of one all-gather buffer:
+    part_stride = elements between parts."""
+    return _merge_parts("nidx_merge_topk", ids, scores, device, part_stride, out)
+
+
+def merge_vector_parts(ids, scores, device=0, part_stride=0, out=None):
+    """The vector merge (nidx_merge_vector_parts): merge_vector_responses' kmerge_by(score >=) over the parts in the order given,
+    same arguments and results as merge_topk."""
+    return _merge_parts("nidx_merge_vector_parts", ids, scores, device, part_stride, out)
 
 
 def _pack_keys(keys):

@@ -29,6 +29,7 @@ def main():
     import torch.distributed as dist
 
     import oracle as O
+    from merge_model import merge_vector_responses
     from nucliadb_b200 import _lib
     from nucliadb_b200.dist import ShardComm
     from nucliadb_b200.segment import TextSegment, VectorSegment
@@ -61,11 +62,11 @@ def main():
         segs.append(s)
     local_res = [s.search(q, k, ef=64, method=_lib.NIDX_METHOD_HNSW) for s in segs]
 
-    # ---- dedup = 0: merge_vector_responses (kmerge by score; ties: lower part first) ----
+    # ---- dedup = 0: merge_vector_responses (kmerge_by(score >=) over the parts in rank order; ties as itertools' heap orders them) ----
     ids, sc, part, cnt = comm.search_vectors(segs[rank], q, k, ef=64, dedup=False)
     for i in range(nq):
-        cand = sorted(((-float(local_res[r][1][i, j]), r, j) for r in range(world) for j in range(int(local_res[r][2][i]))))[:k]
-        exp = [(r, int(local_res[r][0][i, j]), -ns) for ns, r, j in cand]
+        cand = merge_vector_responses([local_res[r][1][i, :int(local_res[r][2][i])].tolist() for r in range(world)], k)
+        exp = [(r, int(local_res[r][0][i, j]), float(local_res[r][1][i, j])) for r, j in cand]
         got = [(int(part[i, j]), int(ids[i, j]), float(sc[i, j])) for j in range(int(cnt[i]))]
         assert got == exp, (rank, i, got, exp)
     # ---- dedup = 1: Fssc, with and without byte-identical suppression; device and host paths ----

@@ -1,6 +1,6 @@
 """The N>1 exchange path on CPU: world_size 2 over gloo.  Checks the all_gather plumbing and the global
-id mapping of nucliadb_b200.dist against a numpy restatement of shard_merge.rs:332-348 (the CUDA merge
-kernel itself is covered by the gpu tests)."""
+id mapping of nucliadb_b200.dist against the host model of shard_merge.rs:332-348 (tests/merge_model.py; the CUDA
+merge kernels themselves are covered by the gpu tests)."""
 import os
 import socket
 
@@ -9,6 +9,7 @@ import pytest
 import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
+from merge_model import merge_vector_responses
 
 
 def _free_port():
@@ -31,12 +32,12 @@ def _worker(rank, world, port, out_dir):
     ids = rng.integers(0, 1000, (nq, k)).astype(np.int32)
     ids_all, sc_all = gather_partials(torch.from_numpy(ids), torch.from_numpy(scores))
     assert ids_all.shape == (world, nq, k)
-    # numpy restatement of merge_vector_responses: kmerge_by(score >=) of per-rank lists, take k
+    # merge_vector_responses: kmerge_by(score >=) of per-rank lists in rank order, take k
     merged_ids, merged_part = [], []
     for q in range(nq):
-        items = sorted(((-float(sc_all[r, q, j]), r, j) for r in range(world) for j in range(k)))[:k]
-        merged_ids.append([int(ids_all[r, q, j]) for _, r, j in items])
-        merged_part.append([r for _, r, j in items])
+        items = merge_vector_responses([sc_all[r, q].tolist() for r in range(world)], k)
+        merged_ids.append([int(ids_all[r, q, j]) for r, j in items])
+        merged_part.append([r for r, j in items])
     g = global_ids(torch.tensor(merged_ids, dtype=torch.int32), torch.tensor(merged_part, dtype=torch.int32), 1000)
     np.save(os.path.join(out_dir, f"r{rank}.npy"), g.numpy())
     dist.barrier()
@@ -51,8 +52,22 @@ def test_world_size_2_gather_and_global_ids(tmp_path):
     assert ((a >= 0) & (a < 2000)).all() and (a >= 1000).any() and (a < 1000).any()
 
 
-def _np_merge(slot, nq, k):
-    """shard_merge.rs:332-348 on the gathered exchange buffer [world, 2, nq, k] (ids, score bits): k-way merge by score >=."""
+def _vector_merge(slot, nq, k):
+    """merge_vector_responses (shard_merge.rs:332-348) on the gathered exchange buffer [world, 2, nq, k] (ids, score bits)."""
+    g = slot["gathered"].numpy()
+    ids, sc = g[:, 0], g[:, 1].view(np.float32)
+    out_ids = np.empty((nq, k), dtype=np.int32)
+    out_part = np.empty((nq, k), dtype=np.int32)
+    for q in range(nq):
+        items = merge_vector_responses([sc[r, q].tolist() for r in range(g.shape[0])], k)
+        out_ids[q] = [ids[r, q, j] for r, j in items]
+        out_part[q] = [r for r, j in items]
+    return out_ids, out_part
+
+
+def _text_merge(slot, nq, k):
+    """The text merge (nidx_merge_topk) on the gathered buffer: (score desc, part asc, position asc) -- the parts are segments of
+    one index, so part order is docaddr order."""
     g = slot["gathered"].numpy()
     ids, sc = g[:, 0], g[:, 1].view(np.float32)
     out_ids = np.empty((nq, k), dtype=np.int32)
@@ -78,7 +93,7 @@ def _pipeline_worker(rank, world, port, out_dir):
         slot["local"][0].copy_(torch.from_numpy(rng.integers(0, 1000, (nq, k)).astype(np.int32)))
         slot["local"][1].copy_(torch.from_numpy(sc.view(np.int32)))
 
-    s = ShardedSearcher(None, nq, k, "cpu", local_search=local_search, merge=lambda slot: _np_merge(slot, nq, k))
+    s = ShardedSearcher(None, nq, k, "cpu", local_search=local_search, merge=lambda slot: _vector_merge(slot, nq, k))
     sequential = [s.search(b, 0) for b in range(n_batches)]
     pipelined = []
     for b in range(n_batches):                  # two batches in flight: exchange of b overlaps the search of b + 1
@@ -123,7 +138,7 @@ def _text_worker(rank, world, port, out_dir):
         slot["local"][1].copy_(torch.from_numpy(sc.view(np.int32)))
         slot["total"].copy_(torch.full((nq,), 10 + rank, dtype=torch.int64))
 
-    s = ShardedTextSearcher(None, nq, k, "cpu", local_search=local_search, merge=lambda slot: _np_merge(slot, nq, k))
+    s = ShardedTextSearcher(None, nq, k, "cpu", local_search=local_search, merge=lambda slot: _text_merge(slot, nq, k))
     docs, part, total = s.search(0, None)
     assert (total == 10 + 11).all()                                   # Count collector: summed over the parts
     g = s.slots[0]["gathered"].numpy()

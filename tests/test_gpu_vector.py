@@ -127,7 +127,9 @@ def test_gpu_build_equals_oracle_batch_build():
 
 
 def test_parts_merge_matches_kmerge():
-    """shard_merge.rs:332-348: kmerge_by(score >=) of per-part sorted lists, take k (ties: lower part first)."""
+    """The text merge (nidx_merge_topk): per-part sorted lists of the segments of one index merged (score desc, part asc,
+    position asc), take k -- part order is docaddr order there.  The vector merge, whose ties follow kmerge_by's heap instead,
+    is tested in test_gpu_shard_merge.py."""
     import torch
 
     from nucliadb_b200.segment import merge_topk
