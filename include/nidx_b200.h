@@ -206,9 +206,10 @@ int nidx_merge_topk(int32_t device, const uint32_t* ids, const float* scores, in
 int nidx_merge_vector_parts(int32_t device, const uint32_t* ids, const float* scores, int32_t n_parts, int64_t part_stride, int32_t nq, int32_t k,
                             uint32_t* out_ids, float* out_scores, int32_t* out_part, void* stream);
 
-/* Counters of the last HNSW search / build on this segment (0 after an exhaustive f32 scan; for the roofline accounting,
- * SURVEY 8d): [0] similarity evaluations, [1] node expansions, [2] visited-set overflows.  Every search call counts into its
- * own workspace, so concurrent searches never mix their counts; "last" = the call that was issued last. */
+/* Counters of the last HNSW search / build on this segment (for the roofline accounting, SURVEY 8d): [0] similarity
+ * evaluations, [1] node expansions, [2] visited-set overflows.  Every search call resets them, whatever its method, so they are
+ * 0 after a search that does not walk the graph (a scan, an empty segment, nothing matching).  Every search call counts into
+ * its own workspace, so concurrent searches never mix their counts; "last" = the call that was issued last. */
 int nidx_vec_counters(nidx_vec_segment* seg, uint64_t out[3]);
 /* The same with the quantised walk's: [0] exact similarities computed, [1] expansions, [2] visited-set overflows, [3] closest_up
  * overflows, [4] RaBitQ estimates, [5] exact similarities the sequential rerank_top needed (<= the share of [0] spent there). */

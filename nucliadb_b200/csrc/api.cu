@@ -69,21 +69,18 @@ struct DevBuf {
         return 0;
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    ~DevBuf() { release(); }
     template <class T> T* as() { return reinterpret_cast<T*>(p); }
 };
 #define ENSURE(buf, bytes) do { int r__ = (buf).ensure(bytes); if (r__) return r__; } while (0)
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
-    DevBuf queries, qnorms, out_ids, out_scores, out_counts, scores, partial, filter, misc, sched, facets;
+    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets;
     cudaEvent_t done = nullptr;
     cudaStream_t last_stream = nullptr;
     bool busy = false;
-    ~Workspace() {
-        queries.release(); qnorms.release(); out_ids.release(); out_scores.release(); out_counts.release();
-        scores.release(); partial.release(); filter.release(); misc.release(); sched.release(); facets.release();
-        if (done) cudaEventDestroy(done);
-    }
+    ~Workspace() { if (done) cudaEventDestroy(done); }
 };
 
 struct WorkspacePool {
@@ -126,6 +123,61 @@ struct WsGuard {
     WorkspacePool& pool; Workspace* w; cudaStream_t s;
     WsGuard(WorkspacePool& p, cudaStream_t st) : pool(p), w(p.acquire(st)), s(st) {}
     ~WsGuard() { pool.release(w, s); }
+};
+
+// Workspaces of the calls that belong to no segment, per device
+static WorkspacePool* plan_pool(int device) {
+    static std::mutex mu;
+    static WorkspacePool* pools[64] = {nullptr};
+    std::lock_guard<std::mutex> g(mu);
+    if (device < 0 || device >= 64) return nullptr;
+    if (!pools[device]) pools[device] = new WorkspacePool();
+    return pools[device];
+}
+
+// The `mem` contract of include/nidx_b200.h for one call.  in() and out() hand out a device pointer for each caller buffer: the
+// caller's own on the device path, else a 16-byte-aligned slice of one staging buffer that place() lays out (uploading the host
+// inputs) and finish() copies back (then synchronises the stream, once).  A NULL output gets a scratch slice that is never copied
+// back; a NULL input stays NULL.  Inputs and outputs may lie on different sides (host queries, device outputs).  On the device path
+// nothing is copied, set or synchronised here.
+struct Stage {
+    cudaStream_t stream;
+    bool qhost, ohost;
+    struct Slot { void* var; const void* in; void* out; size_t bytes; void* dev; };   // var: the caller's T* to point at the slice
+    std::vector<Slot> slots;
+    size_t total = 0;
+    Stage(cudaStream_t s, bool qh, bool oh) : stream(s), qhost(qh), ohost(oh) {}
+    void add(void* var, const void* in, void* out, size_t bytes) {
+        slots.push_back({var, in, out, bytes, nullptr});
+        total += (bytes + 15) / 16 * 16;
+    }
+    template <class T> void in(const T* src, size_t n, const T** dev) {
+        *dev = src;
+        if (qhost && src) add(dev, src, nullptr, n * sizeof(T));
+    }
+    template <class T> void out(T* dst, size_t n, T** dev) {
+        *dev = dst;
+        if (ohost || !dst) add(dev, nullptr, ohost ? dst : nullptr, n * sizeof(T));
+    }
+    int place(DevBuf& buf) {
+        ENSURE(buf, total);
+        unsigned char* p = buf.as<unsigned char>();
+        for (Slot& s : slots) {
+            s.dev = p;
+            p += (s.bytes + 15) / 16 * 16;
+            memcpy(s.var, &s.dev, sizeof(void*));
+            if (s.in && s.bytes) CU(cudaMemcpyAsync(s.dev, s.in, s.bytes, cudaMemcpyHostToDevice, stream));
+        }
+        return 0;
+    }
+    // sync: synchronise on the device path too (a call that reads a count back)
+    int finish(bool sync = false) {
+        if (ohost)
+            for (const Slot& s : slots)
+                if (s.out && s.bytes) CU(cudaMemcpyAsync(s.out, s.dev, s.bytes, cudaMemcpyDeviceToHost, stream));
+        if (ohost || sync) CU(cudaStreamSynchronize(stream));
+        return 0;
+    }
 };
 
 struct nidx_vec_segment {
@@ -344,6 +396,16 @@ static int make_row_tensor_map(CUtensorMap* map, const float* base, uint64_t row
     return 0;
 }
 
+// A per-row array the caller sets (n values from the host, into *dev, allocated on first use) or clears (host == NULL)
+template <class T>
+static int set_rows(int device, T** dev, const T* host, size_t n) {
+    CU(cudaSetDevice(device));
+    if (!host) { cudaFree(*dev); *dev = nullptr; return 0; }
+    if (!*dev) CU(cudaMalloc(dev, std::max<size_t>(n, 1) * sizeof(T)));
+    CU(cudaMemcpy(*dev, host, n * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+}
+
 extern "C" {
 
 const char* nidx_last_error(void) { return g_err.c_str(); }
@@ -445,6 +507,31 @@ static int new_segment(const nidx_vec_config* cfg, nidx_vec_segment** out) {
     return 0;
 }
 
+// The segment's n rows into d_vecs ([n][ld], zero padded).  Source rows are row_bytes apart and start with the d floats; `whole`:
+// they are [ld] floats already, copied as they are.
+static int upload_rows(nidx_vec_segment* s, const void* rows, size_t row_bytes, bool host, bool whole) {
+    const uint64_t n = s->n;
+    CU(cudaMalloc(&s->d_vecs, std::max<size_t>((size_t)n * s->ld * 4, 16)));
+    if (n == 0) return 0;
+    if (whole) {
+        CU(cudaMemcpy(s->d_vecs, rows, (size_t)n * row_bytes, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
+        return 0;
+    }
+    const unsigned char* src = static_cast<const unsigned char*>(rows);
+    void* staged = nullptr;
+    if (host) {
+        CU(cudaMalloc(&staged, (size_t)n * row_bytes));
+        CU(cudaMemcpy(staged, rows, (size_t)n * row_bytes, cudaMemcpyHostToDevice));
+        src = static_cast<const unsigned char*>(staged);
+    }
+    pad_rows_kernel<<<s->sm_count * 8, 256>>>(src, row_bytes, s->d, s->d_vecs, s->ld, n);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaDeviceSynchronize());
+    if (staged) cudaFree(staged);
+    return 0;
+}
+
 int nidx_vec_create(const nidx_vec_config* cfg, const float* vectors, uint64_t n, int32_t ld, int mem, const uint32_t* paragraph_of,
                     nidx_vec_segment** out) {
     nidx_vec_segment* s = nullptr;
@@ -453,29 +540,7 @@ int nidx_vec_create(const nidx_vec_config* cfg, const float* vectors, uint64_t n
     if (n >= (1ull << 31)) { delete s; return fail(NIDX_EINVAL, "at most 2^31-1 vectors per segment"); }
     if (ld < s->d) { delete s; return fail(NIDX_EINVAL, "ld %d < dimension %d (VectorErr::InconsistentDimensions)", ld, s->d); }
     s->n = n;
-    r = [&]() -> int {
-        CU(cudaMalloc(&s->d_vecs, std::max<size_t>((size_t)n * s->ld * 4, 16)));
-        if (n == 0) return 0;
-        if (mem == NIDX_MEM_HOST && ld == s->ld) {
-            CU(cudaMemcpy(s->d_vecs, vectors, (size_t)n * ld * 4, cudaMemcpyHostToDevice));
-        } else if (mem == NIDX_MEM_DEVICE && ld == s->ld) {
-            CU(cudaMemcpy(s->d_vecs, vectors, (size_t)n * ld * 4, cudaMemcpyDeviceToDevice));
-        } else {
-            const unsigned char* src = reinterpret_cast<const unsigned char*>(vectors);
-            void* staged = nullptr;
-            if (mem == NIDX_MEM_HOST) {
-                CU(cudaMalloc(&staged, (size_t)n * ld * 4));
-                CU(cudaMemcpy(staged, vectors, (size_t)n * ld * 4, cudaMemcpyHostToDevice));
-                src = reinterpret_cast<const unsigned char*>(staged);
-            }
-            pad_rows_kernel<<<s->sm_count * 8, 256>>>(src, (size_t)ld * 4, s->d, s->d_vecs, s->ld, n);
-            LAUNCHED();
-            CU(cudaGetLastError());
-            CU(cudaDeviceSynchronize());
-            if (staged) cudaFree(staged);
-        }
-        return 0;
-    }();
+    r = upload_rows(s, vectors, (size_t)ld * 4, mem == NIDX_MEM_HOST, ld == s->ld);
     if (!r) r = finish_create(s, paragraph_of);
     if (r) { nidx_vec_close(s); return r; }
     *out = s;
@@ -506,12 +571,11 @@ __global__ void __launch_bounds__(NRM_WARPS * 32) normalize_rows_kernel(float* _
 }
 
 int nidx_normalize_vectors(int32_t device, float* vectors, uint64_t n, int32_t d, int32_t ld, int mem, void* stream_) {
-    int dc = 0;
-    if (cudaGetDeviceCount(&dc) != cudaSuccess || dc == 0) return fail(NIDX_ENODEVICE, "no CUDA device (there is no CPU fallback)");
+    int r = check_device(device);
+    if (r) return r;
     if (d <= 0 || ld < d || !vectors) return fail(NIDX_EINVAL, "normalize: d %d, ld %d", d, ld);
     if ((size_t)d * 4 * NRM_WARPS > 200 * 1024) return fail(NIDX_EINVAL, "normalize: dimension %d too large", d);
     if (n == 0) return 0;
-    CU(cudaSetDevice(device));
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
     float* dv = vectors;
     void* staged = nullptr;
@@ -625,45 +689,21 @@ int nidx_vec_get_graph(const nidx_vec_segment* s, uint8_t* level, uint32_t* adj0
     return 0;
 }
 
-int nidx_vec_counters_ex(nidx_vec_segment* s, uint64_t out[6]) {
+// The counters of the last search call (of the last build before any search) into out: out[i] = h[pick[i]] of the eight, the
+// visited-set and closest_up overflows (h[2] + h[3]) where pick[i] is -1
+static int read_counters(nidx_vec_segment* s, uint64_t* out, std::initializer_list<int> pick) {
     if (!s || !out) return fail(NIDX_EINVAL, "null argument");
     CU(cudaSetDevice(s->cfg.device));
     unsigned long long h[8];
     unsigned long long* src = s->last_counters.load();
     CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
-    for (int i = 0; i < 6; ++i) out[i] = h[i];
+    for (int i : pick) *out++ = i < 0 ? h[2] + h[3] : h[i];
     return 0;
 }
-
-int nidx_vec_counters(nidx_vec_segment* s, uint64_t out[3]) {
-    if (!s) return fail(NIDX_EINVAL, "null segment");
-    CU(cudaSetDevice(s->cfg.device));
-    unsigned long long h[4];
-    unsigned long long* src = s->last_counters.load();
-    CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
-    out[0] = h[0]; out[1] = h[1]; out[2] = h[2] + h[3];
-    return 0;
-}
-
-int nidx_vec_exact_rows(nidx_vec_segment* s, uint64_t* out) {
-    if (!s || !out) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(s->cfg.device));
-    unsigned long long h[8];
-    unsigned long long* src = s->last_counters.load();
-    CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
-    *out = h[6];
-    return 0;
-}
-
-int nidx_vec_scan_counters(nidx_vec_segment* s, uint64_t out[2]) {
-    if (!s || !out) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(s->cfg.device));
-    unsigned long long h[8];
-    unsigned long long* src = s->last_counters.load();
-    CU(cudaMemcpy(h, src ? src : s->d_counters, sizeof(h), cudaMemcpyDeviceToHost));
-    out[0] = h[6]; out[1] = h[7];
-    return 0;
-}
+int nidx_vec_counters_ex(nidx_vec_segment* s, uint64_t out[6]) { return read_counters(s, out, {0, 1, 2, 3, 4, 5}); }
+int nidx_vec_counters(nidx_vec_segment* s, uint64_t out[3]) { return read_counters(s, out, {0, 1, -1}); }
+int nidx_vec_exact_rows(nidx_vec_segment* s, uint64_t* out) { return read_counters(s, out, {6}); }
+int nidx_vec_scan_counters(nidx_vec_segment* s, uint64_t out[2]) { return read_counters(s, out, {6, 7}); }
 
 // ---- RaBitQ --------------------------------------------------------------------------------------
 static int rabitq_check(const nidx_vec_segment* s) {
@@ -698,30 +738,39 @@ int nidx_vec_rabitq_codes(const nidx_vec_segment* s, uint8_t* out) {
     return 0;
 }
 
-// queries -> padded device copy + RaBitQ planes/params in the workspace; returns device pointers
-static int rabitq_prepare_queries(nidx_vec_segment* s, Workspace& w, const float* queries, int nq, int ldq, bool host, cudaStream_t stream, float** dq_out,
-                                  uint32_t** planes_out, RabitqQueryParams** params_out) {
+// What the RaBitQ scan and the quantised walk need of the segment
+static int rabitq_ready(const nidx_vec_segment* s) {
+    int r = rabitq_check(s);
+    if (r) return r;
+    if (!s->d_quant) return fail(NIDX_ESTATE, "segment has no RaBitQ codes (call nidx_vec_rabitq_encode)");
+    return 0;
+}
+
+// The queries as [nq][ld] zero-padded rows on the device.  `queries` is device memory: the caller's, or (staged) the call's own
+// copy of host rows, which is used as it is when it needs no padding.
+static int upload_queries(nidx_vec_segment* s, Workspace& w, const float* queries, int nq, int ldq, bool staged, cudaStream_t stream, const float** dq) {
+    *dq = queries;
+    if (ldq == s->ld && staged) return 0;
     ENSURE(w.queries, (size_t)nq * s->ld * 4);
-    float* dq = w.queries.as<float>();
+    *dq = w.queries.as<float>();
     if (ldq == s->ld) {
-        CU(cudaMemcpyAsync(dq, queries, (size_t)nq * ldq * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, stream));
+        CU(cudaMemcpyAsync(w.queries.p, queries, (size_t)nq * ldq * 4, cudaMemcpyDeviceToDevice, stream));
     } else {
-        const unsigned char* src = reinterpret_cast<const unsigned char*>(queries);
-        if (host) {
-            ENSURE(w.misc, (size_t)nq * ldq * 4);
-            CU(cudaMemcpyAsync(w.misc.p, queries, (size_t)nq * ldq * 4, cudaMemcpyHostToDevice, stream));
-            src = w.misc.as<unsigned char>();
-        }
-        pad_rows_kernel<<<std::min(nq, 1024), 256, 0, stream>>>(src, (size_t)ldq * 4, s->d, dq, s->ld, (uint64_t)nq);
+        pad_rows_kernel<<<std::min(nq, 1024), 256, 0, stream>>>(reinterpret_cast<const unsigned char*>(queries), (size_t)ldq * 4, s->d, w.queries.as<float>(),
+                                                               s->ld, (uint64_t)nq);
         LAUNCHED();
     }
-    size_t plane_bytes = (size_t)nq * 4 * (s->d / 32) * 4;
-    ENSURE(w.qnorms, plane_bytes + (size_t)nq * sizeof(RabitqQueryParams) + 64);
-    uint32_t* planes = w.qnorms.as<uint32_t>();
-    RabitqQueryParams* params = reinterpret_cast<RabitqQueryParams*>(w.qnorms.as<unsigned char>() + ((plane_bytes + 15) / 16) * 16);
-    rabitq_query_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(dq, s->ld, s->d, nq, planes, params);
+    return 0;
+}
+
+// The RaBitQ query planes and parameters of the padded queries, in w.misc
+static int rabitq_query_planes(nidx_vec_segment* s, Workspace& w, const float* dq, int nq, cudaStream_t stream, uint32_t** planes, RabitqQueryParams** params) {
+    size_t plane_bytes = ((size_t)nq * 4 * (s->d / 32) * 4 + 15) / 16 * 16;
+    ENSURE(w.misc, plane_bytes + (size_t)nq * sizeof(RabitqQueryParams) + 64);
+    *planes = w.misc.as<uint32_t>();
+    *params = reinterpret_cast<RabitqQueryParams*>(w.misc.as<unsigned char>() + plane_bytes);
+    rabitq_query_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(dq, s->ld, s->d, nq, *planes, *params);
     LAUNCHED();
-    *dq_out = dq; *planes_out = planes; *params_out = params;
     return 0;
 }
 
@@ -733,26 +782,25 @@ int nidx_vec_rabitq_estimate(nidx_vec_segment* s, const float* queries, int32_t 
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     WsGuard g(s->pool, stream);
     Workspace& w = *g.w;
-    bool host = mem == NIDX_MEM_HOST;
-    float* dq; uint32_t* planes; RabitqQueryParams* params;
-    int r = rabitq_prepare_queries(s, w, queries, nq, ldq, host, stream, &dq, &planes, &params);
+    const bool host = mem == NIDX_MEM_HOST;
+    Stage st(stream, host, host);
+    const float* d_q;
+    float *d_est, *d_err;
+    st.in(queries, (size_t)nq * ldq, &d_q);
+    st.out(out_est, (size_t)nq * s->n, &d_est);
+    st.out(out_err, (size_t)nq * s->n, &d_err);
+    int r = st.place(w.stage);
+    const float* dq;
+    if (!r) r = upload_queries(s, w, d_q, nq, ldq, host, stream, &dq);
+    uint32_t* planes; RabitqQueryParams* params;
+    if (!r) r = rabitq_query_planes(s, w, dq, nq, stream, &planes, &params);
     if (r) return r;
-    float *d_est = out_est, *d_err = out_err;
-    if (host) {
-        ENSURE(w.scores, (size_t)nq * s->n * 8);
-        d_est = w.scores.as<float>(); d_err = d_est + (size_t)nq * s->n;
-    }
     if (s->n) {
         rabitq_estimate_kernel<<<dim3((unsigned)((s->n + 255) / 256), nq), 256, 0, stream>>>(s->d_quant, s->quant_stride, (uint32_t)s->n, s->d, planes, params, d_est, d_err);
         LAUNCHED();
         CU(cudaGetLastError());
     }
-    if (host) {
-        CU(cudaMemcpyAsync(out_est, d_est, (size_t)nq * s->n * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_err, d_err, (size_t)nq * s->n * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 int nidx_vec_last_kernel_ms(nidx_vec_segment* s, float* ms) {
@@ -983,8 +1031,44 @@ struct FilterEval {
     }
 };
 
+// The layout of w.filter: [words] filter ∧ alive | 8 words: its match count | [n_nodes + 1][words] a formula's node bitsets | the
+// formula's posting ranges (range_bytes).  Sized for a formula of n_nodes nodes (0: none).
+struct FilterBufs {
+    size_t words;
+    uint64_t* bits;
+    unsigned long long* count;
+    uint64_t* nodes;
+    uint64_t* ranges;
+};
+static int filter_bufs(const nidx_vec_segment* s, Workspace& w, int n_nodes, size_t range_bytes, FilterBufs& f) {
+    f.words = ((size_t)s->n_par + 63) / 64;
+    const size_t node_words = n_nodes ? ((size_t)n_nodes + 1) * f.words : 0;
+    ENSURE(w.filter, (f.words + 8 + node_words) * 8 + range_bytes);
+    f.bits = w.filter.as<uint64_t>();
+    f.count = reinterpret_cast<unsigned long long*>(f.bits + f.words);
+    f.nodes = f.bits + f.words + 8;
+    f.ranges = f.nodes + node_words;
+    return 0;
+}
+
+// filter ∧ alive (segment.rs:516-534) into `out` (NULL: the workspace's filter bits), returned in *bits.  With h_count, the number of
+// set bits is copied back to it (the caller synchronises).
+static int filter_and_alive(nidx_vec_segment* s, Workspace& w, const uint64_t* filter, uint64_t* out, unsigned long long* h_count, cudaStream_t stream,
+                            const uint64_t** bits) {
+    FilterBufs f;
+    int r = filter_bufs(s, w, 0, 0, f);
+    if (r) return r;
+    if (!out) out = f.bits;
+    CU(cudaMemsetAsync(f.count, 0, 8, stream));
+    and_bits_kernel<<<std::min<size_t>((f.words + 255) / 256, 1024), 256, 0, stream>>>(filter, s->d_alive, out, f.words, f.count);
+    LAUNCHED();
+    if (h_count) CU(cudaMemcpyAsync(h_count, f.count, 8, cudaMemcpyDeviceToHost, stream));
+    *bits = out;
+    return 0;
+}
+
 // ParagraphInvertedIndexes::filter on the device: nodes (pre-order; several top-level nodes are not allowed: wrap them in an AND /
-// OR node) -> bitset in `w.filter` (first `words` words), returns the device pointer in *out
+// OR node) -> bitset among the node buffers of `w.filter`, returns the device pointer in *out
 static int filter_formula_device(nidx_vec_segment* s, Workspace& w, const nidx_filter_node* nodes, int n_nodes, cudaStream_t stream, uint64_t** out) {
     if (!nodes || n_nodes <= 0) return fail(NIDX_EINVAL, "empty filter formula");
     size_t words = ((size_t)s->n_par + 63) / 64;
@@ -999,10 +1083,11 @@ static int filter_formula_device(nidx_vec_segment* s, Workspace& w, const nidx_f
     ev.atom_ranges.assign(n_nodes, {0, 0});
     if (ev.collect(0) != n_nodes) return fail(NIDX_EINVAL, "malformed filter formula (operand counts do not add up to %d nodes)", n_nodes);
     size_t range_bytes = ev.ranges.size() * 8;
-    ENSURE(w.filter, ((size_t)n_nodes + 3) * words * 8 + 64 + range_bytes + 64);
-    uint64_t* base = w.filter.as<uint64_t>();
-    ev.bufs = base + 2 * words + 8;          // the first 2 * words + 8 words are vec_search_impl's (filter AND alive, count)
-    ev.d_ranges = ev.bufs + ((size_t)n_nodes + 1) * words;
+    FilterBufs f;
+    int r = filter_bufs(s, w, n_nodes, range_bytes, f);
+    if (r) return r;
+    ev.bufs = f.nodes;
+    ev.d_ranges = f.ranges;
     if (range_bytes) CU(cudaMemcpyAsync(ev.d_ranges, ev.ranges.data(), range_bytes, cudaMemcpyHostToDevice, stream));
     int next = 0;
     uint64_t* res = ev.eval(0, &next);
@@ -1023,134 +1108,41 @@ static bool use_tc_filter(const nidx_vec_segment* s, int nq, int k) {
     return nq >= 64;
 }
 
-// The body of nidx_vec_search.  qhost: the queries (and filter bits) are host pointers; ohost: the outputs are host pointers
-// (copied back and the stream synchronised before returning).  The sharded entry point (shard.cuh) passes host queries with
-// device outputs: the partial results go straight into the exchange buffer.
-static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq, int32_t ldq, bool qhost, bool ohost, const nidx_vec_search_params* p,
-                           uint32_t* out_ids, float* out_scores, int32_t* out_counts, cudaStream_t stream, const nidx_filter_node* formula = nullptr,
-                           int32_t n_formula = 0) {
-    if (!s || !p || (!queries && nq > 0) || !out_ids || !out_scores) return fail(NIDX_EINVAL, "null argument");
-    if (nq <= 0) return 0;
-    if (ldq < s->d) return fail(NIDX_EINVAL, "query dimension %d != index dimension %d (VectorErr::InconsistentDimensions)", ldq, s->d);
-    int k = p->k;
-    if (k <= 0) return fail(NIDX_EINVAL, "k must be positive");
-    CU(cudaSetDevice(s->cfg.device));
-    WsGuard g(s->pool, stream);
-    Workspace& w = *g.w;
-    bool host = qhost;
-    VecDev V = s->vdev();
+// One vector search call as its method sees it: the padded queries and their norms, filter ∧ alive (NULL: every paragraph), the
+// outputs (device pointers) and this call's counters.
+struct VecCall {
+    nidx_vec_segment* s;
+    Workspace& w;
+    cudaStream_t stream;
+    const nidx_vec_search_params* p;
+    VecDev V;
+    int nq, k;
+    const float* dq;
+    float* qnorms;
+    const uint64_t* bits;
+    uint32_t* ids;
+    float* scores;
+    int* counts;
+    unsigned long long* counters;   // [8], zeroed for this call; the 64 bytes before them (w.sched) hold the kernels' work counter
 
-    // queries -> [nq][ld] zero padded on device, norms
-    ENSURE(w.queries, (size_t)nq * s->ld * 4);
-    ENSURE(w.qnorms, (size_t)nq * 4);
-    float* dq = w.queries.as<float>();
-    if (ldq == s->ld) {
-        CU(cudaMemcpyAsync(dq, queries, (size_t)nq * ldq * 4, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, stream));
-    } else {
-        const unsigned char* src = reinterpret_cast<const unsigned char*>(queries);
-        if (host) {
-            ENSURE(w.misc, (size_t)nq * ldq * 4);
-            CU(cudaMemcpyAsync(w.misc.p, queries, (size_t)nq * ldq * 4, cudaMemcpyHostToDevice, stream));
-            src = w.misc.as<unsigned char>();
-        }
-        pad_rows_kernel<<<std::min(nq, 1024), 256, 0, stream>>>(src, (size_t)ldq * 4, s->d, dq, s->ld, (uint64_t)nq);
-        LAUNCHED();
-    }
-    if (s->cfg.similarity != NIDX_SIM_DOT) {
-        row_norms_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(dq, s->ld, (uint64_t)nq, w.qnorms.as<float>());
-        LAUNCHED();
-    }
-
-    // filter ∧ alive (segment.rs:516-534)
-    const uint64_t* bits = s->d_alive;
-    size_t words = ((size_t)s->n_par + 63) / 64;
-    uint64_t matching = s->d_alive ? s->alive_count : s->n_par;
-    const bool filtered = p->filter_bits || formula;
-    if (filtered) {
-        const uint64_t* fsrc = p->filter_bits;
-        bool fhost = host;
-        if (formula) {   // the formula is evaluated on the device (inverted_index/paragraph.rs:124-186): no host bitset, no copy
-            uint64_t* fdev = nullptr;
-            int fr = filter_formula_device(s, w, formula, n_formula, stream, &fdev);
-            if (fr) return fr;
-            fsrc = fdev; fhost = false;
-        } else ENSURE(w.filter, words * 8 * 2 + 64);
-        uint64_t* d_in = w.filter.as<uint64_t>();
-        uint64_t* d_out = d_in + words;
-        unsigned long long* d_cnt = reinterpret_cast<unsigned long long*>(d_out + words);
-        if (fhost) { CU(cudaMemcpyAsync(d_in, p->filter_bits, words * 8, cudaMemcpyHostToDevice, stream)); fsrc = d_in; }
-        CU(cudaMemsetAsync(d_cnt, 0, 8, stream));
-        and_bits_kernel<<<std::min<size_t>((words + 255) / 256, 1024), 256, 0, stream>>>(fsrc, s->d_alive, d_out, words, d_cnt);
-        LAUNCHED();
-        bits = d_out;
-        matching = formula ? 0 : p->filter_matching;
-        if (matching == 0) {   // segment.rs:531: the reference counts the matches of every filtered request (8 bytes back, one sync)
-            unsigned long long h = 0;
-            CU(cudaMemcpyAsync(&h, d_cnt, 8, cudaMemcpyDeviceToHost, stream));
-            CU(cudaStreamSynchronize(stream));
-            matching = h;
-        }
-    }
-
-    if (matching == 0) {   // segment.rs:532-534: nothing can match (everything deleted / filtered out) -> empty, whatever the method
-        uint32_t* e_ids = out_ids; float* e_sc = out_scores; int* e_cnt = out_counts;
-        if (ohost) {
-            for (size_t i = 0; i < (size_t)nq * k; ++i) { e_ids[i] = NIDX_NIL; e_sc[i] = 0.0f; }
-            if (e_cnt) for (int i = 0; i < nq; ++i) e_cnt[i] = 0;
-            CU(cudaStreamSynchronize(stream));
-        } else {
-            CU(cudaMemsetAsync(e_ids, 0xFF, (size_t)nq * k * 4, stream));
-            CU(cudaMemsetAsync(e_sc, 0, (size_t)nq * k * 4, stream));
-            if (e_cnt) CU(cudaMemsetAsync(e_cnt, 0, (size_t)nq * 4, stream));
-        }
+    // Every id NIDX_NIL, every score and count 0
+    int write_empty() const {
+        CU(cudaMemsetAsync(ids, 0xFF, (size_t)nq * k * 4, stream));
+        CU(cudaMemsetAsync(scores, 0, (size_t)nq * k * 4, stream));
+        CU(cudaMemsetAsync(counts, 0, (size_t)nq * 4, stream));
         return 0;
     }
-    int method = p->method;
-    if (method == NIDX_METHOD_AUTO) {
-        if (!s->has_graph) method = NIDX_METHOD_BRUTE;
-        else if (matching == 0 && filtered) method = NIDX_METHOD_BRUTE;
-        else {
-            // a segment that carries codes is searched with a RaBitQ query on either path (segment.rs:506-513: `rabitq` =
-            // has_quantized): the quantised walk (hnsw/search.rs:332-366) or the quantised scan (segment.rs:581-608)
-            bool walk_ok = s->d_quant && s->cfg.similarity == NIDX_SIM_DOT;
-            bool scan_ok = walk_ok && !s->d_par_first && k <= 1024;
-            if (use_hnsw_cost(s->n_par, matching, (size_t)k, (size_t)s->cfg.m, walk_ok)) method = walk_ok ? NIDX_METHOD_HNSW_RABITQ : NIDX_METHOD_HNSW;
-            else method = scan_ok ? NIDX_METHOD_BRUTE_RABITQ : NIDX_METHOD_BRUTE;
-            // A walk keeps its list and visited set in shared memory: a very large top_k (the reference has no limit on it) does not
-            // fit one CTA.  AUTO then takes the exhaustive scan -- exact results -- instead of failing the request.
-            if (method == NIDX_METHOD_HNSW || method == NIDX_METHOD_HNSW_RABITQ) {
-                int last_k, list_cap, cu_cap, hash_bits;
-                size_t bytes;
-                bool fits = method == NIDX_METHOD_HNSW
-                                ? hnsw_search_smem(s, std::max(k, p->ef > 0 ? p->ef : s->cfg.ef_search), k, &list_cap, &cu_cap, &hash_bits, &bytes)
-                                : rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &bytes);
-                if (!fits && k <= 1024) method = NIDX_METHOD_BRUTE;
-            }
-        }
-    }
-    if ((method == NIDX_METHOD_HNSW || method == NIDX_METHOD_HNSW_RABITQ) && !s->has_graph) return fail(NIDX_ESTATE, "HNSW search requested but the segment has no graph");
 
-    // outputs
-    uint32_t* d_ids = out_ids; float* d_sc = out_scores; int* d_cnt = out_counts;
-    if (ohost || !out_counts) {
-        ENSURE(w.out_ids, (size_t)nq * k * 4);
-        ENSURE(w.out_scores, (size_t)nq * k * 4);
-        ENSURE(w.out_counts, (size_t)nq * 4);
-        if (ohost) { d_ids = w.out_ids.as<uint32_t>(); d_sc = w.out_scores.as<float>(); }
-        if (ohost || !out_counts) d_cnt = w.out_counts.as<int>();
-    }
-
-    if (method == NIDX_METHOD_BRUTE_RABITQ && s->n != 0) {
-        // segment.rs:581-608 with SearchVector::RabitQ: estimate every vector from its 1-bit code, keep upper_bound >= min_score,
-        // rerank_top with the raw vectors (sequential semantics preserved, see rabitq_rerank_kernel)
-        int rr = rabitq_check(s);
-        if (rr) return rr;
-        if (!s->d_quant) return fail(NIDX_ESTATE, "segment has no RaBitQ codes (call nidx_vec_rabitq_encode)");
+    // segment.rs:581-608 with SearchVector::RabitQ: estimate every vector from its 1-bit code, keep upper_bound >= min_score,
+    // rerank_top with the raw vectors (sequential semantics preserved, see rabitq_rerank_kernel)
+    int rabitq_scan() {
+        int r = rabitq_ready(s);
+        if (r) return r;
         if (s->d_par_first) return fail(NIDX_EINVAL, "RaBitQ scan of multi-vector paragraphs is not implemented");
         if (k > 1024) return fail(NIDX_EINVAL, "k above 1024 not supported");
-        uint32_t* planes; RabitqQueryParams* params; float* dq2;
-        rr = rabitq_prepare_queries(s, w, queries, nq, ldq, host, stream, &dq2, &planes, &params);
-        if (rr) return rr;
+        uint32_t* planes; RabitqQueryParams* params;
+        r = rabitq_query_planes(s, w, dq, nq, stream, &planes, &params);
+        if (r) return r;
         int qgroup = (int)std::max<size_t>(1, std::min<size_t>((size_t)nq, ((size_t)4 << 30) / ((size_t)s->n * 8)));
         ENSURE(w.scores, (size_t)qgroup * s->n * 8);
         size_t smem_rr = rr_smem_bytes(s->ld, k);
@@ -1160,21 +1152,21 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
             float* d_est = w.scores.as<float>();
             float* d_err = d_est + (size_t)nqg * s->n;
             if (q0 == 0) CU(cudaEventRecord(s->ev_k0, stream));
-            rabitq_estimate_kernel<<<dim3((unsigned)((s->n + 255) / 256), nqg), 256, 0, stream>>>(s->d_quant, s->quant_stride, (uint32_t)s->n, s->d,
-                                                                                                   planes + (size_t)q0 * 4 * (s->d / 32), params + q0, d_est, d_err);
+            const uint32_t* qplanes = planes + (size_t)q0 * 4 * (s->d / 32);
+            rabitq_estimate_kernel<<<dim3((unsigned)((s->n + 255) / 256), nqg), 256, 0, stream>>>(s->d_quant, s->quant_stride, (uint32_t)s->n, s->d, qplanes,
+                                                                                                     params + q0, d_est, d_err);
             if (q0 == 0) CU(cudaEventRecord(s->ev_k1, stream));
             LAUNCHED();
-            rabitq_rerank_kernel<<<nqg, RR_THREADS, smem_rr, stream>>>(V, dq2 + (size_t)q0 * s->ld, d_est, d_err, bits, p->min_score, k, d_ids + (size_t)q0 * k,
-                                                                       d_sc + (size_t)q0 * k, d_cnt + q0, nullptr);
+            rabitq_rerank_kernel<<<nqg, RR_THREADS, smem_rr, stream>>>(V, dq + (size_t)q0 * s->ld, d_est, d_err, bits, p->min_score, k,
+                                                                         ids + (size_t)q0 * k, scores + (size_t)q0 * k, counts + q0, nullptr);
             LAUNCHED();
         }
         CU(cudaGetLastError());
-    } else if (s->n == 0) {
-        CU(cudaMemsetAsync(d_ids, 0xFF, (size_t)nq * k * 4, stream));
-        CU(cudaMemsetAsync(d_sc, 0, (size_t)nq * k * 4, stream));
-        CU(cudaMemsetAsync(d_cnt, 0, (size_t)nq * 4, stream));
-    } else if (method == NIDX_METHOD_BRUTE && use_tc_filter(s, nq, k)) {
-        // large batch: TF32 tensor-core filter + bit-exact refine (scan_tc2.cuh); nothing of size [Q x N] touches HBM
+        return 0;
+    }
+
+    // Large batches: TF32 tensor-core filter + bit-exact refine (scan_tc2.cuh); nothing of size [Q x N] touches HBM
+    int tc_filter_scan() {
         int n_chunks = (int)((s->n + TC2_CHUNK - 1) / TC2_CHUNK), n_qblocks = (nq + TC2_M - 1) / TC2_M;
         {
             std::lock_guard<std::mutex> lk(s->map_mu);
@@ -1191,16 +1183,12 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         int slots = std::max(1, std::min(grid / n_qblocks, n_chunks));   // CTAs per query block; 1 when there are more blocks than CTAs
         size_t cand_n = (size_t)nq * slots * TC2_LISTS * TC2_L;
         ENSURE(w.scores, cand_n * 8 + 64);
-        ENSURE(w.sched, 128);
-        unsigned long long* call_counters = reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64);
         Tc2Args ta;
-        ta.nq = nq; ta.n_qblocks = n_qblocks; ta.n_chunks = n_chunks; ta.slots = slots; ta.qnorms = w.qnorms.as<float>(); ta.bits = bits;
+        ta.nq = nq; ta.n_qblocks = n_qblocks; ta.n_chunks = n_chunks; ta.slots = slots; ta.qnorms = qnorms; ta.bits = bits;
         ta.cand_score = w.scores.as<float>(); ta.cand_id = reinterpret_cast<uint32_t*>(w.scores.as<float>() + cand_n);
         ta.work_counter = w.sched.as<unsigned int>();
         CU(cudaFuncSetAttribute(scan_tc_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC2_SMEM_BYTES));
         grid = n_qblocks <= grid ? n_qblocks * slots : grid;
-        CU(cudaMemsetAsync(w.sched.p, 0, 128, stream));
-        s->last_counters.store(call_counters);
         CU(cudaEventRecord(s->ev_k0, stream));
         scan_tc_filter_kernel<<<grid, TC2_THREADS, TC2_SMEM_BYTES, stream>>>(map_q, s->map_v, V, ta);
         CU(cudaEventRecord(s->ev_k1, stream));
@@ -1208,15 +1196,16 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         int cap = topk_cap(k, 256);
         size_t smem_rf = tc2_refine_smem(s->ld, cap);
         if (smem_rf > 48 * 1024) CU(cudaFuncSetAttribute(scan_tc_refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rf));
-        scan_tc_refine_kernel<<<nq, 256, smem_rf, stream>>>(V, dq, w.qnorms.as<float>(), slots * TC2_LISTS, ta.cand_score, ta.cand_id, bits, s->max_norm, p->min_score, k, cap,
-                                                            d_ids, d_sc, d_cnt, call_counters + 6);
+        scan_tc_refine_kernel<<<nq, 256, smem_rf, stream>>>(V, dq, qnorms, slots * TC2_LISTS, ta.cand_score, ta.cand_id, bits, s->max_norm,
+                                                              p->min_score, k, cap, ids, scores, counts, counters + 6);
         LAUNCHED();
         CU(cudaGetLastError());
-    } else if (method == NIDX_METHOD_BRUTE) {
+        return 0;
+    }
+
+    // The exhaustive scan on the CUDA cores: score matrix per query group, per-chunk top-k, merge
+    int exact_scan() {
         if (k > 1024) return fail(NIDX_EINVAL, "brute-force k above 1024 not supported");
-        ENSURE(w.sched, 128);   // zero counters for this call: nidx_vec_scan_counters then reports that the filter did not run
-        CU(cudaMemsetAsync(w.sched.p, 0, 128, stream));
-        s->last_counters.store(reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64));
         int cap = topk_cap(k, 256);
         int n_chunks = (int)std::min<uint64_t>(std::max<uint64_t>(1, ((uint64_t)s->sm_count * 4 + nq - 1) / nq), (s->n_par + 4095) / 4096);
         n_chunks = std::max(n_chunks, 1);
@@ -1241,30 +1230,58 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
             uint64_t grid = n_vchunks * n_qtiles;
             if (grid > 0x7FFFFFFFull) return fail(NIDX_EINVAL, "scan grid too large");
             if (q0 == 0) CU(cudaEventRecord(s->ev_k0, stream));
-            scan_kern<<<(unsigned)grid, SCAN_WARPS * 32, smem_scan, stream>>>(V, dq + (size_t)q0 * s->ld, w.qnorms.as<float>() + q0, nqg, n_qtiles,
-                                                                                 w.scores.as<float>());
+            scan_kern<<<(unsigned)grid, SCAN_WARPS * 32, smem_scan, stream>>>(V, dq + (size_t)q0 * s->ld, qnorms + q0, nqg, n_qtiles, w.scores.as<float>());
             if (q0 == 0) CU(cudaEventRecord(s->ev_k1, stream));
             LAUNCHED();
-            scan_select_kernel<<<dim3(n_chunks, nqg), 256, (size_t)cap * 8, stream>>>(w.scores.as<float>(), (uint32_t)s->n, s->n_par, s->d_par_first, nullptr, bits,
-                                                                                      p->min_score, k, cap, n_chunks, w.partial.as<uint64_t>());
+            scan_select_kernel<<<dim3(n_chunks, nqg), 256, (size_t)cap * 8, stream>>>(w.scores.as<float>(), (uint32_t)s->n, s->n_par, s->d_par_first, nullptr,
+                                                                                        bits, p->min_score, k, cap, n_chunks, w.partial.as<uint64_t>());
             LAUNCHED();
-            topk_merge_kernel<<<nqg, 256, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), n_chunks * k, k, cap, d_ids + (size_t)q0 * k, d_sc + (size_t)q0 * k,
-                                                                    d_cnt + q0);
+            topk_merge_kernel<<<nqg, 256, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), n_chunks * k, k, cap, ids + (size_t)q0 * k,
+                                                                       scores + (size_t)q0 * k, counts + q0);
             LAUNCHED();
         }
         CU(cudaGetLastError());
-    } else if (method == NIDX_METHOD_HNSW_RABITQ) {
-        // hnsw/search.rs:306-383 with SearchVector::RabitQ: estimate-ranked walk, k * 100 layer-0 results, exact rerank + closest_up
-        int rr = rabitq_check(s);
-        if (rr) return rr;
-        if (!s->d_quant) return fail(NIDX_ESTATE, "segment has no RaBitQ codes (call nidx_vec_rabitq_encode)");
-        int nw = s->d / 32;
-        size_t plane_bytes = (size_t)nq * 4 * nw * 4;
-        ENSURE(w.misc, ((plane_bytes + 15) / 16) * 16 + (size_t)nq * sizeof(RabitqQueryParams) + 64);
-        uint32_t* planes = w.misc.as<uint32_t>();
-        RabitqQueryParams* params = reinterpret_cast<RabitqQueryParams*>(w.misc.as<unsigned char>() + ((plane_bytes + 15) / 16) * 16);
-        rabitq_query_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(dq, s->ld, s->d, nq, planes, params);
+        return 0;
+    }
+
+    // SearchArgs of a walk (mode 0) of this call
+    SearchArgs walk_args(int ef0, int list_cap, int cu_cap, int hash_bits) const {
+        SearchArgs a;
+        memset(&a, 0, sizeof(a));
+        a.mode = 0; a.nq = nq; a.queries = dq; a.qnorms = qnorms; a.k = k; a.ef0 = ef0; a.min_score = p->min_score;
+        a.with_duplicates = p->with_duplicates; a.multi_vector = s->cfg.multi_vector; a.filter = bits;
+        a.out_ids = ids; a.out_scores = scores; a.out_counts = counts;
+        a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = cu_cap;
+        a.work_counter = w.sched.as<unsigned int>();   // the scheduler counter lives in the workspace: concurrent calls must not share it
+        a.counters = counters;
+        return a;
+    }
+
+    // The grid of a walk: as many CTAs as are resident at once, at most one per query
+    int walk_grid(hs_kernel_t kern, int threads, size_t smem, int* grid) const {
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int occ = 0;
+        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
+        *grid = std::min(nq, std::max(1, occ) * s->sm_count);
+        return 0;
+    }
+
+    int launch_walk(hs_kernel_t kern, int grid, int threads, size_t smem, const VecDev& Vw, const SearchArgs& a) const {
+        CU(cudaEventRecord(s->ev_k0, stream));
+        kern<<<grid, threads, smem, stream>>>(Vw, s->gdev(), a);
+        CU(cudaEventRecord(s->ev_k1, stream));
         LAUNCHED();
+        CU(cudaGetLastError());
+        return 0;
+    }
+
+    // hnsw/search.rs:306-383 with SearchVector::RabitQ: estimate-ranked walk, k * 100 layer-0 results, exact rerank + closest_up
+    int quantised_walk() {
+        int r = rabitq_ready(s);
+        if (r) return r;
+        uint32_t* planes; RabitqQueryParams* params;
+        r = rabitq_query_planes(s, w, dq, nq, stream, &planes, &params);
+        if (r) return r;
         int last_k, cu_cap, list_cap, hash_bits;
         size_t smem;
         if (!rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &smem))
@@ -1275,80 +1292,132 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
         // 8 warps per query: 4 CTAs per SM; 4 warps: 7 per SM.  The 4-warp shape is taken when the batch does not fit one wave of the
         // 8-warp shape (NIDX_B200_RQ_W = 4 / 8 forces one).
         hs_kernel_t kern = pick_rabitq_walk_kernel(s->ld);
-        int threads = HS_THREADS;
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int occ = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
-        {
-            const char* ew = getenv("NIDX_B200_RQ_W");
-            int force = ew ? atoi(ew) : 0;
-            if (force == 4 || (force != 8 && nq > std::max(1, occ) * s->sm_count)) {
-                kern = pick_rabitq_walk_kernel_w4(s->ld);
-                threads = 128;
-                CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
-            }
+        int threads = HS_THREADS, grid = 0;
+        r = walk_grid(kern, threads, smem, &grid);
+        const char* ew = getenv("NIDX_B200_RQ_W");
+        const int force = ew ? atoi(ew) : 0;
+        if (!r && (force == 4 || (force != 8 && nq > grid))) {
+            kern = pick_rabitq_walk_kernel_w4(s->ld);
+            threads = 128;
+            r = walk_grid(kern, threads, smem, &grid);
         }
-        int grid = std::min(nq, std::max(1, occ) * s->sm_count);
+        if (r) return r;
         ENSURE(w.scores, ((size_t)grid << gv_bits) * 4);
-        SearchArgs a;
-        memset(&a, 0, sizeof(a));
-        a.mode = 0; a.nq = nq; a.queries = dq; a.qnorms = w.qnorms.as<float>(); a.k = k; a.ef0 = last_k; a.min_score = p->min_score;
-        a.with_duplicates = p->with_duplicates; a.multi_vector = s->cfg.multi_vector; a.filter = bits;
-        a.out_ids = d_ids; a.out_scores = d_sc; a.out_counts = d_cnt;
-        a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = cu_cap;
+        SearchArgs a = walk_args(last_k, list_cap, cu_cap, hash_bits);
         a.codes = s->d_quant; a.code_stride = s->quant_stride; a.planes = planes; a.qparams = params;
         a.gvisited = w.scores.as<uint32_t>(); a.gv_bits = gv_bits; a.last_k = last_k;
-        ENSURE(w.sched, 128);
-        a.work_counter = w.sched.as<unsigned int>();
-        a.counters = reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64);   // per call, in the call's workspace
-        CU(cudaMemsetAsync(a.work_counter, 0, 128, stream));
-        s->last_counters.store(a.counters);
-        CU(cudaEventRecord(s->ev_k0, stream));
-        kern<<<grid, threads, smem, stream>>>(V, s->gdev(), a);
-        CU(cudaEventRecord(s->ev_k1, stream));
-        LAUNCHED();
-        CU(cudaGetLastError());
-    } else {
+        return launch_walk(kern, grid, threads, smem, V, a);
+    }
+
+    // hnsw/search.rs:306-383 on the f32 vectors, screened on the fp16 copy when the segment has one
+    int dense_walk() {
         int ef = p->ef > 0 ? p->ef : s->cfg.ef_search;
         int ef0 = std::max(k, ef);  // search.rs:338-345
         int list_cap, cu_cap, hash_bits;
         size_t smem;
         if (!hnsw_search_smem(s, ef0, k, &list_cap, &cu_cap, &hash_bits, &smem))
             return fail(NIDX_EINVAL, "HNSW search needs %zu bytes of shared memory (ef=%d, k=%d, dim=%d): too large", smem, ef0, k, s->d);
-        int r = attach_half_copy(s, &V);
-        if (r) return r;
-        SearchArgs a;
-        memset(&a, 0, sizeof(a));
-        a.mode = 0; a.nq = nq; a.queries = dq; a.qnorms = w.qnorms.as<float>(); a.k = k; a.ef0 = ef0; a.min_score = p->min_score;
-        a.with_duplicates = p->with_duplicates; a.multi_vector = s->cfg.multi_vector; a.filter = bits;
-        a.out_ids = d_ids; a.out_scores = d_sc; a.out_counts = d_cnt;
-        a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = cu_cap;
-        // the scheduler counter lives in the workspace: concurrent calls must not share it
-        ENSURE(w.sched, 128);
-        a.work_counter = w.sched.as<unsigned int>();
-        a.counters = reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64);   // per call, in the call's workspace
-        CU(cudaMemsetAsync(a.work_counter, 0, 128, stream));
-        s->last_counters.store(a.counters);
+        VecDev Vh = V;   // with the screening copy attached
+        int r = attach_half_copy(s, &Vh);
         hs_kernel_t kern = pick_search_kernel(s->ld);
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int occ = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, HS_THREADS, smem));
-        int grid = std::min(nq, std::max(1, occ) * s->sm_count);
-        CU(cudaEventRecord(s->ev_k0, stream));
-        kern<<<grid, HS_THREADS, smem, stream>>>(V, s->gdev(), a);
-        CU(cudaEventRecord(s->ev_k1, stream));
+        int grid = 0;
+        if (!r) r = walk_grid(kern, HS_THREADS, smem, &grid);
+        if (r) return r;
+        return launch_walk(kern, grid, HS_THREADS, smem, Vh, walk_args(ef0, list_cap, cu_cap, hash_bits));
+    }
+};
+
+// NIDX_METHOD_AUTO: the walk or the exhaustive scan by the reference's cost model.  A segment that carries codes is searched with a
+// RaBitQ query on either path (segment.rs:506-513: `rabitq` = has_quantized): the quantised walk (hnsw/search.rs:332-366) or the
+// quantised scan (segment.rs:581-608).
+static int choose_method(const nidx_vec_segment* s, uint64_t matching, int k, int ef) {
+    if (!s->has_graph) return NIDX_METHOD_BRUTE;
+    bool walk_ok = s->d_quant && s->cfg.similarity == NIDX_SIM_DOT;
+    bool scan_ok = walk_ok && !s->d_par_first && k <= 1024;
+    if (!use_hnsw_cost(s->n_par, matching, (size_t)k, (size_t)s->cfg.m, walk_ok)) return scan_ok ? NIDX_METHOD_BRUTE_RABITQ : NIDX_METHOD_BRUTE;
+    // A walk keeps its list and visited set in shared memory: a very large top_k (the reference has no limit on it) does not fit one
+    // CTA.  AUTO then takes the exhaustive scan -- exact results -- instead of failing the request.
+    int last_k, list_cap, cu_cap, hash_bits;
+    size_t bytes;
+    bool fits = walk_ok ? rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &bytes)
+                        : hnsw_search_smem(s, std::max(k, ef > 0 ? ef : s->cfg.ef_search), k, &list_cap, &cu_cap, &hash_bits, &bytes);
+    if (!fits && k <= 1024) return NIDX_METHOD_BRUTE;
+    return walk_ok ? NIDX_METHOD_HNSW_RABITQ : NIDX_METHOD_HNSW;
+}
+
+// The body of nidx_vec_search.  qhost: the queries (and filter bits) are host pointers; ohost: the outputs are host pointers
+// (copied back and the stream synchronised before returning).  The sharded entry point (shard.cuh) passes host queries with
+// device outputs: the partial results go straight into the exchange buffer.
+static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq, int32_t ldq, bool qhost, bool ohost, const nidx_vec_search_params* p,
+                           uint32_t* out_ids, float* out_scores, int32_t* out_counts, cudaStream_t stream, const nidx_filter_node* formula = nullptr,
+                           int32_t n_formula = 0) {
+    if (!s || !p || (!queries && nq > 0) || !out_ids || !out_scores) return fail(NIDX_EINVAL, "null argument");
+    if (nq <= 0) return 0;
+    if (ldq < s->d) return fail(NIDX_EINVAL, "query dimension %d != index dimension %d (VectorErr::InconsistentDimensions)", ldq, s->d);
+    const int k = p->k;
+    if (k <= 0) return fail(NIDX_EINVAL, "k must be positive");
+    CU(cudaSetDevice(s->cfg.device));
+    WsGuard g(s->pool, stream);
+    Workspace& w = *g.w;
+    VecCall c{s, w, stream, p, s->vdev(), nq, k};
+    Stage st(stream, qhost, ohost);
+    const float* d_q;
+    const uint64_t* d_filter;
+    st.in(queries, (size_t)nq * ldq, &d_q);
+    st.in(formula ? nullptr : p->filter_bits, ((size_t)s->n_par + 63) / 64, &d_filter);
+    st.out(out_ids, (size_t)nq * k, &c.ids);
+    st.out(out_scores, (size_t)nq * k, &c.scores);
+    st.out(out_counts, (size_t)nq, &c.counts);
+    int r = st.place(w.stage);
+    if (r) return r;
+    // this call's counters, zero whatever the method: the getters report them until the next search
+    ENSURE(w.sched, 128);
+    CU(cudaMemsetAsync(w.sched.p, 0, 128, stream));
+    c.counters = reinterpret_cast<unsigned long long*>(w.sched.as<unsigned char>() + 64);
+    s->last_counters.store(c.counters);
+
+    // queries -> [nq][ld] zero padded on device, norms
+    r = upload_queries(s, w, d_q, nq, ldq, qhost, stream, &c.dq);
+    if (r) return r;
+    ENSURE(w.qnorms, (size_t)nq * 4);
+    c.qnorms = w.qnorms.as<float>();
+    if (s->cfg.similarity != NIDX_SIM_DOT) {
+        row_norms_kernel<<<(nq + 7) / 8, 256, 0, stream>>>(c.dq, s->ld, (uint64_t)nq, c.qnorms);
         LAUNCHED();
-        CU(cudaGetLastError());
     }
 
-    if (ohost) {
-        CU(cudaMemcpyAsync(out_ids, d_ids, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        if (out_counts) CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
+    // filter ∧ alive (segment.rs:516-534)
+    c.bits = s->d_alive;
+    uint64_t matching = s->d_alive ? s->alive_count : s->n_par;
+    if (d_filter || formula) {
+        if (formula) {   // the formula is evaluated on the device (inverted_index/paragraph.rs:124-186): no host bitset, no copy
+            uint64_t* fdev = nullptr;
+            r = filter_formula_device(s, w, formula, n_formula, stream, &fdev);
+            if (r) return r;
+            d_filter = fdev;
+        }
+        matching = formula ? 0 : p->filter_matching;
+        unsigned long long h = 0;   // segment.rs:531: the reference counts the matches of every filtered request (8 bytes back, one sync)
+        r = filter_and_alive(s, w, d_filter, nullptr, matching ? nullptr : &h, stream, &c.bits);
+        if (r) return r;
+        if (matching == 0) {
+            CU(cudaStreamSynchronize(stream));
+            matching = h;
+        }
     }
-    return 0;
+
+    const int method = p->method == NIDX_METHOD_AUTO ? choose_method(s, matching, k, p->ef) : p->method;
+    const bool walk = method == NIDX_METHOD_HNSW || method == NIDX_METHOD_HNSW_RABITQ;
+    if (matching == 0) r = c.write_empty();   // segment.rs:532-534: nothing can match (everything deleted / filtered out), whatever the method
+    else if (walk && !s->has_graph) return fail(NIDX_ESTATE, "HNSW search requested but the segment has no graph");
+    else if (s->n == 0) r = c.write_empty();
+    else if (method == NIDX_METHOD_BRUTE_RABITQ) r = c.rabitq_scan();
+    else if (method == NIDX_METHOD_BRUTE && use_tc_filter(s, nq, k)) r = c.tc_filter_scan();
+    else if (method == NIDX_METHOD_BRUTE) r = c.exact_scan();
+    else if (method == NIDX_METHOD_HNSW_RABITQ) r = c.quantised_walk();
+    else r = c.dense_walk();
+    if (r) return r;
+    return st.finish();
 }
 
 extern "C" {
@@ -1394,20 +1463,30 @@ int nidx_vec_filter(nidx_vec_segment* s, const nidx_filter_node* nodes, int32_t 
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     WsGuard g(s->pool, stream);
     Workspace& w = *g.w;
+    const bool host = mem == NIDX_MEM_HOST;
+    Stage st(stream, host, host);
+    uint64_t* d_bits;
+    st.out(out_bits, ((size_t)s->n_par + 63) / 64, &d_bits);
+    int r = st.place(w.stage);
     uint64_t* fdev = nullptr;
-    int r = filter_formula_device(s, w, nodes, n_nodes, stream, &fdev);
-    if (r) return r;
-    size_t words = ((size_t)s->n_par + 63) / 64;
-    uint64_t* d_out = w.filter.as<uint64_t>() + words;
-    unsigned long long* d_cnt = reinterpret_cast<unsigned long long*>(d_out + words);
-    CU(cudaMemsetAsync(d_cnt, 0, 8, stream));
-    and_bits_kernel<<<std::min<size_t>((words + 255) / 256, 1024), 256, 0, stream>>>(fdev, s->d_alive, d_out, words, d_cnt);   // segment.rs:523-526: intersect with the alive set
-    LAUNCHED();
-    if (out_bits) CU(cudaMemcpyAsync(out_bits, d_out, words * 8, mem == NIDX_MEM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, stream));
+    if (!r) r = filter_formula_device(s, w, nodes, n_nodes, stream, &fdev);
     unsigned long long h = 0;
-    CU(cudaMemcpyAsync(&h, d_cnt, 8, cudaMemcpyDeviceToHost, stream));
-    CU(cudaStreamSynchronize(stream));
+    const uint64_t* bits;
+    if (!r) r = filter_and_alive(s, w, fdev, d_bits, &h, stream, &bits);   // segment.rs:523-526: intersect with the alive set
+    if (!r) r = st.finish(true);
+    if (r) return r;
     if (out_matching) *out_matching = h;
+    return 0;
+}
+
+// The text merge of n_parts top-k lists: (score desc, part asc, position asc)
+static int launch_parts_merge(const uint32_t* ids, const float* scores, int n_parts, size_t part_stride, int nq, int k, uint32_t* out_ids, float* out_scores,
+                              int* out_part, cudaStream_t stream) {
+    if (k > 1024 || (long long)n_parts * k >= (1ll << 31)) return fail(NIDX_EINVAL, "k above 1024 not supported");
+    int cap = topk_cap(k, 256);
+    if ((size_t)cap * 8 > 48 * 1024) CU(cudaFuncSetAttribute(parts_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    parts_merge_kernel<<<nq, 256, (size_t)cap * 8, stream>>>(ids, scores, n_parts, part_stride, nq, k, cap, out_ids, out_scores, out_part);
+    LAUNCHED();
     return 0;
 }
 
@@ -1416,11 +1495,9 @@ int nidx_merge_topk(int32_t device, const uint32_t* ids, const float* scores, in
     int r = check_device(device);
     if (r) return r;
     if (!ids || !scores || !out_ids || !out_scores || n_parts <= 0 || nq <= 0 || k <= 0) return fail(NIDX_EINVAL, "bad argument");
-    if (k > 1024 || (long long)n_parts * k >= (1ll << 31)) return fail(NIDX_EINVAL, "k above 1024 not supported");
-    int cap = topk_cap(k, 256);
-    if ((size_t)cap * 8 > 48 * 1024) CU(cudaFuncSetAttribute(parts_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
-    parts_merge_kernel<<<nq, 256, (size_t)cap * 8, reinterpret_cast<cudaStream_t>(stream_)>>>(ids, scores, n_parts, part_stride > 0 ? (size_t)part_stride : (size_t)nq * k, nq, k, cap, out_ids, out_scores, out_part);
-    LAUNCHED();
+    r = launch_parts_merge(ids, scores, n_parts, part_stride > 0 ? (size_t)part_stride : (size_t)nq * k, nq, k, out_ids, out_scores, out_part,
+                           reinterpret_cast<cudaStream_t>(stream_));
+    if (r) return r;
     CU(cudaGetLastError());
     return 0;
 }
@@ -1483,7 +1560,8 @@ static void host_assign_levels(uint64_t n, int M, uint64_t seed, uint8_t* level)
 
 // Batch-synchronous insertion of order[0 .. n) into the segment's graph (which may already hold other nodes):
 // the loop of build.rs:123-166 as search / select / sort / reverse-link kernels per batch (hnsw_build.cuh).
-// entry_after_first (node, layer), if given, becomes the entry point once the first batch has been inserted.
+// entry_after_first (node, layer), if given, becomes the entry point once the first batch has been inserted.  On failure the
+// segment loses its graph.
 static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level, const std::vector<uint32_t>& order, const std::vector<uint32_t>& ends,
                           cudaStream_t stream, const uint32_t* entry_after_first = nullptr) {
     uint64_t n = order.size();
@@ -1616,7 +1694,17 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
         return 0;
     }();
     cleanup();
+    if (r) free_graph(s);
     return r;
+}
+
+// Appends the insertion batches from `done` inserted nodes to n (ends counted from `base`): batch b = min(max_batch, max(1, done/16))
+static void batch_ends(uint64_t done, uint64_t n, uint64_t base, int max_batch, std::vector<uint32_t>& ends) {
+    if (max_batch <= 0) max_batch = 4096;
+    while (done < n) {
+        done += std::min<uint64_t>({(uint64_t)max_batch, std::max<uint64_t>(1, done / 16), n - done});
+        ends.push_back((uint32_t)(done - base));
+    }
 }
 
 extern "C" {
@@ -1633,7 +1721,6 @@ int nidx_vec_build_hnsw(nidx_vec_segment* s, uint64_t seed, int32_t max_batch, v
     CU(cudaSetDevice(s->cfg.device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     uint64_t n = s->n;
-    if (max_batch <= 0) max_batch = 4096;
     std::vector<uint8_t> level(n ? n : 1);
     host_assign_levels(n, s->cfg.m, seed, level.data());
     int r = alloc_graph(s, level.data());
@@ -1641,19 +1728,13 @@ int nidx_vec_build_hnsw(nidx_vec_segment* s, uint64_t seed, int32_t max_batch, v
     s->has_graph = true;
     if (n == 0) return 0;
 
-    // insertion order: entry point first, then ascending id; batch b = min(max_batch, max(1, done/16))
+    // insertion order: entry point first, then ascending id
     std::vector<uint32_t> order(n);
     order[0] = s->entry_node;
     for (uint64_t i = 0, j = 1; i < n; ++i) if (i != s->entry_node) order[j++] = (uint32_t)i;
     std::vector<uint32_t> ends;
-    for (uint64_t done = 0; done < n;) {
-        uint64_t b = std::min<uint64_t>({(uint64_t)max_batch, std::max<uint64_t>(1, done / 16), n - done});
-        done += b;
-        ends.push_back((uint32_t)done);
-    }
-    r = run_insertions(s, level, order, ends, stream);
-    if (r) { free_graph(s); return r; }
-    return 0;
+    batch_ends(0, n, 0, max_batch, ends);
+    return run_insertions(s, level, order, ends, stream);
 }
 
 // merge_indexes' fast path (segment.rs:143-167): the first n_existing vectors of this (merged) segment are the largest
@@ -1669,7 +1750,6 @@ int nidx_vec_extend_hnsw(nidx_vec_segment* s, uint64_t n_existing, const uint8_t
     CU(cudaSetDevice(s->cfg.device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     uint64_t n = s->n;
-    if (max_batch <= 0) max_batch = 4096;
     std::vector<uint8_t> level(n);
     memcpy(level.data(), level_existing, n_existing);
     for (uint64_t i = 0; i < n_existing; ++i)
@@ -1734,14 +1814,8 @@ int nidx_vec_extend_hnsw(nidx_vec_segment* s, uint64_t n_existing, const uint8_t
         if (!raises || i != raised[0]) order.push_back((uint32_t)i);
     std::vector<uint32_t> ends;
     if (raises) ends.push_back(1);
-    for (uint64_t done = n_existing + (raises ? 1 : 0); done < n;) {
-        uint64_t b = std::min<uint64_t>({(uint64_t)max_batch, std::max<uint64_t>(1, done / 16), n - done});
-        done += b;
-        ends.push_back((uint32_t)(done - n_existing));
-    }
-    r = run_insertions(s, level, order, ends, stream, raises ? raised : nullptr);
-    if (r) { free_graph(s); return r; }
-    return 0;
+    batch_ends(n_existing + (raises ? 1 : 0), n, n_existing, max_batch, ends);
+    return run_insertions(s, level, order, ends, stream, raises ? raised : nullptr);
 }
 
 // ---- segment files ----------------------------------------------------------------------------
@@ -1759,20 +1833,7 @@ int nidx_vec_open(const nidx_vec_config* cfg, const char* dir, nidx_vec_segment*
     s->n = n;
     std::vector<uint32_t> par(n);
     for (uint64_t i = 0; i < n; ++i) memcpy(&par[i], raw.data() + i * rec + (size_t)s->d * 4, 4);
-    r = [&]() -> int {
-        CU(cudaMalloc(&s->d_vecs, std::max<size_t>((size_t)n * s->ld * 4, 16)));
-        if (n) {
-            void* staged = nullptr;
-            CU(cudaMalloc(&staged, raw.size()));
-            CU(cudaMemcpy(staged, raw.data(), raw.size(), cudaMemcpyHostToDevice));
-            pad_rows_kernel<<<s->sm_count * 8, 256>>>(reinterpret_cast<unsigned char*>(staged), rec, s->d, s->d_vecs, s->ld, n);
-            LAUNCHED();
-            CU(cudaGetLastError());
-            CU(cudaDeviceSynchronize());
-            cudaFree(staged);
-        }
-        return 0;
-    }();
+    r = upload_rows(s, raw.data(), rec, true, false);
     if (!r) r = finish_create(s, n ? par.data() : nullptr);
     if (r) { nidx_vec_close(s); return r; }
     // hnsw.graph (+ hnsw.edges) if present
@@ -1975,12 +2036,7 @@ int nidx_txt_set_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t total_
 
 int nidx_txt_set_alive(nidx_txt_segment* t, const uint64_t* alive_bits) {
     if (!t) return fail(NIDX_EINVAL, "null segment");
-    CU(cudaSetDevice(t->device));
-    if (!alive_bits) { cudaFree(t->d_alive); t->d_alive = nullptr; return 0; }
-    size_t words = ((size_t)t->n_docs + 63) / 64;
-    if (!t->d_alive) CU(cudaMalloc(&t->d_alive, std::max<size_t>(words, 1) * 8));
-    CU(cudaMemcpy(t->d_alive, alive_bits, words * 8, cudaMemcpyHostToDevice));
-    return 0;
+    return set_rows(t->device, &t->d_alive, alive_bits, ((size_t)t->n_docs + 63) / 64);
 }
 
 void nidx_txt_close(nidx_txt_segment* t) {
@@ -2155,11 +2211,6 @@ static int facet_args(const nidx_txt_segment* t, const FacetPlan& P, Workspace& 
     return 0;
 }
 
-typedef void (*bm_kernel_t)(TxtDev, Bm25Args);
-typedef void (*bm_facet_kernel_t)(TxtDev, Bm25Args, FacetArgs);
-typedef void (*bm_order_kernel_t)(TxtDev, Bm25Args, OrderArgs);
-typedef void (*bm_order_facet_kernel_t)(TxtDev, Bm25Args, FacetArgs, OrderArgs);
-
 // The body of nidx_txt_search (facets == nullptr), nidx_txt_search_faceted and nidx_txt_search_ordered (order != nullptr: dates to
 // out_dates instead of scores to out_scores).  qhost / ohost as in vec_search_impl.
 static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, bool qhost, bool ohost,
@@ -2192,30 +2243,29 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     int max_terms = 0;
     for (int i = 0; i < nq; ++i) max_terms = std::max<int>(max_terms, h_off[i + 1] - h_off[i]);
     if (max_terms > BM_MAX_TERMS) return fail(NIDX_EINVAL, "queries with more than %d terms are not supported", BM_MAX_TERMS);
-    const uint32_t *d_qt = query_terms, *d_qo = query_off;
-    if (qhost) {
-        ENSURE(w.queries, ((size_t)n_qt + nq + 1) * 4 + 16);
-        uint32_t* base = w.queries.as<uint32_t>();
-        CU(cudaMemcpyAsync(base, query_off, ((size_t)nq + 1) * 4, cudaMemcpyHostToDevice, stream));
-        if (n_qt) CU(cudaMemcpyAsync(base + nq + 1, query_terms, (size_t)n_qt * 4, cudaMemcpyHostToDevice, stream));
-        d_qo = base; d_qt = base + nq + 1;
-    }
     bool conj = p->mode == NIDX_BM25_AND;
     int cap = topk_cap(k, BM_THREADS);
     size_t smem = bm_smem_bytes(cap, conj);
     if (smem > 220 * 1024) return fail(NIDX_EINVAL, "BM25 needs %zu bytes of shared memory (k=%d): too large", smem, k);
     ENSURE(w.partial, (size_t)nq * k * 8);
-    ENSURE(w.misc, (size_t)nq * 8);
-    uint32_t* d_docs = out_docs; float* d_sc = out_scores; int* d_cnt = out_counts;
-    unsigned long long* d_total = reinterpret_cast<unsigned long long*>(out_total);
-    if (ohost) {
-        ENSURE(w.out_ids, (size_t)nq * k * 4);
-        ENSURE(w.out_scores, (size_t)nq * k * (order ? 8 : 4));
-        ENSURE(w.out_counts, (size_t)nq * 4);
-        d_docs = w.out_ids.as<uint32_t>(); d_sc = w.out_scores.as<float>(); d_cnt = w.out_counts.as<int>();
-        d_total = w.misc.as<unsigned long long>();
-    }
-    int64_t* d_dates = ohost ? w.out_scores.as<int64_t>() : out_dates;
+    const size_t nb = plan.b_req.size();
+    Stage st(stream, qhost, ohost);
+    const uint32_t *d_qt, *d_qo;
+    uint32_t *d_docs, *d_fc = nullptr;
+    float* d_sc = nullptr;
+    int64_t* d_dates = nullptr;
+    int* d_cnt;
+    uint64_t* d_total;
+    st.in(query_off, (size_t)nq + 1, &d_qo);
+    st.in(query_terms, n_qt, &d_qt);
+    st.out(out_docs, (size_t)nq * k, &d_docs);
+    if (order) st.out(out_dates, (size_t)nq * k, &d_dates);
+    else st.out(out_scores, (size_t)nq * k, &d_sc);
+    st.out(out_counts, (size_t)nq, &d_cnt);
+    st.out(out_total, (size_t)nq, &d_total);
+    if (facets) st.out(out_facet_counts, (size_t)nq * nb, &d_fc);
+    int r = st.place(w.stage);
+    if (r) return r;
     TxtDev T;
     T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
     T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
@@ -2223,64 +2273,43 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     a.query_terms = d_qt; a.query_off = d_qo; a.nq = nq; a.k = k; a.cap = cap;
     a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
-    a.out_keys = w.partial.as<uint64_t>(); a.out_total = d_total; a.error_flag = t->d_error;
+    a.out_keys = w.partial.as<uint64_t>(); a.out_total = reinterpret_cast<unsigned long long*>(d_total); a.error_flag = t->d_error;
     if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after
-    if (order && !facets) {
-        bm_order_kernel_t kern = conj ? bm25_order_kernel<true> : bm25_order_kernel<false>;
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    auto launch = [&](auto kern, size_t bytes, auto... extra) -> int {   // the BM25 pass, between the roofline events
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         CU(cudaEventRecord(t->ev_k0, stream));
-        kern<<<nq, BM_THREADS, smem, stream>>>(T, a, O);
+        kern<<<nq, BM_THREADS, bytes, stream>>>(T, a, extra...);
         CU(cudaEventRecord(t->ev_k1, stream));
         LAUNCHED();
-    } else if (!facets) {
-        bm_kernel_t kern = conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>);
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CU(cudaEventRecord(t->ev_k0, stream));
-        kern<<<nq, BM_THREADS, smem, stream>>>(T, a);
-        CU(cudaEventRecord(t->ev_k1, stream));
-        LAUNCHED();
-    } else {
-        const size_t nb = plan.b_req.size();
-        uint32_t* d_fc = out_facet_counts;
-        if (ohost) { ENSURE(w.scores, std::max<size_t>((size_t)nq * nb, 1) * 4); d_fc = w.scores.as<uint32_t>(); }
-        FacetArgs F;
-        int r = facet_args(t, plan, w, d_fc, stream, F);
+        return 0;
+    };
+    FacetArgs F;
+    size_t fsmem = smem;
+    if (facets) {
+        r = facet_args(t, plan, w, d_fc, stream, F);
         if (r) return r;
         if (F.smem && smem + nb * 4 > 220 * 1024) F.smem = 0;
         if (!F.smem && nb) CU(cudaMemsetAsync(d_fc, 0, (size_t)nq * nb * 4, stream));
-        const size_t fsmem = smem + (F.smem ? nb * 4 : 0);
-        if (order) {
-            bm_order_facet_kernel_t kern = conj ? bm25_order_facet_kernel<true> : bm25_order_facet_kernel<false>;
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-            CU(cudaEventRecord(t->ev_k0, stream));
-            kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F, O);
-            CU(cudaEventRecord(t->ev_k1, stream));
-        } else {
-            bm_facet_kernel_t kern = conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
-                                          : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>);
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-            CU(cudaEventRecord(t->ev_k0, stream));
-            kern<<<nq, BM_THREADS, fsmem, stream>>>(T, a, F);
-            CU(cudaEventRecord(t->ev_k1, stream));
-        }
-        LAUNCHED();
-        if (ohost && nb) CU(cudaMemcpyAsync(out_facet_counts, d_fc, (size_t)nq * nb * 4, cudaMemcpyDeviceToHost, stream));
+        fsmem += F.smem ? nb * 4 : 0;
     }
+    if (order && !facets) r = launch(conj ? bm25_order_kernel<true> : bm25_order_kernel<false>, smem, O);
+    else if (!facets)
+        r = launch(conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>),
+                   smem);
+    else if (order) r = launch(conj ? bm25_order_facet_kernel<true> : bm25_order_facet_kernel<false>, fsmem, F, O);
+    else
+        r = launch(conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
+                        : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>), fsmem, F);
+    if (r) return r;
     if (order) date_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, O.secs, d_docs, d_dates, d_cnt);
     else bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
     LAUNCHED();
     CU(cudaGetLastError());
-    if (ohost) {
-        CU(cudaMemcpyAsync(out_docs, d_docs, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        if (order) CU(cudaMemcpyAsync(out_dates, d_dates, (size_t)nq * k * 8, cudaMemcpyDeviceToHost, stream));
-        else CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
-        if (out_total) CU(cudaMemcpyAsync(out_total, d_total, (size_t)nq * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-        unsigned int err = 0;   // an accumulator table that filled up would mean incomplete sums: report, never return them silently
-        CU(cudaMemcpy(&err, t->d_error, 4, cudaMemcpyDeviceToHost));
-        if (err) { cudaMemset(t->d_error, 0, 4); return fail(NIDX_EOVERFLOW, "BM25 accumulator table overflow"); }
-    }
+    r = st.finish();
+    if (r || !ohost) return r;
+    unsigned int err = 0;   // an accumulator table that filled up would mean incomplete sums: report, never return them silently
+    CU(cudaMemcpy(&err, t->d_error, 4, cudaMemcpyDeviceToHost));
+    if (err) { cudaMemset(t->d_error, 0, 4); return fail(NIDX_EOVERFLOW, "BM25 accumulator table overflow"); }
     return 0;
 }
 
@@ -2326,10 +2355,12 @@ int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* 
     CU(cudaSetDevice(t->device));
     WsGuard g(t->pool, stream);
     Workspace& w = *g.w;
-    uint32_t* d_fc = out_facet_counts;
-    if (host) { ENSURE(w.scores, nb * 4); d_fc = w.scores.as<uint32_t>(); }
+    Stage st(stream, host, host);
+    uint32_t* d_fc;
+    st.out(out_facet_counts, nb, &d_fc);
+    r = st.place(w.stage);
     FacetArgs F;
-    r = facet_args(t, plan, w, d_fc, stream, F);
+    if (!r) r = facet_args(t, plan, w, d_fc, stream, F);
     if (r) return r;
     CU(cudaMemsetAsync(d_fc, 0, nb * 4, stream));
     const int threads = 256;
@@ -2339,11 +2370,7 @@ int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* 
     CU(cudaEventRecord(t->ev_k1, stream));
     LAUNCHED();
     CU(cudaGetLastError());
-    if (host) {
-        CU(cudaMemcpyAsync(out_facet_counts, d_fc, nb * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 int nidx_txt_search_ordered(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem, const nidx_txt_search_params* p,
@@ -2372,34 +2399,29 @@ int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int3
     const int blocks = std::max(1, std::min<int>(t->sm_count * 2, (int)(((size_t)t->n_docs + threads * DATE_PT - 1) / (threads * DATE_PT))));
     const int cap = topk_cap(k, threads);
     ENSURE(w.partial, (size_t)blocks * k * 8);
-    ENSURE(w.misc, 8);
-    uint32_t* d_docs = out_docs; int64_t* d_dates = out_dates; int* d_cnt = out_count;
-    unsigned long long* d_total = reinterpret_cast<unsigned long long*>(out_total);
-    if (host || !out_total) d_total = w.misc.as<unsigned long long>();
-    if (host) {
-        ENSURE(w.out_ids, (size_t)k * 4);
-        ENSURE(w.out_scores, (size_t)k * 8);
-        ENSURE(w.out_counts, 4);
-        d_docs = w.out_ids.as<uint32_t>(); d_dates = w.out_scores.as<int64_t>(); d_cnt = w.out_counts.as<int>();
-    }
+    Stage st(stream, host, host);
+    uint32_t* d_docs;
+    int64_t* d_dates;
+    int* d_cnt;
+    uint64_t* d_total;
+    st.out(out_docs, (size_t)k, &d_docs);
+    st.out(out_dates, (size_t)k, &d_dates);
+    st.out(out_count, 1, &d_cnt);
+    st.out(out_total, 1, &d_total);
+    r = st.place(w.stage);
+    if (r) return r;
     CU(cudaFuncSetAttribute(date_topk_all_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
     CU(cudaFuncSetAttribute(date_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
     CU(cudaMemsetAsync(d_total, 0, 8, stream));
     CU(cudaEventRecord(t->ev_k0, stream));
-    date_topk_all_kernel<<<blocks, threads, (size_t)cap * 8, stream>>>(t->n_docs, t->d_alive, O, k, cap, w.partial.as<uint64_t>(), d_total);
+    date_topk_all_kernel<<<blocks, threads, (size_t)cap * 8, stream>>>(t->n_docs, t->d_alive, O, k, cap, w.partial.as<uint64_t>(),
+                                                                      reinterpret_cast<unsigned long long*>(d_total));
     LAUNCHED();
     date_merge_kernel<<<1, threads, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), blocks * k, k, cap, O.secs, d_docs, d_dates, d_cnt);
     LAUNCHED();
     CU(cudaEventRecord(t->ev_k1, stream));
     CU(cudaGetLastError());
-    if (host) {
-        CU(cudaMemcpyAsync(out_docs, d_docs, (size_t)k * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_dates, d_dates, (size_t)k * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_count, d_cnt, 4, cudaMemcpyDeviceToHost, stream));
-        if (out_total) CU(cudaMemcpyAsync(out_total, d_total, 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 // ---- sharded search (shard.cuh) -------------------------------------------------------------------
@@ -2407,7 +2429,7 @@ struct nidx_shard_comm {
     int rank = 0, world = 1, device = 0;
     nccl_comm_t comm = nullptr;
     std::mutex mu;          // collectives on one communicator must be issued in the same order by every rank: one call at a time
-    DevBuf local, gathered, total;
+    DevBuf local, gathered, stage;   // this rank's record, every rank's, staged outputs
 };
 
 #define NC(expr)                                                                                                   \
@@ -2447,17 +2469,12 @@ void nidx_shard_destroy(nidx_shard_comm* c) {
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     if (c->comm) nccl_api().CommDestroy(c->comm);
-    c->local.release(); c->gathered.release(); c->total.release();
     delete c;
 }
 
 int nidx_vec_set_paragraph_keys(nidx_vec_segment* s, const uint64_t* keys) {
     if (!s) return fail(NIDX_EINVAL, "null segment");
-    CU(cudaSetDevice(s->cfg.device));
-    if (!keys) { cudaFree(s->d_par_keys); s->d_par_keys = nullptr; return 0; }
-    if (!s->d_par_keys) CU(cudaMalloc(&s->d_par_keys, std::max<size_t>(s->n_par, 1) * 8));
-    CU(cudaMemcpy(s->d_par_keys, keys, (size_t)s->n_par * 8, cudaMemcpyHostToDevice));
-    return 0;
+    return set_rows(s->cfg.device, &s->d_par_keys, keys, s->n_par);
 }
 
 // How the parts of a sharded search are merged (step 3)
@@ -2467,17 +2484,24 @@ enum class PartsRule {
     fssc,     // vector segments of one index: Fssc with the paragraph / vector keys of the records (shard_fssc_kernel)
 };
 
-// Step 3: merge n_parts records laid end to end (shard_part_words each) into [nq][k] ids / scores / part + counts.  Outputs are
-// device pointers, or (ohost) host pointers staged through `stage` (nq * k * 12 + nq * 4 bytes of device memory) and copied back
-// asynchronously on `stream`.
-static int shard_merge_impl(const uint32_t* gathered, int n_parts, int nq, int k, PartsRule rule, int with_duplicates, bool ohost, uint32_t* stage,
-                            uint32_t* out_ids, float* out_scores, int32_t* out_part, int32_t* out_counts, cudaStream_t stream) {
+// The device outputs of a merge of parts (the caller's, or staged)
+struct MergeOut {
+    uint32_t* ids;
+    float* scores;
+    int* part;
+    int* counts;
+};
+static void stage_merge_outputs(Stage& st, MergeOut& o, int nq, int k, uint32_t* ids, float* scores, int32_t* part, int32_t* counts) {
+    st.out(ids, (size_t)nq * k, &o.ids);
+    st.out(scores, (size_t)nq * k, &o.scores);
+    st.out(part, (size_t)nq * k, &o.part);
+    st.out(counts, (size_t)nq, &o.counts);
+}
+
+// Step 3: merge n_parts records laid end to end (shard_part_words each) into [nq][k] ids / scores / part + counts
+static int shard_merge_impl(const uint32_t* gathered, int n_parts, int nq, int k, PartsRule rule, int with_duplicates, const MergeOut& o,
+                            cudaStream_t stream) {
     size_t words = shard_part_words(nq, k, rule == PartsRule::fssc);
-    uint32_t* d_ids = out_ids; float* d_sc = out_scores; int* d_part = out_part; int* d_cnt = out_counts;
-    if (ohost) {
-        d_ids = stage; d_sc = reinterpret_cast<float*>(stage + (size_t)nq * k); d_part = reinterpret_cast<int*>(stage + 2 * (size_t)nq * k);
-        d_cnt = reinterpret_cast<int*>(stage + 3 * (size_t)nq * k);
-    }
     const float* gathered_scores = reinterpret_cast<const float*>(gathered + (size_t)nq * k);
     if (rule == PartsRule::fssc) {
         size_t per = (size_t)k * 16 + (size_t)n_parts * k * 8;
@@ -2486,43 +2510,37 @@ static int shard_merge_impl(const uint32_t* gathered, int n_parts, int nq, int k
         threads = std::min(threads, nq);
         size_t smem = per * threads;
         if (smem > 48 * 1024) CU(cudaFuncSetAttribute(shard_fssc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        shard_fssc_kernel<<<(nq + threads - 1) / threads, threads, smem, stream>>>(gathered, n_parts, words, nq, k, with_duplicates, d_ids, d_sc, d_part, d_cnt);
+        shard_fssc_kernel<<<(nq + threads - 1) / threads, threads, smem, stream>>>(gathered, n_parts, words, nq, k, with_duplicates, o.ids, o.scores, o.part,
+                                                                                  o.counts);
         LAUNCHED();
     } else if (rule == PartsRule::kmerge) {
-        int r = launch_kmerge(gathered, gathered_scores, n_parts, words, nq, k, d_ids, d_sc, d_part, d_cnt, stream);
+        int r = launch_kmerge(gathered, gathered_scores, n_parts, words, nq, k, o.ids, o.scores, o.part, o.counts, stream);
         if (r) return r;
     } else {
-        if (k > 1024 || (long long)n_parts * k >= (1ll << 31)) return fail(NIDX_EINVAL, "k above 1024 not supported");
-        int cap = topk_cap(k, 256);
-        if ((size_t)cap * 8 > 48 * 1024) CU(cudaFuncSetAttribute(parts_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
-        parts_merge_kernel<<<nq, 256, (size_t)cap * 8, stream>>>(gathered, gathered_scores, n_parts, words, nq, k, cap, d_ids, d_sc, d_part);
+        int r = launch_parts_merge(gathered, gathered_scores, n_parts, words, nq, k, o.ids, o.scores, o.part, stream);
+        if (r) return r;
+        shard_count_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(o.ids, nq, k, o.counts);
         LAUNCHED();
-        if (d_cnt) {
-            shard_count_kernel<<<(nq + 255) / 256, 256, 0, stream>>>(d_ids, nq, k, d_cnt);
-            LAUNCHED();
-        }
     }
     CU(cudaGetLastError());
-    if (ohost) {
-        CU(cudaMemcpyAsync(out_ids, d_ids, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        if (out_part) CU(cudaMemcpyAsync(out_part, d_part, (size_t)nq * k * 4, cudaMemcpyDeviceToHost, stream));
-        if (out_counts) CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
-    }
     return 0;
 }
 
-// common tail: all-gather the local part, merge, deliver (outputs staged behind the gathered parts when they are host pointers)
-static int shard_exchange_and_merge(nidx_shard_comm* c, int nq, int k, PartsRule rule, int with_duplicates, bool ohost, uint32_t* out_ids, float* out_scores,
-                                    int32_t* out_part, int32_t* out_counts, cudaStream_t stream) {
+// The exchange buffers of a sharded search: this rank's record (words long) + nq counts, and every rank's record
+static int shard_buffers(nidx_shard_comm* c, int nq, int k, bool fssc, size_t* words) {
+    *words = shard_part_words(nq, k, fssc);
+    ENSURE(c->local, *words * 4 + (size_t)nq * 4);
+    ENSURE(c->gathered, (size_t)c->world * *words * 4 + 64);
+    return 0;
+}
+
+// Steps 2 and 3: all-gather the local records in rank order, merge them
+static int shard_exchange_and_merge(nidx_shard_comm* c, int nq, int k, PartsRule rule, int with_duplicates, const MergeOut& o, cudaStream_t stream) {
     NcclApi& N = nccl_api();
     size_t words = shard_part_words(nq, k, rule == PartsRule::fssc);
-    uint32_t* local = c->local.as<uint32_t>();
-    uint32_t* gathered = c->gathered.as<uint32_t>();
-    NC(N.AllGather(local, gathered, words * 4, NCCL_INT8, c->comm, stream));
+    NC(N.AllGather(c->local.p, c->gathered.p, words * 4, NCCL_INT8, c->comm, stream));
     LAUNCHED();
-    return shard_merge_impl(gathered, c->world, nq, k, rule, with_duplicates, ohost, gathered + (size_t)c->world * words, out_ids, out_scores, out_part,
-                            out_counts, stream);
+    return shard_merge_impl(c->gathered.as<uint32_t>(), c->world, nq, k, rule, with_duplicates, o, stream);
 }
 
 // Step 1: this part's segment searched into its exchange record (queries from the caller's memory, results straight into the
@@ -2559,18 +2577,18 @@ int nidx_shard_merge(int32_t device, const uint32_t* records, int32_t n_parts, i
     if (r) return r;
     if (!records || !out_ids || !out_scores || n_parts <= 0 || k <= 0) return fail(NIDX_EINVAL, "bad argument");
     if (nq <= 0) return 0;
-    CU(cudaSetDevice(device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    PartsRule rule = dedup ? PartsRule::fssc : PartsRule::kmerge;
-    if (mem != NIDX_MEM_HOST) return shard_merge_impl(records, n_parts, nq, k, rule, with_duplicates, false, nullptr, out_ids, out_scores, out_part, out_counts, stream);
-    DevBuf stage;
-    r = stage.ensure((size_t)nq * k * 12 + (size_t)nq * 4);
-    if (!r) r = shard_merge_impl(records, n_parts, nq, k, rule, with_duplicates, true, stage.as<uint32_t>(), out_ids, out_scores, out_part, out_counts, stream);
-    cudaError_t e = cudaStreamSynchronize(stream);
-    stage.release();
+    WorkspacePool* pool = plan_pool(device);
+    if (!pool) return fail(NIDX_EINVAL, "device %d", device);
+    WsGuard g(*pool, stream);
+    const bool host = mem == NIDX_MEM_HOST;
+    Stage st(stream, host, host);
+    MergeOut o;
+    stage_merge_outputs(st, o, nq, k, out_ids, out_scores, out_part, out_counts);
+    r = st.place(g.w->stage);
+    if (!r) r = shard_merge_impl(records, n_parts, nq, k, dedup ? PartsRule::fssc : PartsRule::kmerge, with_duplicates, o, stream);
     if (r) return r;
-    if (e != cudaSuccess) return fail(NIDX_ECUDA, "cudaStreamSynchronize failed: %s", cudaGetErrorString(e));
-    return 0;
+    return st.finish();
 }
 
 int nidx_vec_search_sharded(nidx_shard_comm* c, nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem, const nidx_vec_search_params* p,
@@ -2584,19 +2602,20 @@ int nidx_vec_search_sharded(nidx_shard_comm* c, nidx_vec_segment* seg, const flo
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     bool host = mem == NIDX_MEM_HOST;
     std::lock_guard<std::mutex> lock(c->mu);
-    size_t words = shard_part_words(nq, k, dedup != 0);
-    ENSURE(c->local, words * 4 + (size_t)nq * 4);
-    ENSURE(c->gathered, (size_t)c->world * words * 4 + (size_t)nq * k * 12 + (size_t)nq * 4 + 64);
+    size_t words;
+    int r = shard_buffers(c, nq, k, dedup != 0, &words);
+    Stage st(stream, false, host);
+    MergeOut o;
+    stage_merge_outputs(st, o, nq, k, out_ids, out_scores, out_part, out_counts);
+    if (!r) r = st.place(c->stage);
+    if (r) return r;
     uint32_t* local = c->local.as<uint32_t>();
     // 1. this rank's segment into the exchange record
-    int r = shard_record_impl(seg, queries, nq, ldq, host, p, c->rank, dedup != 0, local, reinterpret_cast<int*>(local + words), stream);
-    if (r) return r;
+    r = shard_record_impl(seg, queries, nq, ldq, host, p, c->rank, dedup != 0, local, reinterpret_cast<int*>(local + words), stream);
     // 2. + 3. exchange and merge
-    r = shard_exchange_and_merge(c, nq, k, dedup ? PartsRule::fssc : PartsRule::kmerge, p->with_duplicates, host, out_ids, out_scores, out_part, out_counts,
-                                 stream);
+    if (!r) r = shard_exchange_and_merge(c, nq, k, dedup ? PartsRule::fssc : PartsRule::kmerge, p->with_duplicates, o, stream);
     if (r) return r;
-    if (host) CU(cudaStreamSynchronize(stream));
-    return 0;
+    return st.finish();
 }
 
 int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem,
@@ -2611,48 +2630,35 @@ int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uin
     bool host = mem == NIDX_MEM_HOST;
     std::lock_guard<std::mutex> lock(c->mu);
     NcclApi& N = nccl_api();
-    size_t words = shard_part_words(nq, k, false);
-    ENSURE(c->local, words * 4 + (size_t)nq * 4);
-    ENSURE(c->gathered, (size_t)c->world * words * 4 + (size_t)nq * k * 12 + (size_t)nq * 4 + 64);
-    ENSURE(c->total, (size_t)nq * 8);
+    size_t words;
+    int r = shard_buffers(c, nq, k, false, &words);
+    Stage st(stream, false, host);
+    MergeOut o;
+    uint64_t* d_total;
+    stage_merge_outputs(st, o, nq, k, out_docs, out_scores, out_part, out_counts);
+    st.out(out_total, (size_t)nq, &d_total);
+    if (!r) r = st.place(c->stage);
+    if (r) return r;
     uint32_t* local = c->local.as<uint32_t>();
     int* local_cnt = reinterpret_cast<int*>(local + words);
-    uint64_t* d_total = host ? c->total.as<uint64_t>() : (out_total ? out_total : c->total.as<uint64_t>());
     // the min_score cut is applied to the merged list by the caller's convention (reader.rs:302-305 drops below min_score after top-k):
     // every part applies it locally, which commutes with the merge.
-    int r = txt_search_impl(seg, query_terms, query_off, nq, host, false, p, local, reinterpret_cast<float*>(local + (size_t)nq * k), local_cnt, d_total, stream);
+    r = txt_search_impl(seg, query_terms, query_off, nq, host, false, p, local, reinterpret_cast<float*>(local + (size_t)nq * k), local_cnt, d_total, stream);
     if (r) return r;
     NC(N.AllReduce(d_total, d_total, (size_t)nq, NCCL_UINT64, NCCL_SUM, c->comm, stream));   // Count collector over all parts
     LAUNCHED();
-    r = shard_exchange_and_merge(c, nq, k, PartsRule::text, 1, host, out_docs, out_scores, out_part, out_counts, stream);
+    r = shard_exchange_and_merge(c, nq, k, PartsRule::text, 1, o, stream);
     if (r) return r;
-    if (host) {
-        if (out_total) CU(cudaMemcpyAsync(out_total, d_total, (size_t)nq * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 // ---- rank fusion + the fused shard search (SURVEY 8f rank 4) --------------------------------------------------------------
 int nidx_txt_set_doc_keys(nidx_txt_segment* t, const uint64_t* keys) {
     if (!t) return fail(NIDX_EINVAL, "null segment");
-    CU(cudaSetDevice(t->device));
-    if (!keys) { cudaFree(t->d_doc_keys); t->d_doc_keys = nullptr; return 0; }
-    if (!t->d_doc_keys) CU(cudaMalloc(&t->d_doc_keys, std::max<size_t>(t->n_docs, 1) * 8));
-    CU(cudaMemcpy(t->d_doc_keys, keys, (size_t)t->n_docs * 8, cudaMemcpyHostToDevice));
-    return 0;
+    return set_rows(t->device, &t->d_doc_keys, keys, t->n_docs);
 }
 
 }  // extern "C"
-
-static WorkspacePool* plan_pool(int device) {
-    static std::mutex mu;
-    static WorkspacePool* pools[64] = {nullptr};
-    std::lock_guard<std::mutex> g(mu);
-    if (device < 0 || device >= 64) return nullptr;
-    if (!pools[device]) pools[device] = new WorkspacePool();
-    return pools[device];
-}
 
 // sources already on the device; outputs on the device
 static int rrf_launch(const RrfSourceDev* src, int n_sources, int nq, double k, uint64_t* out_keys, double* out_scores, uint32_t* out_refs, int32_t* out_counts,
@@ -2709,47 +2715,27 @@ int nidx_rank_fusion_rrf(int32_t device, const nidx_rrf_source* sources, int32_t
         if (sources[i].k >= (1 << 24)) return fail(NIDX_EINVAL, "rank fusion source %d: k too large", i);
         cap += sources[i].k;
     }
-    RrfSourceDev dev[RF_MAX_SOURCES];
     WorkspacePool* pool = plan_pool(device);
     if (!pool) return fail(NIDX_EINVAL, "device %d", device);
     WsGuard g(*pool, stream);
-    Workspace& w = *g.w;
-    uint64_t* d_keys = out_keys; double* d_sc = out_scores; uint32_t* d_refs = out_refs; int32_t* d_cnt = out_counts;
-    if (host) {
-        size_t in_bytes = 0;
-        auto al16 = [](size_t b) { return (b + 15) / 16 * 16; };
-        for (int i = 0; i < n_sources; ++i) in_bytes += al16((size_t)nq * sources[i].k * 8) + al16((size_t)nq * sources[i].k * 4) + al16((size_t)nq * 4);
-        ENSURE(w.queries, in_bytes);
-        ENSURE(w.scores, (size_t)nq * cap * 20 + (size_t)nq * 4 + 128);
-        unsigned char* p = w.queries.as<unsigned char>();
-        for (int i = 0; i < n_sources; ++i) {
-            size_t nk = (size_t)nq * sources[i].k;
-            uint64_t* dk = reinterpret_cast<uint64_t*>(p); p += al16(nk * 8);
-            float* ds = reinterpret_cast<float*>(p); p += al16(nk * 4);
-            int32_t* dc = reinterpret_cast<int32_t*>(p); p += al16((size_t)nq * 4);
-            CU(cudaMemcpyAsync(dk, sources[i].keys, nk * 8, cudaMemcpyHostToDevice, stream));
-            CU(cudaMemcpyAsync(ds, sources[i].scores, nk * 4, cudaMemcpyHostToDevice, stream));
-            if (sources[i].counts) CU(cudaMemcpyAsync(dc, sources[i].counts, (size_t)nq * 4, cudaMemcpyHostToDevice, stream));
-            dev[i] = RrfSourceDev{dk, ds, sources[i].counts ? dc : nullptr, sources[i].k, sources[i].weight};
-        }
-        unsigned char* o = w.scores.as<unsigned char>();
-        d_keys = reinterpret_cast<uint64_t*>(o); o += (size_t)nq * cap * 8;
-        d_sc = reinterpret_cast<double*>(o); o += (size_t)nq * cap * 8;
-        d_refs = reinterpret_cast<uint32_t*>(o); o += al16((size_t)nq * cap * 4);
-        d_cnt = reinterpret_cast<int32_t*>(o);
-    } else {
-        for (int i = 0; i < n_sources; ++i) dev[i] = RrfSourceDev{sources[i].keys, sources[i].scores, sources[i].counts, sources[i].k, sources[i].weight};
+    Stage st(stream, host, host);
+    RrfSourceDev dev[RF_MAX_SOURCES];
+    for (int i = 0; i < n_sources; ++i) {
+        const size_t nk = (size_t)nq * sources[i].k;
+        dev[i] = RrfSourceDev{nullptr, nullptr, nullptr, sources[i].k, sources[i].weight};
+        st.in(sources[i].keys, nk, &dev[i].keys);
+        st.in(sources[i].scores, nk, &dev[i].scores);
+        st.in(sources[i].counts, (size_t)nq, &dev[i].counts);
     }
-    r = rrf_launch(dev, n_sources, nq, k, d_keys, d_sc, d_refs, d_cnt, stream);
+    uint64_t* d_keys; double* d_sc; uint32_t* d_refs; int32_t* d_cnt;
+    st.out(out_keys, (size_t)nq * cap, &d_keys);
+    st.out(out_scores, (size_t)nq * cap, &d_sc);
+    st.out(out_refs, (size_t)nq * cap, &d_refs);
+    st.out(out_counts, (size_t)nq, &d_cnt);
+    r = st.place(g.w->stage);
+    if (!r) r = rrf_launch(dev, n_sources, nq, k, d_keys, d_sc, d_refs, d_cnt, stream);
     if (r) return r;
-    if (host) {
-        CU(cudaMemcpyAsync(out_keys, d_keys, (size_t)nq * cap * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_scores, d_sc, (size_t)nq * cap * 8, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_refs, d_refs, (size_t)nq * cap * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaMemcpyAsync(out_counts, d_cnt, (size_t)nq * 4, cudaMemcpyDeviceToHost, stream));
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_response* rs, int mem, void* stream_) {
@@ -2767,7 +2753,6 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
     if (fuse && (!rs->fused_keys || !rs->fused_scores || !rs->fused_refs || !rs->fused_counts)) return fail(NIDX_EINVAL, "rank fusion: outputs are required");
     int r = check_device(device);
     if (r) return r;
-    CU(cudaSetDevice(device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const bool host = mem == NIDX_MEM_HOST;
     PlanStreams& ps = g_plan_streams;
@@ -2777,49 +2762,47 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
     if ((rq->vec && kv <= 0) || (rq->par && kp <= 0) || (rq->doc && kd <= 0)) return fail(NIDX_EINVAL, "k must be positive");
     WorkspacePool* pool = plan_pool(device);
     WsGuard g(*pool, stream);
-    Workspace& w = *g.w;
-    // device-side results (the callers' buffers, or staging when they are host buffers) + fusion scratch
-    size_t nv = (size_t)nq * kv, np = (size_t)nq * kp, nd = (size_t)nq * kd, nf = (size_t)nq * (kv + kp), cw = ((size_t)nq * 4 + 15) / 16 * 16;
-    size_t stage_bytes = host ? nv * 8 + np * 8 + nd * 8 + 3 * cw + 2 * (size_t)nq * 8 + nf * 20 + cw : 0;
-    size_t key_bytes = fuse ? (nv + np) * 8 : 0;
-    ENSURE(w.scores, stage_bytes + key_bytes + 512);
-    unsigned char* p = w.scores.as<unsigned char>();
-    auto take = [&](size_t bytes) { unsigned char* q = p; p += (bytes + 15) / 16 * 16; return q; };
-    uint32_t *d_vid = rs->vec_ids, *d_pdoc = rs->par_docs, *d_ddoc = rs->doc_docs, *d_frf = rs->fused_refs;
-    float *d_vsc = rs->vec_scores, *d_psc = rs->par_scores, *d_dsc = rs->doc_scores;
-    int32_t *d_vcnt = rs->vec_counts, *d_pcnt = rs->par_counts, *d_dcnt = rs->doc_counts, *d_fcnt = rs->fused_counts;
-    uint64_t *d_ptot = rs->par_total, *d_dtot = rs->doc_total, *d_fkey = rs->fused_keys;
-    double* d_fsc = rs->fused_scores;
-    if (host) {
-        if (rq->vec) { d_vid = (uint32_t*)take(nv * 4); d_vsc = (float*)take(nv * 4); d_vcnt = (int32_t*)take(cw); }
-        if (rq->par) { d_pdoc = (uint32_t*)take(np * 4); d_psc = (float*)take(np * 4); d_pcnt = (int32_t*)take(cw); d_ptot = (uint64_t*)take((size_t)nq * 8); }
-        if (rq->doc) { d_ddoc = (uint32_t*)take(nd * 4); d_dsc = (float*)take(nd * 4); d_dcnt = (int32_t*)take(cw); d_dtot = (uint64_t*)take((size_t)nq * 8); }
-        if (fuse) { d_fkey = (uint64_t*)take(nf * 8); d_fsc = (double*)take(nf * 8); d_frf = (uint32_t*)take(nf * 4); d_fcnt = (int32_t*)take(cw); }
+    // device-side results (the callers' buffers, or staged when they are host buffers) + fusion scratch
+    const size_t nv = (size_t)nq * kv, np = (size_t)nq * kp, nd = (size_t)nq * kd, nf = (size_t)nq * (kv + kp);
+    Stage st(stream, host, host);
+    uint32_t *d_vid, *d_pdoc, *d_ddoc, *d_frf;
+    float *d_vsc, *d_psc, *d_dsc;
+    int32_t *d_vcnt, *d_pcnt, *d_dcnt, *d_fcnt;
+    uint64_t *d_ptot, *d_dtot, *d_fkey, *d_vkey = nullptr, *d_pkey = nullptr;
+    double* d_fsc;
+    if (rq->vec) { st.out(rs->vec_ids, nv, &d_vid); st.out(rs->vec_scores, nv, &d_vsc); st.out(rs->vec_counts, (size_t)nq, &d_vcnt); }
+    if (rq->par) {
+        st.out(rs->par_docs, np, &d_pdoc); st.out(rs->par_scores, np, &d_psc); st.out(rs->par_counts, (size_t)nq, &d_pcnt);
+        st.out(rs->par_total, (size_t)nq, &d_ptot);
     }
-    uint64_t *d_vkey = nullptr, *d_pkey = nullptr;
-    if (fuse) { d_vkey = (uint64_t*)take(nv * 8); d_pkey = (uint64_t*)take(np * 8); }
+    if (rq->doc) {
+        st.out(rs->doc_docs, nd, &d_ddoc); st.out(rs->doc_scores, nd, &d_dsc); st.out(rs->doc_counts, (size_t)nq, &d_dcnt);
+        st.out(rs->doc_total, (size_t)nq, &d_dtot);
+    }
+    if (fuse) {
+        st.out(rs->fused_keys, nf, &d_fkey); st.out(rs->fused_scores, nf, &d_fsc); st.out(rs->fused_refs, nf, &d_frf);
+        st.out(rs->fused_counts, (size_t)nq, &d_fcnt);
+        st.out((uint64_t*)nullptr, nv, &d_vkey);   // scratch: the keys of the two fused lists
+        st.out((uint64_t*)nullptr, np, &d_pkey);
+    }
+    r = st.place(g.w->stage);
+    if (r) return r;
 
     // fork: the three index searches run on their own streams, each ordered after whatever the caller enqueued before this call
     CU(cudaEventRecord(ps.fork, stream));
     for (int i = 0; i < 3; ++i) CU(cudaStreamWaitEvent(ps.s[i], ps.fork, 0));
     // (text searches first: with host queries they enqueue without waiting; the vector search may wait for a filter count)
-    if (rq->par) {
-        r = txt_search_impl(rq->par, rq->par_terms, rq->par_off, nq, host, false, rq->par_params, d_pdoc, d_psc, d_pcnt, d_ptot, ps.s[1]);
+    for (int i : {1, 2, 0}) {
+        if (i == 1 && rq->par)
+            r = txt_search_impl(rq->par, rq->par_terms, rq->par_off, nq, host, false, rq->par_params, d_pdoc, d_psc, d_pcnt, d_ptot, ps.s[1]);
+        else if (i == 2 && rq->doc)
+            r = txt_search_impl(rq->doc, rq->doc_terms, rq->doc_off, nq, host, false, rq->doc_params, d_ddoc, d_dsc, d_dcnt, d_dtot, ps.s[2]);
+        else if (i == 0 && rq->vec)
+            r = vec_search_impl(rq->vec, rq->queries, nq, rq->ldq, host, false, rq->vec_params, d_vid, d_vsc, d_vcnt, ps.s[0], rq->formula, rq->n_formula);
+        else continue;
         if (r) return r;
-        CU(cudaEventRecord(ps.join[1], ps.s[1]));
-        CU(cudaStreamWaitEvent(stream, ps.join[1], 0));
-    }
-    if (rq->doc) {
-        r = txt_search_impl(rq->doc, rq->doc_terms, rq->doc_off, nq, host, false, rq->doc_params, d_ddoc, d_dsc, d_dcnt, d_dtot, ps.s[2]);
-        if (r) return r;
-        CU(cudaEventRecord(ps.join[2], ps.s[2]));
-        CU(cudaStreamWaitEvent(stream, ps.join[2], 0));
-    }
-    if (rq->vec) {
-        r = vec_search_impl(rq->vec, rq->queries, nq, rq->ldq, host, false, rq->vec_params, d_vid, d_vsc, d_vcnt, ps.s[0], rq->formula, rq->n_formula);
-        if (r) return r;
-        CU(cudaEventRecord(ps.join[0], ps.s[0]));
-        CU(cudaStreamWaitEvent(stream, ps.join[0], 0));
+        CU(cudaEventRecord(ps.join[i], ps.s[i]));
+        CU(cudaStreamWaitEvent(stream, ps.join[i], 0));
     }
     // join + rank fusion of the paragraph (keyword) and vector (semantic) results on the caller's stream
     if (fuse) {
@@ -2834,15 +2817,7 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
         r = rrf_launch(src, 2, nq, rq->rrf_k, d_fkey, d_fsc, d_frf, d_fcnt, stream);
         if (r) return r;
     }
-    if (host) {
-        auto back = [&](void* dst, const void* src, size_t bytes) { return dst ? cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, stream) : cudaSuccess; };
-        if (rq->vec) { CU(back(rs->vec_ids, d_vid, nv * 4)); CU(back(rs->vec_scores, d_vsc, nv * 4)); CU(back(rs->vec_counts, d_vcnt, (size_t)nq * 4)); }
-        if (rq->par) { CU(back(rs->par_docs, d_pdoc, np * 4)); CU(back(rs->par_scores, d_psc, np * 4)); CU(back(rs->par_counts, d_pcnt, (size_t)nq * 4)); CU(back(rs->par_total, d_ptot, (size_t)nq * 8)); }
-        if (rq->doc) { CU(back(rs->doc_docs, d_ddoc, nd * 4)); CU(back(rs->doc_scores, d_dsc, nd * 4)); CU(back(rs->doc_counts, d_dcnt, (size_t)nq * 4)); CU(back(rs->doc_total, d_dtot, (size_t)nq * 8)); }
-        if (fuse) { CU(back(rs->fused_keys, d_fkey, nf * 8)); CU(back(rs->fused_scores, d_fsc, nf * 8)); CU(back(rs->fused_refs, d_frf, nf * 4)); CU(back(rs->fused_counts, d_fcnt, (size_t)nq * 4)); }
-        CU(cudaStreamSynchronize(stream));
-    }
-    return 0;
+    return st.finish();
 }
 
 }  // extern "C"

@@ -300,8 +300,8 @@ class EmulatedLib:
             ids[:], sc[:], cnt[:] = NIL, 0, 0
             return 0
         method = p.method
-        if method == _lib.NIDX_METHOD_AUTO:
-            if s.g is None or (matching == 0 and filtered):
+        if method == _lib.NIDX_METHOD_AUTO:                                 # api.cu: choose_method
+            if s.g is None:
                 method = _lib.NIDX_METHOD_BRUTE
             else:
                 method = _lib.NIDX_METHOD_HNSW if O.use_hnsw(s.n_par, matching, k, M=s.m) else _lib.NIDX_METHOD_BRUTE
