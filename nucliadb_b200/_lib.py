@@ -2,6 +2,12 @@
 
 The CUDA library is the product: if it is missing or no CUDA device is usable the package fails
 loudly -- there is no CPU fallback anywhere in ``nucliadb_b200``.
+
+``SIGNATURES`` declares every function of the header once: name -> (restype, argtypes), applied to the library by ``load()``.
+Scalars take their exact width (``int`` = ``int32_t``); data buffers, handles, out-handles and streams are ``void*``; pointers to
+the ABI's own structs are typed, so passing the wrong struct raises.  ctypes then converts plain Python values at every call
+site and rejects too few arguments or a wrong type.  It does not catch extra trailing arguments, and it does not range-check
+integers (``-1`` passed for a ``uint64_t`` arrives as 2^64 - 1).
 """
 from __future__ import annotations
 
@@ -20,22 +26,6 @@ NIDX_ORDER_CREATED, NIDX_ORDER_MODIFIED = 0, 1   # OrderBy.OrderField
 NIDX_ORDER_DESC, NIDX_ORDER_ASC = 0, 1           # OrderBy.OrderType
 NIDX_DATE_NONE = -(1 << 63)                      # a document without a date
 NIL = 0xFFFFFFFF
-
-# every symbol include/nidx_b200.h declares (tests check the .so exports exactly these)
-SYMBOLS = [
-    "nidx_last_error", "nidx_device_count", "nidx_launch_count",
-    "nidx_vec_create", "nidx_vec_open", "nidx_vec_save", "nidx_vec_close", "nidx_vec_len", "nidx_vec_device_vectors",
-    "nidx_use_hnsw", "nidx_hnsw_levels", "nidx_normalize_vectors", "nidx_vec_build_hnsw", "nidx_vec_extend_hnsw", "nidx_vec_graph_dims", "nidx_vec_set_graph", "nidx_vec_get_graph", "nidx_vec_set_alive",
-    "nidx_vec_set_inverted_index", "nidx_vec_filter", "nidx_vec_search_formula",
-    "nidx_vec_search", "nidx_merge_topk", "nidx_merge_vector_parts", "nidx_vec_counters", "nidx_vec_counters_ex", "nidx_vec_exact_rows", "nidx_vec_scan_counters", "nidx_vec_last_kernel_ms",
-    "nidx_vec_rabitq_encode", "nidx_vec_rabitq_codes", "nidx_vec_rabitq_estimate",
-    "nidx_txt_create", "nidx_txt_set_stats", "nidx_txt_set_alive", "nidx_txt_close", "nidx_txt_search", "nidx_txt_last_kernel_ms",
-    "nidx_txt_set_facets", "nidx_txt_facet_buckets", "nidx_txt_search_faceted", "nidx_txt_facet_count_all",
-    "nidx_txt_set_dates", "nidx_txt_search_ordered", "nidx_txt_list_ordered",
-    "nidx_shard_unique_id", "nidx_shard_init", "nidx_shard_destroy", "nidx_vec_set_paragraph_keys", "nidx_vec_search_sharded",
-    "nidx_vec_shard_record", "nidx_shard_merge", "nidx_txt_search_sharded",
-    "nidx_txt_set_doc_keys", "nidx_rank_fusion_rrf", "nidx_shard_search",
-]
 
 
 class NidxError(RuntimeError):
@@ -95,6 +85,70 @@ class ShardSearchResponse(C.Structure):
                                            "doc_docs", "doc_scores", "doc_counts", "doc_total", "fused_keys", "fused_scores", "fused_refs", "fused_counts")]
 
 
+# every function include/nidx_b200.h declares (tests check the table against the header and the .so's exports)
+i32, u32, i64, u64, f64, P = C.c_int32, C.c_uint32, C.c_int64, C.c_uint64, C.c_double, C.c_void_p
+CFG, VSP, NODES, TSP = C.POINTER(VecConfig), C.POINTER(VecSearchParams), C.POINTER(FilterNode), C.POINTER(TxtSearchParams)
+REQ, ORDER, RRF = C.POINTER(TxtFacetRequest), C.POINTER(TxtOrder), C.POINTER(RrfSource)
+SIGNATURES = {
+    "nidx_last_error": (C.c_char_p, []),
+    "nidx_device_count": (i32, []),
+    "nidx_launch_count": (u64, []),
+    "nidx_vec_create": (i32, [CFG, P, u64, i32, i32, P, P]),
+    "nidx_vec_open": (i32, [CFG, C.c_char_p, P]),
+    "nidx_vec_save": (i32, [P, C.c_char_p]),
+    "nidx_vec_close": (None, [P]),
+    "nidx_vec_len": (u64, [P]),
+    "nidx_vec_device_vectors": (P, [P, P]),
+    "nidx_vec_build_hnsw": (i32, [P, u64, i32, P]),
+    "nidx_hnsw_levels": (i32, [u64, i32, u64, P]),
+    "nidx_normalize_vectors": (i32, [i32, P, u64, i32, i32, i32, P]),
+    "nidx_use_hnsw": (i32, [u64, u64, u64, i32, i32]),
+    "nidx_vec_extend_hnsw": (i32, [P, u64, P, P, P, P, P, u32, u32, u64, i32, P]),
+    "nidx_vec_graph_dims": (i32, [P, P, P, P, P, P]),
+    "nidx_vec_set_graph": (i32, [P, P, P, P, P, P]),
+    "nidx_vec_get_graph": (i32, [P, P, P, P, P, P]),
+    "nidx_vec_set_alive": (i32, [P, P, i32]),
+    "nidx_vec_search": (i32, [P, P, i32, i32, i32, VSP, P, P, P, P]),
+    "nidx_vec_set_inverted_index": (i32, [P, i32, u32, P, P, P, P]),
+    "nidx_vec_filter": (i32, [P, NODES, i32, P, i32, P, P]),
+    "nidx_vec_search_formula": (i32, [P, P, i32, i32, i32, VSP, NODES, i32, P, P, P, P]),
+    "nidx_merge_topk": (i32, [i32, P, P, i32, i64, i32, i32, P, P, P, P]),
+    "nidx_merge_vector_parts": (i32, [i32, P, P, i32, i64, i32, i32, P, P, P, P]),
+    "nidx_vec_counters": (i32, [P, P]),
+    "nidx_vec_counters_ex": (i32, [P, P]),
+    "nidx_vec_exact_rows": (i32, [P, P]),
+    "nidx_vec_scan_counters": (i32, [P, P]),
+    "nidx_vec_rabitq_encode": (i32, [P, P]),
+    "nidx_vec_rabitq_codes": (i32, [P, P]),
+    "nidx_vec_rabitq_estimate": (i32, [P, P, i32, i32, i32, P, P, P]),
+    "nidx_vec_last_kernel_ms": (i32, [P, P]),
+    "nidx_txt_create": (i32, [i32, u32, u32, P, P, P, P, P]),
+    "nidx_txt_set_stats": (i32, [P, u64, u64, P]),
+    "nidx_txt_set_alive": (i32, [P, P]),
+    "nidx_txt_close": (None, [P]),
+    "nidx_txt_search": (i32, [P, P, P, i32, i32, TSP, P, P, P, P, P]),
+    "nidx_txt_last_kernel_ms": (i32, [P, P]),
+    "nidx_txt_set_facets": (i32, [P, u32, P, P, P, P]),
+    "nidx_txt_facet_buckets": (i32, [P, REQ, P, P, u32, P]),
+    "nidx_txt_search_faceted": (i32, [P, P, P, i32, i32, TSP, REQ, P, P, P, P, P, P]),
+    "nidx_txt_facet_count_all": (i32, [P, REQ, i32, P, P]),
+    "nidx_txt_set_dates": (i32, [P, P, P]),
+    "nidx_txt_search_ordered": (i32, [P, P, P, i32, i32, TSP, ORDER, REQ, P, P, P, P, P, P]),
+    "nidx_txt_list_ordered": (i32, [P, ORDER, i32, i32, P, P, P, P, P]),
+    "nidx_shard_unique_id": (i32, [P]),
+    "nidx_shard_init": (i32, [P, i32, i32, i32, P]),
+    "nidx_shard_destroy": (None, [P]),
+    "nidx_vec_set_paragraph_keys": (i32, [P, P]),
+    "nidx_vec_search_sharded": (i32, [P, P, P, i32, i32, i32, VSP, i32, P, P, P, P, P]),
+    "nidx_vec_shard_record": (i32, [P, P, i32, i32, i32, VSP, i32, i32, P, P]),
+    "nidx_shard_merge": (i32, [i32, P, i32, i32, i32, i32, i32, i32, P, P, P, P, P]),
+    "nidx_txt_search_sharded": (i32, [P, P, P, P, i32, i32, TSP, P, P, P, P, P, P]),
+    "nidx_txt_set_doc_keys": (i32, [P, P]),
+    "nidx_rank_fusion_rrf": (i32, [i32, RRF, i32, i32, f64, i32, P, P, P, P, P]),
+    "nidx_shard_search": (i32, [C.POINTER(ShardSearchRequest), C.POINTER(ShardSearchResponse), i32, P]),
+}
+SYMBOLS = list(SIGNATURES)
+
 _lib = None
 
 
@@ -107,13 +161,9 @@ def load():
         raise ImportError(f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                           "(nvcc, sm_90a). nucliadb_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
-    L.nidx_last_error.restype = C.c_char_p
-    L.nidx_launch_count.restype = C.c_uint64
-    L.nidx_vec_len.restype = C.c_uint64
-    L.nidx_vec_device_vectors.restype = C.c_void_p
-    L.nidx_vec_close.restype = None
-    L.nidx_txt_close.restype = None
-    L.nidx_shard_destroy.restype = None
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(L, name)
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 

@@ -117,51 +117,37 @@ def shard_record(segment, queries, k, rank=0, dedup=False, ef=0, min_score=-1.0,
     import ctypes as C
 
     import numpy as np
-    import torch
 
     from . import _lib
-    from .segment import _is_torch, _torch_stream
+    from .segment import _is_torch, _stage
 
-    dev = segment.cfg.device
-    p = _lib.VecSearchParams(k, ef, min_score, int(with_duplicates), _lib.NIDX_METHOD_AUTO if method is None else method, None, 0)
+    _, stream, alloc = _stage(segment.cfg.device, True)     # the record is device memory, whatever memory the queries are in
     if _is_torch(queries):
         mem = _lib.NIDX_MEM_DEVICE
-        if filter_bits is not None:
-            p.filter_bits = filter_bits.data_ptr()
     else:
         mem = _lib.NIDX_MEM_HOST
         queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
-        if filter_bits is not None:
-            filter_bits = np.ascontiguousarray(filter_bits, dtype=np.uint64)
-            p.filter_bits = filter_bits.ctypes.data
+        filter_bits = None if filter_bits is None else np.ascontiguousarray(filter_bits, dtype=np.uint64)
+    p = _lib.VecSearchParams(k, ef, min_score, int(with_duplicates), _lib.NIDX_METHOD_AUTO if method is None else method, _lib.ptr(filter_bits), 0)
     nq, ldq = queries.shape
-    if out is None:
-        out = torch.empty(nq * k * (6 if dedup else 2), dtype=torch.int32, device=torch.device("cuda", dev))
-    _lib.check(_lib.load().nidx_vec_shard_record(segment._h, _lib.ptr(queries), C.c_int32(nq), C.c_int32(ldq), mem, C.byref(p), C.c_int32(rank),
-                                                 C.c_int32(int(dedup)), _lib.ptr(out), _torch_stream(dev)))
+    out = out if out is not None else alloc(nq * k * (6 if dedup else 2), np.uint32)
+    _lib.check(_lib.load().nidx_vec_shard_record(segment._h, _lib.ptr(queries), nq, ldq, mem, C.byref(p), rank, int(dedup), _lib.ptr(out), stream))
     return out
 
 
 def shard_merge(records, n_parts, nq, k, dedup=False, with_duplicates=True, device=0, host=False):
     """nidx_shard_merge over n_parts records laid end to end in one torch CUDA tensor -> (ids local to their part, scores, part,
     counts): torch tensors on the device (asynchronous on the current stream), or numpy arrays with host=True."""
-    import ctypes as C
-
     import numpy as np
-    import torch
 
     from . import _lib
-    from .segment import _torch_stream
+    from .segment import _stage, _torch_stream
 
-    if host:
-        out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty((nq, k), dtype=np.int32), np.empty(nq, dtype=np.int32))
-    else:
-        dev = records.device
-        out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-               torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int32, device=dev))
-    _lib.check(_lib.load().nidx_shard_merge(C.c_int32(device), _lib.ptr(records), C.c_int32(n_parts), C.c_int32(nq), C.c_int32(k), C.c_int32(int(dedup)),
-                                            C.c_int32(int(with_duplicates)), _lib.NIDX_MEM_HOST if host else _lib.NIDX_MEM_DEVICE,
-                                            _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]), _torch_stream(device)))
+    mem, _, alloc = _stage(device, not host)
+    out = (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc((nq, k), np.int32), alloc(nq, np.int32))
+    # the records are device memory: the merge runs on the current torch stream whatever memory the outputs are in
+    _lib.check(_lib.load().nidx_shard_merge(device, _lib.ptr(records), n_parts, nq, k, int(dedup), int(with_duplicates), mem, *map(_lib.ptr, out),
+                                            _torch_stream(device)))
     return out
 
 
@@ -247,7 +233,7 @@ class ShardComm:
             payload = exchange(payload)
         ident = (C.c_uint8 * 128).from_buffer_copy(payload)
         self._h = C.c_void_p()
-        _lib.check(L.nidx_shard_init(ident, C.c_int32(rank), C.c_int32(world), C.c_int32(device), C.byref(self._h)))
+        _lib.check(L.nidx_shard_init(ident, rank, world, device, C.byref(self._h)))
         self.rank, self.world, self.device = rank, world, device
 
     def close(self):
@@ -271,29 +257,16 @@ class ShardComm:
         import numpy as np
 
         from . import _lib
-        from .segment import _is_torch, _torch_stream
+        from .segment import _is_torch, _stage
 
-        L = _lib.load()
         p = _lib.VecSearchParams(k, ef, min_score, int(with_duplicates), _lib.NIDX_METHOD_HNSW if method is None else method, None, 0)
-        if _is_torch(queries):
-            import torch
-
-            nq, ldq = queries.shape
-            dev = queries.device
-            if out is None:
-                out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-                       torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int32, device=dev))
-            _lib.check(L.nidx_vec_search_sharded(self._h, segment._h, _lib.ptr(queries), C.c_int32(nq), C.c_int32(ldq), _lib.NIDX_MEM_DEVICE, C.byref(p),
-                                                 C.c_int32(int(dedup)), _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]),
-                                                 _torch_stream(self.device)))
-            return out
-        queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
+        mem, stream, alloc = _stage(self.device, _is_torch(queries), stream)
+        if mem == _lib.NIDX_MEM_HOST:
+            queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
         nq, ldq = queries.shape
-        if out is None:
-            out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty((nq, k), dtype=np.int32), np.empty(nq, dtype=np.int32))
-        _lib.check(L.nidx_vec_search_sharded(self._h, segment._h, _lib.ptr(queries), C.c_int32(nq), C.c_int32(ldq), _lib.NIDX_MEM_HOST, C.byref(p),
-                                             C.c_int32(int(dedup)), _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]),
-                                             C.c_void_p(stream) if stream else None))
+        out = out or (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc((nq, k), np.int32), alloc(nq, np.int32))
+        _lib.check(_lib.load().nidx_vec_search_sharded(self._h, segment._h, _lib.ptr(queries), nq, ldq, mem, C.byref(p), int(dedup), *map(_lib.ptr, out),
+                                                       stream))
         return out
 
     def search_text(self, segment, query_terms, query_off, k, mode=0, use_tf=True, min_score=0.0, out=None):
@@ -303,28 +276,10 @@ class ShardComm:
         import numpy as np
 
         from . import _lib
-        from .segment import _is_torch, _torch_stream
 
-        L = _lib.load()
         p = _lib.TxtSearchParams(k, mode, int(use_tf), min_score, 0, 0.0, 0, 0)
-        if _is_torch(query_terms):
-            import torch
-
-            nq = query_off.numel() - 1
-            dev = query_terms.device
-            if out is None:
-                out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-                       torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int32, device=dev),
-                       torch.empty((nq,), dtype=torch.int64, device=dev))
-            _lib.check(L.nidx_txt_search_sharded(self._h, segment._h, _lib.ptr(query_terms), _lib.ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_DEVICE, C.byref(p),
-                                                 _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]), _lib.ptr(out[4]), _torch_stream(self.device)))
-            return out
-        query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
-        query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
-        nq = len(query_off) - 1
-        if out is None:
-            out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty((nq, k), dtype=np.int32), np.empty(nq, dtype=np.int32),
-                   np.empty(nq, dtype=np.uint64))
-        _lib.check(L.nidx_txt_search_sharded(self._h, segment._h, _lib.ptr(query_terms), _lib.ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_HOST, C.byref(p),
-                                             _lib.ptr(out[0]), _lib.ptr(out[1]), _lib.ptr(out[2]), _lib.ptr(out[3]), _lib.ptr(out[4]), None))
+        mem, stream, alloc, query_terms, query_off, nq = segment._queries(query_terms, query_off)
+        out = out or (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc((nq, k), np.int32), alloc(nq, np.int32), alloc(nq, np.uint64))
+        _lib.check(_lib.load().nidx_txt_search_sharded(self._h, segment._h, _lib.ptr(query_terms), _lib.ptr(query_off), nq, mem, C.byref(p), *map(_lib.ptr, out),
+                                                       stream))
         return out

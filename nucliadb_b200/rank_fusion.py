@@ -50,8 +50,8 @@ class ReciprocalRankFusion:
             cap += kk
         out_keys, out_scores = np.empty((1, cap), dtype=np.uint64), np.empty((1, cap), dtype=np.float64)
         out_refs, out_counts = np.empty((1, cap), dtype=np.uint32), np.empty(1, dtype=np.int32)
-        check(L.nidx_rank_fusion_rrf(C.c_int32(self.device), structs, C.c_int32(len(names)), C.c_int32(1), C.c_double(self._k), _lib.NIDX_MEM_HOST,
-                                     ptr(out_keys), ptr(out_scores), ptr(out_refs), ptr(out_counts), None))
+        check(L.nidx_rank_fusion_rrf(self.device, structs, len(names), 1, self._k, _lib.NIDX_MEM_HOST, ptr(out_keys), ptr(out_scores), ptr(out_refs),
+                                     ptr(out_counts), None))
         fused = []
         types = [_TYPE_OF.get(name, "RELATION_RELEVANCE") for name in names]
         for j in range(int(out_counts[0])):

@@ -27,6 +27,35 @@ def _torch_stream(device: int):
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+_SIGNED = {"uint32": "int32", "uint64": "int64"}   # torch has no usable unsigned 32 / 64-bit tensors
+
+
+def _stage(device: int, on_device: bool, stream: Optional[int] = None):
+    """Where a call's buffers live -> (mem, stream, alloc).  On the device the call is asynchronous on the current torch stream and
+    alloc(shape, numpy dtype) returns an uninitialised torch CUDA tensor of the same width (uint32 -> int32, uint64 -> int64).  On
+    the host the call runs on `stream` (a cudaStream_t as int; None = the default stream) and alloc returns a numpy array, zeroed
+    with zero=True (device outputs are left to the kernel: no fill is launched)."""
+    if on_device:
+        import torch
+
+        def alloc(shape, dtype, zero=False):
+            name = np.dtype(dtype).name
+            return torch.empty(shape, dtype=getattr(torch, _SIGNED.get(name, name)), device=torch.device("cuda", device))
+
+        return _lib.NIDX_MEM_DEVICE, _torch_stream(device), alloc
+    return _lib.NIDX_MEM_HOST, C.c_void_p(stream) if stream else None, lambda shape, dtype, zero=False: (np.zeros if zero else np.empty)(shape, dtype)
+
+
+def normalize(vectors: np.ndarray, device: int = 0) -> np.ndarray:
+    """utils::normalize_vector (nidx_vector/src/utils.rs:20-23) through nidx_normalize_vectors, in place: one vector [d] or rows
+    [n][d] of a C-contiguous float32 array.  The f32 fold runs sequentially on the device, bit-identical to the reference's."""
+    assert vectors.dtype == np.float32 and vectors.flags.c_contiguous   # else the rows below would be a copy
+    if vectors.size:
+        rows = vectors.reshape(-1, vectors.shape[-1])
+        check(_lib.require_device().nidx_normalize_vectors(device, ptr(rows), rows.shape[0], rows.shape[1], rows.shape[1], _lib.NIDX_MEM_HOST, None))
+    return vectors
+
+
 class VectorSegment:
     def __init__(self, handle, cfg: VecConfig):
         self._h, self.cfg = handle, cfg
@@ -47,7 +76,7 @@ class VectorSegment:
             n, ld = vectors.shape if vectors.ndim == 2 else (0, dimension)
             mem = _lib.NIDX_MEM_HOST
         par = None if paragraph_of is None else np.ascontiguousarray(paragraph_of, dtype=np.uint32)
-        check(L.nidx_vec_create(C.byref(cfg), ptr(vectors) if n else None, C.c_uint64(n), C.c_int32(ld), mem, ptr(par), C.byref(h)))
+        check(L.nidx_vec_create(C.byref(cfg), ptr(vectors) if n else None, n, ld, mem, ptr(par), C.byref(h)))
         return cls(h, cfg)
 
     @classmethod
@@ -78,7 +107,7 @@ class VectorSegment:
 
     # ---- graph ----------------------------------------------------------------------------------------
     def build_hnsw(self, seed=2, max_batch=4096):
-        check(_lib.load().nidx_vec_build_hnsw(self._h, C.c_uint64(seed), C.c_int32(max_batch), None))
+        check(_lib.load().nidx_vec_build_hnsw(self._h, seed, max_batch, None))
 
     def extend_hnsw(self, n_existing, level, adj0, adjU, w0, wU, entry_node, entry_layer, seed=2, max_batch=4096):
         """Reuse the graph of the first n_existing vectors and insert the rest (segment.rs:143-167)."""
@@ -87,8 +116,8 @@ class VectorSegment:
         adjU = np.ascontiguousarray(adjU, dtype=np.uint32)
         w0 = np.ascontiguousarray(w0, dtype=np.float32)
         wU = np.ascontiguousarray(wU, dtype=np.float32)
-        check(_lib.load().nidx_vec_extend_hnsw(self._h, C.c_uint64(n_existing), ptr(level), ptr(adj0), ptr(w0), ptr(adjU), ptr(wU), C.c_uint32(entry_node),
-                                               C.c_uint32(entry_layer), C.c_uint64(seed), C.c_int32(max_batch), None))
+        check(_lib.load().nidx_vec_extend_hnsw(self._h, n_existing, ptr(level), ptr(adj0), ptr(w0), ptr(adjU), ptr(wU), entry_node, entry_layer, seed,
+                                               max_batch, None))
 
     def graph_dims(self):
         s0, su, rows, en, el = C.c_int32(), C.c_int32(), C.c_uint64(), C.c_uint32(), C.c_uint32()
@@ -123,40 +152,46 @@ class VectorSegment:
         keys = None if keys is None else np.ascontiguousarray(keys, dtype=np.uint64)
         check(_lib.load().nidx_vec_set_paragraph_keys(self._h, ptr(keys)))
 
+    # ---- filters (ParagraphInvertedIndexes, inverted_index/paragraph.rs) ----------------------------------
+    def set_inverted_index(self, which, keys, postings):
+        """ParagraphInvertedIndexes::build (inverted_index/paragraph.rs:74-106) for one index (_lib.NIDX_INV_*): keys (bytes) sorted
+        bytewise as in the fst, and for each key its paragraphs, ascending.  The postings go to HBM, where filter formulas are
+        evaluated."""
+        key_bytes, key_off = _pack_keys(keys)
+        post_off = np.zeros(len(keys) + 1, dtype=np.uint64)
+        post_off[1:] = np.cumsum([len(p) for p in postings]) if len(keys) else []
+        flat = np.asarray([p for ps in postings for p in ps] or [0], dtype=np.uint32)
+        check(_lib.load().nidx_vec_set_inverted_index(self._h, which, len(keys), ptr(key_bytes), ptr(key_off), ptr(post_off), ptr(flat)))
+
+    def filter(self, nodes, n, out_bits: Optional[np.ndarray] = None) -> int:
+        """nidx_vec_filter: the formula (n FilterNodes in pre-order) AND the alive set, on the device -> the number of matching
+        paragraphs; the bitset goes to out_bits (host uint64 words, (paragraphs + 63) // 64) when given."""
+        matching = C.c_uint64()
+        check(_lib.load().nidx_vec_filter(self._h, nodes, n, ptr(out_bits), _lib.NIDX_MEM_HOST, C.byref(matching), None))
+        return matching.value
+
     # ---- search ----------------------------------------------------------------------------------------
     def search(self, queries, k: int, ef: int = 0, min_score: float = -1.0, with_duplicates=True, method=_lib.NIDX_METHOD_AUTO,
-               filter_bits=None, filter_matching: int = 0, out=None, stream: Optional[int] = None):
+               filter_bits=None, filter_matching: int = 0, formula=None, out=None, stream: Optional[int] = None):
         """Batch search.  numpy in -> numpy out (host path, synchronous); torch CUDA tensors in -> torch
         CUDA tensors out (device path, asynchronous on the current stream).  `stream` (a cudaStream_t as int) lets concurrent
-        host-path callers overlap their copies with each other's kernels.  Returns (ids, scores, counts)."""
-        L = _lib.load()
-        p = VecSearchParams(k, ef, min_score, int(with_duplicates), method, None, filter_matching)
-        if _is_torch(queries):
+        host-path callers overlap their copies with each other's kernels.  `formula` (a FilterNode array in pre-order) is a filter
+        evaluated on the device (nidx_vec_search_formula) instead of filter_bits.  Returns (ids, scores, counts)."""
+        mem, stream, alloc = _stage(self.cfg.device, _is_torch(queries), stream)
+        if mem == _lib.NIDX_MEM_DEVICE:
             import torch
 
             assert queries.is_cuda and queries.is_contiguous() and queries.dtype == torch.float32
-            nq, ldq = queries.shape
-            dev = queries.device
-            if out is None:
-                out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-                       torch.empty((nq,), dtype=torch.int32, device=dev))
-            if filter_bits is not None:
-                p.filter_bits = filter_bits.data_ptr()
-            check(L.nidx_vec_search(self._h, ptr(queries), C.c_int32(nq), C.c_int32(ldq), _lib.NIDX_MEM_DEVICE, C.byref(p), ptr(out[0]), ptr(out[1]),
-                                    ptr(out[2]), _torch_stream(self.cfg.device)))
-            return out
-        queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
+        else:
+            queries = np.ascontiguousarray(np.atleast_2d(queries), dtype=np.float32)
+            filter_bits = None if filter_bits is None else np.ascontiguousarray(filter_bits, dtype=np.uint64)
         nq, ldq = queries.shape
-        ids = np.empty((nq, k), dtype=np.uint32)
-        scores = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.int32)
-        keep = None
-        if filter_bits is not None:
-            keep = np.ascontiguousarray(filter_bits, dtype=np.uint64)
-            p.filter_bits = keep.ctypes.data
-        check(L.nidx_vec_search(self._h, ptr(queries), C.c_int32(nq), C.c_int32(ldq), _lib.NIDX_MEM_HOST, C.byref(p), ptr(ids), ptr(scores), ptr(counts),
-                                C.c_void_p(stream) if stream else None))
-        return ids, scores, counts
+        out = out or (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc(nq, np.int32))
+        p = VecSearchParams(k, ef, min_score, int(with_duplicates), method, ptr(filter_bits), filter_matching)
+        L = _lib.load()
+        fn, by_formula = (L.nidx_vec_search, ()) if formula is None else (L.nidx_vec_search_formula, (formula, len(formula)))
+        check(fn(self._h, ptr(queries), nq, ldq, mem, C.byref(p), *by_formula, ptr(out[0]), ptr(out[1]), ptr(out[2]), stream))
+        return out
 
     # ---- RaBitQ (vector_types/rabitq.rs) ----------------------------------------------------------------
     def rabitq_encode(self):
@@ -172,7 +207,7 @@ class VectorSegment:
         nq = queries.shape[0]
         est = np.empty((nq, len(self)), dtype=np.float32)
         err = np.empty((nq, len(self)), dtype=np.float32)
-        check(_lib.load().nidx_vec_rabitq_estimate(self._h, ptr(queries), C.c_int32(nq), C.c_int32(queries.shape[1]), _lib.NIDX_MEM_HOST, ptr(est), ptr(err), None))
+        check(_lib.load().nidx_vec_rabitq_estimate(self._h, ptr(queries), nq, queries.shape[1], _lib.NIDX_MEM_HOST, ptr(est), ptr(err), None))
         return est, err
 
     def last_kernel_ms(self) -> float:
@@ -205,14 +240,10 @@ class VectorSegment:
 
 
 def _merge_parts(entry, ids, scores, device, part_stride, out):
-    import torch
-
     n_parts, nq, k = ids.shape
-    if out is None:
-        out = (torch.empty((nq, k), dtype=ids.dtype, device=ids.device), torch.empty((nq, k), dtype=torch.float32, device=ids.device),
-               torch.empty((nq, k), dtype=torch.int32, device=ids.device))
-    check(getattr(_lib.load(), entry)(C.c_int32(device), ptr(ids), ptr(scores), C.c_int32(n_parts), C.c_int64(part_stride), C.c_int32(nq), C.c_int32(k),
-                                      ptr(out[0]), ptr(out[1]), ptr(out[2]), _torch_stream(device)))
+    _, stream, alloc = _stage(device, True)
+    out = out or (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc((nq, k), np.int32))
+    check(getattr(_lib.load(), entry)(device, ptr(ids), ptr(scores), n_parts, part_stride, nq, k, ptr(out[0]), ptr(out[1]), ptr(out[2]), stream))
     return out
 
 
@@ -242,6 +273,14 @@ def _facet_request(facets):
     return _lib.TxtFacetRequest(len(facets), ptr(kb), ptr(ko)), (kb, ko)
 
 
+def _txt_params(k, mode=_lib.NIDX_BM25_OR, use_tf=True, min_score=0.0, after=None, docaddr_base=0):
+    """nidx_txt_search_params; after = (score, mode, docaddr) with mode 1 Drop / 2 KeepAfter / 3 Keep (nidx_paragraph SearchAfter)."""
+    p = TxtSearchParams(k, mode, int(use_tf), min_score, 0, 0.0, 0, docaddr_base)
+    if after is not None:
+        p.after_score, p.after_mode, p.after_docaddr = float(after[0]), int(after[1]), int(after[2])
+    return p
+
+
 class TextSegment:
     def __init__(self, handle, n_docs, n_terms, device):
         self._h, self.n_docs, self.n_terms, self.device = handle, n_docs, n_terms, device
@@ -254,46 +293,32 @@ class TextSegment:
         post_tf = np.ascontiguousarray(post_tf, dtype=np.uint32)
         fieldnorm_id = np.ascontiguousarray(fieldnorm_id, dtype=np.uint8)
         h = C.c_void_p()
-        check(L.nidx_txt_create(C.c_int32(device), C.c_uint32(n_docs), C.c_uint32(n_terms), ptr(term_off), ptr(post_doc), ptr(post_tf), ptr(fieldnorm_id),
-                                C.byref(h)))
+        check(L.nidx_txt_create(device, n_docs, n_terms, ptr(term_off), ptr(post_doc), ptr(post_tf), ptr(fieldnorm_id), C.byref(h)))
         return cls(h, n_docs, n_terms, device)
 
     def set_stats(self, total_docs: int, total_tokens: int, doc_freq: Optional[np.ndarray] = None):
         df = None if doc_freq is None else np.ascontiguousarray(doc_freq, dtype=np.uint64)
-        check(_lib.load().nidx_txt_set_stats(self._h, C.c_uint64(total_docs), C.c_uint64(total_tokens), ptr(df)))
+        check(_lib.load().nidx_txt_set_stats(self._h, total_docs, total_tokens, ptr(df)))
 
     def set_alive(self, alive_bits: Optional[np.ndarray]):
         check(_lib.load().nidx_txt_set_alive(self._h, ptr(alive_bits)))
 
+    def _queries(self, query_terms, query_off):
+        """-> (mem, stream, alloc, query_terms, query_off, nq): torch CUDA int32 -> device path, anything else -> host uint32."""
+        mem, stream, alloc = _stage(self.device, _is_torch(query_terms))
+        if mem == _lib.NIDX_MEM_DEVICE:
+            return mem, stream, alloc, query_terms, query_off, query_off.numel() - 1
+        query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
+        return mem, stream, alloc, np.ascontiguousarray(query_terms, dtype=np.uint32), query_off, len(query_off) - 1
+
     def search(self, query_terms, query_off, k, mode=_lib.NIDX_BM25_OR, use_tf=True, min_score=0.0, out=None, after=None, docaddr_base=0):
         """query i = query_terms[query_off[i]:query_off[i+1]].  numpy -> host path, torch CUDA int32 -> device path.
         Returns (docs, scores, counts, total)."""
-        L = _lib.load()
-        # after = (score, mode, docaddr) with mode 1 Drop / 2 KeepAfter / 3 Keep (nidx_paragraph SearchAfter)
-        p = TxtSearchParams(k, mode, int(use_tf), min_score, 0, 0.0, 0, docaddr_base)
-        if after is not None:
-            p.after_score, p.after_mode, p.after_docaddr = float(after[0]), int(after[1]), int(after[2])
-        if _is_torch(query_terms):
-            import torch
-
-            nq = query_off.numel() - 1
-            dev = query_terms.device
-            if out is None:
-                out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-                       torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev))
-            check(L.nidx_txt_search(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_DEVICE, C.byref(p), ptr(out[0]), ptr(out[1]),
-                                    ptr(out[2]), ptr(out[3]), _torch_stream(self.device)))
-            return out
-        query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
-        query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
-        nq = len(query_off) - 1
-        docs = np.empty((nq, k), dtype=np.uint32)
-        scores = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.int32)
-        total = np.empty(nq, dtype=np.uint64)
-        check(L.nidx_txt_search(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_HOST, C.byref(p), ptr(docs), ptr(scores), ptr(counts),
-                                ptr(total), None))
-        return docs, scores, counts, total
+        p = _txt_params(k, mode, use_tf, min_score, after, docaddr_base)
+        mem, stream, alloc, query_terms, query_off, nq = self._queries(query_terms, query_off)
+        out = out or (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc(nq, np.int32), alloc(nq, np.uint64))
+        check(_lib.load().nidx_txt_search(self._h, ptr(query_terms), ptr(query_off), nq, mem, C.byref(p), *map(ptr, out), stream))
+        return out
 
     # ---- facets (tantivy FacetCollector; keys in the encoded form of include/nidx_b200.h: segments joined by 0x00) -----------
     def set_facets(self, keys, doc_off, doc_ords):
@@ -301,57 +326,35 @@ class TextSegment:
         kb, ko = _pack_keys(keys)
         doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
         doc_ords = np.ascontiguousarray(doc_ords, dtype=np.uint32)
-        check(_lib.load().nidx_txt_set_facets(self._h, C.c_uint32(len(keys)), ptr(kb), ptr(ko), ptr(doc_off), ptr(doc_ords)))
+        check(_lib.load().nidx_txt_set_facets(self._h, len(keys), ptr(kb), ptr(ko), ptr(doc_off), ptr(doc_ords)))
 
     def facet_buckets(self, facets):
         """facets: encoded facet keys -> (bucket_req, bucket_ord) uint32 arrays (include/nidx_b200.h nidx_txt_facet_buckets)."""
         req, _keep = _facet_request(facets)
         n = C.c_uint32()
-        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), None, None, C.c_uint32(0), C.byref(n)))
+        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), None, None, 0, C.byref(n)))
         b_req, b_ord = np.empty(n.value, dtype=np.uint32), np.empty(n.value, dtype=np.uint32)
-        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), ptr(b_req), ptr(b_ord), C.c_uint32(n.value), C.byref(n)))
+        check(_lib.load().nidx_txt_facet_buckets(self._h, C.byref(req), ptr(b_req), ptr(b_ord), n.value, C.byref(n)))
         return b_req, b_ord
 
     def search_faceted(self, query_terms, query_off, k, facets, mode=_lib.NIDX_BM25_OR, use_tf=True, min_score=0.0, after=None, docaddr_base=0):
         """search() + per-query facet bucket counts in the same pass: (docs, scores, counts, total, facet_counts[nq][n_buckets]).
         numpy -> host path, torch CUDA -> device path (as search())."""
-        L = _lib.load()
-        p = TxtSearchParams(k, mode, int(use_tf), min_score, 0, 0.0, 0, docaddr_base)
-        if after is not None:
-            p.after_score, p.after_mode, p.after_docaddr = float(after[0]), int(after[1]), int(after[2])
+        p = _txt_params(k, mode, use_tf, min_score, after, docaddr_base)
         nb = len(self.facet_buckets(facets)[0])
         req, _keep = _facet_request(facets)
-        if _is_torch(query_terms):
-            import torch
-
-            nq, dev = query_off.numel() - 1, query_terms.device
-            out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.float32, device=dev),
-                   torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev),
-                   torch.empty((nq, nb), dtype=torch.int32, device=dev))
-            check(L.nidx_txt_search_faceted(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_DEVICE, C.byref(p), C.byref(req),
-                                            *[ptr(o) for o in out], _torch_stream(self.device)))
-            return out
-        query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
-        query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
-        nq = len(query_off) - 1
-        out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.float32), np.empty(nq, dtype=np.int32), np.empty(nq, dtype=np.uint64),
-               np.zeros((nq, nb), dtype=np.uint32))
-        check(L.nidx_txt_search_faceted(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), _lib.NIDX_MEM_HOST, C.byref(p), C.byref(req),
-                                        *[ptr(o) for o in out], None))
+        mem, stream, alloc, query_terms, query_off, nq = self._queries(query_terms, query_off)
+        out = (alloc((nq, k), np.uint32), alloc((nq, k), np.float32), alloc(nq, np.int32), alloc(nq, np.uint64), alloc((nq, nb), np.uint32, zero=True))
+        check(_lib.load().nidx_txt_search_faceted(self._h, ptr(query_terms), ptr(query_off), nq, mem, C.byref(p), C.byref(req), *map(ptr, out), stream))
         return out
 
     def facet_count_all(self, facets, device_out=False):
         """Bucket counts over every alive document (uint32 [n_buckets]; device_out: a torch CUDA int32 tensor, device path)."""
         nb = len(self.facet_buckets(facets)[0])
         req, _keep = _facet_request(facets)
-        if device_out:
-            import torch
-
-            out = torch.empty(nb, dtype=torch.int32, device=f"cuda:{self.device}")
-            check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), _lib.NIDX_MEM_DEVICE, ptr(out), _torch_stream(self.device)))
-            return out
-        out = np.zeros(nb, dtype=np.uint32)
-        check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), _lib.NIDX_MEM_HOST, ptr(out), None))
+        mem, stream, alloc = _stage(self.device, device_out)
+        out = alloc(nb, np.uint32, zero=True)
+        check(_lib.load().nidx_txt_facet_count_all(self._h, C.byref(req), mem, ptr(out), stream))
         return out
 
     # ---- order by date (TopDocs::order_by_fast_field; seconds, NIDX_DATE_NONE = no date) ----------------------------------------
@@ -365,45 +368,26 @@ class TextSegment:
     def search_ordered(self, query_terms, query_off, k, field=_lib.NIDX_ORDER_CREATED, order=_lib.NIDX_ORDER_DESC, mode=_lib.NIDX_BM25_OR, facets=None):
         """search() ordered by date: (docs, dates, counts, total) plus the facet counts [nq][n_buckets] when `facets` (encoded keys)
         is given.  numpy -> host path, torch CUDA -> device path (as search())."""
-        L = _lib.load()
         p = TxtSearchParams(k, mode, 0, 0.0, 0, 0.0, 0, 0)
         o = _lib.TxtOrder(field, order)
         req, _keep = _facet_request(facets) if facets is not None else (None, None)
-        nb = len(self.facet_buckets(facets)[0]) if facets is not None else 0
-        if _is_torch(query_terms):
-            import torch
-
-            nq, dev = query_off.numel() - 1, query_terms.device
-            out = (torch.empty((nq, k), dtype=torch.int32, device=dev), torch.empty((nq, k), dtype=torch.int64, device=dev),
-                   torch.empty((nq,), dtype=torch.int32, device=dev), torch.empty((nq,), dtype=torch.int64, device=dev),
-                   torch.empty((nq, nb), dtype=torch.int32, device=dev))
-            stream, mem = _torch_stream(self.device), _lib.NIDX_MEM_DEVICE
-        else:
-            query_terms = np.ascontiguousarray(query_terms, dtype=np.uint32)
-            query_off = np.ascontiguousarray(query_off, dtype=np.uint32)
-            nq = len(query_off) - 1
-            out = (np.empty((nq, k), dtype=np.uint32), np.empty((nq, k), dtype=np.int64), np.empty(nq, dtype=np.int32), np.empty(nq, dtype=np.uint64),
-                   np.zeros((nq, nb), dtype=np.uint32))
-            stream, mem = None, _lib.NIDX_MEM_HOST
-        check(L.nidx_txt_search_ordered(self._h, ptr(query_terms), ptr(query_off), C.c_int32(nq), mem, C.byref(p), C.byref(o),
-                                        C.byref(req) if req is not None else None, ptr(out[0]), ptr(out[1]), ptr(out[2]), ptr(out[3]),
-                                        ptr(out[4]) if facets is not None else None, stream))
-        return out if facets is not None else out[:4]
+        mem, stream, alloc, query_terms, query_off, nq = self._queries(query_terms, query_off)
+        out = (alloc((nq, k), np.uint32), alloc((nq, k), np.int64), alloc(nq, np.int32), alloc(nq, np.uint64))
+        if facets is not None:
+            out += (alloc((nq, len(self.facet_buckets(facets)[0])), np.uint32, zero=True),)
+        check(_lib.load().nidx_txt_search_ordered(self._h, ptr(query_terms), ptr(query_off), nq, mem, C.byref(p), C.byref(o),
+                                                  C.byref(req) if req is not None else None, *map(ptr, out[:4]), ptr(out[4]) if facets is not None else None,
+                                                  stream))
+        return out
 
     def list_ordered(self, k, field=_lib.NIDX_ORDER_CREATED, order=_lib.NIDX_ORDER_DESC, device_out=False):
-        """The empty body ordered by date: the top k alive documents -> (docs [k], dates [k], count, total alive)."""
+        """The empty body ordered by date: the top k alive documents -> (docs [k], dates [k], count, total alive); with device_out
+        all four are torch CUDA tensors (count and total of one element), on the device path."""
         o = _lib.TxtOrder(field, order)
-        if device_out:
-            import torch
-
-            dev = f"cuda:{self.device}"
-            out = (torch.empty(k, dtype=torch.int32, device=dev), torch.empty(k, dtype=torch.int64, device=dev), torch.empty(1, dtype=torch.int32, device=dev),
-                   torch.empty(1, dtype=torch.int64, device=dev))
-            check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), C.c_int32(k), _lib.NIDX_MEM_DEVICE, *[ptr(x) for x in out], _torch_stream(self.device)))
-            return out
-        docs, dates, count, total = np.empty(k, dtype=np.uint32), np.empty(k, dtype=np.int64), np.zeros(1, dtype=np.int32), np.zeros(1, dtype=np.uint64)
-        check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), C.c_int32(k), _lib.NIDX_MEM_HOST, ptr(docs), ptr(dates), ptr(count), ptr(total), None))
-        return docs, dates, int(count[0]), int(total[0])
+        mem, stream, alloc = _stage(self.device, device_out)
+        out = (alloc(k, np.uint32), alloc(k, np.int64), alloc(1, np.int32, zero=True), alloc(1, np.uint64, zero=True))
+        check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), k, mem, *map(ptr, out), stream))
+        return out if device_out else (out[0], out[1], int(out[2][0]), int(out[3][0]))
 
     def set_doc_keys(self, keys: Optional[np.ndarray]):
         """Caller keys of the documents (paragraph ids) for rank fusion; None = the document number."""

@@ -26,7 +26,8 @@ from typing import Iterable, Optional, Sequence, Union
 import numpy as np
 
 from . import _lib
-from ._lib import NIL, NidxError, VecConfig, VecSearchParams, check, ptr
+from ._lib import NidxError
+from .segment import VectorSegment, normalize
 
 
 class Similarity(enum.Enum):  # config.rs:33-37 (+ L2: an extension, the reference has no Euclidean similarity)
@@ -60,10 +61,11 @@ class VectorConfig:
     ef_search: int = 30
     device: int = 0
 
-    def _c(self) -> VecConfig:
-        return VecConfig(self.dimension, {Similarity.Cosine: _lib.NIDX_SIM_COSINE, Similarity.Dot: _lib.NIDX_SIM_DOT, Similarity.L2: _lib.NIDX_SIM_L2}[self.similarity],
-                         int(self.vector_cardinality == VectorCardinality.Multi), self.m, self.m0, self.ef_construction, self.ef_search,
-                         self.device)
+    def _segment_kw(self) -> dict:
+        """VectorSegment.create / open's keyword arguments."""
+        return dict(similarity={Similarity.Cosine: _lib.NIDX_SIM_COSINE, Similarity.Dot: _lib.NIDX_SIM_DOT, Similarity.L2: _lib.NIDX_SIM_L2}[self.similarity],
+                    m=self.m, m0=self.m0, ef_construction=self.ef_construction, ef_search=self.ef_search, device=self.device,
+                    multi_vector=self.vector_cardinality == VectorCardinality.Multi)
 
 
 # ---- nidx_types::query_language::BooleanExpression ----------------------------------------------
@@ -173,11 +175,12 @@ def _labels_key(label: str) -> str:  # inverted_index/paragraph.rs:64-66
 
 
 class OpenSegment:
-    """segment.rs OpenSegment: device-resident vectors + graph, host-resident paragraph metadata."""
+    """segment.rs OpenSegment: device-resident vectors + graph (``segment``, a VectorSegment; None for a host-only view),
+    host-resident paragraph metadata."""
 
-    def __init__(self, config: VectorConfig, handle, keys, labels, metadata, first_vec, tags=frozenset()):
+    def __init__(self, config: VectorConfig, segment: Optional[VectorSegment], keys, labels, metadata, first_vec, tags=frozenset()):
         self.config = config
-        self._h = handle
+        self.segment = segment
         self.keys, self.labels, self.metadata = list(keys), [tuple(l) for l in labels], list(metadata)
         self.first_vec = np.asarray(first_vec, dtype=np.uint32)  # [n_par + 1]
         self.records = len(self.keys)
@@ -192,23 +195,16 @@ class OpenSegment:
         for p, fk in enumerate(self._field_keys):
             if fk is not None:
                 self._field_index.setdefault(fk, []).append(p)
-        if handle is not None:
-            self._upload_inverted_indexes()
+        if segment is not None:   # the label and field indexes go to the library, so that filter formulas are evaluated on the device
+            for which, index in ((_lib.NIDX_INV_LABELS, {k.encode(): v for k, v in self._label_index.items()}), (_lib.NIDX_INV_FIELDS, self._field_index)):
+                keys = sorted(index)
+                segment.set_inverted_index(which, keys, [sorted(index[k]) for k in keys])
 
-    def _upload_inverted_indexes(self):
-        """ParagraphInvertedIndexes::build (inverted_index/paragraph.rs:74-106): the label and field indexes go to the library --
-        keys sorted bytewise as in the fst, postings to HBM -- so that filter formulas are evaluated on the device."""
-        L = _lib.load()
-        for which, index in ((_lib.NIDX_INV_LABELS, {k.encode(): v for k, v in self._label_index.items()}), (_lib.NIDX_INV_FIELDS, self._field_index)):
-            keys = sorted(index)
-            key_off = np.zeros(len(keys) + 1, dtype=np.uint64)
-            post_off = np.zeros(len(keys) + 1, dtype=np.uint64)
-            if keys:
-                key_off[1:] = np.cumsum([len(k) for k in keys])
-                post_off[1:] = np.cumsum([len(index[k]) for k in keys])
-            key_bytes = np.frombuffer(b"".join(keys) or b"\0", dtype=np.uint8).copy()
-            postings = np.asarray([p for k in keys for p in sorted(index[k])] or [0], dtype=np.uint32)
-            check(L.nidx_vec_set_inverted_index(self._h, C.c_int32(which), C.c_uint32(len(keys)), ptr(key_bytes), ptr(key_off), ptr(post_off), ptr(postings)))
+    @property
+    def _h(self):
+        """The C handle of the owned VectorSegment, for callers that pass it to the C ABI themselves.  It stays owned by `segment`,
+        which alone closes it."""
+        return self.segment._h
 
     # -- filter formulas for the device (formula.rs:40-100 -> nidx_filter_node, pre-order) ----------
     def formula_nodes(self, clauses, operator_and=True):
@@ -254,15 +250,14 @@ class OpenSegment:
         """nidx_vec_filter: the formula's bitset AND the alive set, computed on the device -> (bool mask over paragraphs, matching)."""
         nodes, n, keep = self.formula_nodes(clauses, operator_and)
         words = np.zeros((self.records + 63) // 64, dtype=np.uint64)
-        matching = C.c_uint64()
-        check(_lib.load().nidx_vec_filter(self._h, nodes, C.c_int32(n), ptr(words), _lib.NIDX_MEM_HOST, C.byref(matching), None))
-        return np.unpackbits(words.view(np.uint8), bitorder="little")[: self.records].astype(bool), int(matching.value)
+        matching = self.segment.filter(nodes, n, words)
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[: self.records].astype(bool), matching
 
     # -- lifecycle -----------------------------------------------------------------------------
     @classmethod
     def create(cls, elems: Sequence[Elem], config: VectorConfig, tags=frozenset(), build_graph=True, seed=2, max_batch=4096):
         """segment::create (segment.rs:199-286): data store + HNSW (GPU build)."""
-        L = _lib.require_device()
+        _lib.require_device()
         dim = config.dimension
         vecs, par_of, first = [], [], [0]
         for p, e in enumerate(elems):
@@ -275,18 +270,13 @@ class OpenSegment:
                 par_of.append(p)
             first.append(len(vecs))
         arr = np.stack(vecs).astype(np.float32) if vecs else np.zeros((0, dim), dtype=np.float32)
-        if config.normalize_vectors and len(arr):  # indexer.rs:94-146 normalises at index time (utils.rs:20-23)
-            arr = np.ascontiguousarray(arr, dtype=np.float32)   # sequential f32 fold on the device, bit-identical to the reference's
-            check(L.nidx_normalize_vectors(C.c_int32(config.device), ptr(arr), C.c_uint64(len(arr)), C.c_int32(dim), C.c_int32(dim), _lib.NIDX_MEM_HOST, None))
-        par = np.asarray(par_of, dtype=np.uint32)
-        h = C.c_void_p()
-        cfg = config._c()
-        check(L.nidx_vec_create(C.byref(cfg), ptr(arr), C.c_uint64(len(arr)), C.c_int32(dim), _lib.NIDX_MEM_HOST, ptr(par) if len(par) else None,
-                                C.byref(h)))
-        seg = cls(config, h, [e.key for e in elems], [e.labels for e in elems], [e.metadata for e in elems], first, tags)
+        if config.normalize_vectors:  # indexer.rs:94-146 normalises at index time (utils.rs:20-23)
+            normalize(arr, config.device)
+        segment = VectorSegment.create(arr, dim, **config._segment_kw(), paragraph_of=np.asarray(par_of, dtype=np.uint32) if par_of else None)
+        seg = cls(config, segment, [e.key for e in elems], [e.labels for e in elems], [e.metadata for e in elems], first, tags)
         seg.host_vectors = arr
         if build_graph and len(arr):
-            check(L.nidx_vec_build_hnsw(h, C.c_uint64(seed), C.c_int32(max_batch), None))
+            segment.build_hnsw(seed, max_batch)
         return seg
 
     def save(self, directory: str):
@@ -296,7 +286,7 @@ class OpenSegment:
         (segment.rs:183)."""
         from . import paragraph_store as PS
 
-        check(_lib.load().nidx_vec_save(self._h, directory.encode()))
+        self.segment.save(directory)
         PS.write_paragraphs(directory, ((self.keys[p], self.labels[p], self.metadata[p], int(self.first_vec[p]), int(self.first_vec[p + 1] - self.first_vec[p]))
                                         for p in range(self.records)))
 
@@ -306,7 +296,7 @@ class OpenSegment:
         metadata of the paragraphs stay on the host."""
         from . import paragraph_store as PS
 
-        L = _lib.require_device()
+        _lib.require_device()
         paragraphs = PS.read_paragraphs(directory)
         first = [p[3] for p in paragraphs] + [paragraphs[-1][3] + paragraphs[-1][4] if paragraphs else 0]
         for i, p in enumerate(paragraphs):
@@ -316,23 +306,14 @@ class OpenSegment:
         stored = np.fromfile(os.path.join(directory, "vectors.bin"), dtype=record)
         if len(stored) != first[-1]:
             raise NidxError(-1, f"vectors.bin holds {len(stored)} vectors, paragraphs.bin accounts for {first[-1]}")
-        h = C.c_void_p()
-        cfg = config._c()
-        check(L.nidx_vec_open(C.byref(cfg), directory.encode(), C.byref(h)))
-        seg = cls(config, h, [p[0] for p in paragraphs], [p[1] for p in paragraphs], [p[2] for p in paragraphs], first, tags)
+        segment = VectorSegment.open(directory, config.dimension, **config._segment_kw())
+        seg = cls(config, segment, [p[0] for p in paragraphs], [p[1] for p in paragraphs], [p[2] for p in paragraphs], first, tags)
         seg.host_vectors = np.ascontiguousarray(stored["vector"])
         return seg
 
     def close(self):
-        if self._h is not None:
-            _lib.load().nidx_vec_close(self._h)
-            self._h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        if self.segment is not None:
+            self.segment.close()
 
     # -- deletions (segment.rs:428-445, lib.rs:166-200) -------------------------------------------
     def apply_deletions(self, deleted_keys: Iterable[str]):
@@ -346,7 +327,7 @@ class OpenSegment:
         bits = np.packbits(self.alive, bitorder="little")
         words = np.zeros((self.records + 63) // 64 * 8, dtype=np.uint8)
         words[: len(bits)] = bits
-        check(_lib.load().nidx_vec_set_alive(self._h, ptr(words.view(np.uint64)), _lib.NIDX_MEM_HOST))
+        self.segment.set_alive(words.view(np.uint64))
 
     # -- filters (inverted_index/paragraph.rs:124-186) ---------------------------------------------
     def _clause(self, clause) -> np.ndarray:
@@ -391,38 +372,17 @@ class OpenSegment:
 
     def search_batch(self, queries: np.ndarray, top_k, min_score=0.0, with_duplicates=False, clauses=(), operator_and=True,
                      method=_lib.NIDX_METHOD_AUTO, ef=0):
-        L = _lib.load()
         queries = np.ascontiguousarray(queries, dtype=np.float32)
-        nq, dim = queries.shape
-        if dim != self.config.dimension:
-            raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {dim}")
-        ids = np.empty((nq, top_k), dtype=np.uint32)
-        scores = np.empty((nq, top_k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.int32)
-        p = VecSearchParams(top_k, ef, min_score, int(with_duplicates), method, None, 0)
+        if queries.shape[1] != self.config.dimension:
+            raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {queries.shape[1]}")
+        # a formula goes to the library as it is: postings -> bitset -> algebra -> AND alive -> count, all in HBM (segment.rs:516-534)
         clauses = list(clauses)
-        if clauses:   # the formula goes to the library as it is: postings -> bitset -> algebra -> AND alive -> count, all in HBM (segment.rs:516-534)
-            nodes, n_nodes, keep = self.formula_nodes(clauses, operator_and)
-            check(L.nidx_vec_search_formula(self._h, ptr(queries), C.c_int32(nq), C.c_int32(dim), _lib.NIDX_MEM_HOST, C.byref(p), nodes, C.c_int32(n_nodes),
-                                            ptr(ids), ptr(scores), ptr(counts), None))
-            return ids, scores, counts
-        check(L.nidx_vec_search(self._h, ptr(queries), C.c_int32(nq), C.c_int32(dim), _lib.NIDX_MEM_HOST, C.byref(p), ptr(ids), ptr(scores), ptr(counts),
-                                None))
-        return ids, scores, counts
+        nodes, _, keep = self.formula_nodes(clauses, operator_and) if clauses else (None, 0, None)
+        return self.segment.search(queries, top_k, ef, min_score, with_duplicates, method, formula=nodes)
 
     def _raw_search(self, queries, k, filter_bits):
         """exact scan restricted to a paragraph bitset, no min_score: per (query, paragraph) the best vector's similarity."""
-        L = _lib.load()
-        queries = np.ascontiguousarray(queries, dtype=np.float32)
-        nq = queries.shape[0]
-        ids = np.empty((nq, k), dtype=np.uint32)
-        scores = np.empty((nq, k), dtype=np.float32)
-        counts = np.empty(nq, dtype=np.int32)
-        keep = np.ascontiguousarray(filter_bits, dtype=np.uint64)
-        p = VecSearchParams(k, 0, float(np.finfo(np.float32).min), 1, _lib.NIDX_METHOD_BRUTE, keep.ctypes.data, 0)
-        check(L.nidx_vec_search(self._h, ptr(queries), C.c_int32(nq), C.c_int32(queries.shape[1]), _lib.NIDX_MEM_HOST, C.byref(p), ptr(ids), ptr(scores),
-                                ptr(counts), None))
-        return ids, scores, counts
+        return self.segment.search(queries, k, 0, float(np.finfo(np.float32).min), True, _lib.NIDX_METHOD_BRUTE, filter_bits=filter_bits)
 
     def paragraph_of(self, vector_addr: int) -> int:
         return int(np.searchsorted(self.first_vec, vector_addr, side="right") - 1)
@@ -491,7 +451,7 @@ class VectorSearcher:
         operator_and = request.filter_operator == FilterOperator.And
         query = np.asarray(request.vector, dtype=np.float32)
         if self.config.normalize_vectors and self.config.vector_cardinality != VectorCardinality.Multi:  # searcher.rs:246-252, utils.rs:20-23
-            query = self._normalize(query)
+            query = normalize(query.copy(), self.config.device)
         multi = self.config.vector_cardinality == VectorCardinality.Multi
         if (len(query) != self.config.dimension) if not multi else (len(query) % self.config.dimension != 0 or len(query) == 0):
             raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {len(query)}")
@@ -520,7 +480,7 @@ class VectorSearcher:
         k = request.result_per_page
         qv = np.asarray(request.vector, dtype=np.float32).reshape(-1, d)
         if self.config.normalize_vectors:
-            qv = self._normalize(qv)
+            qv = normalize(qv.copy(), self.config.device)
         if k <= 0 or prefilter.kind == "none":
             return VectorSearchResponse([])
         first_k = max(k, 10)
@@ -548,14 +508,6 @@ class VectorSearcher:
         docs = [DocumentScored(seg.keys[p], sc, list(seg.labels[p]), seg.metadata[p]) for sc, seg, p in scored[:k]]
         return VectorSearchResponse(docs)
 
-    def _normalize(self, v):
-        """utils.rs:20-23 through the C ABI (nidx_normalize_vectors): one vector [d] or rows [n][d]."""
-        a = np.array(v, dtype=np.float32, ndmin=2)
-        if a.size:
-            check(_lib.require_device().nidx_normalize_vectors(C.c_int32(self.config.device), ptr(a), C.c_uint64(a.shape[0]), C.c_int32(a.shape[1]),
-                                                               C.c_int32(a.shape[1]), _lib.NIDX_MEM_HOST, None))
-        return a.reshape(np.shape(v))
-
     @staticmethod
     def _vector_bytes(seg: OpenSegment, addr: int) -> bytes:
         # Fssc's exact-duplicate test hashes the raw vector bytes (searcher.rs:175-183); the host copy
@@ -577,8 +529,6 @@ class VectorIndexer:
         data store.  If that first segment has no deletions its HNSW is reused (its vector addresses are a prefix of the
         merged store's) and only the other segments' vectors are inserted (merge_indexes, segment.rs:143-167); otherwise the
         graph is built from scratch.  Both on the GPU."""
-        from .segment import VectorSegment
-
         opened = []
         for seg, seq in segments:
             dels = [k for k, dseq in deletions if dseq > seq]
@@ -595,24 +545,18 @@ class VectorIndexer:
                 elems.append(Elem(seg.keys[p], [seg.host_vectors[i] for i in range(a, b)], seg.labels[p], seg.metadata[p]))
         merged_cfg = VectorConfig(**{**config.__dict__, "normalize_vectors": False})   # vectors were normalised when first indexed
         first = opened[0]
-        view = VectorSegment(first._h, None)        # borrowed handles: the OpenSegments own them
-        tgt = VectorSegment(None, None)
-        try:
-            reuse = bool(first.alive.all()) and len(first.host_vectors) > 0
-            if reuse:
-                try:
-                    g = view.get_graph()
-                except NidxError:                       # the first segment was created without a graph
-                    reuse = False
-            if reuse:
-                out = OpenSegment.create(elems, merged_cfg, frozenset(first.tags), build_graph=False)
-                tgt._h = out._h
-                rows = max(int(g["upper_rows"]), 1)
-                tgt.extend_hnsw(len(first.host_vectors), g["level"], g["adj0"], g["adjU"][:rows], g["w0"], g["wU"][:rows], g["entry_node"], g["entry_layer"],
-                                seed=kw.get("seed", 2), max_batch=kw.get("max_batch", 4096))
-            else:
-                out = OpenSegment.create(elems, merged_cfg, frozenset(first.tags), **kw)
-        finally:
-            view._h = tgt._h = None
+        reuse = bool(first.alive.all()) and len(first.host_vectors) > 0
+        if reuse:
+            try:
+                g = first.segment.get_graph()
+            except NidxError:                       # the first segment was created without a graph
+                reuse = False
+        if reuse:
+            out = OpenSegment.create(elems, merged_cfg, frozenset(first.tags), build_graph=False)
+            rows = max(int(g["upper_rows"]), 1)
+            out.segment.extend_hnsw(len(first.host_vectors), g["level"], g["adj0"], g["adjU"][:rows], g["w0"], g["wU"][:rows], g["entry_node"], g["entry_layer"],
+                                    seed=kw.get("seed", 2), max_batch=kw.get("max_batch", 4096))
+        else:
+            out = OpenSegment.create(elems, merged_cfg, frozenset(first.tags), **kw)
         out.config = config
         return out

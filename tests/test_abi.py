@@ -18,6 +18,108 @@ def header_functions():
     return sorted(set(re.findall(r"\b(nidx_[a-z0-9_]+)\s*\(", text)))
 
 
+def header_prototypes():
+    """-> {name: (return type, [parameter declarations])} of every function include/nidx_b200.h declares."""
+    text = open(os.path.join(ROOT, "include", "nidx_b200.h")).read()
+    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
+    text = "\n".join(l for l in text.splitlines() if not l.lstrip().startswith("#"))
+    protos = {}
+    for stmt in text.split(";"):
+        stmt = stmt.split("{")[-1].split("}")[-1]
+        m = re.fullmatch(r"\s*(.+?)\s*\b(nidx_\w+)\s*\((.*)\)\s*", stmt, flags=re.S)
+        if m:
+            params = [p.strip() for p in m.group(3).split(",")]
+            protos[m.group(2)] = (m.group(1), [] if params == ["void"] else params)
+    return protos
+
+
+def ctype_of(decl):
+    """The ctypes type _lib.SIGNATURES gives a C declaration: scalars by exact width, `const char*` as c_char_p, pointers to the
+    ABI's structs typed, every other pointer or array (buffers, handles, out-handles, streams) void*; void -> None."""
+    structs = {"nidx_vec_config": _lib.VecConfig, "nidx_vec_search_params": _lib.VecSearchParams, "nidx_filter_node": _lib.FilterNode,
+               "nidx_txt_search_params": _lib.TxtSearchParams, "nidx_txt_facet_request": _lib.TxtFacetRequest, "nidx_txt_order": _lib.TxtOrder,
+               "nidx_rrf_source": _lib.RrfSource, "nidx_shard_search_request": _lib.ShardSearchRequest,
+               "nidx_shard_search_response": _lib.ShardSearchResponse}
+    scalars = {"int": C.c_int32, "int32_t": C.c_int32, "uint32_t": C.c_uint32, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "float": C.c_float,
+               "double": C.c_double}
+    base = re.findall(r"\w+", re.sub(r"\bconst\b", " ", decl))[0]
+    if "*" in decl or "[" in decl:
+        return C.c_char_p if base == "char" else C.POINTER(structs[base]) if base in structs else C.c_void_p
+    return None if base == "void" else scalars[base]
+
+
+def test_signature_table_matches_the_header():
+    """Every prototype of include/nidx_b200.h against _lib.SIGNATURES, parameter by parameter (a scalar of the wrong width, or
+    a missing parameter, reaches the library as a wrong value without an error)."""
+    protos = header_prototypes()
+    assert len(protos) == len(header_functions())
+    assert sorted(_lib.SIGNATURES) == sorted(protos)
+    for name, (ret, params) in protos.items():
+        restype, argtypes = _lib.SIGNATURES[name]
+        assert restype is ctype_of(ret), (name, ret, restype)
+        assert len(argtypes) == len(params), (name, params, argtypes)
+        for i, (decl, t) in enumerate(zip(params, argtypes)):
+            assert t is ctype_of(decl), (name, i, decl, t)
+    L = _lib.load()
+    assert L.nidx_vec_search.argtypes == _lib.SIGNATURES["nidx_vec_search"][1] and L.nidx_vec_len.restype is C.c_uint64
+
+
+def test_wrappers_agree_with_the_signature_table():
+    """Every VectorSegment / TextSegment wrapper that reaches its ABI call with numpy inputs, driven over a NULL handle: the
+    library refuses it (NidxError).  A ctypes.ArgumentError or TypeError would mean a call site disagrees with the table.
+    Not driven here (the GPU suite covers them): create / open (require_device first), close / len (no refusal to see), and
+    the torch device path."""
+    from nucliadb_b200.segment import TextSegment, VectorSegment
+
+    vec = VectorSegment(None, _lib.VecConfig(8, _lib.NIDX_SIM_DOT, 0, 0, 0, 0, 0, 0))
+    txt = TextSegment(None, 4, 3, 0)
+    txt.facet_buckets = lambda facets: (np.zeros(2, np.uint32), np.zeros(2, np.uint32))   # reach the faceted calls themselves
+    nodes = (_lib.FilterNode * 1)(_lib.FilterNode(_lib.NIDX_F_NOT, 0, None, None))
+    q = np.zeros((2, 8), np.float32)
+    qt, qoff = np.array([0, 1], np.uint32), np.array([0, 1, 2], np.uint32)
+    level, adj = np.zeros(2, np.uint8), np.zeros((2, 4), np.uint32)
+    calls = {
+        "VectorSegment.save": lambda: vec.save("/nonexistent"),
+        "VectorSegment.build_hnsw": lambda: vec.build_hnsw(seed=3, max_batch=64),
+        "VectorSegment.extend_hnsw": lambda: vec.extend_hnsw(1, level, adj, adj, adj, adj, 0, 0, seed=3, max_batch=64),
+        "VectorSegment.graph_dims": vec.graph_dims,
+        "VectorSegment.get_graph": vec.get_graph,
+        "VectorSegment.set_graph": lambda: vec.set_graph(level, adj, adj, adj, adj),
+        "VectorSegment.set_alive": lambda: vec.set_alive(np.ones(1, np.uint64)),
+        "VectorSegment.set_paragraph_keys": lambda: vec.set_paragraph_keys(np.arange(2)),
+        "VectorSegment.set_inverted_index": lambda: vec.set_inverted_index(_lib.NIDX_INV_LABELS, [b"a", b"b"], [[0], [0, 1]]),
+        "VectorSegment.filter": lambda: vec.filter(nodes, 1, np.zeros(1, np.uint64)),
+        "VectorSegment.search": lambda: vec.search(q, 3, ef=16, min_score=0.5, with_duplicates=False, method=_lib.NIDX_METHOD_BRUTE),
+        "VectorSegment.search(filter_bits)": lambda: vec.search(q, 3, filter_bits=np.ones(1, np.uint64), filter_matching=2),
+        "VectorSegment.search(formula)": lambda: vec.search(q, 3, formula=nodes),
+        "VectorSegment.rabitq_encode": vec.rabitq_encode,
+        "VectorSegment.rabitq_codes": vec.rabitq_codes,
+        "VectorSegment.rabitq_estimate": lambda: vec.rabitq_estimate(q),
+        "VectorSegment.last_kernel_ms": vec.last_kernel_ms,
+        "VectorSegment.counters": vec.counters,
+        "VectorSegment.counters_ex": vec.counters_ex,
+        "VectorSegment.exact_rows": vec.exact_rows,
+        "VectorSegment.scan_counters": vec.scan_counters,
+        "TextSegment.set_stats": lambda: txt.set_stats(4, 10, np.ones(3)),
+        "TextSegment.set_alive": lambda: txt.set_alive(np.ones(1, np.uint64)),
+        "TextSegment.search": lambda: txt.search(qt, qoff, 3, mode=_lib.NIDX_BM25_AND, use_tf=False, min_score=0.1, after=(1.0, 2, 5), docaddr_base=1 << 32),
+        "TextSegment.set_facets": lambda: txt.set_facets([b"a", b"a\0b"], np.zeros(5), np.zeros(0)),
+        "TextSegment.facet_buckets": lambda: TextSegment.facet_buckets(txt, [b"a"]),
+        "TextSegment.search_faceted": lambda: txt.search_faceted(qt, qoff, 3, [b"a"], after=(1.0, 1, 0)),
+        "TextSegment.facet_count_all": lambda: txt.facet_count_all([b"a"]),
+        "TextSegment.set_dates": lambda: txt.set_dates(np.zeros(4), np.zeros(4)),
+        "TextSegment.search_ordered": lambda: txt.search_ordered(qt, qoff, 3, field=_lib.NIDX_ORDER_MODIFIED, order=_lib.NIDX_ORDER_ASC),
+        "TextSegment.search_ordered(facets)": lambda: txt.search_ordered(qt, qoff, 3, facets=[b"a"]),
+        "TextSegment.list_ordered": lambda: txt.list_ordered(3),
+        "TextSegment.set_doc_keys": lambda: txt.set_doc_keys(np.arange(4)),
+        "TextSegment.last_kernel_ms": txt.last_kernel_ms,
+    }
+    for name, call in calls.items():
+        with pytest.raises(_lib.NidxError):
+            call()
+            pytest.fail(f"{name} was not refused")
+
+
 def test_library_exports_every_header_symbol():
     L = _lib.load()
     names = header_functions()
@@ -61,8 +163,7 @@ def test_cost_model_is_a_host_function_equal_to_the_oracle():
     import oracle as O
 
     L = _lib.load()
-    L.nidx_use_hnsw.restype = C.c_int
-    call = lambda t, mt, k, rq, m=30: bool(L.nidx_use_hnsw(C.c_uint64(t), C.c_uint64(mt), C.c_uint64(k), C.c_int(int(rq)), C.c_int(m)))
+    call =lambda t, mt, k, rq, m=30: bool(L.nidx_use_hnsw(C.c_uint64(t), C.c_uint64(mt), C.c_uint64(k), C.c_int(int(rq)), C.c_int(m)))
     assert call(100_000, 100_000, 10, False) and not call(100_000, 500, 10, False)
     for total in (1, 7, 640, 5_000, 100_000, 10_000_000):
         for frac in (1.0, 0.3, 0.01, 0.0001):

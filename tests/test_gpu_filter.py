@@ -73,7 +73,7 @@ def test_search_with_a_device_formula_matches_the_bitset_path():
             import ctypes as C
 
             i2, s2, c2 = np.empty_like(ids), np.empty_like(sc), np.empty_like(cnt)
-            _lib.check(_lib.load().nidx_vec_search(seg._h, _lib.ptr(q), C.c_int32(len(q)), C.c_int32(64), _lib.NIDX_MEM_HOST, C.byref(p), _lib.ptr(i2), _lib.ptr(s2),
+            _lib.check(_lib.load().nidx_vec_search(seg.segment._h, _lib.ptr(q), C.c_int32(len(q)), C.c_int32(64), _lib.NIDX_MEM_HOST, C.byref(p), _lib.ptr(i2), _lib.ptr(s2),
                                                    _lib.ptr(c2), None))
             assert (cnt == c2).all() and (ids == i2).all() and np.array_equal(sc, s2)
             assert all(mask[seg.paragraph_of(int(v))] for v in ids[ids != 0xFFFFFFFF])
@@ -88,4 +88,4 @@ def test_malformed_formulas_are_rejected():
     nodes[1].kind, nodes[1].n = _lib.NIDX_F_NOT, 0
     m = C.c_uint64()
     with pytest.raises(_lib.NidxError):
-        _lib.check(_lib.load().nidx_vec_filter(seg._h, nodes, C.c_int32(2), None, _lib.NIDX_MEM_HOST, C.byref(m), None))
+        _lib.check(_lib.load().nidx_vec_filter(seg.segment._h, nodes, C.c_int32(2), None, _lib.NIDX_MEM_HOST, C.byref(m), None))

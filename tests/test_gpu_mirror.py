@@ -221,14 +221,7 @@ def test_merge_segments_with_deletions():  # nidx_vector/src/segment/tests.rs me
     both = V.VectorIndexer.merge(cfg, [(V.VectorIndexer.index_elems([V.Elem(f"{RID}/a/title/0-{i}", [sentence(i)]) for i in range(5)], cfg), 1), (merged, 4)])
     assert both.records == 35 and both.keys[0].startswith(other)                         # largest segment first (segment.rs:103-105)
     # merge_indexes reuses the first operand's graph when it has no deletions (segment.rs:143-167)
-    def graph_of(seg):
-        view = VectorSegment(seg._h, None)
-        try:
-            return view.get_graph()
-        finally:
-            view._h = None
-
-    g2, gm, gb = graph_of(seg2), graph_of(merged), graph_of(both)
+    g2, gm, gb = seg2.segment.get_graph(), merged.segment.get_graph(), both.segment.get_graph()
     assert np.array_equal(g2["adj0"], gm["adj0"]) and np.array_equal(g2["level"], gm["level"])      # nothing to insert: the graph is seg2's
     assert np.array_equal(gb["level"][:30], gm["level"]) and (gb["adj0"][30:, 0] != 0xFFFFFFFF).all()  # the 5 new nodes are linked in
     r = V.VectorSearcher.open(cfg, [(both, 5)]).search(V.VectorSearchRequest(vector=sentence(3), result_per_page=1, min_score=-1.0), method=_lib.NIDX_METHOD_HNSW)
