@@ -165,7 +165,8 @@ int nidx_vec_search(nidx_vec_segment* seg, const float* queries, int32_t nq, int
 #define NIDX_INV_FIELDS 1  /* field index: key = FieldKey bytes (utils.rs:80-117), looked up EXACTLY (get) */
 /* One inverted index of the segment: n_keys byte strings, strictly ascending in memcmp order (the fst's order), key i =
  * key_bytes[key_off[i] .. key_off[i + 1]), its paragraph addresses = postings[post_off[i] .. post_off[i + 1]).  The keys stay on the
- * host side of the library (the lookup is the fst's job: a binary search), the postings live in HBM.  Host pointers. */
+ * host side of the library (the lookup is the fst's job: a binary search), the postings live in HBM.  Host pointers.  A call that
+ * fails (rejected input included) leaves the segment's previous index in place. */
 int nidx_vec_set_inverted_index(nidx_vec_segment* seg, int32_t which, uint32_t n_keys, const uint8_t* key_bytes, const uint64_t* key_off,
                                 const uint64_t* post_off, const uint32_t* postings);
 
@@ -297,7 +298,8 @@ int nidx_txt_last_kernel_ms(nidx_txt_segment* seg, float* ms);
  * key_bytes[key_off[i] .. key_off[i + 1]); document d carries the ords doc_ords[doc_off[d] .. doc_off[d + 1]) (strictly
  * ascending; doc_off has n_docs + 1 entries).  The keys stay on the host side of the library (a request is resolved by binary
  * search: the descendants of a facet are one ord range), the ords live in HBM.  Segments of one index should be given the same
- * dictionary, so that a bucket means the same child in every segment and per-segment counts add up as arrays.  Host pointers. */
+ * dictionary, so that a bucket means the same child in every segment and per-segment counts add up as arrays.  Host pointers.  A
+ * call that fails (rejected input included) leaves the segment's previous facets in place. */
 int nidx_txt_set_facets(nidx_txt_segment* seg, uint32_t n_facets, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
                         const uint32_t* doc_ords);
 
@@ -344,7 +346,8 @@ typedef struct nidx_txt_order {
 } nidx_txt_order;
 
 /* Every document's created and modified seconds (n_docs each, NIDX_DATE_NONE = none; host pointers).  The seconds and, per field,
- * each document's dense rank among the segment's distinct dates (built on the device) live in HBM. */
+ * each document's dense rank among the segment's distinct dates (built on the device) live in HBM.  A call that fails leaves the
+ * segment's previous dates in place. */
 int nidx_txt_set_dates(nidx_txt_segment* seg, const int64_t* created, const int64_t* modified);
 
 /* nidx_txt_search (facets == NULL) or nidx_txt_search_faceted with TopDocs ordered by date: the matched set, out_total and the facet

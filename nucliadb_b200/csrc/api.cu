@@ -11,6 +11,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -54,25 +55,43 @@ static int fail(int code, const char* fmt, ...) {
 static int next_pow2(int x) { int p = 1; while (p < x) p <<= 1; return p; }
 static int ilog2(int x) { int b = 0; while ((1 << b) < x) ++b; return b; }
 
-struct DevBuf {
-    void* p = nullptr;
+// The owner of every device allocation: move-only, freed when it is destroyed, released or allocated again.  Sizes are in bytes.
+// alloc() takes exactly the size asked for (segment arrays, whose sizes include the padding kernels read into), ensure() grows
+// with slack (per-call scratch), try_alloc() reports a failure to its caller only (an allocation with a fallback).  It converts to
+// the raw pointer that kernels and copies take.
+template <class T>
+struct DevArray {
+    T* p = nullptr;
     size_t cap = 0;
-    int ensure(size_t bytes) {
-        if (bytes <= cap) return 0;
-        if (p) cudaFree(p);
-        p = nullptr; cap = 0;
-        size_t want = bytes + bytes / 4 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) { e = cudaMalloc(&p, bytes); want = bytes; }
-        if (e != cudaSuccess) return fail(NIDX_ECUDA, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-        cap = want;
-        return 0;
+    DevArray() = default;
+    DevArray(DevArray&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevArray& operator=(DevArray&& o) noexcept {
+        if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+        return *this;
     }
+    ~DevArray() { release(); }
+    operator T*() const { return p; }
+    template <class U> U* as() const { return reinterpret_cast<U*>(p); }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-    ~DevBuf() { release(); }
-    template <class T> T* as() { return reinterpret_cast<T*>(p); }
+    cudaError_t try_alloc(size_t bytes) {
+        release();
+        cudaError_t e = cudaMalloc(&p, bytes);
+        if (e == cudaSuccess) cap = bytes;
+        else { p = nullptr; (void)cudaGetLastError(); }   // not left for the next cudaGetLastError() to report
+        return e;
+    }
+    int alloc(size_t bytes) {
+        cudaError_t e = try_alloc(bytes);
+        return e == cudaSuccess ? 0 : fail(NIDX_ECUDA, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+    }
+    int ensure(size_t bytes) {
+        if (bytes <= cap || try_alloc(bytes + bytes / 4 + 256) == cudaSuccess) return 0;
+        return alloc(bytes);
+    }
 };
+using DevBuf = DevArray<unsigned char>;
 #define ENSURE(buf, bytes) do { int r__ = (buf).ensure(bytes); if (r__) return r__; } while (0)
+#define ALLOC(buf, bytes) do { int r__ = (buf).alloc(bytes); if (r__) return r__; } while (0)
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
@@ -185,49 +204,54 @@ struct nidx_vec_segment {
     uint64_t n = 0;
     int d = 0, ld = 0;
     int sm_count = 0;
-    float* d_vecs = nullptr;
-    float* d_norms = nullptr;
-    uint32_t* d_par_of = nullptr;
-    uint32_t* d_par_first = nullptr;
+    DevArray<float> d_vecs;
+    DevArray<float> d_norms;
+    DevArray<uint32_t> d_par_of;
+    DevArray<uint32_t> d_par_first;
     uint32_t n_par = 0;
-    uint64_t* d_alive = nullptr;
+    DevArray<uint64_t> d_alive;
     uint64_t alive_count = 0;         // set bits of d_alive (counted in nidx_vec_set_alive): `matching` of an unfiltered search
-    uint64_t* d_par_keys = nullptr;   // [n_par] caller-supplied paragraph keys for the cross-segment de-duplication (shard.cuh)
+    DevArray<uint64_t> d_par_keys;    // [n_par] caller-supplied paragraph keys for the cross-segment de-duplication (shard.cuh)
     struct InvIndex {                 // one inverted index (inverted_index/fst_index.rs + map.rs): sorted keys on the host, postings in HBM
         std::vector<unsigned char> key_bytes;
         std::vector<uint64_t> key_off, post_off;
-        uint32_t* d_post = nullptr;
+        DevArray<uint32_t> d_post;
         uint32_t n_keys = 0;
     } inv[2];
     // graph
     bool has_graph = false;
     std::vector<uint8_t> h_level;
-    uint8_t* d_level = nullptr;
+    DevArray<uint8_t> d_level;
     uint32_t entry_node = 0, entry_layer = 0;
     int s0 = 0, su = 0;
     uint64_t upper_rows = 0;
-    uint32_t* d_adj0 = nullptr; float* d_w0 = nullptr;
-    uint64_t* d_upper_off = nullptr;
-    uint32_t* d_adjU = nullptr; float* d_wU = nullptr;
+    DevArray<uint32_t> d_adj0; DevArray<float> d_w0;
+    DevArray<uint64_t> d_upper_off;
+    DevArray<uint32_t> d_adjU; DevArray<float> d_wU;
     float max_norm = 0.0f;              // max |v| (error bound of the tensor-core filter for Dot)
     bool tc_rows_ok = false;            // every row meets the filter's bound (max_norm_kernel): else batches take the exact scan
     CUtensorMap map_v;                  // TMA descriptor of the vector block (scan_tc2.cuh), built on first use
     bool map_v_ready = false;
     std::mutex map_mu;
-    unsigned char* d_quant = nullptr;   // RaBitQ codes [n][quant_stride] (vectors.quant records, padded)
+    DevArray<unsigned char> d_quant;    // RaBitQ codes [n][quant_stride] (vectors.quant records, padded)
     int quant_stride = 0;
-    unsigned long long* d_counters = nullptr;  // [8] the build's counters
+    DevArray<unsigned long long> d_counters;   // [8] the build's counters
     std::atomic<unsigned long long*> last_counters{nullptr};   // counters of the LAST search call (they live in that call's workspace: concurrent
                                                                // searches never add into each other's), read by nidx_vec_counters*
-    unsigned int* d_work_counter = nullptr;
+    DevArray<unsigned int> d_work_counter;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around the dominant kernel of the last search (bench roofline)
     WorkspacePool pool;
     // fp16 screening copy of the vectors for the HNSW walk (hs_half_kernel), made once by ensure_half_copy
-    __half* d_hvecs = nullptr;
-    float4* d_hrec = nullptr;
+    DevArray<__half> d_hvecs;
+    DevArray<float4> d_hrec;
     int ldh = 0;
     bool half_decided = false;          // the copy was made, or was found not to fit (the walk then reads f32 rows only)
     std::mutex half_mu;
+
+    ~nidx_vec_segment() {
+        if (ev_k0) cudaEventDestroy(ev_k0);
+        if (ev_k1) cudaEventDestroy(ev_k1);
+    }
 
     VecDev vdev() const {
         VecDev v;
@@ -248,8 +272,7 @@ static int stride0_for(int M0) { return (M0 + 31) / 32 * 32; }
 static int strideU_for(int M) { return (M + 15) / 16 * 16; }
 
 static void free_graph(nidx_vec_segment* s) {
-    cudaFree(s->d_level); cudaFree(s->d_adj0); cudaFree(s->d_w0); cudaFree(s->d_upper_off); cudaFree(s->d_adjU); cudaFree(s->d_wU);
-    s->d_level = nullptr; s->d_adj0 = nullptr; s->d_w0 = nullptr; s->d_upper_off = nullptr; s->d_adjU = nullptr; s->d_wU = nullptr;
+    s->d_level.release(); s->d_adj0.release(); s->d_w0.release(); s->d_upper_off.release(); s->d_adjU.release(); s->d_wU.release();
     s->has_graph = false;
 }
 
@@ -270,12 +293,12 @@ static int alloc_graph(nidx_vec_segment* s, const uint8_t* level) {
     s->s0 = stride0_for(s->cfg.m0);
     s->su = strideU_for(s->cfg.m);
     size_t n0 = (size_t)n * s->s0, nu = (size_t)std::max<uint64_t>(rows, 1) * s->su;
-    CU(cudaMalloc(&s->d_level, std::max<uint64_t>(n, 1)));
-    CU(cudaMalloc(&s->d_adj0, n0 * 4 + 16));
-    CU(cudaMalloc(&s->d_w0, n0 * 4 + 16));
-    CU(cudaMalloc(&s->d_upper_off, std::max<uint64_t>(n, 1) * 8));
-    CU(cudaMalloc(&s->d_adjU, nu * 4));
-    CU(cudaMalloc(&s->d_wU, nu * 4));
+    ALLOC(s->d_level, std::max<uint64_t>(n, 1));
+    ALLOC(s->d_adj0, n0 * 4 + 16);
+    ALLOC(s->d_w0, n0 * 4 + 16);
+    ALLOC(s->d_upper_off, std::max<uint64_t>(n, 1) * 8);
+    ALLOC(s->d_adjU, nu * 4);
+    ALLOC(s->d_wU, nu * 4);
     CU(cudaMemcpy(s->d_level, level, n, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(s->d_upper_off, off.data(), n * 8, cudaMemcpyHostToDevice));
     CU(cudaMemset(s->d_adj0, 0xFF, n0 * 4));
@@ -357,10 +380,8 @@ static int attach_half_copy(nidx_vec_segment* s, VecDev* V) {
         size_t free_b = 0, total_b = 0;
         CU(cudaMemGetInfo(&free_b, &total_b));
         if (free_b < hbytes + rbytes + HS_HALF_MARGIN) return 0;
-        if (cudaMalloc(&s->d_hvecs, hbytes) != cudaSuccess || cudaMalloc(&s->d_hrec, rbytes) != cudaSuccess) {
-            (void)cudaGetLastError();   // out of memory is not an error here: the f32-only walk runs
-            cudaFree(s->d_hvecs); cudaFree(s->d_hrec);
-            s->d_hvecs = nullptr; s->d_hrec = nullptr;
+        if (s->d_hvecs.try_alloc(hbytes) != cudaSuccess || s->d_hrec.try_alloc(rbytes) != cudaSuccess) {
+            s->d_hvecs.release();   // out of memory is not an error here: the f32-only walk runs
             return 0;
         }
         hs_half_kernel<<<s->sm_count * 8, 256>>>(s->vdev(), s->n, ldh, s->d_hvecs, s->d_hrec);
@@ -398,11 +419,11 @@ static int make_row_tensor_map(CUtensorMap* map, const float* base, uint64_t row
 
 // A per-row array the caller sets (n values from the host, into *dev, allocated on first use) or clears (host == NULL)
 template <class T>
-static int set_rows(int device, T** dev, const T* host, size_t n) {
+static int set_rows(int device, DevArray<T>& dev, const T* host, size_t n) {
     CU(cudaSetDevice(device));
-    if (!host) { cudaFree(*dev); *dev = nullptr; return 0; }
-    if (!*dev) CU(cudaMalloc(dev, std::max<size_t>(n, 1) * sizeof(T)));
-    CU(cudaMemcpy(*dev, host, n * sizeof(T), cudaMemcpyHostToDevice));
+    if (!host) { dev.release(); return 0; }
+    if (!dev) ALLOC(dev, std::max<size_t>(n, 1) * sizeof(T));
+    CU(cudaMemcpy(dev, host, n * sizeof(T), cudaMemcpyHostToDevice));
     return 0;
 }
 
@@ -439,7 +460,7 @@ static int fill_defaults(nidx_vec_config* c) {
 // Common tail of create/open: vectors are in d_vecs; compute norms, paragraph CSR.
 static int finish_create(nidx_vec_segment* s, const uint32_t* paragraph_of_host) {
     uint64_t n = s->n;
-    CU(cudaMalloc(&s->d_norms, std::max<uint64_t>(n, 1) * 4));
+    ALLOC(s->d_norms, std::max<uint64_t>(n, 1) * 4);
     if (n) {
         int blocks = (int)std::min<uint64_t>((n + 7) / 8, (uint64_t)s->sm_count * 16);
         row_norms_kernel<<<blocks, 256>>>(s->d_vecs, s->ld, n, s->d_norms);
@@ -462,48 +483,48 @@ static int finish_create(nidx_vec_segment* s, const uint32_t* paragraph_of_host)
         first.push_back((uint32_t)n);
         s->n_par = (uint32_t)first.size() - 1;
         if (s->n_par != n) {  // only materialise when some paragraph has several vectors
-            CU(cudaMalloc(&s->d_par_of, n * 4));
+            ALLOC(s->d_par_of, n * 4);
             CU(cudaMemcpy(s->d_par_of, paragraph_of_host, n * 4, cudaMemcpyHostToDevice));
-            CU(cudaMalloc(&s->d_par_first, first.size() * 4));
+            ALLOC(s->d_par_first, first.size() * 4);
             CU(cudaMemcpy(s->d_par_first, first.data(), first.size() * 4, cudaMemcpyHostToDevice));
         }
     }
     if (n) {   // max |v| for the Dot error bound of the tensor-core filter, and whether every row meets the bound
-        unsigned int* d_bits = nullptr;
-        CU(cudaMalloc(&d_bits, 8));
+        DevArray<unsigned int> d_bits;
+        ALLOC(d_bits, 8);
         CU(cudaMemset(d_bits, 0, 8));
         max_norm_kernel<<<std::min<uint64_t>((n + 255) / 256, (uint64_t)s->sm_count * 8), 256>>>(s->vdev(), n, d_bits);
         LAUNCHED();
         unsigned int hb[2] = {0, 0};
         CU(cudaMemcpy(hb, d_bits, 8, cudaMemcpyDeviceToHost));
-        cudaFree(d_bits);
         memcpy(&s->max_norm, &hb[0], 4);
         s->tc_rows_ok = hb[1] == 0;
     }
-    CU(cudaMalloc(&s->d_counters, 8 * sizeof(unsigned long long)));
+    ALLOC(s->d_counters, 8 * sizeof(unsigned long long));
     CU(cudaMemset(s->d_counters, 0, 8 * sizeof(unsigned long long)));
-    CU(cudaMalloc(&s->d_work_counter, 64));
+    ALLOC(s->d_work_counter, 64);
     CU(cudaEventCreate(&s->ev_k0));
     CU(cudaEventCreate(&s->ev_k1));
     CU(cudaDeviceSynchronize());
     return 0;
 }
 
-static int new_segment(const nidx_vec_config* cfg, nidx_vec_segment** out) {
-    if (!cfg || !out) return fail(NIDX_EINVAL, "null argument");
+// A new segment, freed with everything it holds unless the call that creates it succeeds and releases it to the caller
+static int new_segment(const nidx_vec_config* cfg, std::unique_ptr<nidx_vec_segment>& out) {
+    if (!cfg) return fail(NIDX_EINVAL, "null argument");
     nidx_vec_config c = *cfg;
     int r = fill_defaults(&c);
     if (r) return r;
     r = check_device(c.device);
     if (r) return r;
-    nidx_vec_segment* s = new nidx_vec_segment();
+    out.reset(new nidx_vec_segment());
+    nidx_vec_segment* s = out.get();
     s->cfg = c;
     s->d = c.dimension;
     s->ld = (c.dimension + 3) / 4 * 4;
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, c.device);
     s->sm_count = prop.multiProcessorCount;
-    *out = s;
     return 0;
 }
 
@@ -511,39 +532,39 @@ static int new_segment(const nidx_vec_config* cfg, nidx_vec_segment** out) {
 // they are [ld] floats already, copied as they are.
 static int upload_rows(nidx_vec_segment* s, const void* rows, size_t row_bytes, bool host, bool whole) {
     const uint64_t n = s->n;
-    CU(cudaMalloc(&s->d_vecs, std::max<size_t>((size_t)n * s->ld * 4, 16)));
+    ALLOC(s->d_vecs, std::max<size_t>((size_t)n * s->ld * 4, 16));
     if (n == 0) return 0;
     if (whole) {
         CU(cudaMemcpy(s->d_vecs, rows, (size_t)n * row_bytes, host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice));
         return 0;
     }
     const unsigned char* src = static_cast<const unsigned char*>(rows);
-    void* staged = nullptr;
+    DevBuf staged;
     if (host) {
-        CU(cudaMalloc(&staged, (size_t)n * row_bytes));
+        ALLOC(staged, (size_t)n * row_bytes);
         CU(cudaMemcpy(staged, rows, (size_t)n * row_bytes, cudaMemcpyHostToDevice));
-        src = static_cast<const unsigned char*>(staged);
+        src = staged;
     }
     pad_rows_kernel<<<s->sm_count * 8, 256>>>(src, row_bytes, s->d, s->d_vecs, s->ld, n);
     LAUNCHED();
     CU(cudaGetLastError());
     CU(cudaDeviceSynchronize());
-    if (staged) cudaFree(staged);
     return 0;
 }
 
 int nidx_vec_create(const nidx_vec_config* cfg, const float* vectors, uint64_t n, int32_t ld, int mem, const uint32_t* paragraph_of,
                     nidx_vec_segment** out) {
-    nidx_vec_segment* s = nullptr;
-    int r = new_segment(cfg, &s);
+    if (!out) return fail(NIDX_EINVAL, "null argument");
+    std::unique_ptr<nidx_vec_segment> s;
+    int r = new_segment(cfg, s);
     if (r) return r;
-    if (n >= (1ull << 31)) { delete s; return fail(NIDX_EINVAL, "at most 2^31-1 vectors per segment"); }
-    if (ld < s->d) { delete s; return fail(NIDX_EINVAL, "ld %d < dimension %d (VectorErr::InconsistentDimensions)", ld, s->d); }
+    if (n >= (1ull << 31)) return fail(NIDX_EINVAL, "at most 2^31-1 vectors per segment");
+    if (ld < s->d) return fail(NIDX_EINVAL, "ld %d < dimension %d (VectorErr::InconsistentDimensions)", ld, s->d);
     s->n = n;
-    r = upload_rows(s, vectors, (size_t)ld * 4, mem == NIDX_MEM_HOST, ld == s->ld);
-    if (!r) r = finish_create(s, paragraph_of);
-    if (r) { nidx_vec_close(s); return r; }
-    *out = s;
+    r = upload_rows(s.get(), vectors, (size_t)ld * 4, mem == NIDX_MEM_HOST, ld == s->ld);
+    if (!r) r = finish_create(s.get(), paragraph_of);
+    if (r) return r;
+    *out = s.release();
     return 0;
 }
 
@@ -578,13 +599,13 @@ int nidx_normalize_vectors(int32_t device, float* vectors, uint64_t n, int32_t d
     if (n == 0) return 0;
     cudaStream_t st = static_cast<cudaStream_t>(stream_);
     float* dv = vectors;
-    void* staged = nullptr;
+    DevArray<float> staged;
     size_t bytes = (size_t)n * ld * 4;
     if (mem == NIDX_MEM_HOST) {
-        CU(cudaMalloc(&staged, bytes));
-        dv = static_cast<float*>(staged);
+        ALLOC(staged, bytes);
+        dv = staged;
         cudaError_t e = cudaMemcpyAsync(dv, vectors, bytes, cudaMemcpyHostToDevice, st);
-        if (e != cudaSuccess) { cudaFree(staged); return fail(NIDX_ECUDA, "normalize: H2D failed: %s", cudaGetErrorString(e)); }
+        if (e != cudaSuccess) return fail(NIDX_ECUDA, "normalize: H2D failed: %s", cudaGetErrorString(e));
     }
     int sm = 0;
     cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device);
@@ -597,7 +618,6 @@ int nidx_normalize_vectors(int32_t device, float* vectors, uint64_t n, int32_t d
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess && staged) e = cudaMemcpyAsync(vectors, dv, bytes, cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess && staged) e = cudaStreamSynchronize(st);
-    if (staged) cudaFree(staged);
     if (e != cudaSuccess) return fail(NIDX_ECUDA, "normalize failed: %s", cudaGetErrorString(e));
     return 0;
 }
@@ -606,12 +626,6 @@ void nidx_vec_close(nidx_vec_segment* s) {
     if (!s) return;
     cudaSetDevice(s->cfg.device);
     cudaDeviceSynchronize();
-    free_graph(s);
-    cudaFree(s->d_vecs); cudaFree(s->d_norms); cudaFree(s->d_par_of); cudaFree(s->d_par_first); cudaFree(s->d_alive);
-    cudaFree(s->d_counters); cudaFree(s->d_work_counter); cudaFree(s->d_quant); cudaFree(s->d_par_keys); cudaFree(s->inv[0].d_post); cudaFree(s->inv[1].d_post);
-    cudaFree(s->d_hvecs); cudaFree(s->d_hrec);
-    if (s->ev_k0) cudaEventDestroy(s->ev_k0);
-    if (s->ev_k1) cudaEventDestroy(s->ev_k1);
     delete s;
 }
 
@@ -625,9 +639,9 @@ const float* nidx_vec_device_vectors(const nidx_vec_segment* s, int32_t* ld_out)
 int nidx_vec_set_alive(nidx_vec_segment* s, const uint64_t* alive_bits, int mem) {
     if (!s) return fail(NIDX_EINVAL, "null segment");
     CU(cudaSetDevice(s->cfg.device));
-    if (!alive_bits) { cudaFree(s->d_alive); s->d_alive = nullptr; return 0; }
+    if (!alive_bits) { s->d_alive.release(); return 0; }
     size_t words = ((size_t)s->n_par + 63) / 64;
-    if (!s->d_alive) CU(cudaMalloc(&s->d_alive, std::max<size_t>(words, 1) * 8 + 8));
+    if (!s->d_alive) ALLOC(s->d_alive, std::max<size_t>(words, 1) * 8 + 8);
     CU(cudaMemcpy(s->d_alive, alive_bits, words * 8, mem == NIDX_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
     // the number of alive paragraphs: what the reference counts per request (segment.rs:531) when there is no filter
     std::vector<uint64_t> h(words);
@@ -719,7 +733,7 @@ int nidx_vec_rabitq_encode(nidx_vec_segment* s, void* stream_) {
     CU(cudaSetDevice(s->cfg.device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     s->quant_stride = rabitq_stride(s->d);
-    if (!s->d_quant) CU(cudaMalloc(&s->d_quant, std::max<size_t>((size_t)s->n * s->quant_stride, 16)));
+    if (!s->d_quant) ALLOC(s->d_quant, std::max<size_t>((size_t)s->n * s->quant_stride, 16));
     if (s->n) {
         rabitq_encode_kernel<<<(unsigned)((s->n + 7) / 8), 256, 0, stream>>>(s->vdev(), s->d_quant, s->quant_stride);
         LAUNCHED();
@@ -1440,9 +1454,8 @@ int nidx_vec_set_inverted_index(nidx_vec_segment* s, int32_t which, uint32_t n_k
     if (!s || (which != NIDX_INV_LABELS && which != NIDX_INV_FIELDS)) return fail(NIDX_EINVAL, "bad argument");
     if (n_keys && (!key_off || !post_off || (!key_bytes && key_off[n_keys]) || (!postings && post_off[n_keys]))) return fail(NIDX_EINVAL, "null argument");
     CU(cudaSetDevice(s->cfg.device));
-    nidx_vec_segment::InvIndex& ix = s->inv[which];
-    cudaFree(ix.d_post); ix.d_post = nullptr; ix.n_keys = 0;
-    if (!n_keys) { ix.key_bytes.clear(); ix.key_off.assign(1, 0); ix.post_off.assign(1, 0); return 0; }
+    nidx_vec_segment::InvIndex ix;
+    if (!n_keys) { ix.key_off.assign(1, 0); ix.post_off.assign(1, 0); s->inv[which] = std::move(ix); return 0; }
     for (uint32_t i = 0; i + 1 < n_keys; ++i)
         if (FilterEval::cmp_key(key_bytes + key_off[i], key_off[i + 1] - key_off[i], key_bytes + key_off[i + 1], key_off[i + 2] - key_off[i + 1]) >= 0)
             return fail(NIDX_EINVAL, "inverted index keys must be strictly ascending (key %u)", i + 1);
@@ -1451,9 +1464,10 @@ int nidx_vec_set_inverted_index(nidx_vec_segment* s, int32_t which, uint32_t n_k
     ix.key_bytes.assign(key_bytes, key_bytes + key_off[n_keys]);
     ix.key_off.assign(key_off, key_off + n_keys + 1);
     ix.post_off.assign(post_off, post_off + n_keys + 1);
-    CU(cudaMalloc(&ix.d_post, std::max<uint64_t>(np, 1) * 4));
+    ALLOC(ix.d_post, std::max<uint64_t>(np, 1) * 4);
     if (np) CU(cudaMemcpy(ix.d_post, postings, np * 4, cudaMemcpyHostToDevice));
     ix.n_keys = n_keys;
+    s->inv[which] = std::move(ix);   // only now: a rejected or failed call leaves the previous index in place
     return 0;
 }
 
@@ -1560,12 +1574,10 @@ static void host_assign_levels(uint64_t n, int M, uint64_t seed, uint8_t* level)
 
 // Batch-synchronous insertion of order[0 .. n) into the segment's graph (which may already hold other nodes):
 // the loop of build.rs:123-166 as search / select / sort / reverse-link kernels per batch (hnsw_build.cuh).
-// entry_after_first (node, layer), if given, becomes the entry point once the first batch has been inserted.  On failure the
-// segment loses its graph.
-static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level, const std::vector<uint32_t>& order, const std::vector<uint32_t>& ends,
-                          cudaStream_t stream, const uint32_t* entry_after_first = nullptr) {
+// entry_after_first (node, layer), if given, becomes the entry point once the first batch has been inserted.
+static int insert_batches(nidx_vec_segment* s, const std::vector<uint8_t>& level, const std::vector<uint32_t>& order, const std::vector<uint32_t>& ends,
+                          cudaStream_t stream, const uint32_t* entry_after_first) {
     uint64_t n = order.size();
-    int r = 0;
     // work items (node position, layer), insertion order, layer ascending
     std::vector<uint64_t> wstart(n + 1);
     uint64_t W = 0;
@@ -1581,119 +1593,118 @@ static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level
         max_w = std::max<uint64_t>(max_w, wstart[ends[b]] - wstart[begin]);
     }
     int efC = s->cfg.ef_construction, M = s->cfg.m;
-    uint32_t *d_order = nullptr, *d_wpos = nullptr, *d_rev_x = nullptr, *d_idx = nullptr, *d_idx_sorted = nullptr, *d_heads = nullptr;
-    unsigned int* d_head_ctr = nullptr;  // [0] number of heads, [1] work counter
-    unsigned char* d_wlayer = nullptr;
-    uint64_t *d_found = nullptr, *d_rev_key = nullptr, *d_key_sorted = nullptr;
-    int* d_found_count = nullptr;
-    float* d_rev_sim = nullptr;
-    void* d_cub = nullptr;
+    DevArray<uint32_t> d_order, d_wpos, d_rev_x, d_idx, d_idx_sorted, d_heads;
+    DevArray<unsigned int> d_head_ctr;  // [0] number of heads, [1] work counter
+    DevArray<unsigned char> d_wlayer;
+    DevArray<uint64_t> d_found, d_rev_key, d_key_sorted;
+    DevArray<int> d_found_count;
+    DevArray<float> d_rev_sim;
+    DevBuf d_cub;
     size_t cub_bytes = 0;
     size_t max_rev = (size_t)max_w * M;
-    auto cleanup = [&]() {
-        cudaFree(d_order); cudaFree(d_wpos); cudaFree(d_wlayer); cudaFree(d_found); cudaFree(d_found_count); cudaFree(d_rev_key); cudaFree(d_rev_x);
-        cudaFree(d_rev_sim); cudaFree(d_key_sorted); cudaFree(d_idx); cudaFree(d_idx_sorted); cudaFree(d_cub); cudaFree(d_heads); cudaFree(d_head_ctr);
-    };
-    r = [&]() -> int {
-        CU(cudaMalloc(&d_order, n * 4));
-        CU(cudaMalloc(&d_wpos, W * 4));
-        CU(cudaMalloc(&d_wlayer, W));
-        CU(cudaMalloc(&d_found, (size_t)max_b * HS_MAX_LAYERS * efC * 8));
-        CU(cudaMalloc(&d_found_count, (size_t)max_b * HS_MAX_LAYERS * 4));
-        CU(cudaMalloc(&d_rev_key, max_rev * 8));
-        CU(cudaMalloc(&d_key_sorted, max_rev * 8));
-        CU(cudaMalloc(&d_rev_x, max_rev * 4));
-        CU(cudaMalloc(&d_rev_sim, max_rev * 4));
-        CU(cudaMalloc(&d_idx, max_rev * 4));
-        CU(cudaMalloc(&d_idx_sorted, max_rev * 4));
-        CU(cudaMalloc(&d_heads, max_rev * 4));
-        CU(cudaMalloc(&d_head_ctr, 64));
-        CU(cudaMemcpyAsync(d_order, order.data(), n * 4, cudaMemcpyHostToDevice, stream));
-        CU(cudaMemcpyAsync(d_wpos, w_pos.data(), W * 4, cudaMemcpyHostToDevice, stream));
-        CU(cudaMemcpyAsync(d_wlayer, w_layer.data(), W, cudaMemcpyHostToDevice, stream));
-        {
-            std::vector<uint32_t> iota(max_rev);
-            for (size_t i = 0; i < max_rev; ++i) iota[i] = (uint32_t)i;
-            CU(cudaMemcpyAsync(d_idx, iota.data(), max_rev * 4, cudaMemcpyHostToDevice, stream));
-            CU(cudaStreamSynchronize(stream));
-        }
-        CU(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, d_rev_key, d_key_sorted, d_idx, d_idx_sorted, (int)max_rev, 0, 40, stream));
-        CU(cudaMalloc(&d_cub, cub_bytes));
-
-        // shared-memory plans
-
-        int list_cap = efC, hash_bits;
-        int slots = next_pow2(std::max(2048, (efC * s->s0 * 3) / 2));
-        slots = std::max(slots, next_pow2(4 * list_cap));
-        hash_bits = ilog2(slots);
-        size_t smem_search = hs_smem_bytes(s->ld, list_cap, hash_bits);
-        if (smem_search > 200 * 1024) return fail(NIDX_EINVAL, "HNSW build search needs %zu bytes of shared memory", smem_search);
-        hs_kernel_t kern = pick_search_kernel(s->ld);
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_search));
-        int occ = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, HS_THREADS, smem_search));
-        size_t row_bytes = (size_t)s->ld * 4;
-        size_t budget = 96 * 1024;
-        int cache_sel = (int)std::min<size_t>(M, budget / row_bytes);
-        int prune_max = std::max(s->cfg.m0, M) * 95 / 100;
-        int cache_rev = (int)std::min<size_t>(prune_max, budget / row_bytes);
-        size_t smem_sel = hb_smem_bytes(s->ld, cache_sel), smem_rev = hb_smem_bytes(s->ld, cache_rev);
-        CU(cudaFuncSetAttribute(select_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sel));
-        CU(cudaFuncSetAttribute(reverse_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rev));
-        int occ_rev = 0;
-        CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_rev, reverse_link_kernel, HB_THREADS, smem_rev));
-        int rev_grid = std::max(1, occ_rev) * s->sm_count;
-        CU(cudaMemsetAsync(s->d_counters, 0, 8 * sizeof(unsigned long long), stream));
-        s->last_counters.store(nullptr);   // the getters report the build's counters until the next search
-
-
-        VecDev V = s->vdev();
-        int hr = attach_half_copy(s, &V);
-        if (hr) return hr;
-        GraphDev G = s->gdev();
-        uint32_t begin = 0;
-        for (size_t b = 0; b < ends.size(); ++b) {
-            uint32_t end = ends[b];
-            int nb = (int)(end - begin);
-            int nw = (int)(wstart[end] - wstart[begin]);
-            SearchArgs a;
-            memset(&a, 0, sizeof(a));
-            a.mode = 1; a.nq = nb; a.nodes = d_order + begin; a.efC = efC; a.found = d_found; a.found_count = d_found_count;
-            a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = 0; a.work_counter = s->d_work_counter; a.counters = s->d_counters;
-            CU(cudaMemsetAsync(s->d_work_counter, 0, 4, stream));
-            int grid = std::min(nb, std::max(1, occ) * s->sm_count);
-            kern<<<grid, HS_THREADS, smem_search, stream>>>(V, G, a);
-            LAUNCHED();
-            BuildArgs ba;
-            ba.n_work = nw; ba.w_pos = d_wpos + wstart[begin]; ba.w_layer = d_wlayer + wstart[begin]; ba.order = d_order; ba.batch_begin = begin;
-            ba.efC = efC; ba.M = M; ba.found = d_found; ba.found_count = d_found_count; ba.rev_key = d_rev_key; ba.rev_x = d_rev_x; ba.rev_sim = d_rev_sim;
-            ba.cache_cap = cache_sel;
-            select_link_kernel<<<nw, HB_THREADS, smem_sel, stream>>>(V, G, ba);
-            LAUNCHED();
-            int n_rev = nw * M;
-            size_t tmp = cub_bytes;
-            CU(cub::DeviceRadixSort::SortPairs(d_cub, tmp, d_rev_key, d_key_sorted, d_idx, d_idx_sorted, n_rev, 0, 40, stream));
-            LAUNCHED();
-            ReverseArgs ra;
-            ra.n_rev = n_rev; ra.key_sorted = d_key_sorted; ra.idx_sorted = d_idx_sorted; ra.rev_x = d_rev_x; ra.rev_sim = d_rev_sim; ra.cache_cap = cache_rev;
-            ra.heads = d_heads; ra.n_heads = d_head_ctr; ra.work_counter = d_head_ctr + 1;
-            CU(cudaMemsetAsync(d_head_ctr, 0, 8, stream));
-            collect_heads_kernel<<<(n_rev + 255) / 256, 256, 0, stream>>>(d_key_sorted, n_rev, d_heads, d_head_ctr);
-            LAUNCHED();
-            reverse_link_kernel<<<std::min(n_rev, rev_grid), HB_THREADS, smem_rev, stream>>>(V, G, ra);
-            LAUNCHED();
-            begin = end;
-            if (b == 0 && entry_after_first) {   // kernel arguments travel by value: later batches start from the new entry point
-                s->entry_node = entry_after_first[0];
-                s->entry_layer = entry_after_first[1];
-                G = s->gdev();
-            }
-        }
-        CU(cudaGetLastError());
+    ALLOC(d_order, n * 4);
+    ALLOC(d_wpos, W * 4);
+    ALLOC(d_wlayer, W);
+    ALLOC(d_found, (size_t)max_b * HS_MAX_LAYERS * efC * 8);
+    ALLOC(d_found_count, (size_t)max_b * HS_MAX_LAYERS * 4);
+    ALLOC(d_rev_key, max_rev * 8);
+    ALLOC(d_key_sorted, max_rev * 8);
+    ALLOC(d_rev_x, max_rev * 4);
+    ALLOC(d_rev_sim, max_rev * 4);
+    ALLOC(d_idx, max_rev * 4);
+    ALLOC(d_idx_sorted, max_rev * 4);
+    ALLOC(d_heads, max_rev * 4);
+    ALLOC(d_head_ctr, 64);
+    CU(cudaMemcpyAsync(d_order, order.data(), n * 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_wpos, w_pos.data(), W * 4, cudaMemcpyHostToDevice, stream));
+    CU(cudaMemcpyAsync(d_wlayer, w_layer.data(), W, cudaMemcpyHostToDevice, stream));
+    {
+        std::vector<uint32_t> iota(max_rev);
+        for (size_t i = 0; i < max_rev; ++i) iota[i] = (uint32_t)i;
+        CU(cudaMemcpyAsync(d_idx, iota.data(), max_rev * 4, cudaMemcpyHostToDevice, stream));
         CU(cudaStreamSynchronize(stream));
-        return 0;
-    }();
-    cleanup();
+    }
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, d_rev_key.p, d_key_sorted.p, d_idx.p, d_idx_sorted.p, (int)max_rev, 0, 40, stream));
+    ALLOC(d_cub, cub_bytes);
+
+    // shared-memory plans
+
+    int list_cap = efC, hash_bits;
+    int slots = next_pow2(std::max(2048, (efC * s->s0 * 3) / 2));
+    slots = std::max(slots, next_pow2(4 * list_cap));
+    hash_bits = ilog2(slots);
+    size_t smem_search = hs_smem_bytes(s->ld, list_cap, hash_bits);
+    if (smem_search > 200 * 1024) return fail(NIDX_EINVAL, "HNSW build search needs %zu bytes of shared memory", smem_search);
+    hs_kernel_t kern = pick_search_kernel(s->ld);
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_search));
+    int occ = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, HS_THREADS, smem_search));
+    size_t row_bytes = (size_t)s->ld * 4;
+    size_t budget = 96 * 1024;
+    int cache_sel = (int)std::min<size_t>(M, budget / row_bytes);
+    int prune_max = std::max(s->cfg.m0, M) * 95 / 100;
+    int cache_rev = (int)std::min<size_t>(prune_max, budget / row_bytes);
+    size_t smem_sel = hb_smem_bytes(s->ld, cache_sel), smem_rev = hb_smem_bytes(s->ld, cache_rev);
+    CU(cudaFuncSetAttribute(select_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_sel));
+    CU(cudaFuncSetAttribute(reverse_link_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rev));
+    int occ_rev = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_rev, reverse_link_kernel, HB_THREADS, smem_rev));
+    int rev_grid = std::max(1, occ_rev) * s->sm_count;
+    CU(cudaMemsetAsync(s->d_counters, 0, 8 * sizeof(unsigned long long), stream));
+    s->last_counters.store(nullptr);   // the getters report the build's counters until the next search
+
+
+    VecDev V = s->vdev();
+    int hr = attach_half_copy(s, &V);
+    if (hr) return hr;
+    GraphDev G = s->gdev();
+    uint32_t begin = 0;
+    for (size_t b = 0; b < ends.size(); ++b) {
+        uint32_t end = ends[b];
+        int nb = (int)(end - begin);
+        int nw = (int)(wstart[end] - wstart[begin]);
+        SearchArgs a;
+        memset(&a, 0, sizeof(a));
+        a.mode = 1; a.nq = nb; a.nodes = d_order + begin; a.efC = efC; a.found = d_found; a.found_count = d_found_count;
+        a.hash_bits = hash_bits; a.list_cap = list_cap; a.cu_cap = 0; a.work_counter = s->d_work_counter; a.counters = s->d_counters;
+        CU(cudaMemsetAsync(s->d_work_counter, 0, 4, stream));
+        int grid = std::min(nb, std::max(1, occ) * s->sm_count);
+        kern<<<grid, HS_THREADS, smem_search, stream>>>(V, G, a);
+        LAUNCHED();
+        BuildArgs ba;
+        ba.n_work = nw; ba.w_pos = d_wpos + wstart[begin]; ba.w_layer = d_wlayer + wstart[begin]; ba.order = d_order; ba.batch_begin = begin;
+        ba.efC = efC; ba.M = M; ba.found = d_found; ba.found_count = d_found_count; ba.rev_key = d_rev_key; ba.rev_x = d_rev_x; ba.rev_sim = d_rev_sim;
+        ba.cache_cap = cache_sel;
+        select_link_kernel<<<nw, HB_THREADS, smem_sel, stream>>>(V, G, ba);
+        LAUNCHED();
+        int n_rev = nw * M;
+        size_t tmp = cub_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(d_cub.p, tmp, d_rev_key.p, d_key_sorted.p, d_idx.p, d_idx_sorted.p, n_rev, 0, 40, stream));
+        LAUNCHED();
+        ReverseArgs ra;
+        ra.n_rev = n_rev; ra.key_sorted = d_key_sorted; ra.idx_sorted = d_idx_sorted; ra.rev_x = d_rev_x; ra.rev_sim = d_rev_sim; ra.cache_cap = cache_rev;
+        ra.heads = d_heads; ra.n_heads = d_head_ctr; ra.work_counter = d_head_ctr + 1;
+        CU(cudaMemsetAsync(d_head_ctr, 0, 8, stream));
+        collect_heads_kernel<<<(n_rev + 255) / 256, 256, 0, stream>>>(d_key_sorted, n_rev, d_heads, d_head_ctr);
+        LAUNCHED();
+        reverse_link_kernel<<<std::min(n_rev, rev_grid), HB_THREADS, smem_rev, stream>>>(V, G, ra);
+        LAUNCHED();
+        begin = end;
+        if (b == 0 && entry_after_first) {   // kernel arguments travel by value: later batches start from the new entry point
+            s->entry_node = entry_after_first[0];
+            s->entry_layer = entry_after_first[1];
+            G = s->gdev();
+        }
+    }
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(stream));
+    return 0;
+}
+
+// insert_batches; on failure the segment loses its graph
+static int run_insertions(nidx_vec_segment* s, const std::vector<uint8_t>& level, const std::vector<uint32_t>& order, const std::vector<uint32_t>& ends,
+                          cudaStream_t stream, const uint32_t* entry_after_first = nullptr) {
+    int r = insert_batches(s, level, order, ends, stream, entry_after_first);
     if (r) free_graph(s);
     return r;
 }
@@ -1821,32 +1832,31 @@ int nidx_vec_extend_hnsw(nidx_vec_segment* s, uint64_t n_existing, const uint8_t
 // ---- segment files ----------------------------------------------------------------------------
 int nidx_vec_open(const nidx_vec_config* cfg, const char* dir, nidx_vec_segment** out) {
     if (!dir) return fail(NIDX_EINVAL, "null dir");
-    nidx_vec_segment* s = nullptr;
-    int r = new_segment(cfg, &s);
+    if (!out) return fail(NIDX_EINVAL, "null argument");
+    std::unique_ptr<nidx_vec_segment> s;
+    int r = new_segment(cfg, s);
     if (r) return r;
     std::string err;
     std::vector<unsigned char> raw;
-    if (!segio::read_file(std::string(dir) + "/vectors.bin", raw, err)) { delete s; return fail(NIDX_EIO, "%s", err.c_str()); }
+    if (!segio::read_file(std::string(dir) + "/vectors.bin", raw, err)) return fail(NIDX_EIO, "%s", err.c_str());
     size_t rec = (size_t)s->d * 4 + 4;  // vector_store.rs:33-68: [dim x f32 LE][paragraph_addr u32]
-    if (raw.size() % rec) { delete s; return fail(NIDX_EIO, "vectors.bin size %zu is not a multiple of the record length %zu", raw.size(), rec); }
+    if (raw.size() % rec) return fail(NIDX_EIO, "vectors.bin size %zu is not a multiple of the record length %zu", raw.size(), rec);
     uint64_t n = raw.size() / rec;
     s->n = n;
     std::vector<uint32_t> par(n);
     for (uint64_t i = 0; i < n; ++i) memcpy(&par[i], raw.data() + i * rec + (size_t)s->d * 4, 4);
-    r = upload_rows(s, raw.data(), rec, true, false);
-    if (!r) r = finish_create(s, n ? par.data() : nullptr);
-    if (r) { nidx_vec_close(s); return r; }
+    r = upload_rows(s.get(), raw.data(), rec, true, false);
+    if (!r) r = finish_create(s.get(), n ? par.data() : nullptr);
+    if (r) return r;
     // hnsw.graph (+ hnsw.edges) if present
     std::vector<unsigned char> graph, edges;
     if (segio::read_file(std::string(dir) + "/hnsw.graph", graph, err) && !graph.empty()) {
         segio::read_file(std::string(dir) + "/hnsw.edges", edges, err);
         segio::FlatGraph fg;
-        if (!segio::parse_graph_v2(graph, edges, n, stride0_for(s->cfg.m0), strideU_for(s->cfg.m), HS_MAX_LAYERS, fg, err)) {
-            nidx_vec_close(s);
+        if (!segio::parse_graph_v2(graph, edges, n, stride0_for(s->cfg.m0), strideU_for(s->cfg.m), HS_MAX_LAYERS, fg, err))
             return fail(NIDX_EIO, "hnsw.graph: %s", err.c_str());
-        }
-        r = nidx_vec_set_graph(s, fg.level.data(), fg.adj0.data(), fg.w0.empty() ? nullptr : fg.w0.data(), fg.adjU.data(), fg.wU.empty() ? nullptr : fg.wU.data());
-        if (r) { nidx_vec_close(s); return r; }
+        r = nidx_vec_set_graph(s.get(), fg.level.data(), fg.adj0.data(), fg.w0.empty() ? nullptr : fg.w0.data(), fg.adjU.data(), fg.wU.empty() ? nullptr : fg.wU.data());
+        if (r) return r;
         s->entry_node = fg.entry_node;   // the file's entry point (ram_hnsw.rs: hash-order dependent in the reference)
         s->entry_layer = fg.entry_layer;
     }
@@ -1855,17 +1865,13 @@ int nidx_vec_open(const nidx_vec_config* cfg, const char* dir, nidx_vec_segment*
     std::vector<unsigned char> quant;
     if (s->cfg.similarity == NIDX_SIM_DOT && s->d % 64 == 0 && s->d / 32 <= RQ_MAX_WORDS32 && segio::read_file(std::string(dir) + "/vectors.quant", quant, err) && !quant.empty()) {
         size_t rec_q = (size_t)s->d / 8 + 8;
-        if (quant.size() != rec_q * n) { nidx_vec_close(s); return fail(NIDX_EIO, "vectors.quant holds %zu bytes, expected %zu records of %zu", quant.size(), (size_t)n, rec_q); }
+        if (quant.size() != rec_q * n) return fail(NIDX_EIO, "vectors.quant holds %zu bytes, expected %zu records of %zu", quant.size(), (size_t)n, rec_q);
         s->quant_stride = rabitq_stride(s->d);
-        r = [&]() -> int {
-            CU(cudaMalloc(&s->d_quant, std::max<size_t>((size_t)n * s->quant_stride, 16)));
-            CU(cudaMemset(s->d_quant, 0, std::max<size_t>((size_t)n * s->quant_stride, 16)));
-            CU(cudaMemcpy2D(s->d_quant, (size_t)s->quant_stride, quant.data(), rec_q, rec_q, (size_t)n, cudaMemcpyHostToDevice));
-            return 0;
-        }();
-        if (r) { nidx_vec_close(s); return r; }
+        ALLOC(s->d_quant, std::max<size_t>((size_t)n * s->quant_stride, 16));
+        CU(cudaMemset(s->d_quant, 0, std::max<size_t>((size_t)n * s->quant_stride, 16)));
+        CU(cudaMemcpy2D(s->d_quant, (size_t)s->quant_stride, quant.data(), rec_q, rec_q, (size_t)n, cudaMemcpyHostToDevice));
     }
-    *out = s;
+    *out = s.release();
     return 0;
 }
 
@@ -1910,29 +1916,33 @@ struct nidx_txt_segment {
     int device = 0, sm_count = 0;
     uint32_t n_docs = 0, n_terms = 0;
     uint64_t n_post = 0;
-    uint64_t* d_term_off = nullptr;
-    uint2* d_post = nullptr;          // (doc, tf << 8 | fieldnorm id)
-    uint32_t* d_skip_row = nullptr;   // [n_terms]
-    uint32_t* d_skip = nullptr;       // [rows][n_fine + 1]
+    DevArray<uint64_t> d_term_off;
+    DevArray<uint2> d_post;           // (doc, tf << 8 | fieldnorm id)
+    DevArray<uint32_t> d_skip_row;    // [n_terms]
+    DevArray<uint32_t> d_skip;        // [rows][n_fine + 1]
     uint32_t n_fine = 0;
-    uint64_t* d_alive = nullptr;
-    float* d_weight = nullptr;   // [n_terms]
-    float* d_norm_cache = nullptr;  // [256]
-    unsigned int* d_error = nullptr;
-    uint64_t* d_doc_keys = nullptr;   // [n_docs] caller keys of the documents (paragraph ids) for rank fusion (nidx_txt_set_doc_keys)
+    DevArray<uint64_t> d_alive;
+    DevArray<float> d_weight;         // [n_terms]
+    DevArray<float> d_norm_cache;     // [256]
+    DevArray<uint64_t> d_doc_keys;    // [n_docs] caller keys of the documents (paragraph ids) for rank fusion (nidx_txt_set_doc_keys)
     std::vector<uint64_t> own_df;
     uint64_t own_tokens = 0;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around bm25_kernel of the last search (bench roofline)
     // facets (nidx_txt_set_facets): the dictionary on the host in facet order, every document's ords (CSR) in HBM
     std::vector<std::string> facet_keys;
-    uint32_t* d_fdoc_off = nullptr;   // [n_docs + 1]
-    uint32_t* d_ford = nullptr;       // [n_facet_ords]
+    DevArray<uint32_t> d_fdoc_off;    // [n_docs + 1]
+    DevArray<uint32_t> d_ford;        // [n_facet_ords]
     uint64_t n_facet_ords = 0;
     // dates (nidx_txt_set_dates), per field (NIDX_ORDER_CREATED, NIDX_ORDER_MODIFIED): the seconds and every document's dense rank
-    int64_t* d_secs[2] = {nullptr, nullptr};     // [n_docs]
-    uint32_t* d_rank[2] = {nullptr, nullptr};    // [n_docs rounded up to 8], 0 = no date
+    DevArray<int64_t> d_secs[2];      // [n_docs]
+    DevArray<uint32_t> d_rank[2];     // [n_docs rounded up to 8], 0 = no date
     uint32_t n_ranks[2] = {0, 0};
     WorkspacePool pool;
+
+    ~nidx_txt_segment() {
+        if (ev_k0) cudaEventDestroy(ev_k0);
+        if (ev_k1) cudaEventDestroy(ev_k1);
+    }
 };
 
 // tantivy fieldnorm code -> token count (Lucene SmallFloat.byte4ToInt) [recalled]
@@ -1963,68 +1973,62 @@ int nidx_txt_create(int32_t device, uint32_t n_docs, uint32_t n_terms, const uin
     int r = check_device(device);
     if (r) return r;
     if (n_docs >= (1u << 31)) return fail(NIDX_EINVAL, "at most 2^31-1 documents per segment");
-    nidx_txt_segment* t = new nidx_txt_segment();
+    std::unique_ptr<nidx_txt_segment> t(new nidx_txt_segment());   // freed with everything it holds unless the call succeeds
     t->device = device; t->n_docs = n_docs; t->n_terms = n_terms; t->n_post = term_off[n_terms];
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     t->sm_count = prop.multiProcessorCount;
-    r = [&]() -> int {
-        t->n_fine = (n_docs + BM_FINE - 1) / BM_FINE;
-        CU(cudaMalloc(&t->d_term_off, ((size_t)n_terms + 1) * 8));
-        CU(cudaMalloc(&t->d_post, std::max<uint64_t>(t->n_post, 1) * 8));
-        CU(cudaMalloc(&t->d_weight, std::max<uint32_t>(n_terms, 1) * 4));
-        CU(cudaMalloc(&t->d_norm_cache, 1024));
-        CU(cudaMalloc(&t->d_skip_row, std::max<uint32_t>(n_terms, 1) * 4));
-        CU(cudaMalloc(&t->d_error, 4));
-        CU(cudaMemset(t->d_error, 0, 4));
-        CU(cudaEventCreate(&t->ev_k0));
-        CU(cudaEventCreate(&t->ev_k1));
-        CU(cudaMemcpy(t->d_term_off, term_off, ((size_t)n_terms + 1) * 8, cudaMemcpyHostToDevice));
-        if (t->n_post) {
-            // staged only to be packed into the 8-byte posting records
-            uint32_t *d_doc = nullptr, *d_tf = nullptr;
-            unsigned char* d_fn = nullptr;
-            CU(cudaMalloc(&d_doc, t->n_post * 4));
-            CU(cudaMalloc(&d_fn, std::max<uint32_t>(n_docs, 1)));
-            CU(cudaMemcpy(d_doc, post_doc, t->n_post * 4, cudaMemcpyHostToDevice));
-            CU(cudaMemcpy(d_fn, fieldnorm_id, n_docs, cudaMemcpyHostToDevice));
-            if (post_tf) {
-                CU(cudaMalloc(&d_tf, t->n_post * 4));
-                CU(cudaMemcpy(d_tf, post_tf, t->n_post * 4, cudaMemcpyHostToDevice));
-            }
-            bm25_pack_kernel<<<t->sm_count * 8, 256>>>(d_doc, d_tf, d_fn, t->n_post, t->d_post);
-            LAUNCHED();
-            CU(cudaGetLastError());
-            CU(cudaDeviceSynchronize());
-            cudaFree(d_doc); cudaFree(d_tf); cudaFree(d_fn);
+    t->n_fine = (n_docs + BM_FINE - 1) / BM_FINE;
+    ALLOC(t->d_term_off, ((size_t)n_terms + 1) * 8);
+    ALLOC(t->d_post, std::max<uint64_t>(t->n_post, 1) * 8);
+    ALLOC(t->d_weight, std::max<uint32_t>(n_terms, 1) * 4);
+    ALLOC(t->d_norm_cache, 1024);
+    ALLOC(t->d_skip_row, std::max<uint32_t>(n_terms, 1) * 4);
+    CU(cudaEventCreate(&t->ev_k0));
+    CU(cudaEventCreate(&t->ev_k1));
+    CU(cudaMemcpy(t->d_term_off, term_off, ((size_t)n_terms + 1) * 8, cudaMemcpyHostToDevice));
+    if (t->n_post) {
+        // staged only to be packed into the 8-byte posting records
+        DevArray<uint32_t> d_doc, d_tf;
+        DevArray<unsigned char> d_fn;
+        ALLOC(d_doc, t->n_post * 4);
+        ALLOC(d_fn, std::max<uint32_t>(n_docs, 1));
+        CU(cudaMemcpy(d_doc, post_doc, t->n_post * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_fn, fieldnorm_id, n_docs, cudaMemcpyHostToDevice));
+        if (post_tf) {
+            ALLOC(d_tf, t->n_post * 4);
+            CU(cudaMemcpy(d_tf, post_tf, t->n_post * 4, cudaMemcpyHostToDevice));
         }
-        // skip rows for the terms with enough postings
-        std::vector<uint32_t> skip_row(n_terms, NIDX_NIL), row_term;
-        for (uint32_t i = 0; i < n_terms; ++i)
-            if (term_off[i + 1] - term_off[i] >= (uint64_t)BM_SKIP_DF) { skip_row[i] = (uint32_t)row_term.size(); row_term.push_back(i); }
-        if (n_terms) CU(cudaMemcpy(t->d_skip_row, skip_row.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice));
-        size_t skip_words = std::max<size_t>(row_term.size(), 1) * ((size_t)t->n_fine + 1);
-        CU(cudaMalloc(&t->d_skip, skip_words * 4));
-        if (!row_term.empty()) {
-            uint32_t* d_row_term = nullptr;
-            CU(cudaMalloc(&d_row_term, row_term.size() * 4));
-            CU(cudaMemcpy(d_row_term, row_term.data(), row_term.size() * 4, cudaMemcpyHostToDevice));
-            bm25_build_skip_kernel<<<t->sm_count * 8, 256>>>(t->d_term_off, t->d_post, d_row_term, (uint32_t)row_term.size(), t->n_fine, t->d_skip);
-            LAUNCHED();
-            CU(cudaGetLastError());
-            CU(cudaDeviceSynchronize());
-            cudaFree(d_row_term);
-        }
-        t->own_df.resize(n_terms);
-        for (uint32_t i = 0; i < n_terms; ++i) t->own_df[i] = term_off[i + 1] - term_off[i];
-        // a segment alone only knows the quantised lengths; the exact token total comes with set_stats
-        uint64_t tokens = 0;
-        for (uint32_t i = 0; i < n_docs; ++i) tokens += fieldnorm_id_to_value(fieldnorm_id[i]);
-        t->own_tokens = tokens;
-        return txt_upload_stats(t, std::max<uint32_t>(n_docs, 1), std::max<uint64_t>(tokens, 1), t->own_df.data());
-    }();
-    if (r) { nidx_txt_close(t); return r; }
-    *out = t;
+        bm25_pack_kernel<<<t->sm_count * 8, 256>>>(d_doc, d_tf, d_fn, t->n_post, t->d_post);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        CU(cudaDeviceSynchronize());
+    }
+    // skip rows for the terms with enough postings
+    std::vector<uint32_t> skip_row(n_terms, NIDX_NIL), row_term;
+    for (uint32_t i = 0; i < n_terms; ++i)
+        if (term_off[i + 1] - term_off[i] >= (uint64_t)BM_SKIP_DF) { skip_row[i] = (uint32_t)row_term.size(); row_term.push_back(i); }
+    if (n_terms) CU(cudaMemcpy(t->d_skip_row, skip_row.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice));
+    size_t skip_words = std::max<size_t>(row_term.size(), 1) * ((size_t)t->n_fine + 1);
+    ALLOC(t->d_skip, skip_words * 4);
+    if (!row_term.empty()) {
+        DevArray<uint32_t> d_row_term;
+        ALLOC(d_row_term, row_term.size() * 4);
+        CU(cudaMemcpy(d_row_term, row_term.data(), row_term.size() * 4, cudaMemcpyHostToDevice));
+        bm25_build_skip_kernel<<<t->sm_count * 8, 256>>>(t->d_term_off, t->d_post, d_row_term, (uint32_t)row_term.size(), t->n_fine, t->d_skip);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        CU(cudaDeviceSynchronize());
+    }
+    t->own_df.resize(n_terms);
+    for (uint32_t i = 0; i < n_terms; ++i) t->own_df[i] = term_off[i + 1] - term_off[i];
+    // a segment alone only knows the quantised lengths; the exact token total comes with set_stats
+    uint64_t tokens = 0;
+    for (uint32_t i = 0; i < n_docs; ++i) tokens += fieldnorm_id_to_value(fieldnorm_id[i]);
+    t->own_tokens = tokens;
+    r = txt_upload_stats(t.get(), std::max<uint32_t>(n_docs, 1), std::max<uint64_t>(tokens, 1), t->own_df.data());
+    if (r) return r;
+    *out = t.release();
     return 0;
 }
 
@@ -2036,18 +2040,13 @@ int nidx_txt_set_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t total_
 
 int nidx_txt_set_alive(nidx_txt_segment* t, const uint64_t* alive_bits) {
     if (!t) return fail(NIDX_EINVAL, "null segment");
-    return set_rows(t->device, &t->d_alive, alive_bits, ((size_t)t->n_docs + 63) / 64);
+    return set_rows(t->device, t->d_alive, alive_bits, ((size_t)t->n_docs + 63) / 64);
 }
 
 void nidx_txt_close(nidx_txt_segment* t) {
     if (!t) return;
     cudaSetDevice(t->device);
     cudaDeviceSynchronize();
-    cudaFree(t->d_term_off); cudaFree(t->d_post); cudaFree(t->d_skip_row); cudaFree(t->d_skip); cudaFree(t->d_alive); cudaFree(t->d_weight);
-    cudaFree(t->d_norm_cache); cudaFree(t->d_error); cudaFree(t->d_doc_keys); cudaFree(t->d_fdoc_off); cudaFree(t->d_ford);
-    for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); }
-    if (t->ev_k0) cudaEventDestroy(t->ev_k0);
-    if (t->ev_k1) cudaEventDestroy(t->ev_k1);
     delete t;
 }
 
@@ -2080,13 +2079,13 @@ int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* k
             if (doc_ords[i] >= n_facets || (i > doc_off[d] && doc_ords[i] <= doc_ords[i - 1]))
                 return fail(NIDX_EINVAL, "document %u: facet ords must be < n_facets and strictly ascending", d);
     CU(cudaSetDevice(t->device));
-    cudaFree(t->d_fdoc_off); cudaFree(t->d_ford);
-    t->d_fdoc_off = nullptr; t->d_ford = nullptr;
-    t->facet_keys.clear(); t->n_facet_ords = 0;
-    CU(cudaMalloc(&t->d_fdoc_off, ((size_t)t->n_docs + 1) * 4));
-    CU(cudaMalloc(&t->d_ford, std::max<uint64_t>(nnz, 1) * 4));
-    CU(cudaMemcpy(t->d_fdoc_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    if (nnz) CU(cudaMemcpy(t->d_ford, doc_ords, nnz * 4, cudaMemcpyHostToDevice));
+    DevArray<uint32_t> fdoc_off, ford;
+    ALLOC(fdoc_off, ((size_t)t->n_docs + 1) * 4);
+    ALLOC(ford, std::max<uint64_t>(nnz, 1) * 4);
+    CU(cudaMemcpy(fdoc_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (nnz) CU(cudaMemcpy(ford, doc_ords, nnz * 4, cudaMemcpyHostToDevice));
+    t->d_fdoc_off = std::move(fdoc_off);   // only now: a rejected or failed call leaves the previous facets in place
+    t->d_ford = std::move(ford);
     t->facet_keys = std::move(keys);
     t->n_facet_ords = nnz;
     return 0;
@@ -2095,56 +2094,54 @@ int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* k
 int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_t* modified) {
     if (!t || !created || !modified) return fail(NIDX_EINVAL, "null argument");
     CU(cudaSetDevice(t->device));
-    for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); t->d_secs[f] = nullptr; t->d_rank[f] = nullptr; t->n_ranks[f] = 0; }
     const uint32_t n = t->n_docs;
     const size_t padded = std::max<size_t>(((size_t)n + 7) & ~(size_t)7, 8);
     // ranks: sort (seconds, doc) on the device, flag the first document of every distinct date, inclusive prefix sum, scatter
-    int64_t* d_sorted = nullptr;
-    uint32_t *d_doc = nullptr, *d_doc_sorted = nullptr, *d_flag = nullptr, *d_incl = nullptr;
-    void* d_cub = nullptr;
-    int r = [&]() -> int {
-        size_t sort_bytes = 0, scan_bytes = 0;
-        if (n) {
-            CU(cudaMalloc(&d_sorted, (size_t)n * 8));
-            CU(cudaMalloc(&d_doc, (size_t)n * 4));
-            CU(cudaMalloc(&d_doc_sorted, (size_t)n * 4));
-            CU(cudaMalloc(&d_flag, (size_t)n * 4));
-            CU(cudaMalloc(&d_incl, (size_t)n * 4));
-            std::vector<uint32_t> iota(n);
-            for (uint32_t i = 0; i < n; ++i) iota[i] = i;
-            CU(cudaMemcpy(d_doc, iota.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-            CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const int64_t*)nullptr, d_sorted, d_doc, d_doc_sorted, (int)n));
-            CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, d_flag, d_incl, (int)n));
-            CU(cudaMalloc(&d_cub, std::max(sort_bytes, scan_bytes)));
-        }
-        const int blocks = std::max(1, std::min<int>(t->sm_count * 8, (int)((n + 255) / 256)));
-        for (int f = 0; f < 2; ++f) {
-            CU(cudaMalloc(&t->d_secs[f], std::max<size_t>(n, 1) * 8));
-            CU(cudaMalloc(&t->d_rank[f], padded * 4));
-            CU(cudaMemset(t->d_rank[f], 0, padded * 4));
-            if (!n) continue;
-            CU(cudaMemcpy(t->d_secs[f], f == 0 ? created : modified, (size_t)n * 8, cudaMemcpyHostToDevice));
-            size_t tmp = sort_bytes;
-            CU(cub::DeviceRadixSort::SortPairs(d_cub, tmp, (const int64_t*)t->d_secs[f], d_sorted, d_doc, d_doc_sorted, (int)n));
-            LAUNCHED();
-            date_flag_kernel<<<blocks, 256>>>(d_sorted, n, d_flag);
-            LAUNCHED();
-            tmp = scan_bytes;
-            CU(cub::DeviceScan::InclusiveSum(d_cub, tmp, d_flag, d_incl, (int)n));
-            LAUNCHED();
-            date_scatter_kernel<<<blocks, 256>>>(d_incl, d_doc_sorted, n, t->d_rank[f]);
-            LAUNCHED();
-            CU(cudaGetLastError());
-            CU(cudaMemcpy(&t->n_ranks[f], d_incl + n - 1, 4, cudaMemcpyDeviceToHost));
-        }
-        CU(cudaDeviceSynchronize());
-        return 0;
-    }();
-    cudaFree(d_sorted); cudaFree(d_doc); cudaFree(d_doc_sorted); cudaFree(d_flag); cudaFree(d_incl); cudaFree(d_cub);
-    if (r) {
-        for (int f = 0; f < 2; ++f) { cudaFree(t->d_secs[f]); cudaFree(t->d_rank[f]); t->d_secs[f] = nullptr; t->d_rank[f] = nullptr; t->n_ranks[f] = 0; }
+    DevArray<int64_t> d_sorted, secs[2];
+    DevArray<uint32_t> d_doc, d_doc_sorted, d_flag, d_incl, rank[2];
+    DevBuf d_cub;
+    uint32_t n_ranks[2] = {0, 0};
+    size_t sort_bytes = 0, scan_bytes = 0;
+    if (n) {
+        ALLOC(d_sorted, (size_t)n * 8);
+        ALLOC(d_doc, (size_t)n * 4);
+        ALLOC(d_doc_sorted, (size_t)n * 4);
+        ALLOC(d_flag, (size_t)n * 4);
+        ALLOC(d_incl, (size_t)n * 4);
+        std::vector<uint32_t> iota(n);
+        for (uint32_t i = 0; i < n; ++i) iota[i] = i;
+        CU(cudaMemcpy(d_doc, iota.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
+        CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const int64_t*)nullptr, d_sorted.p, d_doc.p, d_doc_sorted.p, (int)n));
+        CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, d_flag.p, d_incl.p, (int)n));
+        ALLOC(d_cub, std::max(sort_bytes, scan_bytes));
     }
-    return r;
+    const int blocks = std::max(1, std::min<int>(t->sm_count * 8, (int)((n + 255) / 256)));
+    for (int f = 0; f < 2; ++f) {
+        ALLOC(secs[f], std::max<size_t>(n, 1) * 8);
+        ALLOC(rank[f], padded * 4);
+        CU(cudaMemset(rank[f], 0, padded * 4));
+        if (!n) continue;
+        CU(cudaMemcpy(secs[f], f == 0 ? created : modified, (size_t)n * 8, cudaMemcpyHostToDevice));
+        size_t tmp = sort_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(d_cub.p, tmp, (const int64_t*)secs[f].p, d_sorted.p, d_doc.p, d_doc_sorted.p, (int)n));
+        LAUNCHED();
+        date_flag_kernel<<<blocks, 256>>>(d_sorted, n, d_flag);
+        LAUNCHED();
+        tmp = scan_bytes;
+        CU(cub::DeviceScan::InclusiveSum(d_cub.p, tmp, d_flag.p, d_incl.p, (int)n));
+        LAUNCHED();
+        date_scatter_kernel<<<blocks, 256>>>(d_incl, d_doc_sorted, n, rank[f]);
+        LAUNCHED();
+        CU(cudaGetLastError());
+        CU(cudaMemcpy(&n_ranks[f], d_incl + n - 1, 4, cudaMemcpyDeviceToHost));
+    }
+    CU(cudaDeviceSynchronize());
+    for (int f = 0; f < 2; ++f) {   // only now: a failed call leaves the previous dates in place
+        t->d_secs[f] = std::move(secs[f]);
+        t->d_rank[f] = std::move(rank[f]);
+        t->n_ranks[f] = n_ranks[f];
+    }
+    return 0;
 }
 
 }  // extern "C"
@@ -2273,7 +2270,7 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     a.query_terms = d_qt; a.query_off = d_qo; a.nq = nq; a.k = k; a.cap = cap;
     a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
-    a.out_keys = w.partial.as<uint64_t>(); a.out_total = reinterpret_cast<unsigned long long*>(d_total); a.error_flag = t->d_error;
+    a.out_keys = w.partial.as<uint64_t>(); a.out_total = reinterpret_cast<unsigned long long*>(d_total);
     if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after
     auto launch = [&](auto kern, size_t bytes, auto... extra) -> int {   // the BM25 pass, between the roofline events
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
@@ -2305,12 +2302,7 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     else bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
     LAUNCHED();
     CU(cudaGetLastError());
-    r = st.finish();
-    if (r || !ohost) return r;
-    unsigned int err = 0;   // an accumulator table that filled up would mean incomplete sums: report, never return them silently
-    CU(cudaMemcpy(&err, t->d_error, 4, cudaMemcpyDeviceToHost));
-    if (err) { cudaMemset(t->d_error, 0, 4); return fail(NIDX_EOVERFLOW, "BM25 accumulator table overflow"); }
-    return 0;
+    return st.finish();
 }
 
 extern "C" {
@@ -2474,7 +2466,7 @@ void nidx_shard_destroy(nidx_shard_comm* c) {
 
 int nidx_vec_set_paragraph_keys(nidx_vec_segment* s, const uint64_t* keys) {
     if (!s) return fail(NIDX_EINVAL, "null segment");
-    return set_rows(s->cfg.device, &s->d_par_keys, keys, s->n_par);
+    return set_rows(s->cfg.device, s->d_par_keys, keys, s->n_par);
 }
 
 // How the parts of a sharded search are merged (step 3)
@@ -2655,7 +2647,7 @@ int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uin
 // ---- rank fusion + the fused shard search (SURVEY 8f rank 4) --------------------------------------------------------------
 int nidx_txt_set_doc_keys(nidx_txt_segment* t, const uint64_t* keys) {
     if (!t) return fail(NIDX_EINVAL, "null segment");
-    return set_rows(t->device, &t->d_doc_keys, keys, t->n_docs);
+    return set_rows(t->device, t->d_doc_keys, keys, t->n_docs);
 }
 
 }  // extern "C"

@@ -83,7 +83,6 @@ struct Bm25Args {
     uint64_t after_docaddr, docaddr_base;
     uint64_t* out_keys;         // [nq][k] rank keys (score desc, doc asc), 0 = none
     unsigned long long* out_total;  // [nq] matching documents (Count collector)
-    unsigned int* error_flag;   // reserved (an accumulator that could fill up would report here; this design cannot)
 };
 
 // ---- index-time kernels ---------------------------------------------------------------------------------
