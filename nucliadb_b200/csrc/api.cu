@@ -851,60 +851,6 @@ __global__ void and_bits_kernel(const uint64_t* a, const uint64_t* b, uint64_t* 
     if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
-// hnsw_search_kernel is instantiated for the common row lengths (ld = NG * 128 floats); other dimensions use
-// the run-time loop (NG = 0).
-typedef void (*hs_kernel_t)(VecDev, GraphDev, SearchArgs);
-static hs_kernel_t pick_search_kernel(int ld) {
-    if (ld % 128 == 0) switch (ld / 128) {
-        case 1: return hnsw_search_kernel<1>;
-        case 2: return hnsw_search_kernel<2>;
-        case 3: return hnsw_search_kernel<3>;
-        case 4: return hnsw_search_kernel<4>;
-        case 6: return hnsw_search_kernel<6>;
-        case 8: return hnsw_search_kernel<8>;
-        default: break;
-    }
-    return hnsw_search_kernel<0>;
-}
-
-static hs_kernel_t pick_rabitq_walk_kernel_w4(int ld) {
-    if (ld % 128 == 0) switch (ld / 128) {
-        case 2: return hnsw_rabitq_kernel<2, 4>;
-        case 3: return hnsw_rabitq_kernel<3, 4>;
-        case 4: return hnsw_rabitq_kernel<4, 4>;
-        case 6: return hnsw_rabitq_kernel<6, 4>;
-        case 8: return hnsw_rabitq_kernel<8, 4>;
-        default: break;
-    }
-    return hnsw_rabitq_kernel<0, 4>;
-}
-
-static hs_kernel_t pick_rabitq_walk_kernel(int ld) {
-    if (ld % 128 == 0) switch (ld / 128) {
-        case 2: return hnsw_rabitq_kernel<2>;
-        case 3: return hnsw_rabitq_kernel<3>;
-        case 4: return hnsw_rabitq_kernel<4>;
-        case 6: return hnsw_rabitq_kernel<6>;
-        case 8: return hnsw_rabitq_kernel<8>;
-        default: break;
-    }
-    return hnsw_rabitq_kernel<0>;
-}
-
-typedef void (*scan_kernel_t)(VecDev, const float*, const float*, int, int, float*);
-static scan_kernel_t pick_scan_kernel(int ld) {
-    if (ld % 128 == 0) switch (ld / 128) {
-        case 1: return scan_scores_kernel_t<1, 4>;
-        case 2: return scan_scores_kernel_t<2, 4>;
-        case 3: return scan_scores_kernel_t<3, 4>;
-        case 4: return scan_scores_kernel_t<4, 2>;
-        case 6: return scan_scores_kernel_t<6, 2>;
-        case 8: return scan_scores_kernel_t<8, 2>;
-        default: break;
-    }
-    return scan_scores_kernel;
-}
-
 // Shared-memory plans of the two walks, used by AUTO's choice and by the launch alike.  Each returns false when the plan does not
 // fit one CTA (the list and the visited set grow with ef and k).
 static bool hnsw_search_smem(const nidx_vec_segment* s, int ef0, int k, int* list_cap, int* cu_cap, int* hash_bits, size_t* bytes) {
@@ -931,6 +877,35 @@ static bool rq_walk_smem(const nidx_vec_segment* s, int k, int* last_k, int* cu_
 }
 
 }  // extern "C"
+
+// The vector kernels are instantiated for the common row lengths, ld = NG * 128 floats with NG among NGs; other dimensions use the
+// run-time loop (NG = 0).  `inst(std::integral_constant<int, NG>())` names the instance.
+template <int... NGs, typename F>
+static auto pick_ng(int ld, F inst) {
+    auto k = inst(std::integral_constant<int, 0>());
+    auto match = [&](auto ng) { if (ld == ng * 128) k = inst(ng); };
+    (match(std::integral_constant<int, NGs>()), ...);
+    return k;
+}
+
+typedef void (*hs_kernel_t)(VecDev, GraphDev, SearchArgs);
+static hs_kernel_t pick_search_kernel(int ld) {
+    return pick_ng<1, 2, 3, 4, 6, 8>(ld, [](auto ng) -> hs_kernel_t { return hnsw_search_kernel<ng>; });
+}
+
+// w4: the 4-warp CTA shape (quantised_walk)
+static hs_kernel_t pick_rabitq_walk_kernel(int ld, bool w4) {
+    return pick_ng<2, 3, 4, 6, 8>(ld, [w4](auto ng) -> hs_kernel_t { return w4 ? hnsw_rabitq_kernel<ng, 4> : hnsw_rabitq_kernel<ng>; });
+}
+
+// four vectors in flight per warp for rows of up to 384 floats, two for longer ones
+typedef void (*scan_kernel_t)(VecDev, const float*, const float*, int, int, float*);
+static scan_kernel_t pick_scan_kernel(int ld) {
+    return pick_ng<1, 2, 3, 4, 6, 8>(ld, [](auto ng) -> scan_kernel_t {
+        if constexpr (ng == 0) return scan_scores_kernel;
+        else return scan_scores_kernel_t<ng, ng <= 3 ? 4 : 2>;
+    });
+}
 
 // ---- filter formulas on the device (inverted_index/paragraph.rs:124-186) ---------------------------------------------
 // ranges[2r], ranges[2r + 1] = [begin, end) into the postings of one inverted index; one block per range sets the bits
@@ -1305,13 +1280,13 @@ struct VecCall {
         // CTA shape: the walk is bound by the ~1 000 dependent hops of a query, so what counts is how many queries are resident.
         // 8 warps per query: 4 CTAs per SM; 4 warps: 7 per SM.  The 4-warp shape is taken when the batch does not fit one wave of the
         // 8-warp shape (NIDX_B200_RQ_W = 4 / 8 forces one).
-        hs_kernel_t kern = pick_rabitq_walk_kernel(s->ld);
+        hs_kernel_t kern = pick_rabitq_walk_kernel(s->ld, false);
         int threads = HS_THREADS, grid = 0;
         r = walk_grid(kern, threads, smem, &grid);
         const char* ew = getenv("NIDX_B200_RQ_W");
         const int force = ew ? atoi(ew) : 0;
         if (!r && (force == 4 || (force != 8 && nq > grid))) {
-            kern = pick_rabitq_walk_kernel_w4(s->ld);
+            kern = pick_rabitq_walk_kernel(s->ld, true);
             threads = 128;
             r = walk_grid(kern, threads, smem, &grid);
         }

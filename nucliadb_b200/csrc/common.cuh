@@ -165,6 +165,7 @@ __device__ __forceinline__ void cp_async4(void* smem_dst, const void* gmem_src) 
 __device__ __forceinline__ void cp_async_commit_wait_all() {
     asm volatile("cp.async.commit_group;\n\tcp.async.wait_all;" ::: "memory");
 }
+__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 
 // dense_f32.rs:29-33 with simsimd's edge cases; na, nb = precomputed ordered norms.
 __device__ __forceinline__ float cosine_from_parts(float ab, float na, float nb) {

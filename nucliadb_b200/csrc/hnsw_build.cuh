@@ -62,13 +62,13 @@ __device__ inline int select_neighbours_heuristic(const VecDev& V, HeurSmem& h, 
     constexpr int AHEAD = 4;
     const int lines = (V.ld * 4 + 127) >> 7;
     if (warp < AHEAD && warp < nc)
-        for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(reinterpret_cast<const char*>(V.vecs + (size_t)h.cand_id[warp] * V.ld) + (size_t)l * 128));
+        for (int l = lane; l < lines; l += 32) prefetch_l2(reinterpret_cast<const char*>(V.vecs + (size_t)h.cand_id[warp] * V.ld) + (size_t)l * 128);
     for (int i = 0; i < nc && nsel < k; ++i) {  // 66-69: stop once k are kept
         uint32_t x = h.cand_id[i];
         float sim = h.cand_sim[i];
         if (threadIdx.x == 0) *h.s_fail = 0;
         if (warp == HB_WARPS - 1 && i + AHEAD < nc)
-            for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(reinterpret_cast<const char*>(V.vecs + (size_t)h.cand_id[i + AHEAD] * V.ld) + (size_t)l * 128));
+            for (int l = lane; l < lines; l += 32) prefetch_l2(reinterpret_cast<const char*>(V.vecs + (size_t)h.cand_id[i + AHEAD] * V.ld) + (size_t)l * 128);
         __syncthreads();
         const float4* xv = reinterpret_cast<const float4*>(V.vecs + (size_t)x * V.ld);
         float xn = V.sim != SIM_DOT ? V.norms[x] : 0.0f;

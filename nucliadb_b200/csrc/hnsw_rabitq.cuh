@@ -37,9 +37,7 @@ struct RqCtx {
     int nw;
     float low, delta, root_dim;
     uint32_t sum_quantized;
-    uint32_t* gvis;           // this CTA's slice of the global visited table
-    uint32_t gv_mask;
-    int gv_bits, gv_limit;
+    VisitedSet gvis;          // layer 0: this CTA's slice of the global visited table
     unsigned long long n_quant, n_rerank;
 };
 
@@ -107,15 +105,12 @@ __device__ __forceinline__ void rq_estimate(const RqCtx& r, const unsigned char*
 // shuffles add the eight partial sums (integers: exact in any order).  The group's first lane tests the visited set (global
 // table: the atomicCAS and the code loads are in flight together, codes of visited neighbours are fetched for nothing) and
 // finishes the estimate.  Admitted keys are compacted into todo_key[0 .. nadmit) (their order does not matter: hs_merge ranks
-// by key).  The last warp first prefetches the adjacency row of the predicted next candidate (as hs_expand) and publishes its
-// list position (*s_pred) for the caller's nothing-admitted fast path.
-// Counters live in s_cnt[parity of the hop][admitted, fresh, overflow]: thread 0 folds them after the barrier and clears the
-// other parity for the next hop, so no extra barrier is needed to reset them.
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
-
+// by key).  The last warp first prefetches the adjacency row of the predicted next candidate (hs_prefetch_next) and publishes its
+// list position (HopRec::pred) for the caller's nothing-admitted fast path.
+// The hop's record collects the counts; thread 0 folds them after the barrier and resets the other record for the next hop, so no
+// extra barrier is needed to reset them (hs_reseed resets both before a layer search's first hop).
 template <bool GLOBAL_VIS, int W>
-__device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchArgs& a, RqCtx& r, uint32_t node, int layer, int ef, int best,
-                                 int (*s_cnt)[4], int* s_pred, unsigned long long* s_maxtodo) {
+__device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchArgs& a, RqCtx& r, uint32_t node, int layer, int ef, int best) {
     // LPN lanes per neighbour, so that the CTA covers one adjacency row of 32 per pass: 8 lanes (one 16-byte chunk each per 128 bytes
     // of code) with 8 warps, 4 lanes (two chunks each) with 4 warps -- the float tail of the estimate then runs once per warp for
     // eight neighbours instead of four.
@@ -126,31 +121,16 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
     const int sub = lane & (LPN - 1);
     const int stride = G.stride(layer);
     const unsigned cur = c.hop & 1u;
-    int* cnt = s_cnt[cur];
-    c.s_ntodo = cnt;        // hs_merge reads the number of todo keys and of admitted keys: both = cnt[0]
-    c.s_nadmit = cnt;
-    c.s_maxtodo = &s_maxtodo[cur];
+    HopRec& h = c.hops[cur];
+    const VisitedSet& vis = GLOBAL_VIS ? r.gvis : c.vis;
     const int len = *c.s_len;
     const bool full = len >= ef;
     const float wscore = full ? key_score(c.A[len - 1]) : 0.0f;
     const int visited = *c.s_hash_count;       // stable during the expansion (thread 0 updates it after the barrier)
-    if (threadIdx.x == 0) *c.s_best_next = INT_MAX;   // hs_merge's atomicMin target: reset before the barrier below
     const int nchunks = a.code_stride >> 4;
     if (warp == W - 1) {
-        int pred = -1;
-        for (int i0 = best + 1; i0 < len && pred < 0; i0 += 32) {
-            int i = i0 + lane;
-            unsigned m = __ballot_sync(0xFFFFFFFFu, i < len && (c.A[i] & 1ull));
-            if (m) pred = i0 + __ffs(m) - 1;
-        }
-        uint32_t pnode = NIL;
-        if (pred >= 0) {
-            pnode = key_id(c.A[pred]);
-            const uint32_t* row2 = G.row(pnode, layer);
-            uint32_t* dst = c.pref_row + (cur ^ 1u) * HS_MAX_ROW;
-            for (int e = lane; e < stride; e += 32) cp_async4(dst + e, row2 + e);
-        }
-        if (lane == 0) { c.pref_node[cur ^ 1u] = pnode; *s_pred = pred; }
+        const int pred = hs_prefetch_next<false>(G, c, layer, best, len);
+        if (lane == 0) h.pred = pred;
     }
     const uint32_t* prow = c.pref_row + cur * HS_MAX_ROW;
     const bool hit = c.pref_node[cur] == node;
@@ -177,22 +157,9 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
         for (int blk = 0; blk < 2; ++blk)
 #pragma unroll
             for (int cc = 0; cc < CPL; ++cc) w[blk][cc] = make_uint4(0, 0, 0, 0);
-        if (GLOBAL_VIS) {
-            if (valid) load_chunks();
-            if (valid && sub == 0) {
-                if (visited >= r.gv_limit) ov = true;
-                else {
-                    uint32_t h = (y * 2654435761u) >> (32 - r.gv_bits);
-                    while (true) {
-                        uint32_t old = atomicCAS(&r.gvis[h], NIL, y);
-                        if (old == NIL) { fresh = true; break; }
-                        if (old == y) break;
-                        h = (h + 1) & r.gv_mask;
-                    }
-                }
-            }
-        } else {
-            if (valid && sub == 0) fresh = hash_insert(c, y, ov);
+        if (GLOBAL_VIS && valid) load_chunks();
+        if (valid && sub == 0) fresh = vis.insert(y, visited, ov);
+        if (!GLOBAL_VIS) {
             fresh = __shfl_sync(0xFFFFFFFFu, fresh, lane & ~(LPN - 1));
             if (fresh) load_chunks();
         }
@@ -219,13 +186,13 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
             rq_finish(r, idot, w[0][0].x, w[0][0].y, est, err);       // chunk 0 starts with the code's header (dot_quant_original, sum_bits)
             uint64_t key = make_key(est, y, 1);
             if (!full || est > wscore) {                                  // layer_search (search.rs:286): a SCORE above the worst of a full list (a tie is refused whatever the ids)
-                c.todo_key[atomicAdd(&cnt[0], 1)] = key;
-                atomicMax(c.s_maxtodo, (unsigned long long)key);
+                c.todo_key[atomicAdd(&h.nadmit, 1)] = key;
+                atomicMax(&h.maxtodo, (unsigned long long)key);
             }
         }
         unsigned mf = __ballot_sync(0xFFFFFFFFu, sub == 0 && fresh);
-        if (lane == 0 && mf) atomicAdd(&cnt[1], __popc(mf));
-        if (ov) cnt[2] = 1;
+        if (lane == 0 && mf) atomicAdd(&h.nfresh, __popc(mf));
+        if (ov) h.overflow = 1;
     }
     if (warp == W - 1) {
         cp_async_commit_wait_all();
@@ -241,7 +208,7 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
                         const unsigned char* cp = a.codes + (size_t)y2 * a.code_stride;
                         prefetch_l2(cp);
                         if (((uintptr_t)cp & 127) + a.code_stride > 128) prefetch_l2(cp + 128 - ((uintptr_t)cp & 127));
-                        prefetch_l2(&r.gvis[(y2 * 2654435761u) >> (32 - r.gv_bits)]);
+                        prefetch_l2(&r.gvis.slots[r.gvis.slot(y2)]);
                     }
                 }
         }
@@ -249,60 +216,34 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
     c.hop++;
     __syncthreads();
     if (threadIdx.x == 0) {
-        *c.s_hash_count = visited + cnt[1];
+        *c.s_hash_count = visited + h.nfresh;
         c.n_expand++;
-        r.n_quant += cnt[1];
-        if (cnt[2]) c.n_overflow++;
-        int* nxt = s_cnt[cur ^ 1u];
-        nxt[0] = 0; nxt[1] = 0; nxt[2] = 0;
-        s_maxtodo[cur ^ 1u] = 0;
+        r.n_quant += h.nfresh;
+        if (h.overflow) c.n_overflow++;
+        c.hops[cur ^ 1u].clear();
     }
-}
-
-// Start a layer search on the list in c.A: every entry unexpanded, visited set = the list's ids.
-template <bool GLOBAL_VIS>
-__device__ inline void rq_reseed(SearchCtx& c, RqCtx& r) {
-    if (!GLOBAL_VIS) { hs_reseed(c); return; }
-    __syncthreads();
-    uint4 e4 = make_uint4(NIL, NIL, NIL, NIL);
-    for (uint32_t i = threadIdx.x; i < (r.gv_mask + 1) / 4; i += blockDim.x) reinterpret_cast<uint4*>(r.gvis)[i] = e4;
-    if (threadIdx.x == 0) { *c.s_hash_count = 0; *c.s_best = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL; }
-    __syncthreads();
-    int len = *c.s_len;
-    for (int i = threadIdx.x; i < len; i += blockDim.x) {
-        uint64_t key = c.A[i] | 1ull;
-        c.A[i] = key;
-        uint32_t y = key_id(key), h = (y * 2654435761u) >> (32 - r.gv_bits);
-        while (true) {
-            uint32_t old = atomicCAS(&r.gvis[h], NIL, y);
-            if (old == NIL || old == y) break;
-            h = (h + 1) & r.gv_mask;
-        }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) *c.s_hash_count = len;
-    __syncthreads();
 }
 
 template <bool GLOBAL_VIS, int W>
-__device__ inline void rq_layer_search(const GraphDev& G, SearchCtx& c, const SearchArgs& a, RqCtx& r, int layer, int ef, int (*s_cnt)[4], int* s_pred, unsigned long long* s_maxtodo) {
+__device__ inline void rq_layer_search(const GraphDev& G, SearchCtx& c, const SearchArgs& a, RqCtx& r, int layer, int ef) {
     while (true) {
         int best = *c.s_best, len = *c.s_len;
         if (best >= len) break;
         uint64_t ckey = c.A[best];
-        rq_expand<GLOBAL_VIS, W>(G, c, a, r, key_id(ckey), layer, ef, best, s_cnt, s_pred, s_maxtodo);
-        if (*c.s_nadmit == 0) {
+        rq_expand<GLOBAL_VIS, W>(G, c, a, r, key_id(ckey), layer, ef, best);
+        const HopRec& h = c.last_hop();
+        if (h.nadmit == 0) {
             // nothing admitted (the common case once the list is full): the list only loses the expanded flag of `best`, and the
             // next candidate is the first unexpanded entry after it -- the one the prefetching warp has just located.
-            if (threadIdx.x == 0) {    // (every thread read *s_best before rq_expand's barrier and *s_nadmit's slot is not touched until the next one)
+            if (threadIdx.x == 0) {    // (every thread read *s_best before rq_expand's barrier and this record is not touched until the next one)
                 c.A[best] &= ~1ull;
-                int pred = *s_pred;
+                int pred = h.pred;
                 *c.s_best = pred >= 0 ? pred : len;
             }
             __syncthreads();
             continue;
         }
-        hs_merge<false>(c, ef, best);
+        hs_merge<false>(c, ef, best, h.nadmit);
     }
 }
 
@@ -311,23 +252,11 @@ __device__ inline void rq_layer_search(const GraphDev& G, SearchCtx& c, const Se
 template <int NG, int W = HS_WARPS>
 __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_kernel(VecDev V, GraphDev G, SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
-    __shared__ int s_ints[8];
-    __shared__ unsigned int s_work;
     __shared__ int s_wtot[RQ_RC / 32], s_total, s_hlen;
-    __shared__ int s_cnt[2][4], s_pred;
-    __shared__ unsigned long long s_maxtodo[2], s_maxtodo_cu;
     __shared__ float s_best_k;
     SearchCtx c;
     RqCtx r;
-    unsigned char* p = smem;
-    c.qvec = reinterpret_cast<float*>(p); p += (size_t)V.ld * 4;
-    c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
-    c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
-    c.todo_key = reinterpret_cast<uint64_t*>(p); p += HS_MAX_ROW * 8;
-    c.hash = reinterpret_cast<uint32_t*>(p); p += (size_t)4 << a.hash_bits;
-    c.todo_id = reinterpret_cast<uint32_t*>(p); p += HS_MAX_ROW * 4;
-    c.pref_row = reinterpret_cast<uint32_t*>(p); p += 2 * HS_MAX_ROW * 4;
-    c.pref_node = reinterpret_cast<uint32_t*>(p); p += 16;
+    unsigned char* p = hs_setup(c, a, smem, V.ld);
     uint64_t* heap = reinterpret_cast<uint64_t*>(p); p += (size_t)(a.k + 1) * 8;          // rerank_top's `best`, rank keys, descending
     uint32_t* planes = reinterpret_cast<uint32_t*>(p); p += (size_t)4 * (V.d / 32) * 4;
     p = smem + (((size_t)(p - smem) + 15) & ~(size_t)15);
@@ -335,29 +264,15 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
     uint32_t* surv_id = reinterpret_cast<uint32_t*>(p); p += RQ_RC * 4;
     float* surv_up = reinterpret_cast<float*>(p); p += RQ_RC * 4;
     float* surv_real = reinterpret_cast<float*>(p);
-    c.hop = 0;
-    c.s_len = &s_ints[0]; c.s_best = &s_ints[1]; c.s_best_next = &s_ints[2]; c.s_ntodo = &s_ints[3];
-    c.s_bn = &s_ints[2];   // (the lean layer search of hnsw_search.cuh is not used by this kernel)
-    c.s_hash_count = &s_ints[4]; c.s_flag = &s_ints[5]; c.s_nadmit = &s_ints[6];
-    c.hash_bits = a.hash_bits;
-    c.hash_mask = (1u << a.hash_bits) - 1;
-    c.hash_limit = (int)((15u << a.hash_bits) >> 4) - HS_MAX_ROW;
-    c.n_dist = c.n_expand = c.n_overflow = 0;
-    c.qnorm = 0.0f;
     r.planes = planes; r.planes_t = planes_t; r.nw = V.d / 32; r.root_dim = __fsqrt_rn((float)V.d);
-    r.gvis = a.gvisited + ((size_t)blockIdx.x << a.gv_bits);
-    r.gv_bits = a.gv_bits; r.gv_mask = (1u << a.gv_bits) - 1; r.gv_limit = (int)((15u << a.gv_bits) >> 4) - HS_MAX_ROW;
+    r.gvis.init(a.gvisited + ((size_t)blockIdx.x << a.gv_bits), a.gv_bits);
     r.n_quant = r.n_rerank = 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int ng = V.ld >> 2;
     const RabitqQueryParams* qparams = reinterpret_cast<const RabitqQueryParams*>(a.qparams);
 
-    while (true) {
-        __syncthreads();
-        if (threadIdx.x == 0) s_work = atomicAdd(a.work_counter, 1u);
-        __syncthreads();
-        unsigned int q = s_work;
-        if (q >= (unsigned)a.nq) break;
+    unsigned q;
+    while (hs_next_query(a, &q)) {
         const float* qsrc = a.queries + (size_t)q * V.ld;
         for (int i = threadIdx.x; i < ng; i += blockDim.x) reinterpret_cast<float4*>(c.qvec)[i] = reinterpret_cast<const float4*>(qsrc)[i];
         for (int i = threadIdx.x; i < 4 * r.nw; i += blockDim.x) planes[i] = a.planes[(size_t)q * 4 * r.nw + i];
@@ -365,8 +280,6 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
             int ch = i >> 4, kpl = (i >> 2) & 3, wi = ch * 4 + (i & 3) - 2;
             planes_t[i] = (wi >= 0 && wi < r.nw) ? a.planes[(size_t)q * 4 * r.nw + kpl * r.nw + wi] : 0u;
         }
-        if (threadIdx.x < 8) s_cnt[threadIdx.x >> 2][threadIdx.x & 3] = 0;   // closest_up's hops (hs_expand) change the parity between queries
-        if (threadIdx.x < 2) s_maxtodo[threadIdx.x] = 0;
         RabitqQueryParams qp = qparams[q];
         r.low = qp.low; r.delta = qp.delta; r.sum_quantized = qp.sum_quantized;
         __syncthreads();
@@ -382,16 +295,14 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
         }
         __syncthreads();
         for (int layer = (int)G.entry_layer; layer > 0; --layer) {   // search.rs:321-327: one best node per upper layer
-            rq_reseed<false>(c, r);
-            rq_layer_search<false, W>(G, c, a, r, layer, 1, s_cnt, &s_pred, s_maxtodo);
+            hs_reseed(c, c.vis);
+            rq_layer_search<false, W>(G, c, a, r, layer, 1);
             __syncthreads();
         }
-        rq_reseed<true>(c, r);
-        rq_layer_search<true, W>(G, c, a, r, 0, a.last_k, s_cnt, &s_pred, s_maxtodo);             // search.rs:335-345
+        hs_reseed(c, r.gvis);
+        rq_layer_search<true, W>(G, c, a, r, 0, a.last_k);             // search.rs:335-345
         __syncthreads();
 
-        c.s_ntodo = &s_ints[3]; c.s_nadmit = &s_ints[6];   // rq_expand pointed both at its counter slot; closest_up_nodes (hs_expand) needs two
-        c.s_maxtodo = &s_maxtodo_cu;
         // ---- rerank_top (rabitq.rs:222-244) over the list, best estimate first ----
         const int len = *c.s_len;
         if (threadIdx.x == 0) { s_hlen = 0; s_best_k = 0.0f; }
@@ -458,11 +369,8 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
         }
         hs_emit_results<NG, W>(V, G, c, a, q);
     }
-    if (lane == 0 && c.n_dist) atomicAdd(&a.counters[0], c.n_dist);
+    hs_flush_counters(c, a.counters);
     if (threadIdx.x == 0) {
-        if (c.n_expand) atomicAdd(&a.counters[1], c.n_expand);
-        if (c.n_overflow & 0xFFFFFFFFull) atomicAdd(&a.counters[2], c.n_overflow & 0xFFFFFFFFull);
-        if (c.n_overflow >> 32) atomicAdd(&a.counters[3], c.n_overflow >> 32);
         if (r.n_quant) atomicAdd(&a.counters[4], r.n_quant);
         if (r.n_rerank) atomicAdd(&a.counters[5], r.n_rerank);
     }

@@ -62,24 +62,67 @@ struct SearchArgs {
     int last_k;                       // min(k * RERANKING_FACTOR, RERANKING_LIMIT)
 };
 
+// An exact visited set: open addressing over 1 << bits slots of node ids (NIL = free), linear probing.  Threads insert concurrently.
+struct VisitedSet {
+    uint32_t* slots;
+    uint32_t mask;
+    int bits;
+    int limit;   // count at which inserts stop: a pass inserts at most one adjacency row, so the table stays below 15/16 full
+
+    __device__ void init(uint32_t* s, int b) {
+        slots = s; bits = b; mask = (1u << b) - 1;
+        limit = (int)((15u << b) >> 4) - HS_MAX_ROW;
+    }
+    __device__ uint32_t slot(uint32_t y) const { return (y * 2654435761u) >> (32 - bits); }
+    // Every thread of the CTA; 4 << bits bytes, 16-byte aligned.
+    __device__ void clear() const {
+        const uint4 e4 = make_uint4(NIL, NIL, NIL, NIL);
+        for (uint32_t i = threadIdx.x; i < (mask + 1) / 4; i += blockDim.x) reinterpret_cast<uint4*>(slots)[i] = e4;
+    }
+    // True iff y was not in the set (and is now).  `count` is the number of ids the set held when the pass of inserts began: the
+    // callers publish the new count only after the pass.  A full table reports "already visited" and sets `overflow`.
+    __device__ bool insert(uint32_t y, int count, bool& overflow) const {
+        if (count >= limit) { overflow = true; return false; }
+        for (uint32_t h = slot(y);; h = (h + 1) & mask) {
+            const uint32_t old = atomicCAS(&slots[h], NIL, y);
+            if (old == NIL) return true;
+            if (old == y) return false;
+        }
+    }
+};
+
+// What one expansion leaves for hs_merge and for the code after it.  There are two records, used by alternate hops (the parity of
+// SearchCtx::hop), so that one can be reset while threads still read the other: hs_expand resets its own before its first barrier,
+// rq_expand (whose atomics come before its barrier) the next hop's after it, and hs_reseed both.
+struct HopRec {
+    unsigned long long maxtodo;  // the largest admitted key: list entries above it keep their position in the merge
+    int ntodo;                   // hs_expand: todo_key[0, ntodo) holds the scored neighbours, 0 for a refused one
+    int nadmit;                  // admitted keys (rq_expand compacts them into todo_key[0, nadmit))
+    int best_next;               // hs_merge's atomicMin: the first unexpanded entry of the merged list
+    int pred;                    // rq_expand: list position of the predicted next candidate (-1: none)
+    int nfresh;                  // rq_expand: neighbours not visited before
+    int overflow;                // rq_expand: the visited set was full
+
+    __device__ void clear() { maxtodo = 0; nadmit = 0; best_next = INT_MAX; nfresh = 0; overflow = 0; }
+};
+
 struct SearchCtx {
     float* qvec;
     uint64_t *A, *B;
-    uint32_t* hash;
+    VisitedSet vis;       // the shared-memory visited set
     uint32_t* todo_id;
     uint64_t* todo_key;
     uint32_t* pref_row;   // [2][HS_MAX_ROW] speculatively prefetched adjacency rows (double buffered by hop parity)
     uint32_t* pref_node;  // [2] node each buffer belongs to (NIL = none)
-    int *s_len, *s_best, *s_best_next, *s_ntodo, *s_hash_count, *s_flag, *s_nadmit;
-    int* s_bn;                       // [2] parity slots for s_best_next in the barrier-lean layer search
-    unsigned long long* s_maxtodo;   // the largest admitted key of the expansion: list entries above it keep their position
-    unsigned hop;
-    uint32_t hash_mask;
-    int hash_bits, hash_limit;
+    int *s_len, *s_best, *s_hash_count, *s_flag;
+    HopRec* hops;         // [2], by hop parity
+    unsigned hop;         // expansions so far; hs_expand and rq_expand advance it at their end
     float qnorm;
     float qbound;                    // >= |q| (hs_query_bound), for the screen's error bound
     unsigned long long n_dist, n_expand, n_overflow;
     unsigned long long n_skip;       // similarities the screen settled without reading the f32 row
+
+    __device__ HopRec& last_hop() const { return hops[(hop & 1u) ^ 1u]; }   // the record of the expansion that just ran
 };
 
 // An upper bound on |q| for the query in shared memory, the same in every thread: the squares are exact in f64 and the f64 sum
@@ -117,96 +160,140 @@ __host__ __device__ __forceinline__ size_t hs_smem_bytes(int ld, int list_cap, i
     return (size_t)ld * 4 + (size_t)list_cap * 16 + ((size_t)4 << hash_bits) + HS_MAX_ROW * 12 + HS_MAX_ROW * 8 + 16 + 64;
 }
 
-// returns true iff y was not in the set (and is now).  A full table reports "already visited".
-__device__ __forceinline__ bool hash_insert(SearchCtx& c, uint32_t y, bool& overflow) {
-    if (*c.s_hash_count >= c.hash_limit) { overflow = true; return false; }
-    uint32_t h = (y * 2654435761u) >> (32 - c.hash_bits);
-    while (true) {
-        uint32_t old = atomicCAS(&c.hash[h], NIL, y);
-        if (old == NIL) return true;
-        if (old == y) return false;
-        h = (h + 1) & c.hash_mask;
+// The CTA's shared state of a walk: the dynamic shared memory laid out as hs_smem_bytes counts it, from `p` on, and the shared
+// scalars.  Returns the end of the layout, where the quantised walk lays out its own arrays.
+__device__ inline unsigned char* hs_setup(SearchCtx& c, const SearchArgs& a, unsigned char* p, int ld) {
+    __shared__ int s_ints[4];
+    __shared__ HopRec s_hops[2];
+    c.qvec = reinterpret_cast<float*>(p); p += (size_t)ld * 4;
+    c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
+    c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
+    c.todo_key = reinterpret_cast<uint64_t*>(p); p += HS_MAX_ROW * 8;
+    c.vis.init(reinterpret_cast<uint32_t*>(p), a.hash_bits); p += (size_t)4 << a.hash_bits;
+    c.todo_id = reinterpret_cast<uint32_t*>(p); p += HS_MAX_ROW * 4;
+    c.pref_row = reinterpret_cast<uint32_t*>(p); p += 2 * HS_MAX_ROW * 4;
+    c.pref_node = reinterpret_cast<uint32_t*>(p); p += 16;
+    c.s_len = &s_ints[0]; c.s_best = &s_ints[1]; c.s_hash_count = &s_ints[2]; c.s_flag = &s_ints[3];
+    c.hops = s_hops;
+    c.hop = 0;
+    c.qnorm = 0.0f;
+    c.n_dist = c.n_expand = c.n_overflow = c.n_skip = 0;
+    return p;
+}
+
+// The dynamic scheduler: the CTA's next query in *q, false when every query has been taken.
+__device__ inline bool hs_next_query(const SearchArgs& a, unsigned* q) {
+    __shared__ unsigned s_work;
+    __syncthreads();
+    if (threadIdx.x == 0) s_work = atomicAdd(a.work_counter, 1u);
+    __syncthreads();
+    *q = s_work;
+    return *q < (unsigned)a.nq;
+}
+
+// counters [0]-[3]: n_dist lives in lane 0 of every warp, the rest in thread 0
+__device__ inline void hs_flush_counters(const SearchCtx& c, unsigned long long* counters) {
+    if ((threadIdx.x & 31) == 0 && c.n_dist) atomicAdd(&counters[0], c.n_dist);
+    if (threadIdx.x == 0) {
+        if (c.n_expand) atomicAdd(&counters[1], c.n_expand);
+        if (c.n_overflow & 0xFFFFFFFFull) atomicAdd(&counters[2], c.n_overflow & 0xFFFFFFFFull);
+        if (c.n_overflow >> 32) atomicAdd(&counters[3], c.n_overflow >> 32);
     }
 }
 
-// Clear the visited set and seed it with the ids of the current list; mark every entry unexpanded.
-__device__ inline void hs_reseed(SearchCtx& c) {
+// Start a layer search (or closest_up_nodes) on the list in c.A: every entry unexpanded, the visited set `vis` = the list's ids,
+// both hop records reset.
+__device__ inline void hs_reseed(SearchCtx& c, const VisitedSet& vis) {
     __syncthreads();
-    for (int i = threadIdx.x; i <= (int)c.hash_mask; i += blockDim.x) c.hash[i] = NIL;
-    if (threadIdx.x == 0) { *c.s_hash_count = 0; *c.s_best = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL; }
+    vis.clear();
+    if (threadIdx.x == 0) {
+        *c.s_hash_count = 0; *c.s_best = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL;
+        c.hops[0].clear(); c.hops[1].clear();
+    }
     __syncthreads();
     int len = *c.s_len;
     bool ov = false;
     for (int i = threadIdx.x; i < len; i += blockDim.x) {
         uint64_t key = c.A[i] | 1ull;
         c.A[i] = key;
-        hash_insert(c, key_id(key), ov);
+        vis.insert(key_id(key), 0, ov);
     }
     __syncthreads();
     if (threadIdx.x == 0) *c.s_hash_count = len;
     __syncthreads();
 }
 
+// The node expanded next, unless a new neighbour outranks it, is the first unexpanded list entry after `best` (CU: entry 1, the
+// next one once the popped candidate is dropped).  The last warp starts an asynchronous copy (cp.async) of its adjacency row into
+// the other half of the double buffer while the hop works; the row's HBM latency then overlaps the hop's own loads.  The caller
+// waits for the copy before the hop's last barrier.  Returns the entry's list position, -1 if there is none.
+template <bool CU>
+__device__ inline int hs_prefetch_next(const GraphDev& G, SearchCtx& c, int layer, int best, int len) {
+    const int lane = threadIdx.x & 31;
+    const int stride = G.stride(layer);
+    int pred = -1;
+    if (CU) {
+        pred = len > 1 ? 1 : -1;
+    } else {
+        for (int i0 = best + 1; i0 < len && pred < 0; i0 += 32) {
+            int i = i0 + lane;
+            unsigned m = __ballot_sync(0xFFFFFFFFu, i < len && (c.A[i] & 1ull));
+            if (m) pred = i0 + __ffs(m) - 1;
+        }
+    }
+    uint32_t pnode = NIL;
+    if (pred >= 0) {
+        pnode = key_id(c.A[pred]);
+        const uint32_t* row = G.row(pnode, layer);
+        uint32_t* dst = c.pref_row + ((c.hop & 1u) ^ 1u) * HS_MAX_ROW;
+        for (int e = lane; e < stride; e += 32) cp_async4(dst + e, row + e);
+    }
+    if (lane == 0) c.pref_node[(c.hop & 1u) ^ 1u] = pnode;
+    return pred;
+}
+
 // Expand `node` (already chosen): gather unvisited neighbours (warp 0), score them (all warps).
 // Admission: layer_search (search.rs:286) -- when the list holds `ef` entries only keys better than the
 // worst survive; closest_up_nodes (search.rs:231) -- score >= min_score.
-// Speculation: while warp 0 works, the last warp starts an asynchronous copy (cp.async) of the adjacency
-// row of the node that will be expanded next if no new neighbour outranks it -- `pred_idx` in the list --
-// into the other half of a double buffer; the row's HBM latency then overlaps this expansion's vector loads.
-// LEAN (the layer search's hot loop): the list length arrives in a register and s_best_next alternates between two slots, so that
-// hs_merge needs no barrier after thread 0 has published the new length -- three barriers per expansion instead of four.
+// Speculation: while warp 0 works, the last warp prefetches the row of the predicted next node (hs_prefetch_next).
+// The hop's record: warp 0 resets it before the first barrier, the scoring after it adds the admitted keys.
+// LEAN (the layer search's hot loop): the list length arrives in a register, so that hs_merge needs no barrier after thread 0 has
+// published the new length -- three barriers per expansion instead of four.
 template <bool CU, int NG, int W = HS_WARPS, bool LEAN = false>
 __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& c, uint32_t node, int layer, int ef, float min_score, int best, int len_in = -1) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int stride = G.stride(layer);
     unsigned cur = c.hop & 1u;
-    if (LEAN) c.s_best_next = c.s_bn + cur;
+    HopRec& h = c.hops[cur];
     if (warp == 0) {
         const uint32_t* prow = c.pref_row + cur * HS_MAX_ROW;
         bool hit = c.pref_node[cur] == node;
         const uint32_t* row = G.row(node, layer);
+        const int visited = *c.s_hash_count;
         int ntodo = 0;
         bool ov = false;
         for (int e0 = 0; e0 < stride; e0 += 32) {
             uint32_t y = NIL;
             if (e0 + lane < stride) y = hit ? prow[e0 + lane] : __ldg(row + e0 + lane);
-            bool fresh = (y != NIL) && hash_insert(c, y, ov);
+            bool fresh = (y != NIL) && c.vis.insert(y, visited, ov);
             unsigned mask = __ballot_sync(0xFFFFFFFFu, fresh);
             if (fresh) c.todo_id[ntodo + __popc(mask & ((1u << lane) - 1))] = y;
             ntodo += __popc(mask);
         }
         if (__any_sync(0xFFFFFFFFu, ov) && lane == 0) c.n_overflow++;
         if (lane == 0) {
-            *c.s_ntodo = ntodo;
-            *c.s_hash_count += ntodo;
-            *c.s_best_next = INT_MAX;
-            *c.s_nadmit = 0;
-            *c.s_maxtodo = 0;
+            h.ntodo = ntodo;
+            *c.s_hash_count = visited + ntodo;
+            h.best_next = INT_MAX;
+            h.nadmit = 0;
+            h.maxtodo = 0;
             c.n_expand++;
         }
     } else if (warp == W - 1) {
-        int len = LEAN ? len_in : *c.s_len;
-        int pred = -1;
-        if (CU) {
-            pred = len > 1 ? 1 : -1;
-        } else {
-            for (int i0 = best + 1; i0 < len && pred < 0; i0 += 32) {
-                int i = i0 + lane;
-                unsigned m = __ballot_sync(0xFFFFFFFFu, i < len && (c.A[i] & 1ull));
-                if (m) pred = i0 + __ffs(m) - 1;
-            }
-        }
-        uint32_t pnode = NIL;
-        if (pred >= 0) {
-            pnode = key_id(c.A[pred]);
-            const uint32_t* row2 = G.row(pnode, layer);
-            uint32_t* dst = c.pref_row + (cur ^ 1u) * HS_MAX_ROW;
-            for (int e = lane; e < stride; e += 32) cp_async4(dst + e, row2 + e);
-        }
-        if (lane == 0) c.pref_node[cur ^ 1u] = pnode;
+        hs_prefetch_next<CU>(G, c, layer, best, LEAN ? len_in : *c.s_len);
     }
     __syncthreads();
-    int ntodo = *c.s_ntodo, len = LEAN ? len_in : *c.s_len;
+    int ntodo = h.ntodo, len = LEAN ? len_in : *c.s_len;
     uint64_t wkey = (!CU && len >= ef) ? c.A[len - 1] : 0;
     int ng = V.ld >> 2;
     auto finish = [&](int j, uint32_t y, float ab, float vnorm) {
@@ -214,7 +301,7 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
         uint64_t key = make_key(s, y, 1);
         bool admit = CU ? (s >= min_score) : (wkey == 0 || s > key_score(wkey));   // search.rs:286 compares scores: a tie with the worst is refused
         c.todo_key[j] = admit ? key : 0;
-        if (admit) { atomicAdd(c.s_nadmit, 1); atomicMax(c.s_maxtodo, (unsigned long long)key); }
+        if (admit) { atomicAdd(&h.nadmit, 1); atomicMax(&h.maxtodo, (unsigned long long)key); }
         c.n_dist++;
     };
     // Screen (layer search with a full list): a neighbour whose fp16 dot plus its error bound cannot beat wkey is rejected
@@ -230,7 +317,7 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
     const int lines = screen ? (V.ldh * 2 + 127) >> 7 : (V.ld * 4 + 127) >> 7;
     for (int j = warp + W; j < ntodo; j += W) {
         const char* rowp = screen ? reinterpret_cast<const char*>(hrow(c.todo_id[j])) : reinterpret_cast<const char*>(frow(c.todo_id[j]));
-        for (int l = lane; l < lines; l += 32) asm volatile("prefetch.global.L2 [%0];" :: "l"(rowp + (size_t)l * 128));
+        for (int l = lane; l < lines; l += 32) prefetch_l2(rowp + (size_t)l * 128);
     }
     for (int j = warp; j < ntodo; j += W) {
         uint32_t y = c.todo_id[j];
@@ -249,18 +336,20 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
     __syncthreads();
 }
 
-// Merge the admitted todo keys into the sorted list A -> B (rank merge, no sort), keep at most `cap`.
+// Merge the keys todo_key[0, ntodo) of the expansion that just ran (0 = refused; the rest is in its record, c.last_hop()) into
+// the sorted list A -> B (rank merge, no sort), keep at most `cap`.
 // CU: entry 0 (the popped candidate) is dropped.  Afterwards A/B are swapped and s_len/s_best updated.
 // LEAN: `len_io` / `best_io` carry the list length and the next candidate in registers (every thread computes them); no barrier
 // after thread 0's update of the shared copies, which only code outside the hot loop reads (after a barrier of its own).
 template <bool CU, bool LEAN = false>
-__device__ inline void hs_merge(SearchCtx& c, int cap, int best, int* len_io = nullptr, int* best_io = nullptr) {
-    int len = LEAN ? *len_io : *c.s_len, ntodo = *c.s_ntodo;
+__device__ inline void hs_merge(SearchCtx& c, int cap, int best, int ntodo, int* len_io = nullptr, int* best_io = nullptr) {
+    HopRec& h = c.last_hop();
+    int len = LEAN ? *len_io : *c.s_len;
     int first = CU ? 1 : 0;
     int my_best = INT_MAX;
-    const uint64_t maxtodo = *c.s_maxtodo;
-    const int nadmit = *c.s_nadmit;         // final since hs_expand's last barrier; re-zeroed by the next expansion
-    int* const bn = c.s_best_next;
+    const uint64_t maxtodo = h.maxtodo;
+    const int nadmit = h.nadmit;            // final since the expansion's last barrier
+    int* const bn = &h.best_next;
     for (int t = threadIdx.x; t < len - first + ntodo; t += blockDim.x) {
         uint64_t key;
         int p;
@@ -315,9 +404,8 @@ __device__ inline void hs_layer_search(const VecDev& V, const GraphDev& G, Searc
     while (best < len) {
         uint64_t ckey = c.A[best];
         hs_expand<false, NG, W, true>(V, G, c, key_id(ckey), layer, ef, 0.0f, best, len);
-        hs_merge<false, true>(c, ef, best, &len, &best);
+        hs_merge<false, true>(c, ef, best, c.last_hop().ntodo, &len, &best);
     }
-    c.s_best_next = c.s_bn;                    // (callers that use the shared copies come after a barrier)
 }
 
 // NodeFilter::passes (search.rs:147-170) for the popped candidate; warp 0 only, result broadcast by the caller.
@@ -352,7 +440,7 @@ __device__ inline bool hs_passes(const VecDev& V, const SearchArgs& a, uint32_t 
 template <int NG, int W = HS_WARPS>
 __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, uint32_t* out_ids, float* out_scores) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    hs_reseed(c);
+    hs_reseed(c, c.vis);
     int nacc = 0;
     while (true) {
         int len = *c.s_len;
@@ -373,7 +461,7 @@ __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCt
         nacc += *c.s_flag;
         if (nacc == a.k) break;  // 214
         hs_expand<true, NG, W>(V, G, c, node, 0, 0, a.min_score, 0);
-        hs_merge<true>(c, a.cu_cap, 0);
+        hs_merge<true>(c, a.cu_cap, 0, c.last_hop().ntodo);
     }
     return nacc;
 }
@@ -413,39 +501,13 @@ __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, Searc
 template <int NG>
 __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, GraphDev G, SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
-    __shared__ int s_ints[8];
-    __shared__ unsigned int s_work;
-    __shared__ unsigned long long s_maxtodo;
-    __shared__ int s_bn[2];
     SearchCtx c;
-    c.s_bn = s_bn;
-    unsigned char* p = smem;
-    c.qvec = reinterpret_cast<float*>(p); p += (size_t)V.ld * 4;
-    c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
-    c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
-    c.todo_key = reinterpret_cast<uint64_t*>(p); p += HS_MAX_ROW * 8;
-    c.hash = reinterpret_cast<uint32_t*>(p); p += (size_t)4 << a.hash_bits;
-    c.todo_id = reinterpret_cast<uint32_t*>(p); p += HS_MAX_ROW * 4;
-    c.pref_row = reinterpret_cast<uint32_t*>(p); p += 2 * HS_MAX_ROW * 4;
-    c.pref_node = reinterpret_cast<uint32_t*>(p);
-    c.hop = 0;
-    c.s_len = &s_ints[0]; c.s_best = &s_ints[1]; c.s_best_next = &s_bn[0]; c.s_ntodo = &s_ints[3];
-    c.s_hash_count = &s_ints[4]; c.s_flag = &s_ints[5]; c.s_nadmit = &s_ints[6];
-    c.s_maxtodo = &s_maxtodo;
-    c.hash_bits = a.hash_bits;
-    c.hash_mask = (1u << a.hash_bits) - 1;
-    c.hash_limit = (int)((15u << a.hash_bits) >> 4) - HS_MAX_ROW;
-    c.n_dist = c.n_expand = c.n_overflow = c.n_skip = 0;
+    hs_setup(c, a, smem, V.ld);
     int lane = threadIdx.x & 31;
     int ng = V.ld >> 2;
 
-    while (true) {
-        __syncthreads();
-        if (threadIdx.x == 0) s_work = atomicAdd(a.work_counter, 1u);
-        __syncthreads();
-        unsigned int q = s_work;
-        if (q >= (unsigned)a.nq) break;
-
+    unsigned q;
+    while (hs_next_query(a, &q)) {
         const float* qsrc;
         uint32_t self = NIL;
         if (a.mode == 0) { qsrc = a.queries + (size_t)q * V.ld; c.qnorm = V.sim != SIM_DOT ? a.qnorms[q] : 0.0f; }
@@ -471,7 +533,7 @@ __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, Gr
             int ef;
             if (a.mode == 0) ef = layer == 0 ? a.ef0 : 1;
             else ef = layer <= top ? a.efC : 1;
-            hs_reseed(c);
+            hs_reseed(c, c.vis);
             hs_layer_search<NG>(V, G, c, layer, ef);
             __syncthreads();
             if (a.mode == 1 && layer <= top && layer < HS_MAX_LAYERS) {
@@ -493,13 +555,9 @@ __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, Gr
 
         if (a.mode == 0) hs_emit_results<NG>(V, G, c, a, q);
     }
-    // counters: n_dist and n_skip live in lane 0 of every warp, the rest in thread 0; [6] = f32 rows read for a similarity
-    if (lane == 0 && c.n_dist) { atomicAdd(&a.counters[0], c.n_dist); atomicAdd(&a.counters[6], c.n_dist - c.n_skip); }
-    if (threadIdx.x == 0) {
-        if (c.n_expand) atomicAdd(&a.counters[1], c.n_expand);
-        if (c.n_overflow & 0xFFFFFFFFull) atomicAdd(&a.counters[2], c.n_overflow & 0xFFFFFFFFull);
-        if (c.n_overflow >> 32) atomicAdd(&a.counters[3], c.n_overflow >> 32);
-    }
+    hs_flush_counters(c, a.counters);
+    // [6] = f32 rows read for a similarity (n_skip lives in lane 0 of every warp, as n_dist)
+    if (lane == 0 && c.n_dist) atomicAdd(&a.counters[6], c.n_dist - c.n_skip);
 }
 
 }  // namespace nidx
