@@ -358,6 +358,37 @@ int nidx_txt_search_ordered(nidx_txt_segment* seg, const uint32_t* query_terms, 
                             const nidx_txt_search_params* p, const nidx_txt_order* order, const nidx_txt_facet_request* facets, uint32_t* out_docs,
                             int64_t* out_dates, int32_t* out_counts, uint64_t* out_total, uint32_t* out_facet_counts, void* stream);
 
+/* ---- Exact phrases: tantivy's PhraseQuery (slop 0) as one clause of the keyword query (reference: the quoted groups of
+ * nidx_paragraph's body, query_parser/keyword_parser.rs:27-91).  A phrase t_0 .. t_{m-1} occurs in a document freq times, freq = the
+ * number of start positions s such that t_i is at position s + i for every i; the document matches when freq >= 1 and scores
+ * weight * freq / (freq + norm(fieldnorm)), weight = (f32 sum of the terms' idf, in phrase order, repeats counted) * (1 + k1), from
+ * the statistics of nidx_txt_set_stats -- whatever p->use_tf says for the plain terms.  A phrase with a term of no posting in the
+ * segment matches nothing (a term id >= n_terms also weighs 0).  OR: the phrase is one more optional clause; AND: one more required
+ * clause. */
+
+/* Every posting's token positions, in posting order (term by term, doc ascending), each posting's tf of them strictly ascending
+ * (n_positions = the sum of the tf given to nidx_txt_create).  A token's position is its index in the token stream before long
+ * tokens are dropped, so a dropped token leaves a gap.  Host pointer; HBM: 4 bytes per position + 8 per posting.  A segment whose
+ * tf does not fit 24 bits, a count that does not add up or positions out of order are NIDX_EINVAL; a call that fails leaves the
+ * previous positions in place. */
+int nidx_txt_set_positions(nidx_txt_segment* seg, const uint32_t* positions, uint64_t n_positions);
+
+typedef struct nidx_txt_phrases {   /* host memory, whatever `mem` says */
+    const uint32_t* terms;   /* every phrase's term ids, concatenated */
+    const uint32_t* off;     /* [n + 1]: phrase i = terms[off[i] .. off[i + 1]), 2 to 64 terms */
+    const uint32_t* query;   /* [n]: the query of the batch phrase i is a clause of */
+    int32_t n;
+} nidx_txt_phrases;
+
+/* nidx_txt_search (order == NULL, facets == NULL), nidx_txt_search_faceted (facets != NULL) or nidx_txt_search_ordered
+ * (order != NULL: out_dates instead of out_scores) with phrase clauses besides each query's terms.  A query holds at most 128
+ * clauses, a phrase counting as one; the segment needs positions (nidx_txt_set_positions) when phrases->n > 0, else NIDX_EINVAL.
+ * With phrases->n == 0 the outputs are exactly those of the call it stands for. */
+int nidx_txt_search_phrases(nidx_txt_segment* seg, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem,
+                            const nidx_txt_search_params* p, const nidx_txt_phrases* phrases, const nidx_txt_order* order,
+                            const nidx_txt_facet_request* facets, uint32_t* out_docs, float* out_scores, int64_t* out_dates, int32_t* out_counts,
+                            uint64_t* out_total, uint32_t* out_facet_counts, void* stream);
+
 /* The empty body with an order (AllQuery, nidx_text/src/search_query.rs:100-101: the catalogue listing): the top k (1..1024) of every
  * alive document by the order above -> out_docs / out_dates [k], *out_count; *out_total = the alive documents (Count). `mem` applies
  * to the outputs. */

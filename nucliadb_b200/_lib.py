@@ -67,6 +67,10 @@ class TxtOrder(C.Structure):
     _fields_ = [("field", C.c_int32), ("type", C.c_int32)]
 
 
+class TxtPhrases(C.Structure):
+    _fields_ = [("terms", C.c_void_p), ("off", C.c_void_p), ("query", C.c_void_p), ("n", C.c_int32)]
+
+
 class RrfSource(C.Structure):
     _fields_ = [("keys", C.c_void_p), ("scores", C.c_void_p), ("counts", C.c_void_p), ("k", C.c_int32), ("weight", C.c_double)]
 
@@ -135,6 +139,8 @@ SIGNATURES = {
     "nidx_txt_set_dates": (i32, [P, P, P]),
     "nidx_txt_search_ordered": (i32, [P, P, P, i32, i32, TSP, ORDER, REQ, P, P, P, P, P, P]),
     "nidx_txt_list_ordered": (i32, [P, ORDER, i32, i32, P, P, P, P, P]),
+    "nidx_txt_set_positions": (i32, [P, P, u64]),
+    "nidx_txt_search_phrases": (i32, [P, P, P, i32, i32, TSP, P, ORDER, REQ, P, P, P, P, P, P, P]),
     "nidx_shard_unique_id": (i32, [P]),
     "nidx_shard_init": (i32, [P, i32, i32, i32, P]),
     "nidx_shard_destroy": (None, [P]),

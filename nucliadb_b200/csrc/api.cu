@@ -18,6 +18,7 @@
 
 #include "../../include/nidx_b200.h"
 #include "bm25.cuh"
+#include "phrase.cuh"
 #include "common.cuh"
 #include "hnsw_build.cuh"
 #include "hnsw_search.cuh"
@@ -95,7 +96,7 @@ using DevBuf = DevArray<unsigned char>;
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
-    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets;
+    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets, phrases;
     cudaEvent_t done = nullptr;
     cudaStream_t last_stream = nullptr;
     bool busy = false;
@@ -1912,6 +1913,10 @@ struct nidx_txt_segment {
     DevArray<int64_t> d_secs[2];      // [n_docs]
     DevArray<uint32_t> d_rank[2];     // [n_docs rounded up to 8], 0 = no date
     uint32_t n_ranks[2] = {0, 0};
+    // positions (nidx_txt_set_positions): every posting's token positions, in posting order, and where each posting's start
+    DevArray<uint64_t> d_pos_off;     // [n_post + 1]
+    DevArray<uint32_t> d_pos;
+    std::vector<float> idf;           // [n_terms] of the statistics set last: a phrase's weight sums its terms'
     WorkspacePool pool;
 
     ~nidx_txt_segment() {
@@ -1932,13 +1937,15 @@ static int txt_upload_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t t
     float avg = (float)total_tokens / (float)total_docs;
     float cache[256];
     for (int i = 0; i < 256; ++i) cache[i] = K1 * (1.0f - B + B * (float)fieldnorm_id_to_value(i) / avg);
-    std::vector<float> weight(t->n_terms);
+    std::vector<float> weight(t->n_terms), idf(t->n_terms);
     for (uint32_t i = 0; i < t->n_terms; ++i) {
         float x = ((float)(total_docs - df[i]) + 0.5f) / ((float)df[i] + 0.5f);
-        weight[i] = logf(1.0f + x) * (1.0f + K1);
+        idf[i] = logf(1.0f + x);
+        weight[i] = idf[i] * (1.0f + K1);
     }
     CU(cudaMemcpy(t->d_norm_cache, cache, sizeof(cache), cudaMemcpyHostToDevice));
     if (t->n_terms) CU(cudaMemcpy(t->d_weight, weight.data(), (size_t)t->n_terms * 4, cudaMemcpyHostToDevice));
+    t->idf = std::move(idf);
     return 0;
 }
 
@@ -2119,7 +2126,150 @@ int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_
     return 0;
 }
 
+int nidx_txt_set_positions(nidx_txt_segment* t, const uint32_t* positions, uint64_t n_positions) {
+    if (!t || (n_positions && !positions)) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->device));
+    const uint64_t n = t->n_post;
+    DevArray<uint64_t> tf, pos_off;
+    DevArray<uint32_t> pos;
+    DevArray<unsigned int> flags;   // [0] a tf was clamped when packed, [1] positions not strictly ascending
+    DevBuf d_cub;
+    ALLOC(tf, (n + 1) * 8);
+    ALLOC(pos_off, (n + 1) * 8);
+    ALLOC(pos, std::max<uint64_t>(n_positions, 1) * 4);
+    ALLOC(flags, 8);
+    CU(cudaMemset(flags, 0, 8));
+    const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)t->sm_count * 8, (n + 256) / 256));
+    pos_tf_kernel<<<blocks, 256>>>(t->d_post, n, tf, flags);
+    LAUNCHED();
+    size_t scan_bytes = 0;
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tf.p, pos_off.p, n + 1));
+    ALLOC(d_cub, std::max<size_t>(scan_bytes, 1));
+    CU(cub::DeviceScan::ExclusiveSum(d_cub.p, scan_bytes, tf.p, pos_off.p, n + 1));
+    LAUNCHED();
+    unsigned int h_flags[2];
+    uint64_t total = 0;
+    CU(cudaMemcpy(h_flags, flags, 8, cudaMemcpyDeviceToHost));
+    CU(cudaMemcpy(&total, pos_off + n, 8, cudaMemcpyDeviceToHost));
+    if (h_flags[0]) return fail(NIDX_EINVAL, "a term frequency of the segment does not fit 24 bits: its positions cannot be located");
+    if (total != n_positions) return fail(NIDX_EINVAL, "%llu positions given, the postings' term frequencies sum to %llu",
+                                          (unsigned long long)n_positions, (unsigned long long)total);
+    if (n_positions) CU(cudaMemcpy(pos, positions, n_positions * 4, cudaMemcpyHostToDevice));
+    pos_check_kernel<<<blocks, 256>>>(pos_off, pos, n, flags + 1);
+    LAUNCHED();
+    CU(cudaGetLastError());
+    CU(cudaMemcpy(h_flags, flags, 8, cudaMemcpyDeviceToHost));
+    if (h_flags[1]) return fail(NIDX_EINVAL, "the positions of every posting must be strictly ascending");
+    t->d_pos_off = std::move(pos_off);   // only now: a rejected or failed call leaves the previous positions in place
+    t->d_pos = std::move(pos);
+    return 0;
+}
+
 }  // extern "C"
+
+// The phrases of a batch (nidx_txt_phrases) laid out for phrase.cuh and bm25_body: grouped by query (stable), each phrase's driver
+// (its rarest term in the segment) and slots (the driver's df), weight and skip row.  One host buffer, uploaded in one copy.
+struct PhrasePlan {
+    std::vector<unsigned char> buf;
+    size_t o_qoff, o_terms, o_off, o_driver, o_skip_row, o_row_term, o_cap_off, o_weight, o_range, o_post, o_skip;
+    uint32_t nv = 0, n_rows = 0;
+    uint64_t slots = 0;
+    size_t bytes = 0;
+};
+
+static int phrase_plan(const nidx_txt_segment* t, const nidx_txt_phrases* ph, int32_t nq, const std::vector<uint32_t>& h_off, PhrasePlan& P) {
+    if (ph->n < 0 || (ph->n && (!ph->terms || !ph->off || !ph->query))) return fail(NIDX_EINVAL, "bad phrases");
+    if (!t->d_pos) return fail(NIDX_EINVAL, "the segment has no positions (nidx_txt_set_positions)");
+    const uint32_t nv = (uint32_t)ph->n;
+    std::vector<uint32_t> per_q(nq + 1, 0);
+    for (uint32_t i = 0; i < nv; ++i) {
+        const uint32_t m = ph->off[i + 1] - ph->off[i];
+        if (ph->off[i + 1] < ph->off[i] || m < 2 || m > PHRASE_MAX_TERMS) return fail(NIDX_EINVAL, "a phrase has 2 to %d terms", PHRASE_MAX_TERMS);
+        if (ph->query[i] >= (uint32_t)nq) return fail(NIDX_EINVAL, "phrase %u belongs to no query of the batch", i);
+        ++per_q[ph->query[i] + 1];
+    }
+    for (int32_t q = 0; q < nq; ++q) {
+        if (h_off[q + 1] - h_off[q] + per_q[q + 1] > (uint32_t)BM_MAX_TERMS)
+            return fail(NIDX_EINVAL, "queries with more than %d clauses (terms and phrases) are not supported", BM_MAX_TERMS);
+        per_q[q + 1] += per_q[q];
+    }
+    std::vector<uint32_t> order(nv), terms, off(nv + 1, 0), driver(nv), skip_row(nv, NIDX_NIL), row_term;
+    std::vector<uint64_t> cap_off(nv + 1, 0);
+    std::vector<float> weight(nv);
+    {
+        std::vector<uint32_t> at(per_q.begin(), per_q.end() - 1);
+        for (uint32_t i = 0; i < nv; ++i) order[at[ph->query[i]]++] = i;
+    }
+    const float K1 = 1.2f;
+    for (uint32_t v = 0; v < nv; ++v) {
+        const uint32_t i = order[v];
+        bool known = true;
+        uint32_t dv = 0;
+        uint64_t cap = ~0ull;
+        float idf = 0.0f;   // f32 sum in phrase order, repeats counted (Bm25Weight::for_terms) [recalled]
+        for (uint32_t j = ph->off[i]; j < ph->off[i + 1]; ++j) {
+            const uint32_t term = ph->terms[j];
+            terms.push_back(term);
+            if (term >= t->n_terms) { known = false; continue; }
+            idf += t->idf[term];
+            if (t->own_df[term] < cap) { cap = t->own_df[term]; dv = j - ph->off[i]; }
+        }
+        if (!known) cap = 0;   // a term the segment's dictionary lacks: the phrase matches nothing and weighs 0, like the term alone
+        off[v + 1] = (uint32_t)terms.size();
+        driver[v] = dv;
+        cap_off[v + 1] = cap_off[v] + cap;
+        weight[v] = known ? idf * (1.0f + K1) : 0.0f;
+        if (cap >= (uint64_t)BM_SKIP_DF) { skip_row[v] = (uint32_t)row_term.size(); row_term.push_back(2 * v); }
+    }
+    // one buffer: inputs first (copied), then the outputs of the phrase pass
+    auto take = [&](size_t& o, size_t bytes) { o = (P.bytes + 15) & ~(size_t)15; P.bytes = o + bytes; };
+    take(P.o_qoff, per_q.size() * 4);
+    take(P.o_terms, std::max<size_t>(terms.size(), 1) * 4);
+    take(P.o_off, off.size() * 4);
+    take(P.o_driver, std::max<size_t>(nv, 1) * 4);
+    take(P.o_skip_row, std::max<size_t>(nv, 1) * 4);
+    take(P.o_row_term, std::max<size_t>(row_term.size(), 1) * 4);
+    take(P.o_cap_off, cap_off.size() * 8);
+    take(P.o_weight, std::max<size_t>(nv, 1) * 4);
+    const size_t in_bytes = P.bytes;
+    take(P.o_range, std::max<size_t>(nv, 1) * 16);
+    take(P.o_post, std::max<uint64_t>(cap_off[nv], 1) * 8);
+    take(P.o_skip, std::max<size_t>(row_term.size(), 1) * ((size_t)t->n_fine + 1) * 4);
+    P.buf.assign(in_bytes, 0);
+    auto put = [&](size_t o, const auto& v) { if (!v.empty()) memcpy(P.buf.data() + o, v.data(), v.size() * sizeof(v[0])); };
+    put(P.o_qoff, per_q); put(P.o_terms, terms); put(P.o_off, off); put(P.o_driver, driver); put(P.o_skip_row, skip_row);
+    put(P.o_row_term, row_term); put(P.o_cap_off, cap_off); put(P.o_weight, weight);
+    P.nv = nv; P.n_rows = (uint32_t)row_term.size(); P.slots = cap_off[nv];
+    return 0;
+}
+
+// Uploads the plan into w.phrases, runs the phrase pass on `stream` and points a's overlay at its lists.
+static int phrase_pass(nidx_txt_segment* t, const PhrasePlan& P, const TxtDev& T, Workspace& w, cudaStream_t stream, Bm25Args& a) {
+    ENSURE(w.phrases, P.bytes);
+    unsigned char* d = w.phrases.p;
+    CU(cudaMemcpyAsync(d, P.buf.data(), P.buf.size(), cudaMemcpyHostToDevice, stream));
+    PhraseArgs A;
+    A.pos_off = t->d_pos_off; A.pos = t->d_pos;
+    A.terms = reinterpret_cast<const uint32_t*>(d + P.o_terms); A.off = reinterpret_cast<const uint32_t*>(d + P.o_off);
+    A.driver = reinterpret_cast<const uint32_t*>(d + P.o_driver); A.cap_off = reinterpret_cast<const uint64_t*>(d + P.o_cap_off);
+    A.nv = P.nv; A.out = reinterpret_cast<uint2*>(d + P.o_post); A.range = reinterpret_cast<uint64_t*>(d + P.o_range);
+    if (P.slots) {
+        const int blocks = (int)std::min<uint64_t>((uint64_t)t->sm_count * 8, (P.slots + 255) / 256);
+        phrase_match_kernel<<<blocks, 256, 0, stream>>>(T, A);
+        LAUNCHED();
+    }
+    phrase_compact_kernel<<<P.nv, PHRASE_COMPACT_THREADS, 0, stream>>>(A);
+    LAUNCHED();
+    if (P.n_rows) {
+        bm25_build_skip_kernel<<<t->sm_count * 8, 256, 0, stream>>>(A.range, A.out, reinterpret_cast<const uint32_t*>(d + P.o_row_term), P.n_rows, t->n_fine,
+                                                                    reinterpret_cast<uint32_t*>(d + P.o_skip));
+        LAUNCHED();
+    }
+    a.ph_qoff = reinterpret_cast<const uint32_t*>(d + P.o_qoff); a.ph_range = A.range; a.ph_post = A.out;
+    a.ph_skip_row = reinterpret_cast<const uint32_t*>(d + P.o_skip_row); a.ph_skip = reinterpret_cast<const uint32_t*>(d + P.o_skip);
+    a.ph_weight = reinterpret_cast<const float*>(d + P.o_weight);
+    return 0;
+}
 
 // An order resolved against the segment: the field's rank column and seconds.
 static int order_args(const nidx_txt_segment* t, const nidx_txt_order* order, OrderArgs& O) {
@@ -2188,7 +2338,7 @@ static int facet_args(const nidx_txt_segment* t, const FacetPlan& P, Workspace& 
 static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, bool qhost, bool ohost,
                            const nidx_txt_search_params* p, uint32_t* out_docs, float* out_scores, int32_t* out_counts, uint64_t* out_total, cudaStream_t stream,
                            const nidx_txt_facet_request* facets = nullptr, uint32_t* out_facet_counts = nullptr, const nidx_txt_order* order = nullptr,
-                           int64_t* out_dates = nullptr) {
+                           int64_t* out_dates = nullptr, const nidx_txt_phrases* phrases = nullptr) {
     if (!t || !p || !query_off || !out_docs || !(order ? (void*)out_dates : (void*)out_scores) || !out_counts) return fail(NIDX_EINVAL, "null argument");
     FacetPlan plan;
     if (facets) {
@@ -2215,6 +2365,11 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     int max_terms = 0;
     for (int i = 0; i < nq; ++i) max_terms = std::max<int>(max_terms, h_off[i + 1] - h_off[i]);
     if (max_terms > BM_MAX_TERMS) return fail(NIDX_EINVAL, "queries with more than %d terms are not supported", BM_MAX_TERMS);
+    PhrasePlan pp;
+    if (phrases && phrases->n) {
+        int r = phrase_plan(t, phrases, nq, h_off, pp);
+        if (r) return r;
+    }
     bool conj = p->mode == NIDX_BM25_AND;
     int cap = topk_cap(k, BM_THREADS);
     size_t smem = bm_smem_bytes(cap, conj);
@@ -2247,6 +2402,14 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
     a.out_keys = w.partial.as<uint64_t>(); a.out_total = reinterpret_cast<unsigned long long*>(d_total);
     if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after
+    a.ph_qoff = nullptr; a.ph_range = nullptr; a.ph_post = nullptr; a.ph_skip_row = nullptr; a.ph_skip = nullptr; a.ph_weight = nullptr;
+    // a phrase scores its frequency: beside Basic terms the TF kernel runs with the terms' tf taken as 1 (the same two roundings)
+    const bool use_tf = p->use_tf || pp.nv;
+    a.basic_terms = !p->use_tf && pp.nv;
+    if (pp.nv) {
+        r = phrase_pass(t, pp, T, w, stream, a);
+        if (r) return r;
+    }
     auto launch = [&](auto kern, size_t bytes, auto... extra) -> int {   // the BM25 pass, between the roofline events
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         CU(cudaEventRecord(t->ev_k0, stream));
@@ -2266,12 +2429,12 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     }
     if (order && !facets) r = launch(conj ? bm25_order_kernel<true> : bm25_order_kernel<false>, smem, O);
     else if (!facets)
-        r = launch(conj ? (p->use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (p->use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>),
+        r = launch(conj ? (use_tf ? bm25_kernel<true, true> : bm25_kernel<true, false>) : (use_tf ? bm25_kernel<false, true> : bm25_kernel<false, false>),
                    smem);
     else if (order) r = launch(conj ? bm25_order_facet_kernel<true> : bm25_order_facet_kernel<false>, fsmem, F, O);
     else
-        r = launch(conj ? (p->use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
-                        : (p->use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>), fsmem, F);
+        r = launch(conj ? (use_tf ? bm25_facet_kernel<true, true> : bm25_facet_kernel<true, false>)
+                        : (use_tf ? bm25_facet_kernel<false, true> : bm25_facet_kernel<false, false>), fsmem, F);
     if (r) return r;
     if (order) date_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, O.secs, d_docs, d_dates, d_cnt);
     else bm25_finish_kernel<<<nq, 128, 0, stream>>>(w.partial.as<uint64_t>(), nq, k, p->min_score, d_docs, d_sc, d_cnt);
@@ -2347,6 +2510,15 @@ int nidx_txt_search_ordered(nidx_txt_segment* t, const uint32_t* query_terms, co
     bool host = mem == NIDX_MEM_HOST;
     return txt_search_impl(t, query_terms, query_off, nq, host, host, p, out_docs, nullptr, out_counts, out_total, reinterpret_cast<cudaStream_t>(stream_),
                            facets, out_facet_counts, order, out_dates);
+}
+
+int nidx_txt_search_phrases(nidx_txt_segment* t, const uint32_t* query_terms, const uint32_t* query_off, int32_t nq, int mem, const nidx_txt_search_params* p,
+                            const nidx_txt_phrases* phrases, const nidx_txt_order* order, const nidx_txt_facet_request* facets, uint32_t* out_docs,
+                            float* out_scores, int64_t* out_dates, int32_t* out_counts, uint64_t* out_total, uint32_t* out_facet_counts, void* stream_) {
+    if (!phrases) return fail(NIDX_EINVAL, "null argument");
+    bool host = mem == NIDX_MEM_HOST;
+    return txt_search_impl(t, query_terms, query_off, nq, host, host, p, out_docs, order ? nullptr : out_scores, out_counts, out_total,
+                           reinterpret_cast<cudaStream_t>(stream_), facets, out_facet_counts, order, out_dates, phrases);
 }
 
 int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int32_t k, int mem, uint32_t* out_docs, int64_t* out_dates, int32_t* out_count,

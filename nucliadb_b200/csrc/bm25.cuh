@@ -83,7 +83,21 @@ struct Bm25Args {
     uint64_t after_docaddr, docaddr_base;
     uint64_t* out_keys;         // [nq][k] rank keys (score desc, doc asc), 0 = none
     unsigned long long* out_total;  // [nq] matching documents (Count collector)
+    // Phrases (phrase.cuh): query q's clauses are its terms, then the virtual posting lists ph_qoff[q] .. ph_qoff[q + 1), each
+    // scored with its real frequency (a TF kernel runs; basic_terms keeps the terms at tf == 1).  ph_qoff == nullptr: no phrases.
+    const uint32_t* ph_qoff;    // [nq + 1]
+    const uint64_t* ph_range;   // [2 nv] (first, end) posting of list v in ph_post
+    const uint2* ph_post;
+    const uint32_t* ph_skip_row;   // [nv] row in ph_skip or NIL
+    const uint32_t* ph_skip;       // [rows][n_fine + 1] posting index relative to the list's first
+    const float* ph_weight;     // [nv] (sum of the terms' idf) * (1 + k1)
+    int basic_terms;            // TF kernels: the query terms are Basic (tf == 1) and only the phrases count their frequency
 };
+
+// A query term's postings are addressed in 8-byte units of the address space, so that a term's slice is read the same way whether
+// it lies in the segment's postings or in a phrase's virtual list.
+__device__ __forceinline__ uint64_t post_addr(const uint2* p) { return (uint64_t)reinterpret_cast<uintptr_t>(p) >> 3; }
+__device__ __forceinline__ const uint2* post_at(uint64_t a) { return reinterpret_cast<const uint2*>(a << 3); }
 
 // ---- index-time kernels ---------------------------------------------------------------------------------
 __global__ void bm25_pack_kernel(const uint32_t* __restrict__ post_doc, const uint32_t* __restrict__ post_tf, const unsigned char* __restrict__ fieldnorm,
@@ -322,10 +336,10 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
     uint32_t* cnts = reinterpret_cast<uint32_t*>(p); if (CONJ) p += BM_ACC;            // matched-term counters, one BYTE per rank (AND only)
     p = smem + (((size_t)(p - smem) + 15) & ~(size_t)15);
     // per-term state of the resolving warp (kept out of the registers: every thread would pay for them)
-    uint64_t* t_base = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;          // term_off[term]
-    uint64_t* t_end = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;           // term_off[term + 1]
+    uint64_t* t_base = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;          // post_addr of the term's first posting
+    uint64_t* t_end = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;           // post_addr past its last
     uint64_t* t_cur = reinterpret_cast<uint64_t*>(p); p += BM_MAX_TERMS * 8;           // first posting not yet assigned to a tile
-    uint64_t* t_skip = reinterpret_cast<uint64_t*>(p);                                 // offset of the term's skip row, ~0 = none
+    uint64_t* t_skip = reinterpret_cast<uint64_t*>(p);                                 // address of the term's skip row, 0 = none
     const int q = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     uint32_t* fcnt = nullptr;   // FACET: this query's bucket counts (shared memory past the term state, or its row of F.out)
     if (FACET) {
@@ -334,7 +348,9 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
     }
 
     const uint32_t* terms = a.query_terms + a.query_off[q];
-    int nt = (int)(a.query_off[q + 1] - a.query_off[q]);
+    const int n_real = (int)(a.query_off[q + 1] - a.query_off[q]);   // the clauses from n_real on are phrases
+    const uint32_t ph0 = a.ph_qoff ? a.ph_qoff[q] : 0u;
+    int nt = n_real + (a.ph_qoff ? (int)(a.ph_qoff[q + 1] - ph0) : 0);
     if (nt > BM_MAX_TERMS) nt = BM_MAX_TERMS;
     BlockTopK tk;
     tk.init(tk_buf, &tk_count, &tk_thr, a.k, a.cap);
@@ -357,15 +373,29 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
         for (int j = 0; j < BM_TPL; ++j) {
             int i = lane + 32 * j;
             if (i < nt) {
-                uint32_t t = terms[i];
-                bool ok = t < T.n_terms;
-                uint64_t b = ok ? T.term_off[t] : 0, e = ok ? T.term_off[t + 1] : 0;
+                uint64_t b, e;
+                float w;
+                const uint32_t* sk = nullptr;
+                if (i < n_real) {
+                    uint32_t t = terms[i];
+                    bool ok = t < T.n_terms;
+                    b = post_addr(T.post) + (ok ? T.term_off[t] : 0);
+                    e = post_addr(T.post) + (ok ? T.term_off[t + 1] : 0);
+                    w = ok ? a.term_weight[t] : 0.0f;
+                    uint32_t row = ok ? T.skip_row[t] : NIL;
+                    if (row != NIL) sk = T.skip + (uint64_t)row * (T.n_fine + 1);
+                } else {
+                    const uint32_t v = ph0 + (uint32_t)(i - n_real);
+                    b = post_addr(a.ph_post) + a.ph_range[2 * v];
+                    e = post_addr(a.ph_post) + a.ph_range[2 * v + 1];
+                    w = a.ph_weight[v];
+                    uint32_t row = a.ph_skip_row[v];
+                    if (row != NIL) sk = a.ph_skip + (uint64_t)row * (T.n_fine + 1);
+                }
                 t_base[i] = b; t_end[i] = e; t_cur[i] = b;
-                const float w = ok ? a.term_weight[t] : 0.0f;
                 tw[i] = w;   // scaled by 2^shift below (exact: a power of two), so a posting costs one multiply
                 if (!ORDER) wmax = fmaxf(wmax, w);
-                uint32_t row = ok ? T.skip_row[t] : NIL;
-                t_skip[i] = row != NIL ? (uint64_t)row * (T.n_fine + 1) : ~0ull;
+                t_skip[i] = (uint64_t)reinterpret_cast<uintptr_t>(sk);
                 missing |= b == e;
                 my_total += e - b;
             }
@@ -385,7 +415,10 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
     int any_missing = __syncthreads_or(missing);   // an AND query with a term without postings matches nothing
     const bool dead = (CONJ && any_missing) || nt == 0;
     const float scale = ORDER ? 1.0f : (float)(1u << s_shift);
-    if (threadIdx.x < nt) tw[threadIdx.x] = __fmul_rn(tw[threadIdx.x], scale);   // rn(rn(w * frac) * 2^s) == rn((w * 2^s) * frac)
+    if (threadIdx.x < nt) {   // rn(rn(w * frac) * 2^s) == rn((w * 2^s) * frac)
+        const float ws = __fmul_rn(tw[threadIdx.x], scale);
+        tw[threadIdx.x] = TF && a.basic_terms && (int)threadIdx.x < n_real ? -ws : ws;   // a negative weight marks a Basic term
+    }
     const uint32_t n_fine = dead ? 0 : T.n_fine;
     // tile span (fine tiles): the query's postings spread evenly would fill ~80 % of the slots per tile (octet padding takes some)
     uint32_t m = 1;
@@ -411,11 +444,11 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
             uint32_t len = 0;
             if (i < nt) {
                 uint64_t bgn = t_cur[i], end;
-                if (t_skip[i] != ~0ull) {
+                if (t_skip[i] != 0) {
                     end = t_base[i] + t_pf[j];
                 } else {                                                   // rare term: a few postings in total
                     uint64_t l = bgn, e = t_end[i];
-                    while (l < e && T.post[l].x < hi) ++l;
+                    while (l < e && post_at(l)->x < hi) ++l;
                     end = l;
                 }
                 run_b[buf * BM_MAX_TERMS + i] = bgn;
@@ -437,11 +470,11 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
         // request the skip entries of the tile after this one
         uint32_t f2 = f1 + m_next < T.n_fine ? f1 + m_next : T.n_fine;
 #pragma unroll
-        for (int j = 0; j < BM_TPL; ++j) { int i = lane + 32 * j; if (i < nt && t_skip[i] != ~0ull) t_pf[j] = __ldg(T.skip + t_skip[i] + f2); }
+        for (int j = 0; j < BM_TPL; ++j) { int i = lane + 32 * j; if (i < nt && t_skip[i] != 0) t_pf[j] = __ldg(reinterpret_cast<const uint32_t*>(t_skip[i]) + f2); }
     };
     auto load_pf = [&](uint32_t f1) {   // synchronous (re)load of the skip entries for boundary f1
 #pragma unroll
-        for (int j = 0; j < BM_TPL; ++j) { int i = lane + 32 * j; if (i < nt && t_skip[i] != ~0ull) t_pf[j] = __ldg(T.skip + t_skip[i] + f1); }
+        for (int j = 0; j < BM_TPL; ++j) { int i = lane + 32 * j; if (i < nt && t_skip[i] != 0) t_pf[j] = __ldg(reinterpret_cast<const uint32_t*>(t_skip[i]) + f1); }
     };
 
     // omap[o] = run of octet o (last run with pre8[r] <= o), two octets per thread; pre8 of `b` must be complete (barrier)
@@ -538,7 +571,7 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
                         if (within < run_len[buf * BM_MAX_TERMS + r]) {
                             actm |= 1u << u;
                             rpack[u >> 2] |= (uint32_t)r << (8 * (u & 3));
-                            pd[u] = ldg_post(T.post + run_b[buf * BM_MAX_TERMS + r] + within);
+                            pd[u] = ldg_post(post_at(run_b[buf * BM_MAX_TERMS + r] + within));
                         }
                     }
                 }
@@ -625,8 +658,11 @@ __device__ __forceinline__ void bm25_body(const TxtDev& T, const Bm25Args& a, co
                         } else {
                             float wgt = tw[(rpack[u >> 2] >> (8 * (u & 3))) & 0xFFu];
                             float frac;
-                            if (TF) { float tff = (float)(tfn >> 8); frac = __fdiv_rn(tff, __fadd_rn(tff, ntab[tfn & 0xFFu])); }
-                            else frac = ntab[tfn & 0xFFu];
+                            if (TF) {
+                                float tff = (float)(tfn >> 8);
+                                if (wgt < 0.0f) { tff = 1.0f; wgt = -wgt; }   // a Basic term beside phrases (a.basic_terms)
+                                frac = __fdiv_rn(tff, __fadd_rn(tff, ntab[tfn & 0xFFu]));
+                            } else frac = ntab[tfn & 0xFFu];
                             uint32_t fx = (uint32_t)__float2uint_rn(__fmul_rn(wgt, frac));
                             if (fx == 0) fx = 1;
                             uint32_t oldv = atomicAdd(&acc[rank], fx);

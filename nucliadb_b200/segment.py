@@ -380,6 +380,37 @@ class TextSegment:
                                                   stream))
         return out
 
+    # ---- exact phrases (tantivy PhraseQuery, slop 0: include/nidx_b200.h nidx_txt_search_phrases) ------------------------------
+    def set_positions(self, positions):
+        """Every posting's token positions in posting order (uint32; per posting its tf of them, strictly ascending)."""
+        positions = np.ascontiguousarray(positions, dtype=np.uint32)
+        check(_lib.load().nidx_txt_set_positions(self._h, ptr(positions), len(positions)))
+
+    def search_phrases(self, query_terms, query_off, phrases, k, mode=_lib.NIDX_BM25_OR, use_tf=True, min_score=0.0, after=None, docaddr_base=0,
+                       order=None, facets=None):
+        """search() / search_faceted() / search_ordered() with phrase clauses: phrases = [(query index, [term ids])] (host lists).
+        order = (field, type) orders by date (dates in place of scores).  Returns (docs, scores or dates, counts, total) plus the
+        facet counts [nq][n_buckets] when `facets` (encoded keys) is given."""
+        p = _txt_params(k, mode, use_tf, min_score, after, docaddr_base)
+        terms = np.asarray([t for _, ts in phrases for t in ts], dtype=np.uint32)
+        poff = np.zeros(len(phrases) + 1, dtype=np.uint32)
+        poff[1:] = np.cumsum([len(ts) for _, ts in phrases])
+        pq = np.asarray([q for q, _ in phrases], dtype=np.uint32)
+        ph = _lib.TxtPhrases(ptr(terms), ptr(poff), ptr(pq), len(phrases))
+        o = _lib.TxtOrder(*order) if order is not None else None
+        req, _keep = _facet_request(facets) if facets is not None else (None, None)
+        nb = len(self.facet_buckets(facets)[0]) if facets is not None else 0
+        mem, stream, alloc, query_terms, query_off, nq = self._queries(query_terms, query_off)
+        out = (alloc((nq, k), np.uint32), alloc((nq, k), np.int64 if order is not None else np.float32), alloc(nq, np.int32), alloc(nq, np.uint64))
+        if facets is not None:
+            out += (alloc((nq, nb), np.uint32, zero=True),)
+        scores, dates = (None, out[1]) if order is not None else (out[1], None)
+        check(_lib.load().nidx_txt_search_phrases(self._h, ptr(query_terms), ptr(query_off), nq, mem, C.byref(p), C.addressof(ph),
+                                                  C.byref(o) if o is not None else None, C.byref(req) if req is not None else None,
+                                                  ptr(out[0]), ptr(scores), ptr(dates), ptr(out[2]), ptr(out[3]),
+                                                  ptr(out[4]) if facets is not None else None, stream))
+        return out
+
     def list_ordered(self, k, field=_lib.NIDX_ORDER_CREATED, order=_lib.NIDX_ORDER_DESC, device_out=False):
         """The empty body ordered by date: the top k alive documents -> (docs [k], dates [k], count, total alive); with device_out
         all four are torch CUDA tensors (count and total of one element), on the device path."""

@@ -31,6 +31,7 @@ undated documents are fixed here, not taken from the reference.
 from __future__ import annotations
 
 import re
+import unicodedata
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -46,6 +47,95 @@ def tokenize(text: str) -> list:
     """tantivy's "default" analyzer [recalled]: SimpleTokenizer (alphanumeric runs) -> RemoveLongFilter::limit(40), which keeps a
     token iff `token.text.len() < 40` -- a length in UTF-8 BYTES, strictly below the limit -- -> LowerCaser."""
     return [t.lower() for t in _TOKEN.findall(text) if len(t.encode("utf-8")) < 40]
+
+
+def tokenize_with_positions(text: str) -> list:
+    """tokenize() with every token's position: its index in the SimpleTokenizer stream BEFORE RemoveLongFilter, so a dropped long
+    token leaves a gap that a phrase does not match across [recalled].  -> [(position, token)]."""
+    return [(i, t.lower()) for i, t in enumerate(_TOKEN.findall(text)) if len(t.encode("utf-8")) < 40]
+
+
+# Rust's char::is_whitespace (Unicode White_Space) and nom's multispace0 (ASCII space, tab, CR, LF only)
+_WHITE_SPACE = frozenset("\t\n\x0b\x0c\r \x85\xa0\u1680\u2000\u2001\u2002\u2003\u2004\u2005\u2006\u2007\u2008\u2009\u200a"
+                         "\u2028\u2029\u202f\u205f\u3000")
+_MULTISPACE = frozenset(" \t\r\n")
+
+
+def _is_literal_char(c: str) -> bool:
+    return c != '"' and c not in _WHITE_SPACE and unicodedata.category(c) != "Cc"
+
+
+def _grammar(body: str):
+    """nidx_paragraph's query grammar (query_parser/tokenizer.rs:68-127): [(kind, text)] with kind "L" literal, "Q" quoted,
+    "E" excluded (-word), or None on a parse error (a character no rule takes, such as U+00A0 outside quotes)."""
+    n = len(body)
+
+    def ms(i):
+        while i < n and body[i] in _MULTISPACE:
+            i += 1
+        return i
+
+    def word(i):
+        while i < n and _is_literal_char(body[i]):
+            i += 1
+        return i
+
+    out, i = [], ms(0)
+    while i < n:
+        j = ms(i)
+        if j < n and body[j] == '"' and (k := body.find('"', j + 1)) > j + 1:   # "..." (at least one character inside)
+            text = body[j + 1:k]
+            if any(c not in _WHITE_SPACE for c in text):                       # quotes around whitespace only are dropped
+                out.append(("Q", text))
+            i = ms(k + 1)
+        elif body[i] == '"':                                                    # an unclosed quote (or "") is dropped
+            while i < n and body[i] == '"':
+                i += 1
+        elif j < n and body[j] == "-" and word(j + 1) > j + 1:
+            k = word(j + 1)
+            out.append(("E", body[j + 1:k]))
+            i = ms(k)
+        elif word(j) > j:
+            k = word(j)
+            out.append(("L", body[j:k]))
+            i = ms(k)
+        else:
+            return None
+    return out
+
+
+def paragraph_query_tokens(body: str) -> list:
+    """tokenize_query_infallible (query_parser/tokenizer.rs:48-186): the grammar's tokens retokenized by SimpleTokenizer +
+    LowerCaser -> [(kind, text)], a quoted group's words joined by one space; a parse error reads the whole body as one literal."""
+    tokens = _grammar(body)
+    out = []
+    for kind, text in tokens if tokens is not None else [("L", body)]:
+        words = [t.lower() for t in _TOKEN.findall(text)]
+        if kind == "Q":
+            if words:
+                out.append(("Q", " ".join(words)))
+        else:
+            out += [(kind, w) for w in words]
+    return out
+
+
+def parse_paragraph_query(body: str):
+    """paragraph_query_tokens + parse_keyword_query's clauses (keyword_parser.rs:27-91) -> (literal words, phrases as word lists).
+    Literals (and excluded words, searched as literals here) are exactly tokenize()'s words; a quoted group of two or more words is
+    a phrase (no word dropped: a long word is a term the index does not hold, so the phrase matches nothing), of one word a
+    literal.  A parse error reads the whole body as literals."""
+    tokens = _grammar(body)
+    if tokens is None:
+        return tokenize(body), []
+    words, phrases = [], []
+    for kind, text in tokens:
+        if kind == "Q":
+            ws = [t.lower() for t in _TOKEN.findall(text)]
+            if len(ws) >= 2:
+                phrases.append(ws)
+                continue
+        words += tokenize(text)
+    return words, phrases
 
 
 def fieldnorm_to_id(n: int) -> int:
@@ -168,6 +258,12 @@ class TextIndexSegment:
         self.post_doc = np.asarray([p[1] for p in pairs], dtype=np.uint32)
         self.post_tf = np.asarray([tf[p] for p in pairs], dtype=np.uint32)
         self.fieldnorm_id = np.asarray([fieldnorm_to_id(int(x)) for x in self.lens], dtype=np.uint8)
+        pos: dict = {}
+        for i, d in enumerate(self.docs):
+            for p, t in tokenize_with_positions(d.text):
+                pos.setdefault((vocab[t], i), []).append(p)
+        # every posting's positions, in posting order (nidx_txt_set_positions); uploaded on the first phrase query
+        self.positions = np.asarray([p for pr in pairs for p in pos[pr]], dtype=np.uint32)
         self._gpu: Optional[TextSegment] = None
         self.device = device
 
@@ -225,7 +321,7 @@ class TextSearcher:
                              np.asarray([none if d.modified is None else int(d.modified) for d in s.docs], dtype=np.int64))
         self._dates = True
 
-    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None):
+    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None, phrases=()):
         """Counts of the request's facets over the matched set of every segment, summed, then grouped and cut to the top 50.
         With terms: the faceted BM25 search, ordered by date when `order` is given (returns its per-segment (docs, scores or
         dates, counts, total) too); without: every alive document (AllQuery)."""
@@ -243,9 +339,12 @@ class TextSearcher:
         counts = np.zeros(len(b_req), dtype=np.int64)
         hits = []
         for ord_, seg in enumerate(self.segments):
-            if terms:
+            if terms or phrases:
                 qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
-                if order is not None:
+                if phrases:
+                    docs, scores, cnt, total, fc = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k, docaddr_base=ord_ << 32, facets=keys,
+                                                                           order=None if order is None else (order.sort_by, order.type), **params)
+                elif order is not None:
                     docs, scores, cnt, total, fc = seg._gpu.search_ordered(qt, qo, k, order.sort_by, order.type, params["mode"], facets=keys)
                 else:
                     docs, scores, cnt, total, fc = seg._gpu.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
@@ -276,8 +375,12 @@ class TextSearcher:
             terms.append(self.vocab.get(t, 0xFFFFFFF0))  # unknown term: matches nothing
         return terms
 
+    def _clauses(self, body: str):
+        """-> (term ids, phrases as term-id lists).  nidx_text's QueryParser grammar is not restated: no phrases."""
+        return self._terms(body), []
+
     def search(self, request: DocumentSearchRequest) -> DocumentSearchResponse:
-        terms = self._terms(request.body)
+        terms, phrases = self._clauses(request.body)
         k = request.result_per_page
         resp = DocumentSearchResponse(query=request.body)
         after = None
@@ -286,13 +389,13 @@ class TextSearcher:
             after = (sa.score, {"drop": 1, "keep_after": 2, "keep": 3}[sa.tie_break], sa.docaddr)
         params = dict(mode=_lib.NIDX_BM25_AND if self.conjunction else _lib.NIDX_BM25_OR, use_tf=self.use_tf, min_score=0.0, after=after)
         if request.order is not None and not request.only_faceted:   # only_faceted comes first (nidx_text/src/reader.rs:405-414)
-            return self._search_ordered(request, terms, params)
+            return self._search_ordered(request, terms, params, phrases)
         hits = None
         if _facet_request(request.faceted):
-            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params)
+            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, phrases=phrases)
         if request.only_faceted:   # only the facets: no results, total 0 (nidx_text/src/reader.rs:407-414, search_response.rs:111-124)
             return DocumentSearchResponse(facets=resp.facets)
-        if not terms or k <= 0:
+        if not (terms or phrases) or k <= 0:
             return resp
         qt = np.asarray(terms, dtype=np.uint32)
         qo = np.asarray([0, len(terms)], dtype=np.uint32)
@@ -300,6 +403,8 @@ class TextSearcher:
         for ord_, seg in enumerate(self.segments):
             if hits is not None:   # the faceted pass already returned this segment's top-k and Count
                 docs, scores, counts, total = hits[ord_]
+            elif phrases:
+                docs, scores, counts, total = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, docaddr_base=ord_ << 32, **params)
             else:
                 docs, scores, counts, total = seg._gpu.search(qt, qo, k + 1, docaddr_base=ord_ << 32, **params)
             resp.total += int(total[0])
@@ -315,7 +420,7 @@ class TextSearcher:
         return resp
 
 
-    def _search_ordered(self, request: DocumentSearchRequest, terms, params: dict) -> DocumentSearchResponse:
+    def _search_ordered(self, request: DocumentSearchRequest, terms, params: dict, phrases=()) -> DocumentSearchResponse:
         """TopDocs(k + 1) ordered by date beside Count (and the FacetCollector) in one pass per segment; an empty body lists every
         alive document.  convert_int_order (nidx_text/src/reader.rs:226-287): no min_score, next_page = total > k."""
         order, k = request.order, request.result_per_page
@@ -323,16 +428,21 @@ class TextSearcher:
         self._ensure_dates()
         hits = None
         if _facet_request(request.faceted):
-            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, order=order)
+            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, order=order, phrases=phrases)
         if k <= 0:
             return resp
         qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
         rows = []
         for ord_, seg in enumerate(self.segments):
-            if not terms:
+            if not (terms or phrases):
                 docs, dates, count, total = seg._gpu.list_ordered(k + 1, order.sort_by, order.type)
             else:
-                d2, t2, c2, tot2 = hits[ord_] if hits is not None else seg._gpu.search_ordered(qt, qo, k + 1, order.sort_by, order.type, params["mode"])
+                if hits is not None:
+                    d2, t2, c2, tot2 = hits[ord_]
+                elif phrases:
+                    d2, t2, c2, tot2 = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, mode=params["mode"], order=(order.sort_by, order.type))
+                else:
+                    d2, t2, c2, tot2 = seg._gpu.search_ordered(qt, qo, k + 1, order.sort_by, order.type, params["mode"])
                 docs, dates, count, total = d2[0], t2[0], int(c2[0]), int(tot2[0])
             resp.total += int(total)
             rows += [(date_sort_key(int(dates[i]), order.type), ord_, int(docs[i]), int(dates[i])) for i in range(count)]
@@ -352,7 +462,22 @@ def date_sort_key(seconds: Optional[int], order_type: int):
 
 
 class ParagraphSearcher(TextSearcher):
-    """nidx_paragraph keyword search: OR of TermQuery(Basic) => tf == 1 (keyword_parser.rs:27-67)."""
+    """nidx_paragraph keyword search: OR of TermQuery(Basic) => tf == 1 (keyword_parser.rs:27-67), plus a PhraseQuery per quoted
+    group of two or more words (scored with its real frequency): the body is parsed by parse_paragraph_query."""
 
     conjunction = False
     use_tf = False
+
+    def __init__(self, segments: Sequence[TextIndexSegment], vocab: dict):
+        super().__init__(segments, vocab)
+        self._positions = False   # uploaded on the first phrase query
+
+    def _clauses(self, body: str):
+        words, phrases = parse_paragraph_query(body)
+        terms = [self.vocab.get(t, 0xFFFFFFF0) for t in words]   # unknown word: matches nothing
+        phrase_terms = [[self.vocab.get(t, 0xFFFFFFF0) for t in p] for p in phrases]   # an unknown word: the phrase matches nothing
+        if phrase_terms and not self._positions:
+            for s in self.segments:
+                s._gpu.set_positions(s.positions)
+            self._positions = True
+        return terms, phrase_terms
