@@ -284,7 +284,8 @@ int nidx_txt_search(nidx_txt_segment* seg, const uint32_t* query_terms, const ui
 
 /* Device time (CUDA events on the caller's stream) of bm25_kernel in the last nidx_txt_search on this segment (bench roofline),
  * or of the facet kernel of the last nidx_txt_search_faceted / nidx_txt_facet_count_all, of the order kernel of the last
- * nidx_txt_search_ordered, or of the two listing kernels of the last nidx_txt_list_ordered; not meaningful under concurrent searches. */
+ * nidx_txt_search_ordered, of the two listing kernels of the last nidx_txt_list_ordered, or of the pass of the last nidx_txt_prefilter;
+ * not meaningful under concurrent searches. */
 int nidx_txt_last_kernel_ms(nidx_txt_segment* seg, float* ms);
 
 /* ---- Facet counts: tantivy's FacetCollector next to Count and TopDocs
@@ -394,6 +395,50 @@ int nidx_txt_search_phrases(nidx_txt_segment* seg, const uint32_t* query_terms, 
  * to the outputs. */
 int nidx_txt_list_ordered(nidx_txt_segment* seg, const nidx_txt_order* order, int32_t k, int mem, uint32_t* out_docs, int64_t* out_dates,
                           int32_t* out_count, uint64_t* out_total, void* stream);
+
+/* ---- Prefilter: SearchRequest.field_filter evaluated over every document of the segment (reference: TextReaderService::prefilter,
+ * nidx_text/src/reader.rs:147-180, over filter_to_query, nidx_text/src/search_query.rs:156-217).  The strings of the expression are
+ * resolved on the caller's side into ranges of ords of the segment's dictionaries (facets: nidx_txt_set_facets; resources and field
+ * paths: nidx_txt_set_doc_columns), so the device never sees a string. */
+
+/* Every document's resource ord and field ord (n_docs each, host pointers): indexes into the caller's dictionaries of resource ids
+ * and field paths.  The columns live in HBM (8 bytes per document).  A call that fails leaves the previous columns in place. */
+int nidx_txt_set_doc_columns(nidx_txt_segment* seg, const uint32_t* resource_ord, const uint32_t* field_ord);
+
+#define NIDX_P_FACET 0     /* the document carries a facet ord in [lo, hi) */
+#define NIDX_P_FIELD 1     /* the document's field ord is in [lo, hi) */
+#define NIDX_P_RESOURCE 2  /* the document's resource ord is in [lo, hi) */
+#define NIDX_P_DATE 3      /* n = NIDX_ORDER_CREATED | NIDX_ORDER_MODIFIED: lo <= seconds <= hi; a document without that date never matches */
+#define NIDX_P_KEYWORD 4   /* n term ids in `terms`: 1 = the term occurs in the document, 2..64 = the phrase (slop 0) occurs in it (the
+                              segment needs positions), 0 = nothing; an id that is not a term of the segment matches nothing */
+#define NIDX_P_ALL 5       /* every document */
+#define NIDX_P_AND 6       /* intersection of the n operand subtrees that follow; n = 0 matches nothing */
+#define NIDX_P_OR 7        /* union of the n operand subtrees that follow; n = 0 matches nothing */
+#define NIDX_P_NOT 8       /* n = 1: every document that the operand does not match */
+#define NIDX_PREFILTER_MAX_DEPTH 64   /* levels of nesting: a leaf is one level, each AND / OR / NOT adds one */
+typedef struct nidx_prefilter_node {   /* an expression in pre-order */
+    int32_t kind;                      /* NIDX_P_* */
+    int32_t n;                         /* AND / OR / NOT: operands; KEYWORD: terms; DATE: the date field */
+    int64_t lo, hi;                    /* FACET / FIELD / RESOURCE: ord range [lo, hi); DATE: since, until in seconds, both inclusive */
+    const uint32_t* terms;             /* KEYWORD: n term ids (host pointer) */
+} nidx_prefilter_node;
+
+/* The expression AND the alive set over the segment's documents -> out_bits ((n_docs + 63) / 64 words, `mem`, bits past n_docs
+ * zero; may be NULL) and *out_matching (host) = the number of set bits.  The call returns when both are in place.  The program
+ * (at most 4096 instructions: one per leaf and per operand after an operand's first) runs in one pass over the columns; FACET
+ * needs nidx_txt_set_facets, FIELD / RESOURCE nidx_txt_set_doc_columns, DATE nidx_txt_set_dates, a phrase nidx_txt_set_positions
+ * (else NIDX_ESTATE).  A malformed expression, one deeper than NIDX_PREFILTER_MAX_DEPTH or a longer program is NIDX_EINVAL. */
+int nidx_txt_prefilter(nidx_txt_segment* seg, const nidx_prefilter_node* nodes, int32_t n_nodes, uint64_t* out_bits, int mem, uint64_t* out_matching,
+                       void* stream);
+
+/* The hand-off to one vector segment (reference: nidx_vector/src/searcher.rs:300-314 with PrefilterResult::Some): doc_bits over
+ * n_docs text documents and join[n_docs] (u32: the document's key in this segment's NIDX_INV_FIELDS index, or NIDX_NIL; both
+ * `mem`) -> the paragraphs of the matched documents' keys; with a filter formula (nodes, n_nodes > 0; nidx_vec_filter's format)
+ * combined with it under op (NIDX_F_AND | NIDX_F_OR: SearchRequest.filter_operator), then ANDed with the alive set -> out_bits
+ * ((paragraphs + 63) / 64 words, `mem`; may be NULL) and *out_matching (host), to be passed to nidx_vec_search as filter_bits and
+ * filter_matching.  The call returns when both are in place. */
+int nidx_vec_prefilter_bits(nidx_vec_segment* seg, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, const nidx_filter_node* nodes,
+                            int32_t n_nodes, int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Segments sharded over the GPUs of one node: one process (or thread) per GPU, one segment each

@@ -54,6 +54,14 @@ NIDX_INV_LABELS, NIDX_INV_FIELDS = 0, 1
 NIDX_F_LABEL, NIDX_F_KEYS, NIDX_F_AND, NIDX_F_OR, NIDX_F_NOT = 0, 1, 2, 3, 4
 
 
+class PrefilterNode(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("n", C.c_int32), ("lo", C.c_int64), ("hi", C.c_int64), ("terms", C.c_void_p)]
+
+
+NIDX_P_FACET, NIDX_P_FIELD, NIDX_P_RESOURCE, NIDX_P_DATE, NIDX_P_KEYWORD, NIDX_P_ALL, NIDX_P_AND, NIDX_P_OR, NIDX_P_NOT = range(9)
+NIDX_PREFILTER_MAX_DEPTH = 64
+
+
 class TxtSearchParams(C.Structure):
     _fields_ = [("k", C.c_int32), ("mode", C.c_int32), ("use_tf", C.c_int32), ("min_score", C.c_float), ("after_mode", C.c_int32),
                 ("after_score", C.c_float), ("after_docaddr", C.c_uint64), ("docaddr_base", C.c_uint64)]
@@ -141,6 +149,9 @@ SIGNATURES = {
     "nidx_txt_list_ordered": (i32, [P, ORDER, i32, i32, P, P, P, P, P]),
     "nidx_txt_set_positions": (i32, [P, P, u64]),
     "nidx_txt_search_phrases": (i32, [P, P, P, i32, i32, TSP, P, ORDER, REQ, P, P, P, P, P, P, P]),
+    "nidx_txt_set_doc_columns": (i32, [P, P, P]),
+    "nidx_txt_prefilter": (i32, [P, P, i32, P, i32, P, P]),   # nodes: an array of PrefilterNode
+    "nidx_vec_prefilter_bits": (i32, [P, P, u64, P, NODES, i32, i32, P, i32, P, P]),
     "nidx_shard_unique_id": (i32, [P]),
     "nidx_shard_init": (i32, [P, i32, i32, i32, P]),
     "nidx_shard_destroy": (None, [P]),

@@ -70,7 +70,10 @@ def _expr_to_boolean(e) -> Optional[V.BooleanExpression]:
 
 
 def _doc_matches(e, doc: T.TextDoc) -> bool:
-    """nodereader.FilterExpression (field_filter) evaluated on one text document: the prefilter of nidx_text (reader.rs:148-180)."""
+    """nodereader.FilterExpression (field_filter) evaluated on one text document, for the facet / field / resource / and / or / not
+    nodes (every other kind matches).  The search path runs TextSearcher.prefilter on the device instead; this per-document loop is
+    what it replaced, kept for a stand-in library without the prefilter (the ABI emulator of the host-logic tests) and as the
+    reference tests/test_prefilter_model.py compares the prefilter's model with on the nodes both evaluate."""
     kind = e.WhichOneof("expr")
     if kind == "facet":
         return any(l == e.facet.facet or l.startswith(e.facet.facet + "/") for l in doc.labels)
@@ -279,11 +282,14 @@ class NidxBinding:
         k = int(req.result_per_page)
         out = {}
         order = T.OrderBy(sort_by=int(req.order.sort_by), type=int(req.order.type)) if req.HasField("order") else None
-        # prefilter (shard_search.rs:108-137): field_filter on the documents -> the fields that may answer
+        # prefilter (shard_search.rs:108-137): field_filter evaluated on the device over the documents -> the fields that may answer
         prefilter = V.PrefilterResult.all()
         if req.HasField("field_filter") and shard.text_searcher is not None:
-            fields = [V.FieldId(_uuid.UUID(d.uuid), d.field) for seg in shard.text_searcher.segments for d in seg.docs if _doc_matches(req.field_filter, d)]
-            prefilter = V.PrefilterResult.some(fields) if fields else V.PrefilterResult.none()
+            if hasattr(V._lib.load(), "nidx_txt_prefilter"):
+                prefilter = shard.text_searcher.prefilter(req.field_filter)
+            else:   # a stand-in for libnidx_b200.so without the prefilter (the ABI emulator of the host-logic tests): the host loop
+                fields = [V.FieldId(_uuid.UUID(d.uuid), d.field) for seg in shard.text_searcher.segments for d in seg.docs if _doc_matches(req.field_filter, d)]
+                prefilter = V.PrefilterResult.some(fields) if fields else V.PrefilterResult.none()
         if len(req.vector):
             name = req.vectorset
             if name not in shard.vectorsets:

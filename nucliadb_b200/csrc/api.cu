@@ -19,6 +19,7 @@
 #include "../../include/nidx_b200.h"
 #include "bm25.cuh"
 #include "phrase.cuh"
+#include "prefilter.cuh"
 #include "common.cuh"
 #include "hnsw_build.cuh"
 #include "hnsw_search.cuh"
@@ -96,7 +97,7 @@ using DevBuf = DevArray<unsigned char>;
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
-    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets, phrases;
+    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets, phrases, prefilter;
     cudaEvent_t done = nullptr;
     cudaStream_t last_stream = nullptr;
     bool busy = false;
@@ -217,6 +218,7 @@ struct nidx_vec_segment {
         std::vector<unsigned char> key_bytes;
         std::vector<uint64_t> key_off, post_off;
         DevArray<uint32_t> d_post;
+        DevArray<uint64_t> d_post_off;  // post_off in HBM, for the prefilter hand-off (nidx_vec_prefilter_bits)
         uint32_t n_keys = 0;
     } inv[2];
     // graph
@@ -1442,6 +1444,8 @@ int nidx_vec_set_inverted_index(nidx_vec_segment* s, int32_t which, uint32_t n_k
     ix.post_off.assign(post_off, post_off + n_keys + 1);
     ALLOC(ix.d_post, std::max<uint64_t>(np, 1) * 4);
     if (np) CU(cudaMemcpy(ix.d_post, postings, np * 4, cudaMemcpyHostToDevice));
+    ALLOC(ix.d_post_off, ((size_t)n_keys + 1) * 8);
+    CU(cudaMemcpy(ix.d_post_off, post_off, ((size_t)n_keys + 1) * 8, cudaMemcpyHostToDevice));
     ix.n_keys = n_keys;
     s->inv[which] = std::move(ix);   // only now: a rejected or failed call leaves the previous index in place
     return 0;
@@ -1917,6 +1921,8 @@ struct nidx_txt_segment {
     DevArray<uint64_t> d_pos_off;     // [n_post + 1]
     DevArray<uint32_t> d_pos;
     std::vector<float> idf;           // [n_terms] of the statistics set last: a phrase's weight sums its terms'
+    // prefilter columns (nidx_txt_set_doc_columns): every document's resource and field ord
+    DevArray<uint32_t> d_res_ord, d_field_ord;
     WorkspacePool pool;
 
     ~nidx_txt_segment() {
@@ -2561,6 +2567,221 @@ int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int3
     CU(cudaEventRecord(t->ev_k1, stream));
     CU(cudaGetLastError());
     return st.finish();
+}
+
+// ---- prefilter (prefilter.cuh) --------------------------------------------------------------------
+// A handle-taking entry point without a device: NIDX_ENODEVICE (no handle can exist), else a NULL handle is NIDX_EINVAL.
+static int require_handle(const void* h) {
+    if (nidx_device_count() <= 0) return fail(NIDX_ENODEVICE, "no CUDA device available (nidx_b200 has no CPU fallback)");
+    return h ? 0 : fail(NIDX_EINVAL, "null segment");
+}
+
+int nidx_txt_set_doc_columns(nidx_txt_segment* t, const uint32_t* resource_ord, const uint32_t* field_ord) {
+    int r = require_handle(t);
+    if (r) return r;
+    if (t->n_docs && (!resource_ord || !field_ord)) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->device));
+    DevArray<uint32_t> res, fld;
+    const size_t n = t->n_docs;
+    ALLOC(res, std::max<size_t>(n, 1) * 4);
+    ALLOC(fld, std::max<size_t>(n, 1) * 4);
+    if (n) {
+        CU(cudaMemcpy(res, resource_ord, n * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(fld, field_ord, n * 4, cudaMemcpyHostToDevice));
+    }
+    t->d_res_ord = std::move(res);   // only now: a failed call leaves the previous columns in place
+    t->d_field_ord = std::move(fld);
+    return 0;
+}
+
+}  // extern "C"
+
+// An expression (pre-order nidx_prefilter_node) as the pass runs it: leaves and binary AND / OR in post-order, so that the bit stack
+// never holds more than the nesting depth.  Keyword leaves get a bitset slot each: terms first, then phrases.
+struct PrefilterPlan {
+    std::vector<PfOp> prog;
+    std::vector<uint32_t> terms;                       // term leaves, slot = index
+    std::vector<uint32_t> ph_terms, ph_off{0}, ph_query;   // phrase leaves, slot = terms.size() + index
+    bool facets = false, columns = false, dates[2] = {false, false};
+
+    int compile(const nidx_prefilter_node* nodes, int n_nodes, int& i, int depth) {
+        if (i >= n_nodes) return fail(NIDX_EINVAL, "malformed prefilter expression (operand counts do not add up to %d nodes)", n_nodes);
+        if (depth > NIDX_PREFILTER_MAX_DEPTH) return fail(NIDX_EINVAL, "the prefilter expression nests deeper than %d levels", NIDX_PREFILTER_MAX_DEPTH);
+        const nidx_prefilter_node& nd = nodes[i++];
+        PfOp o{};
+        o.lo = nd.lo; o.hi = nd.hi;
+        switch (nd.kind) {
+            case NIDX_P_FACET: o.op = PF_FACET; facets = true; break;
+            case NIDX_P_FIELD: o.op = PF_FIELD; columns = true; break;
+            case NIDX_P_RESOURCE: o.op = PF_RESOURCE; columns = true; break;
+            case NIDX_P_DATE:
+                if (nd.n != NIDX_ORDER_CREATED && nd.n != NIDX_ORDER_MODIFIED) return fail(NIDX_EINVAL, "prefilter node %d: bad date field", i - 1);
+                o.op = PF_DATE; o.arg = (uint32_t)nd.n; dates[nd.n] = true;
+                break;
+            case NIDX_P_KEYWORD:
+                if (nd.n < 0 || nd.n > PHRASE_MAX_TERMS || (nd.n && !nd.terms)) return fail(NIDX_EINVAL, "prefilter node %d: a keyword has 0 to %d terms", i - 1, PHRASE_MAX_TERMS);
+                if (nd.n == 0) { o.op = PF_CONST; o.arg = 0; break; }
+                o.op = PF_BITS;
+                if (nd.n == 1) { o.arg = (uint32_t)terms.size(); terms.push_back(nd.terms[0]); break; }
+                o.arg = 0x80000000u | (uint32_t)ph_query.size();   // a phrase slot, resolved once the number of term leaves is known
+                ph_query.push_back((uint32_t)ph_query.size() / BM_MAX_TERMS);   // at most BM_MAX_TERMS phrases per query of the phrase pass
+                ph_terms.insert(ph_terms.end(), nd.terms, nd.terms + nd.n);
+                ph_off.push_back((uint32_t)ph_terms.size());
+                break;
+            case NIDX_P_ALL: o.op = PF_CONST; o.arg = 1; break;
+            case NIDX_P_AND: case NIDX_P_OR: {
+                if (nd.n < 0) return fail(NIDX_EINVAL, "prefilter node %d: bad operand count", i - 1);
+                if (nd.n == 0) { o.op = PF_CONST; o.arg = 0; break; }   // a BooleanQuery without clauses matches nothing
+                for (int c = 0; c < nd.n; ++c) {
+                    int r = compile(nodes, n_nodes, i, depth + 1);
+                    if (r) return r;
+                    if (c) { PfOp b{}; b.op = nd.kind == NIDX_P_AND ? PF_AND : PF_OR; prog.push_back(b); }
+                }
+                return 0;
+            }
+            case NIDX_P_NOT: {
+                if (nd.n != 1) return fail(NIDX_EINVAL, "prefilter node %d: NOT takes one operand", i - 1);
+                int r = compile(nodes, n_nodes, i, depth + 1);
+                if (r) return r;
+                o.op = PF_NOT;
+                break;
+            }
+            default: return fail(NIDX_EINVAL, "prefilter node %d: bad kind %d", i - 1, nd.kind);
+        }
+        prog.push_back(o);
+        return 0;
+    }
+};
+
+extern "C" {
+
+int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, int32_t n_nodes, uint64_t* out_bits, int mem, uint64_t* out_matching,
+                       void* stream_) {
+    int r = require_handle(t);
+    if (r) return r;
+    if (!nodes || n_nodes <= 0) return fail(NIDX_EINVAL, "empty prefilter expression");
+    PrefilterPlan P;
+    int at = 0;
+    r = P.compile(nodes, n_nodes, at, 1);
+    if (r) return r;
+    if (at != n_nodes) return fail(NIDX_EINVAL, "malformed prefilter expression (operand counts do not add up to %d nodes)", n_nodes);
+    if (P.prog.size() > (size_t)PF_MAX_PROGRAM) return fail(NIDX_EINVAL, "the prefilter program has more than %d instructions", PF_MAX_PROGRAM);
+    if (P.facets && !t->d_fdoc_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
+    if (P.columns && !t->d_res_ord) return fail(NIDX_ESTATE, "the segment has no document columns (nidx_txt_set_doc_columns)");
+    if ((P.dates[0] && !t->d_secs[0]) || (P.dates[1] && !t->d_secs[1])) return fail(NIDX_ESTATE, "the segment has no dates (nidx_txt_set_dates)");
+    if (!P.ph_query.empty() && !t->d_pos) return fail(NIDX_ESTATE, "the segment has no positions (nidx_txt_set_positions)");
+    const uint32_t n_terms = (uint32_t)P.terms.size(), nv = (uint32_t)P.ph_query.size();
+    for (PfOp& o : P.prog)
+        if (o.op == PF_BITS && (o.arg & 0x80000000u)) o.arg = n_terms + (o.arg & 0x7FFFFFFFu);
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(t->device));
+    WsGuard g(t->pool, stream);
+    Workspace& w = *g.w;
+    const size_t words = ((size_t)t->n_docs + 63) / 64, slots = (size_t)n_terms + nv;
+    Stage st(stream, host, host);
+    uint64_t* d_out;
+    st.out(out_bits, words, &d_out);
+    r = st.place(w.stage);
+    if (r) return r;
+    // w.prefilter: [slots][words] keyword bitsets | match count | program | term leaves
+    const size_t o_count = (slots * words * 8 + 15) & ~(size_t)15, o_prog = o_count + 16, o_terms = o_prog + P.prog.size() * sizeof(PfOp);
+    ENSURE(w.prefilter, o_terms + std::max<size_t>(n_terms, 1) * 4);
+    unsigned char* base = w.prefilter.p;
+    uint64_t* kw = reinterpret_cast<uint64_t*>(base);
+    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(base + o_count);
+    PfOp* d_prog = reinterpret_cast<PfOp*>(base + o_prog);
+    uint32_t* d_terms = reinterpret_cast<uint32_t*>(base + o_terms);
+    CU(cudaMemsetAsync(d_count, 0, 8, stream));
+    CU(cudaMemcpyAsync(d_prog, P.prog.data(), P.prog.size() * sizeof(PfOp), cudaMemcpyHostToDevice, stream));
+    if (slots && words) CU(cudaMemsetAsync(kw, 0, slots * words * 8, stream));
+    if (n_terms && words) {
+        CU(cudaMemcpyAsync(d_terms, P.terms.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice, stream));
+        prefilter_scatter_kernel<<<n_terms, 256, 0, stream>>>(t->d_post, t->d_term_off, t->n_terms, d_terms, nullptr, 0, kw, words);
+        LAUNCHED();
+    }
+    PhrasePlan pp;
+    if (nv && words) {   // the phrases' virtual lists (phrase.cuh), as the keyword search makes them, then scattered like terms
+        const int32_t nq = (int32_t)((nv + BM_MAX_TERMS - 1) / BM_MAX_TERMS);
+        const std::vector<uint32_t> no_terms(nq + 1, 0);
+        const nidx_txt_phrases ph{P.ph_terms.data(), P.ph_off.data(), P.ph_query.data(), (int32_t)nv};
+        r = phrase_plan(t, &ph, nq, no_terms, pp);
+        if (r) return r;
+        TxtDev T;
+        T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
+        T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
+        Bm25Args a{};
+        r = phrase_pass(t, pp, T, w, stream, a);
+        if (r) return r;
+        prefilter_scatter_kernel<<<nv, 256, 0, stream>>>(a.ph_post, nullptr, 0, nullptr, a.ph_range, n_terms, kw, words);
+        LAUNCHED();
+    }
+    PrefilterArgs A;
+    A.n_docs = t->n_docs; A.res_ord = t->d_res_ord; A.field_ord = t->d_field_ord; A.fdoc_off = t->d_fdoc_off; A.ford = t->d_ford;
+    A.secs0 = t->d_secs[0]; A.secs1 = t->d_secs[1]; A.kw_bits = kw; A.words = words; A.alive = t->d_alive;
+    A.prog = d_prog; A.n_prog = (uint32_t)P.prog.size(); A.out = reinterpret_cast<uint32_t*>(d_out); A.count = d_count;
+    const size_t smem = P.prog.size() * sizeof(PfOp);
+    CU(cudaFuncSetAttribute(prefilter_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)t->sm_count * 8, (2 * words * 32 + PF_THREADS - 1) / PF_THREADS));
+    CU(cudaEventRecord(t->ev_k0, stream));
+    prefilter_eval_kernel<<<blocks, PF_THREADS, smem, stream>>>(A);
+    CU(cudaEventRecord(t->ev_k1, stream));
+    LAUNCHED();
+    CU(cudaGetLastError());
+    unsigned long long h = 0;
+    CU(cudaMemcpyAsync(&h, d_count, 8, cudaMemcpyDeviceToHost, stream));
+    r = st.finish(true);   // the program and the plans are host temporaries, and the count is read back
+    if (r) return r;
+    if (out_matching) *out_matching = h;
+    return 0;
+}
+
+int nidx_vec_prefilter_bits(nidx_vec_segment* s, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, const nidx_filter_node* nodes,
+                            int32_t n_nodes, int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream_) {
+    int r = require_handle(s);
+    if (r) return r;
+    if (n_docs && (!doc_bits || !join)) return fail(NIDX_EINVAL, "null argument");
+    if (op != NIDX_F_AND && op != NIDX_F_OR) return fail(NIDX_EINVAL, "op must be NIDX_F_AND or NIDX_F_OR");
+    if (n_nodes < 0 || (n_nodes > 0 && !nodes)) return fail(NIDX_EINVAL, "bad filter formula");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(s->cfg.device));
+    WsGuard g(s->pool, stream);
+    Workspace& w = *g.w;
+    const size_t words = ((size_t)s->n_par + 63) / 64;
+    Stage st(stream, host, host);
+    const uint64_t* d_doc;
+    const uint32_t* d_join;
+    uint64_t* d_out;
+    st.in(doc_bits, (size_t)((n_docs + 63) / 64), &d_doc);
+    st.in(join, (size_t)n_docs, &d_join);
+    st.out(out_bits, words, &d_out);
+    r = st.place(w.stage);
+    if (r) return r;
+    ENSURE(w.prefilter, std::max<size_t>(words, 1) * 8);
+    uint64_t* acc = w.prefilter.as<uint64_t>();
+    if (words) CU(cudaMemsetAsync(acc, 0, words * 8, stream));
+    const nidx_vec_segment::InvIndex& ix = s->inv[NIDX_INV_FIELDS];
+    if (n_docs && ix.n_keys) {
+        const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_docs + 255) / 256));
+        prefilter_join_kernel<<<blocks, 256, 0, stream>>>(d_doc, d_join, n_docs, ix.n_keys, ix.d_post_off, ix.d_post, acc);
+        LAUNCHED();
+    }
+    if (n_nodes) {   // the paragraph formula (segment.rs:516-534), combined as the reference combines its clauses
+        uint64_t* fdev = nullptr;
+        r = filter_formula_device(s, w, nodes, n_nodes, stream, &fdev);
+        if (r) return r;
+        bits_combine_kernel<<<(unsigned)std::min<size_t>(std::max<size_t>((words + 255) / 256, 1), 1024), 256, 0, stream>>>(acc, fdev, words, s->n_par,
+                                                                                                                        op == NIDX_F_OR ? 1 : 0);
+        LAUNCHED();
+    }
+    unsigned long long h = 0;
+    const uint64_t* bits;
+    r = words ? filter_and_alive(s, w, acc, d_out, &h, stream, &bits) : 0;   // an empty segment: no words, nothing matches
+    if (!r) r = st.finish(true);
+    if (r) return r;
+    if (out_matching) *out_matching = h;
+    return 0;
 }
 
 // ---- sharded search (shard.cuh) -------------------------------------------------------------------

@@ -1,0 +1,136 @@
+// nidx_b200 — the prefilter of a filtered search on the device (sm_90a).
+//
+// Replaces nidx_text's TextReaderService::prefilter (nidx_text/src/reader.rs:147-180: filter_to_query over every document, the
+// FieldUuidCollector) and the host key set it hands to the vector search (nidx_vector/src/searcher.rs:300-314).
+//   prefilter_scatter_kernel  keyword leaves, before the pass: one CTA per leaf sets the bits of a posting list (a term's, or a
+//                             phrase's virtual list from phrase.cuh) in the leaf's document bitset;
+//   prefilter_eval_kernel     one pass over the documents: a warp covers 32 consecutive documents, every lane runs the program (the
+//                             expression in post-order, in shared memory) for its own document on a bit stack held in a register;
+//                             the warp's ballot is one 32-bit word of the result, ANDed with the alive bits, and counted;
+//   prefilter_join_kernel     text documents -> paragraphs of one vector segment: every matched document with a join entry sets the
+//                             paragraphs of that field key (the NIDX_INV_FIELDS postings).
+// HBM traffic of the pass = per document the columns the program reads (4 B per ord column, 8 B per date column, the facet CSR
+// entry and ords) + 1/8 B of alive bits + 1/8 B per keyword leaf + 1/8 B of output.
+#pragma once
+#include <cstdint>
+
+#include "bm25.cuh"
+
+namespace nidx {
+
+constexpr int PF_MAX_DEPTH = 64;        // the bit stack is one 64-bit register: NIDX_PREFILTER_MAX_DEPTH
+constexpr int PF_MAX_PROGRAM = 4096;    // instructions (32 B each) in shared memory
+constexpr int PF_THREADS = 256;
+
+enum PfOpcode : uint32_t { PF_FACET, PF_FIELD, PF_RESOURCE, PF_DATE, PF_BITS, PF_CONST, PF_AND, PF_OR, PF_NOT };
+
+struct PfOp {          // one instruction: leaves push a bit, AND / OR pop two and push one, NOT flips the top
+    int64_t lo, hi;    // FACET / FIELD / RESOURCE: ord range [lo, hi); DATE: since, until (inclusive)
+    uint32_t op;       // PfOpcode
+    uint32_t arg;      // DATE: the seconds column (0 created, 1 modified); BITS: the keyword leaf's slot; CONST: the bit
+    uint32_t pad[2];
+};
+
+struct PrefilterArgs {
+    uint32_t n_docs;
+    const uint32_t* res_ord;     // [n_docs] (nidx_txt_set_doc_columns)
+    const uint32_t* field_ord;   // [n_docs]
+    const uint32_t* fdoc_off;    // [n_docs + 1] facet CSR (nidx_txt_set_facets)
+    const uint32_t* ford;
+    const int64_t* secs0;        // [n_docs] created, modified seconds (nidx_txt_set_dates); INT64_MIN = no date
+    const int64_t* secs1;
+    const uint64_t* kw_bits;     // [slots][words] keyword leaves
+    size_t words;                // (n_docs + 63) / 64
+    const uint64_t* alive;       // NULL = all alive
+    const PfOp* prog;
+    uint32_t n_prog;
+    uint32_t* out;               // [2 * words]: the result as 32-bit words, padding bits zero
+    unsigned long long* count;   // += set bits of out
+};
+
+__global__ void __launch_bounds__(PF_THREADS) prefilter_eval_kernel(PrefilterArgs A) {
+    extern __shared__ PfOp prog[];
+    for (uint32_t i = threadIdx.x; i < A.n_prog; i += blockDim.x) prog[i] = A.prog[i];
+    __syncthreads();
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t n32 = 2 * (uint64_t)A.words;
+    const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    unsigned long long local = 0;
+    // w is the same for the 32 lanes of a warp: the ballot always has the full warp
+    for (uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n32; w += n_warps) {
+        const uint64_t d = w * 32 + lane;
+        uint32_t bit = 0;
+        if (d < A.n_docs) {
+            uint64_t st = 0;
+            for (uint32_t i = 0; i < A.n_prog; ++i) {
+                const PfOp& o = prog[i];
+                uint64_t b;
+                switch (o.op) {
+                    case PF_FACET: {   // ords ascend: the first one >= lo decides
+                        b = 0;
+                        for (uint32_t j = __ldg(A.fdoc_off + d), e = __ldg(A.fdoc_off + d + 1); j < e; ++j) {
+                            const int64_t u = __ldg(A.ford + j);
+                            if (u >= o.lo) { b = u < o.hi; break; }
+                        }
+                        break;
+                    }
+                    case PF_FIELD: { const int64_t u = __ldg(A.field_ord + d); b = u >= o.lo && u < o.hi; break; }
+                    case PF_RESOURCE: { const int64_t u = __ldg(A.res_ord + d); b = u >= o.lo && u < o.hi; break; }
+                    case PF_DATE: {
+                        const int64_t s = __ldg((o.arg ? A.secs1 : A.secs0) + d);
+                        b = s != INT64_MIN && s >= o.lo && s <= o.hi;
+                        break;
+                    }
+                    case PF_BITS: b = (__ldg(A.kw_bits + (size_t)o.arg * A.words + (d >> 6)) >> (d & 63)) & 1ull; break;
+                    case PF_CONST: b = o.arg; break;
+                    case PF_AND: b = st & (st >> 1) & 1ull; st >>= 2; break;
+                    case PF_OR: b = (st | (st >> 1)) & 1ull; st >>= 2; break;
+                    default: st ^= 1ull; continue;   // PF_NOT
+                }
+                st = (st << 1) | b;
+            }
+            bit = (uint32_t)(st & 1ull);
+        }
+        uint32_t word = __ballot_sync(0xFFFFFFFFu, bit);
+        if (A.alive) word &= __ldg(reinterpret_cast<const uint32_t*>(A.alive) + w);
+        if (lane == 0) { A.out[w] = word; local += __popc(word); }
+    }
+    if (lane == 0 && local) atomicAdd(A.count, local);
+}
+
+// One CTA per keyword leaf (slot0 + blockIdx.x): terms != NULL -> the posting list of terms[blockIdx.x] (none when the id is not a
+// term of the segment), else the range ranges[2 blockIdx.x .. +1] of `post` (a phrase's compacted virtual list).
+__global__ void prefilter_scatter_kernel(const uint2* __restrict__ post, const uint64_t* __restrict__ term_off, uint32_t n_terms,
+                                         const uint32_t* __restrict__ terms, const uint64_t* __restrict__ ranges, uint32_t slot0,
+                                         uint64_t* __restrict__ bits, size_t words) {
+    uint64_t b, e;
+    if (terms) {
+        const uint32_t t = terms[blockIdx.x];
+        if (t >= n_terms) return;
+        b = term_off[t]; e = term_off[t + 1];
+    } else {
+        b = ranges[2 * blockIdx.x]; e = ranges[2 * blockIdx.x + 1];
+    }
+    unsigned long long* out = reinterpret_cast<unsigned long long*>(bits + (size_t)(slot0 + blockIdx.x) * words);
+    for (uint64_t i = b + threadIdx.x; i < e; i += blockDim.x) {
+        const uint32_t doc = __ldg(&post[i].x);
+        atomicOr(out + (doc >> 6), 1ull << (doc & 63));
+    }
+}
+
+// doc_bits [n_docs] -> out (paragraph bits, zeroed by the caller): join[d] = the document's key in the field index (NIL or >= n_keys:
+// none), whose paragraphs are post[post_off[key] .. post_off[key + 1]).
+__global__ void prefilter_join_kernel(const uint64_t* __restrict__ doc_bits, const uint32_t* __restrict__ join, uint64_t n_docs, uint32_t n_keys,
+                                      const uint64_t* __restrict__ post_off, const uint32_t* __restrict__ post, uint64_t* __restrict__ out) {
+    for (uint64_t d = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; d < n_docs; d += (uint64_t)gridDim.x * blockDim.x) {
+        if (!((__ldg(doc_bits + (d >> 6)) >> (d & 63)) & 1ull)) continue;
+        const uint32_t j = __ldg(join + d);
+        if (j >= n_keys) continue;
+        for (uint64_t i = __ldg(post_off + j), e = __ldg(post_off + j + 1); i < e; ++i) {
+            const uint32_t p = __ldg(post + i);
+            atomicOr(reinterpret_cast<unsigned long long*>(out) + (p >> 6), 1ull << (p & 63));
+        }
+    }
+}
+
+}  // namespace nidx

@@ -148,6 +148,12 @@ def _build():
     ff = m.nested_type.add(name="FieldFilter"); _field(ff, "field_type", 1, "string"); _field(ff, "field_id", 2, "string", optional=True)
     kw = m.nested_type.add(name="KeywordFilter"); _field(kw, "keyword", 1, "string")
     fc = m.nested_type.add(name="FacetFilter"); _field(fc, "facet", 1, "string")
+    dr = m.nested_type.add(name="DateRangeFilter")
+    e = dr.enum_type.add(name="DateField"); e.value.add(name="CREATED", number=0); e.value.add(name="MODIFIED", number=1)
+    _field(dr, "field", 1, "enum:.nodereader.FilterExpression.DateRangeFilter.DateField")
+    _field(dr, "since", 2, ".google.protobuf.Timestamp", optional=True); _field(dr, "until", 3, ".google.protobuf.Timestamp", optional=True)
+    rfp = m.nested_type.add(name="ResourceFieldPrefixFilter")
+    _field(rfp, "resource_id", 1, "string"); _field(rfp, "field_type", 2, "string"); _field(rfp, "field_id_prefix", 3, "string")
     m.oneof_decl.add().name = "expr"
     _field(m, "bool_and", 1, ".nodereader.FilterExpression.FilterExpressionList", oneof=0)
     _field(m, "bool_or", 2, ".nodereader.FilterExpression.FilterExpressionList", oneof=0)
@@ -155,7 +161,9 @@ def _build():
     _field(m, "resource", 4, ".nodereader.FilterExpression.ResourceFilter", oneof=0)
     _field(m, "field", 5, ".nodereader.FilterExpression.FieldFilter", oneof=0)
     _field(m, "keyword", 6, ".nodereader.FilterExpression.KeywordFilter", oneof=0)
+    _field(m, "date", 7, ".nodereader.FilterExpression.DateRangeFilter", oneof=0)
     _field(m, "facet", 8, ".nodereader.FilterExpression.FacetFilter", oneof=0)
+    _field(m, "resource_field_prefix", 9, ".nodereader.FilterExpression.ResourceFieldPrefixFilter", oneof=0)
     m = fd.message_type.add(name="SearchAfter")               # :382-386
     _field(m, "score", 1, "float"); _field(m, "shard_id", 2, "bytes"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="SearchRequest")             # :388-437

@@ -170,6 +170,21 @@ class VectorSegment:
         check(_lib.load().nidx_vec_filter(self._h, nodes, n, ptr(out_bits), _lib.NIDX_MEM_HOST, C.byref(matching), None))
         return matching.value
 
+    def prefilter_bits(self, doc_bits, join, n_docs: int, n_paragraphs: int, formula=None, op=_lib.NIDX_F_AND):
+        """nidx_vec_prefilter_bits: text-document bits (uint64 words) and the join table (uint32 [n_docs]: each document's key in the
+        field index, or NIL) -> (paragraph bits, matching): the matched documents' paragraphs, combined with `formula` (a FilterNode
+        array, or None) under `op`, AND alive.  numpy inputs -> numpy words; torch CUDA tensors -> a torch int64 tensor (device path)."""
+        on_device = _is_torch(doc_bits)
+        mem, stream, alloc = _stage(self.cfg.device, on_device)
+        if not on_device:
+            doc_bits = np.ascontiguousarray(doc_bits, dtype=np.uint64)
+            join = np.ascontiguousarray(join, dtype=np.uint32)
+        out = alloc((n_paragraphs + 63) // 64, np.uint64)
+        matching = C.c_uint64()
+        check(_lib.load().nidx_vec_prefilter_bits(self._h, ptr(doc_bits), n_docs, ptr(join), formula, 0 if formula is None else len(formula), op, ptr(out), mem,
+                                                  C.byref(matching), stream))
+        return out, matching.value
+
     # ---- search ----------------------------------------------------------------------------------------
     def search(self, queries, k: int, ef: int = 0, min_score: float = -1.0, with_duplicates=True, method=_lib.NIDX_METHOD_AUTO,
                filter_bits=None, filter_matching: int = 0, formula=None, out=None, stream: Optional[int] = None):
@@ -419,6 +434,25 @@ class TextSegment:
         out = (alloc(k, np.uint32), alloc(k, np.int64), alloc(1, np.int32, zero=True), alloc(1, np.uint64, zero=True))
         check(_lib.load().nidx_txt_list_ordered(self._h, C.byref(o), k, mem, *map(ptr, out), stream))
         return out if device_out else (out[0], out[1], int(out[2][0]), int(out[3][0]))
+
+    # ---- prefilter (TextReaderService::prefilter: include/nidx_b200.h nidx_txt_prefilter) ---------------------------------------
+    def set_doc_columns(self, resource_ord, field_ord):
+        """Every document's resource ord and field ord (uint32 [n_docs]) in the caller's dictionaries."""
+        resource_ord = np.ascontiguousarray(resource_ord, dtype=np.uint32)
+        field_ord = np.ascontiguousarray(field_ord, dtype=np.uint32)
+        assert len(resource_ord) == self.n_docs and len(field_ord) == self.n_docs
+        check(_lib.load().nidx_txt_set_doc_columns(self._h, ptr(resource_ord), ptr(field_ord)))
+
+    def prefilter(self, nodes, out=None):
+        """The expression (a PrefilterNode array in pre-order) AND alive -> (bits, matching): bits = uint64 words [(n_docs + 63) // 64]
+        in a new numpy array, or written into `out` (a torch CUDA int64 tensor of that many words: device path)."""
+        on_device = out is not None and _is_torch(out)
+        mem, stream, alloc = _stage(self.device, on_device)
+        if out is None:
+            out = alloc((self.n_docs + 63) // 64, np.uint64)
+        matching = C.c_uint64()
+        check(_lib.load().nidx_txt_prefilter(self._h, C.addressof(nodes), len(nodes), ptr(out), mem, C.byref(matching), stream))
+        return out, matching.value
 
     def set_doc_keys(self, keys: Optional[np.ndarray]):
         """Caller keys of the documents (paragraph ids) for rank fusion; None = the document number."""

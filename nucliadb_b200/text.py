@@ -32,6 +32,7 @@ from __future__ import annotations
 
 import re
 import unicodedata
+import uuid as _uuid_mod
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -274,7 +275,18 @@ class TextIndexSegment:
         term_off = np.zeros(n_terms + 1, dtype=np.uint64)
         term_off[1:] = np.cumsum(np.bincount(self.post_term, minlength=n_terms))
         self._gpu = TextSegment.create(self.n_docs, n_terms, term_off, self.post_doc, self.post_tf, self.fieldnorm_id, device=self.device)
+        self.alive_count = self.n_docs
         return self._gpu
+
+    def set_alive(self, alive: np.ndarray):
+        """Deletions inside the segment: a bool per document (nidx_txt_set_alive).  The prefilter counts the alive documents for its
+        All class."""
+        alive = np.asarray(alive, dtype=bool)
+        words = np.zeros((self.n_docs + 63) // 64 * 8, dtype=np.uint8)
+        packed = np.packbits(alive, bitorder="little")
+        words[: len(packed)] = packed
+        self._gpu.set_alive(words.view(np.uint64))
+        self.alive_count = int(alive.sum())
 
 
 class TextSearcher:
@@ -296,6 +308,8 @@ class TextSearcher:
             s.upload(n_terms).set_stats(max(total_docs, 1), max(total_tokens, 1), df)
         self.facet_keys: Optional[list] = None   # built on the first faceted request
         self._dates = False                        # uploaded on the first ordered request
+        self._prefilter: Optional[_PrefilterIndex] = None   # built on the first prefilter
+        self._positions = False                    # uploaded on the first phrase (query or keyword filter)
 
     def _ensure_facets(self):
         """The index's facet dictionary (every valid label of every document, in facet order) and each segment's per-document
@@ -320,6 +334,46 @@ class TextSearcher:
             s._gpu.set_dates(np.asarray([none if d.created is None else int(d.created) for d in s.docs], dtype=np.int64),
                              np.asarray([none if d.modified is None else int(d.modified) for d in s.docs], dtype=np.int64))
         self._dates = True
+
+    def _ensure_positions(self):
+        if not self._positions:
+            for s in self.segments:
+                s._gpu.set_positions(s.positions)
+            self._positions = True
+
+    def prefilter(self, expr):
+        """TextReaderService::prefilter (nidx_text/src/reader.rs:147-180) for a nodereader.FilterExpression: evaluated on the device
+        over every segment -> vector.PrefilterResult: none (nothing matched), all (every alive document matched) or some, whose
+        matched documents stay in HBM as a bitset (handed to VectorSearcher.search as they are; `fields` lists them on demand).
+        A malformed expression, an invalid facet or resource UUID, or one the device cannot run (deeper than
+        NIDX_PREFILTER_MAX_DEPTH, a keyword of more than 64 words) is a ValueError."""
+        import torch
+
+        from . import vector as V
+        from ._lib import NidxError
+
+        self._ensure_facets()
+        self._ensure_dates()
+        if self._prefilter is None:
+            self._prefilter = _PrefilterIndex(self)
+        ix = self._prefilter
+        nodes, keep, phrases = ix.compile(expr)
+        if phrases:
+            self._ensure_positions()
+        bits = torch.empty(ix.words_total, dtype=torch.int64, device=torch.device("cuda", self.segments[0].device))
+        matching = 0
+        try:
+            for s, off in zip(self.segments, ix.word_off):
+                matching += s._gpu.prefilter(nodes, out=bits[off: off + (s.n_docs + 63) // 64])[1]
+        except NidxError as e:
+            if e.code == -1:   # NIDX_EINVAL: the expression is not one the device runs
+                raise ValueError(str(e)) from e
+            raise
+        if matching == 0:
+            return V.PrefilterResult.none()
+        if matching == sum(s.alive_count for s in self.segments):
+            return V.PrefilterResult.all()
+        return V.PrefilterResult.from_device(ix, bits, matching)
 
     def _facets(self, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None, phrases=()):
         """Counts of the request's facets over the matched set of every segment, summed, then grouped and cut to the top 50.
@@ -454,6 +508,184 @@ class TextSearcher:
         return resp
 
 
+_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def _prefix_range(keys: list, prefix: bytes, facet: bool):
+    """[lo, hi) of the sorted byte keys that start with `prefix`; facet=True: the facet `prefix` and its descendants (the key itself
+    or prefix + 0x00 ...; the root b"" takes every key)."""
+    import bisect
+
+    lo = bisect.bisect_left(keys, prefix)
+    if facet and prefix:
+        return lo, bisect.bisect_left(keys, prefix + b"\x01")
+    stem = prefix.rstrip(b"\xff")   # the least byte string above every key that starts with `prefix`
+    return lo, bisect.bisect_left(keys, stem[:-1] + bytes([stem[-1] + 1])) if stem else len(keys)
+
+
+class _PrefilterIndex:
+    """What the prefilter of one TextSearcher keeps on the host (built on the first prefilter, once per searcher open): the
+    dictionaries of resource ids and field paths -- field paths in facet order, so that a field filter (a facet term on
+    `schema.field`) and a resource_field_prefix are ranges of ords -- every segment's columns (uploaded with
+    nidx_txt_set_doc_columns), where each segment's documents start in the index-wide bitset (whole 64-bit words), and the join
+    tables to vector segments (one u32 per document of that bitset, in HBM, built on the first hand-off to each)."""
+
+    def __init__(self, searcher: "TextSearcher"):
+        import weakref
+
+        self.searcher = searcher
+        docs = [d for s in searcher.segments for d in s.docs]
+        self.resource_ids, res_ord = np.unique(np.asarray([d.uuid for d in docs], dtype=object).astype(str), return_inverse=True) if docs else ([], [])
+        paths = sorted({d.field for d in docs}, key=lambda p: facet_key(p) if p.startswith("/") else b"\xff" + p.encode())
+        self.field_paths = paths
+        self.field_keys = [facet_key(p) if p.startswith("/") else b"\xff" + p.encode() for p in paths]   # a path without '/' is no facet: matches no filter
+        field_of = {p: i for i, p in enumerate(paths)}
+        fld_ord = np.asarray([field_of[d.field] for d in docs], dtype=np.uint32)
+        res_ord = np.asarray(res_ord, dtype=np.uint32)
+        self.word_off, at, words = [], 0, 0
+        self.doc_base = np.zeros(len(searcher.segments) + 1, dtype=np.int64)
+        for i, s in enumerate(searcher.segments):
+            s._gpu.set_doc_columns(res_ord[at: at + s.n_docs], fld_ord[at: at + s.n_docs])
+            self.word_off.append(words)
+            words += (s.n_docs + 63) // 64
+            at += s.n_docs
+        self.words_total = words
+        self.res_col, self.field_col = res_ord, fld_ord
+        self.by_uuid: dict = {}   # parsed UUID bytes -> resource ords (several spellings of one UUID are several ids)
+        for o, r in enumerate(self.resource_ids):
+            try:
+                self.by_uuid.setdefault(_uuid_mod.UUID(r).bytes, []).append(o)
+            except ValueError:
+                pass
+        self._joins = weakref.WeakKeyDictionary()
+
+    # ---- filter_to_query (nidx_text/src/search_query.rs:156-217) -> nidx_prefilter_node, pre-order ---------------------------------
+    def compile(self, expr):
+        """-> (ctypes PrefilterNode array, keep-alive list, whether a phrase is used)."""
+        flat, keep = [], []
+        phrases = False
+        vocab = self.searcher.vocab
+
+        def node(kind, n=0, lo=0, hi=0, terms=None):
+            flat.append((kind, n, lo, hi, terms))
+
+        def walk(e):
+            nonlocal phrases
+            kind = e.WhichOneof("expr")
+            if kind in ("bool_and", "bool_or"):
+                ops = getattr(e, kind).operands
+                node(_lib.NIDX_P_AND if kind == "bool_and" else _lib.NIDX_P_OR, len(ops))
+                for o in ops:
+                    walk(o)
+            elif kind == "bool_not":
+                node(_lib.NIDX_P_NOT, 1)
+                walk(e.bool_not)
+            elif kind == "facet":
+                key = facet_key(e.facet.facet)
+                if key is None:   # Facet::from asserts a leading '/' [recalled]: the reference fails the request
+                    raise ValueError(f"invalid facet {e.facet.facet!r}: a facet starts with '/'")
+                node(_lib.NIDX_P_FACET, 0, *_prefix_range(self.searcher.facet_keys, key, facet=True))
+            elif kind == "field":
+                f = e.field
+                path = f"/{f.field_type}/{f.field_id}" if f.HasField("field_id") else f"/{f.field_type}"
+                node(_lib.NIDX_P_FIELD, 0, *_prefix_range(self.field_keys, facet_key(path), facet=True))
+            elif kind == "resource":
+                rid = e.resource.resource_id
+                o = int(np.searchsorted(self.resource_ids, rid)) if len(self.resource_ids) else 0
+                hit = o < len(self.resource_ids) and self.resource_ids[o] == rid
+                node(_lib.NIDX_P_RESOURCE, 0, o, o + 1 if hit else o)
+            elif kind == "resource_field_prefix":
+                p = e.resource_field_prefix
+                try:
+                    rb = _uuid_mod.UUID(p.resource_id).bytes
+                except ValueError as err:   # uuid::Uuid::parse_str(..).expect(..): the reference panics
+                    raise ValueError(f"resource_field_prefix: invalid resource id {p.resource_id!r}") from err
+                ords = self.by_uuid.get(rb, [])
+                prefix = facet_key(f"/{p.field_type}/{p.field_id_prefix}")
+                node(_lib.NIDX_P_AND, 2)
+                node(_lib.NIDX_P_OR, len(ords))
+                for o in ords:
+                    node(_lib.NIDX_P_RESOURCE, 0, o, o + 1)
+                node(_lib.NIDX_P_FIELD, 0, *_prefix_range(self.field_keys, prefix, facet=False))
+            elif kind == "date":
+                d = e.date
+                since = d.since.seconds if d.HasField("since") else None
+                until = d.until.seconds if d.HasField("until") else None
+                if since is None and until is None:   # produce_date_range_query -> None: AllQuery
+                    node(_lib.NIDX_P_ALL)
+                else:
+                    node(_lib.NIDX_P_DATE, int(d.field), _I64_MIN if since is None else since, _I64_MAX if until is None else until)
+            elif kind == "keyword":   # translate_keyword_to_text_query (query_io.rs:22-42)
+                words = tokenize(e.keyword.keyword) or [e.keyword.keyword]
+                if len(words) > 64:
+                    raise ValueError("a keyword filter of more than 64 words is not supported")
+                phrases = phrases or len(words) > 1
+                ids = np.asarray([vocab.get(w, 0xFFFFFFF0) for w in words], dtype=np.uint32)   # an unknown word matches nothing
+                keep.append(ids)
+                node(_lib.NIDX_P_KEYWORD, len(ids), terms=ids.ctypes.data)
+            else:
+                raise ValueError(f"filter expression without a known expression: {kind!r}")
+
+        walk(expr)
+        nodes = (_lib.PrefilterNode * len(flat))()
+        for i, (kind, n, lo, hi, terms) in enumerate(flat):
+            nodes[i].kind, nodes[i].n, nodes[i].lo, nodes[i].hi, nodes[i].terms = kind, n, lo, hi, terms
+        return nodes, keep, phrases
+
+    # ---- hand-off to the vector index ---------------------------------------------------------------------------------------
+    def n_docs_total(self) -> int:
+        return 64 * self.words_total
+
+    def join(self, seg):
+        """The join table to one vector OpenSegment (torch int32 [64 * words_total] on the device): for every document of the
+        index-wide bitset, its key in the segment's field index -- the key that FieldId(resource, field) looks up there
+        (searcher.rs:300-314: `{uuid.hex}{field}` through FieldKey) -- or NIL."""
+        j = self._joins.get(seg)
+        if j is not None:
+            return j
+        import torch
+
+        from .vector import field_key
+
+        # (resource ord, field ord) pairs of every field key of the segment: a loop over the segment's keys, not the documents
+        suffix_of: dict = {}
+        for o, path in enumerate(self.field_paths):
+            fk = field_key(f"{_uuid_mod.UUID(int=0).hex}{path}")
+            if fk is not None:
+                suffix_of.setdefault(fk[16:], []).append(o)
+        n_fields = max(len(self.field_paths), 1)
+        codes, vals = [], []
+        for kord, key in enumerate(sorted(seg._field_index)):
+            for r in self.by_uuid.get(key[:16], ()):
+                for f in suffix_of.get(key[16:], ()):
+                    codes.append(r * n_fields + f)
+                    vals.append(kord)
+        codes, vals = np.asarray(codes, dtype=np.int64), np.asarray(vals, dtype=np.uint32)
+        order = np.argsort(codes, kind="stable")
+        codes, vals = codes[order], vals[order]
+        doc_codes = self.res_col.astype(np.int64) * n_fields + self.field_col
+        table = np.full(self.n_docs_total(), _lib.NIL, dtype=np.uint32)
+        if len(codes) and len(doc_codes):
+            at = np.minimum(np.searchsorted(codes, doc_codes), len(codes) - 1)
+            hit = codes[at] == doc_codes
+            docs = np.concatenate([64 * off + np.arange(s.n_docs) for s, off in zip(self.searcher.segments, self.word_off)])
+            table[docs[hit]] = vals[at[hit]]
+        j = torch.from_numpy(table.view(np.int32)).to(torch.device("cuda", self.searcher.segments[0].device))
+        self._joins[seg] = j
+        return j
+
+    def fields(self, bits) -> list:
+        """The matched documents of an index-wide bitset as FieldId(resource, field), segment by segment (FieldUuidCollector)."""
+        from .vector import FieldId
+
+        words = bits.cpu().numpy().view(np.uint64) if hasattr(bits, "cpu") else np.asarray(bits, dtype=np.uint64)
+        out = []
+        for s, off in zip(self.searcher.segments, self.word_off):
+            mask = np.unpackbits(words[off: off + (s.n_docs + 63) // 64].view(np.uint8), bitorder="little")[: s.n_docs].astype(bool)
+            out += [FieldId(_uuid_mod.UUID(s.docs[d].uuid), s.docs[d].field) for d in np.nonzero(mask)[0]]
+        return out
+
+
 def date_sort_key(seconds: Optional[int], order_type: int):
     """Sort key of a date under an order: the requested direction first, documents without a date (None or NIDX_DATE_NONE) last."""
     if seconds is None or seconds == _lib.NIDX_DATE_NONE:
@@ -468,16 +700,10 @@ class ParagraphSearcher(TextSearcher):
     conjunction = False
     use_tf = False
 
-    def __init__(self, segments: Sequence[TextIndexSegment], vocab: dict):
-        super().__init__(segments, vocab)
-        self._positions = False   # uploaded on the first phrase query
-
     def _clauses(self, body: str):
         words, phrases = parse_paragraph_query(body)
         terms = [self.vocab.get(t, 0xFFFFFFF0) for t in words]   # unknown word: matches nothing
         phrase_terms = [[self.vocab.get(t, 0xFFFFFFF0) for t in p] for p in phrases]   # an unknown word: the phrase matches nothing
-        if phrase_terms and not self._positions:
-            for s in self.segments:
-                s._gpu.set_positions(s.positions)
-            self._positions = True
+        if phrase_terms:
+            self._ensure_positions()
         return terms, phrase_terms

@@ -95,10 +95,28 @@ class FieldId:  # nidx_types/src/prefilter.rs
 
 
 class PrefilterResult:
-    """nidx_types/src/prefilter.rs: All | None | Some(fields)."""
+    """nidx_types/src/prefilter.rs: All | None | Some(fields).  A Some made on the device (TextSearcher.prefilter) keeps the matched
+    text documents as a bitset in HBM (`device_bits`: (the text index's prefilter state, the bits, the match count)); its `fields`
+    are listed only when read, and VectorSearcher.search hands the bits to the vector segments without leaving the device."""
 
-    def __init__(self, kind: str, fields: Sequence[FieldId] = ()):
-        self.kind, self.fields = kind, list(fields)
+    def __init__(self, kind: str, fields: Sequence[FieldId] = (), device_bits=None):
+        self.kind, self.device_bits = kind, device_bits
+        self._fields = None if device_bits is not None else list(fields)
+
+    @property
+    def fields(self) -> list:
+        if self._fields is None:
+            index, bits, _ = self.device_bits
+            self._fields = index.fields(bits)
+        return self._fields
+
+    @fields.setter
+    def fields(self, value):
+        self._fields, self.device_bits = list(value), None
+
+    @classmethod
+    def from_device(cls, index, bits, matching: int):
+        return cls("some", device_bits=(index, bits, matching))
 
     @classmethod
     def all(cls):
@@ -380,6 +398,23 @@ class OpenSegment:
         nodes, _, keep = self.formula_nodes(clauses, operator_and) if clauses else (None, 0, None)
         return self.segment.search(queries, top_k, ef, min_score, with_duplicates, method, formula=nodes)
 
+    def search_prefiltered(self, query, prefilter, formula, operator_and, with_duplicates, top_k, min_score, method=_lib.NIDX_METHOD_AUTO, ef=0):
+        """search() restricted by a prefilter made on the device (PrefilterResult.device_bits) instead of a key set: the matched
+        documents' paragraphs (nidx_vec_prefilter_bits through the text index's join table), combined with `formula` under the
+        operator as search() combines its clauses, go to the search as a bitset that never leaves the device."""
+        import torch
+
+        index, doc_bits, _ = prefilter
+        nodes, _, keep = self.formula_nodes([formula]) if formula is not None else (None, 0, None)
+        bits, matching = self.segment.prefilter_bits(doc_bits, index.join(self), index.n_docs_total(), self.records, nodes,
+                                                     _lib.NIDX_F_AND if operator_and else _lib.NIDX_F_OR)
+        if matching == 0:   # segment.rs:532-534: nothing can match
+            return np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.float32)
+        q = torch.as_tensor(np.asarray(query, dtype=np.float32)[None, :]).to(torch.device("cuda", self.config.device))
+        ids, scores, counts = self.segment.search(q, top_k, ef, min_score, with_duplicates, method, filter_bits=bits, filter_matching=matching)
+        c = int(counts[0].item())
+        return ids[0, :c].cpu().numpy().view(np.uint32), scores[0, :c].cpu().numpy()
+
     def _raw_search(self, queries, k, filter_bits):
         """exact scan restricted to a paragraph bitset, no min_score: per (query, paragraph) the best vector's similarity."""
         return self.segment.search(queries, k, 0, float(np.finfo(np.float32).min), True, _lib.NIDX_METHOD_BRUTE, filter_bits=filter_bits)
@@ -443,8 +478,10 @@ class VectorSearcher:
 
     def search(self, request: VectorSearchRequest, prefilter: PrefilterResult = None, method=_lib.NIDX_METHOD_AUTO, ef=0) -> VectorSearchResponse:
         prefilter = prefilter or PrefilterResult.all()
+        multi = self.config.vector_cardinality == VectorCardinality.Multi
+        on_device = prefilter.device_bits if prefilter.kind == "some" and not multi else None
         clauses = []
-        if prefilter.kind == "some":  # searcher.rs:300-314
+        if prefilter.kind == "some" and on_device is None:  # searcher.rs:300-314
             clauses.append(_KeyPrefixSet(frozenset(f"{f.resource_id.hex}{f.field_id}" if f.field_id else f.resource_id.hex for f in prefilter.fields)))
         if request.filtering_formula is not None:
             clauses.append(_map_expression(request.filtering_formula))
@@ -452,7 +489,6 @@ class VectorSearcher:
         query = np.asarray(request.vector, dtype=np.float32)
         if self.config.normalize_vectors and self.config.vector_cardinality != VectorCardinality.Multi:  # searcher.rs:246-252, utils.rs:20-23
             query = normalize(query.copy(), self.config.device)
-        multi = self.config.vector_cardinality == VectorCardinality.Multi
         if (len(query) != self.config.dimension) if not multi else (len(query) % self.config.dimension != 0 or len(query) == 0):
             raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {len(query)}")
         k = request.result_per_page
@@ -463,7 +499,11 @@ class VectorSearcher:
             for seg in self.open_segments:
                 if request.segment_filtering_formula is not None and not _segment_matches(request.segment_filtering_formula, seg.tags):
                     continue
-                addrs, scores = seg.search(query, clauses, operator_and, request.with_duplicates, k, request.min_score, method, ef)
+                if on_device is not None:
+                    addrs, scores = seg.search_prefiltered(query, on_device, request.filtering_formula, operator_and, request.with_duplicates, k,
+                                                           request.min_score, method, ef)
+                else:
+                    addrs, scores = seg.search(query, clauses, operator_and, request.with_duplicates, k, request.min_score, method, ef)
                 for a, s in zip(addrs, scores):
                     p = seg.paragraph_of(int(a))
                     vb = (id(seg), int(a)) if request.with_duplicates else self._vector_bytes(seg, int(a))
