@@ -183,12 +183,15 @@ typedef struct nidx_filter_node {   /* a Formula / Clause tree in pre-order (for
 } nidx_filter_node;
 
 /* ParagraphInvertedIndexes::filter + the intersection with the alive set (segment.rs:516-531): the formula's bitset over the
- * paragraphs, computed in HBM (postings -> bits, bit algebra, popcount).  out_bits (`mem`; (paragraphs + 63) / 64 words) may be NULL;
- * *out_matching = number of set bits (the reference's `bitset.iter().count()`). */
+ * paragraphs, computed in HBM (postings -> bits, then one pass of the formula as a program, ANDed with alive and counted).  out_bits
+ * (`mem`; (paragraphs + 63) / 64 words) may be NULL; *out_matching = number of set bits (the reference's `bitset.iter().count()`).
+ * A formula whose program has more than 4096 instructions is NIDX_EINVAL: the atoms that are operands of one OR are one leaf,
+ * and every other atom, and every operand of an AND / OR / NOT after its first, is one instruction (a NOT adds one more). */
 int nidx_vec_filter(nidx_vec_segment* seg, const nidx_filter_node* nodes, int32_t n_nodes, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
 
 /* nidx_vec_search with the filter given as a formula: evaluated on the device and fed to the search without a host round trip
- * (p->filter_bits must be NULL; NIDX_METHOD_AUTO reads the match count back, 8 bytes, for the cost model as segment.rs:531 does). */
+ * (p->filter_bits must be NULL; NIDX_METHOD_AUTO reads the match count back, 8 bytes, for the cost model as segment.rs:531 does).
+ * The formula has nidx_vec_filter's limit of 4096 instructions. */
 int nidx_vec_search_formula(nidx_vec_segment* seg, const float* queries, int32_t nq, int32_t ldq, int mem, const nidx_vec_search_params* p,
                             const nidx_filter_node* nodes, int32_t n_nodes, uint32_t* out_ids, float* out_scores, int32_t* out_counts, void* stream);
 
@@ -436,7 +439,8 @@ int nidx_txt_prefilter(nidx_txt_segment* seg, const nidx_prefilter_node* nodes, 
  * `mem`) -> the paragraphs of the matched documents' keys; with a filter formula (nodes, n_nodes > 0; nidx_vec_filter's format)
  * combined with it under op (NIDX_F_AND | NIDX_F_OR: SearchRequest.filter_operator), then ANDed with the alive set -> out_bits
  * ((paragraphs + 63) / 64 words, `mem`; may be NULL) and *out_matching (host), to be passed to nidx_vec_search as filter_bits and
- * filter_matching.  The call returns when both are in place. */
+ * filter_matching.  The call returns when both are in place.  The formula has nidx_vec_filter's limit, less two instructions
+ * (the documents' paragraphs and the combination under op). */
 int nidx_vec_prefilter_bits(nidx_vec_segment* seg, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, const nidx_filter_node* nodes,
                             int32_t n_nodes, int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
 

@@ -910,182 +910,205 @@ static scan_kernel_t pick_scan_kernel(int ld) {
     });
 }
 
-// ---- filter formulas on the device (inverted_index/paragraph.rs:124-186) ---------------------------------------------
-// ranges[2r], ranges[2r + 1] = [begin, end) into the postings of one inverted index; one block per range sets the bits
-__global__ void bits_scatter_kernel(const uint32_t* __restrict__ postings, const uint64_t* __restrict__ ranges, uint64_t* __restrict__ out) {
-    uint64_t b = ranges[2 * blockIdx.x], e = ranges[2 * blockIdx.x + 1];
-    for (uint64_t i = b + threadIdx.x; i < e; i += blockDim.x) {
-        uint32_t p = postings[i];
-        atomicOr(reinterpret_cast<unsigned long long*>(out) + (p >> 6), 1ull << (p & 63));
+// ---- filters on the device: running a program of prefilter.cuh ----------------------------------------------------------
+// One run of a compiled program over n_docs documents (A: the document columns the program reads and the alive set; paragraphs have
+// no columns).  w.prefilter holds [n_slots][words] leaf bitsets | the match count | the program | extra_bytes of the caller's leaf
+// data; scatter(slot bits, extra) sets the slots once they are zeroed.  The result goes to out ([words], padding bits zero) and the
+// number of its set bits to *h_count; the caller synchronises before either is read and before the program's storage goes.  A
+// program that is one bitset leaf is ANDed with alive by and_bits_kernel instead of the pass.  ev0 / ev1 (optional) time that kernel or the pass.
+template <class Scatter>
+static int run_program(Workspace& w, cudaStream_t stream, int sm_count, const std::vector<PfOp>& prog, size_t n_slots, PrefilterArgs A,
+                       size_t extra_bytes, Scatter scatter, uint64_t* out, unsigned long long* h_count, cudaEvent_t ev0 = nullptr,
+                       cudaEvent_t ev1 = nullptr) {
+    if (prog.size() > (size_t)PF_MAX_PROGRAM) return fail(NIDX_EINVAL, "the filter program has more than %d instructions", PF_MAX_PROGRAM);
+    const size_t words = A.words;
+    const size_t o_count = (n_slots * words * 8 + 15) & ~(size_t)15, o_prog = o_count + 16, o_extra = o_prog + prog.size() * sizeof(PfOp);
+    ENSURE(w.prefilter, o_extra + extra_bytes);
+    uint64_t* bits = w.prefilter.as<uint64_t>();
+    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(w.prefilter.p + o_count);
+    PfOp* d_prog = reinterpret_cast<PfOp*>(w.prefilter.p + o_prog);
+    CU(cudaMemsetAsync(d_count, 0, 8, stream));
+    if (n_slots && words) {
+        CU(cudaMemsetAsync(bits, 0, n_slots * words * 8, stream));
+        int r = scatter(bits, w.prefilter.p + o_extra);
+        if (r) return r;
     }
-}
-// op 0: a &= b, 1: a |= b, 2: a = ~a (bits beyond n_bits stay clear)
-__global__ void bits_combine_kernel(uint64_t* __restrict__ a, const uint64_t* __restrict__ b, size_t words, uint64_t n_bits, int op) {
-    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < words; i += (size_t)gridDim.x * blockDim.x) {
-        uint64_t v = a[i];
-        if (op == 0) v &= b[i];
-        else if (op == 1) v |= b[i];
-        else {
-            v = ~v;
-            if ((i + 1) * 64 > n_bits) v &= n_bits > i * 64 ? (~0ull >> (64 - (n_bits - i * 64))) : 0ull;
-        }
-        a[i] = v;
+    if (prog.size() == 1 && prog[0].op == PF_BITS) {
+        if (ev0) CU(cudaEventRecord(ev0, stream));
+        and_bits_kernel<<<(unsigned)std::max<size_t>(1, std::min<size_t>((words + 255) / 256, 1024)), 256, 0, stream>>>(
+            bits + (size_t)prog[0].arg * words, A.alive, out, words, d_count);
+    } else {
+        CU(cudaMemcpyAsync(d_prog, prog.data(), prog.size() * sizeof(PfOp), cudaMemcpyHostToDevice, stream));
+        A.kw_bits = bits; A.prog = d_prog; A.n_prog = (uint32_t)prog.size(); A.out = reinterpret_cast<uint32_t*>(out); A.count = d_count;
+        const size_t smem = prog.size() * sizeof(PfOp);
+        CU(cudaFuncSetAttribute(prefilter_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        if (ev0) CU(cudaEventRecord(ev0, stream));
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)sm_count * 8, (2 * words * 32 + PF_THREADS - 1) / PF_THREADS));
+        prefilter_eval_kernel<<<blocks, PF_THREADS, smem, stream>>>(A);
     }
-}
-
-struct FilterEval {
-    nidx_vec_segment* s;
-    const nidx_filter_node* nodes;
-    int n_nodes;
-    uint64_t* bufs;          // [n_nodes + 1][words] device
-    size_t words;
-    cudaStream_t stream;
-    std::vector<uint64_t> ranges;     // all atoms' ranges, uploaded once
-    std::vector<std::pair<size_t, size_t>> atom_ranges;   // per atom node: [first, count) in `ranges`
-    uint64_t* d_ranges = nullptr;
-    int next_buf = 0;
-
-    static int cmp_key(const unsigned char* a, size_t la, const unsigned char* b, size_t lb) {
-        int c = memcmp(a, b, std::min(la, lb));
-        return c ? c : (la < lb ? -1 : (la > lb ? 1 : 0));
-    }
-    // first key >= q
-    static uint32_t lower_bound(const nidx_vec_segment::InvIndex& ix, const unsigned char* q, size_t lq) {
-        uint32_t lo = 0, hi = ix.n_keys;
-        while (lo < hi) {
-            uint32_t mid = (lo + hi) / 2;
-            if (cmp_key(ix.key_bytes.data() + ix.key_off[mid], ix.key_off[mid + 1] - ix.key_off[mid], q, lq) < 0) lo = mid + 1; else hi = mid;
-        }
-        return lo;
-    }
-    // host pass: the key lookups (the fst's job in the reference), in node order
-    int collect(int i) {
-        const nidx_filter_node& nd = nodes[i];
-        if (nd.kind == NIDX_F_LABEL || nd.kind == NIDX_F_KEYS) {
-            const nidx_vec_segment::InvIndex& ix = s->inv[nd.kind == NIDX_F_LABEL ? NIDX_INV_LABELS : NIDX_INV_FIELDS];
-            size_t first = ranges.size() / 2;
-            for (int j = 0; j < nd.n; ++j) {
-                const unsigned char* q = nd.keys[j];
-                size_t lq = nd.key_len[j];
-                uint32_t lo = lower_bound(ix, q, lq), hi = lo;
-                if (nd.kind == NIDX_F_LABEL) {   // get_prefix: every key that starts with q
-                    uint32_t a = lo, b = ix.n_keys;
-                    while (a < b) {
-                        uint32_t mid = (a + b) / 2;
-                        size_t lk = ix.key_off[mid + 1] - ix.key_off[mid];
-                        bool starts = lk >= lq && memcmp(ix.key_bytes.data() + ix.key_off[mid], q, lq) == 0;
-                        if (starts) a = mid + 1; else b = mid;
-                    }
-                    hi = a;
-                } else if (lo < ix.n_keys && cmp_key(ix.key_bytes.data() + ix.key_off[lo], ix.key_off[lo + 1] - ix.key_off[lo], q, lq) == 0) {
-                    hi = lo + 1;                  // get: the exact key
-                }
-                if (hi > lo && ix.post_off[hi] > ix.post_off[lo]) { ranges.push_back(ix.post_off[lo]); ranges.push_back(ix.post_off[hi]); }
-            }
-            atom_ranges[i] = {first, ranges.size() / 2 - first};
-            return i + 1;
-        }
-        int j = i + 1;
-        for (int c = 0; c < nd.n; ++c) { if (j >= n_nodes) return -1; j = collect(j); if (j < 0) return -1; }
-        return j;
-    }
-    // device pass: returns the buffer holding node i's bitset, *next = the node after its subtree
-    uint64_t* eval(int i, int* next) {
-        const nidx_filter_node& nd = nodes[i];
-        uint64_t* out = bufs + (size_t)(next_buf++) * words;
-        if (nd.kind == NIDX_F_LABEL || nd.kind == NIDX_F_KEYS) {
-            cudaMemsetAsync(out, 0, words * 8, stream);
-            auto ar = atom_ranges[i];
-            if (ar.second) {
-                const nidx_vec_segment::InvIndex& ix = s->inv[nd.kind == NIDX_F_LABEL ? NIDX_INV_LABELS : NIDX_INV_FIELDS];
-                bits_scatter_kernel<<<(unsigned)ar.second, 128, 0, stream>>>(ix.d_post, d_ranges + 2 * ar.first, out);
-                LAUNCHED();
-            }
-            *next = i + 1;
-            return out;
-        }
-        int j = i + 1;
-        uint64_t* acc = nullptr;
-        unsigned blocks = (unsigned)std::min<size_t>((words + 255) / 256, 1024);
-        for (int c = 0; c < nd.n; ++c) {
-            int nx;
-            uint64_t* child = eval(j, &nx);
-            j = nx;
-            if (!acc) { cudaMemcpyAsync(out, child, words * 8, cudaMemcpyDeviceToDevice, stream); acc = out; }
-            else {
-                bits_combine_kernel<<<blocks, 256, 0, stream>>>(acc, child, words, s->n_par, nd.kind == NIDX_F_OR ? 1 : 0);   // Not | And => intersect (paragraph.rs:160-164)
-                LAUNCHED();
-            }
-        }
-        if (nd.kind == NIDX_F_NOT) { bits_combine_kernel<<<blocks, 256, 0, stream>>>(acc, nullptr, words, s->n_par, 2); LAUNCHED(); }
-        *next = j;
-        return acc;
-    }
-};
-
-// The layout of w.filter: [words] filter ∧ alive | 8 words: its match count | [n_nodes + 1][words] a formula's node bitsets | the
-// formula's posting ranges (range_bytes).  Sized for a formula of n_nodes nodes (0: none).
-struct FilterBufs {
-    size_t words;
-    uint64_t* bits;
-    unsigned long long* count;
-    uint64_t* nodes;
-    uint64_t* ranges;
-};
-static int filter_bufs(const nidx_vec_segment* s, Workspace& w, int n_nodes, size_t range_bytes, FilterBufs& f) {
-    f.words = ((size_t)s->n_par + 63) / 64;
-    const size_t node_words = n_nodes ? ((size_t)n_nodes + 1) * f.words : 0;
-    ENSURE(w.filter, (f.words + 8 + node_words) * 8 + range_bytes);
-    f.bits = w.filter.as<uint64_t>();
-    f.count = reinterpret_cast<unsigned long long*>(f.bits + f.words);
-    f.nodes = f.bits + f.words + 8;
-    f.ranges = f.nodes + node_words;
+    LAUNCHED();
+    if (ev1) CU(cudaEventRecord(ev1, stream));
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(h_count, d_count, 8, cudaMemcpyDeviceToHost, stream));
     return 0;
 }
 
-// filter ∧ alive (segment.rs:516-534) into `out` (NULL: the workspace's filter bits), returned in *bits.  With h_count, the number of
+static int cmp_key(const unsigned char* a, size_t la, const unsigned char* b, size_t lb) {
+    int c = memcmp(a, b, std::min(la, lb));
+    return c ? c : (la < lb ? -1 : (la > lb ? 1 : 0));
+}
+// The postings [*b, *e) of key q: get_prefix (every key that starts with q) for the label index, get (the exact key) for the fields
+static void key_postings(const nidx_vec_segment::InvIndex& ix, bool prefix, const unsigned char* q, size_t lq, uint64_t* b, uint64_t* e) {
+    uint32_t lo = 0, hi = ix.n_keys;
+    while (lo < hi) {   // the first key >= q
+        uint32_t mid = (lo + hi) / 2;
+        if (cmp_key(ix.key_bytes.data() + ix.key_off[mid], ix.key_off[mid + 1] - ix.key_off[mid], q, lq) < 0) lo = mid + 1; else hi = mid;
+    }
+    if (prefix) {
+        for (uint32_t c = ix.n_keys; hi < c;) {
+            uint32_t mid = (hi + c) / 2;
+            size_t lk = ix.key_off[mid + 1] - ix.key_off[mid];
+            if (lk >= lq && memcmp(ix.key_bytes.data() + ix.key_off[mid], q, lq) == 0) hi = mid + 1; else c = mid;
+        }
+    } else if (lo < ix.n_keys && cmp_key(ix.key_bytes.data() + ix.key_off[lo], ix.key_off[lo + 1] - ix.key_off[lo], q, lq) == 0) {
+        hi = lo + 1;
+    }
+    *b = ix.post_off[lo]; *e = ix.post_off[hi];
+}
+
+// ParagraphInvertedIndexes::filter (inverted_index/paragraph.rs:124-186) as a program over the segment's paragraphs.  The key lookups
+// (the fst's job in the reference) run here; every atom that finds postings is a bitset leaf whose ranges set its slot, and the
+// atoms that are operands of one OR share a slot (the union of their ranges is the OR).  An atom without postings is the constant 0.
+// AND / OR of n operands are n - 1 binary ops, NOT the complement of its operands' intersection (paragraph.rs:160-178).  Operands
+// are emitted heaviest first (Sethi-Ullman), so the bit stack never holds more than log2(leaves) + 1 entries.
+struct FormulaPlan {
+    const nidx_vec_segment* s = nullptr;
+    const nidx_filter_node* nodes = nullptr;
+    int n_nodes = 0;
+    uint32_t slots = 0;                                  // slots below the first one the formula takes belong to the caller
+    std::vector<uint64_t> ranges[2];                     // per inverted index (NIDX_INV_*): [2 r] posting ranges
+    std::vector<uint32_t> range_slot[2];                 // and the slot each one sets
+    std::vector<PfOp> prog;
+
+    static bool atom(const nidx_filter_node& nd) { return nd.kind == NIDX_F_LABEL || nd.kind == NIDX_F_KEYS; }
+    static PfOp leaf(int slot) {   // slot < 0: no postings
+        PfOp o{};
+        o.op = slot >= 0 ? PF_BITS : PF_CONST;
+        o.arg = slot >= 0 ? (uint32_t)slot : 0;
+        return o;
+    }
+    // the atom's ranges into `slot`; false when it has no postings
+    bool lookup(const nidx_filter_node& nd, uint32_t slot) {
+        const int which = nd.kind == NIDX_F_LABEL ? NIDX_INV_LABELS : NIDX_INV_FIELDS;
+        bool any = false;
+        for (int j = 0; j < nd.n; ++j) {
+            uint64_t b, e;
+            key_postings(s->inv[which], nd.kind == NIDX_F_LABEL, nd.keys[j], nd.key_len[j], &b, &e);
+            if (e > b) { ranges[which].push_back(b); ranges[which].push_back(e); range_slot[which].push_back(slot); any = true; }
+        }
+        return any;
+    }
+    // the subtree at node i -> its program (code) and the bit stack entries it needs; returns the node after it, or -1 when the
+    // operand counts do not add up
+    int plan(int i, std::vector<PfOp>& code, int& need) {
+        const nidx_filter_node& nd = nodes[i];
+        need = 1;
+        if (atom(nd)) { code.assign(1, leaf(lookup(nd, slots) ? (int)slots++ : -1)); return i + 1; }
+        std::vector<std::pair<int, std::vector<PfOp>>> v;   // the operands: need, code
+        int or_slot = -1, j = i + 1;                        // or_slot: the slot of this OR's atoms
+        bool or_atoms = false;
+        for (int c = 0; c < nd.n; ++c) {
+            if (j >= n_nodes) return -1;
+            if (nd.kind == NIDX_F_OR && atom(nodes[j])) {
+                or_atoms = true;
+                if (lookup(nodes[j++], or_slot >= 0 ? (uint32_t)or_slot : slots) && or_slot < 0) or_slot = (int)slots++;
+                continue;
+            }
+            v.emplace_back();
+            j = plan(j, v.back().second, v.back().first);
+            if (j < 0) return -1;
+        }
+        if (or_atoms) v.push_back({1, {leaf(or_slot)}});
+        std::stable_sort(v.begin(), v.end(), [](const auto& a, const auto& b) { return a.first > b.first; });
+        need = v.size() > 1 ? std::max(v[0].first, v[1].first + 1) : v[0].first;
+        code = std::move(v[0].second);
+        PfOp op{};
+        op.op = nd.kind == NIDX_F_OR ? PF_OR : PF_AND;   // Not | And => intersect (paragraph.rs:160-164)
+        for (size_t c = 1; c < v.size(); ++c) {
+            code.insert(code.end(), v[c].second.begin(), v[c].second.end());
+            code.push_back(op);
+        }
+        if (nd.kind == NIDX_F_NOT) { op.op = PF_NOT; code.push_back(op); }
+        return j;
+    }
+    int compile(const nidx_vec_segment* seg, const nidx_filter_node* nd, int n) {
+        s = seg; nodes = nd; n_nodes = n;
+        if (!nodes || n_nodes <= 0) return fail(NIDX_EINVAL, "empty filter formula");
+        for (int i = 0; i < n_nodes; ++i) {
+            int kd = nodes[i].kind;
+            if (kd < NIDX_F_LABEL || kd > NIDX_F_NOT || nodes[i].n < 0) return fail(NIDX_EINVAL, "filter node %d: bad kind / count", i);
+            if ((kd == NIDX_F_LABEL || kd == NIDX_F_KEYS) && nodes[i].n > 0 && (!nodes[i].keys || !nodes[i].key_len)) return fail(NIDX_EINVAL, "filter node %d: null keys", i);
+            if ((kd == NIDX_F_AND || kd == NIDX_F_OR || kd == NIDX_F_NOT) && nodes[i].n < 1) return fail(NIDX_EINVAL, "filter node %d: a compound clause needs operands", i);
+        }
+        int need;
+        if (plan(0, prog, need) != n_nodes) return fail(NIDX_EINVAL, "malformed filter formula (operand counts do not add up to %d nodes)", n_nodes);
+        // at most log2(leaves) + 1 <= 13 within the program limit; one entry stays free for nidx_vec_prefilter_bits' combination
+        if (need >= PF_MAX_DEPTH) return fail(NIDX_EINVAL, "the filter formula needs more than %d bit stack entries", PF_MAX_DEPTH - 1);
+        return 0;
+    }
+    // leaf data in w.prefilter after the program: the ranges of both indexes, then their slots
+    size_t extra_bytes() const { return (range_slot[0].size() + range_slot[1].size()) * 20; }
+    int scatter(uint64_t* bits, unsigned char* extra, size_t words, cudaStream_t stream) const {
+        const size_t n0 = range_slot[0].size(), n = n0 + range_slot[1].size();
+        if (!n) return 0;
+        uint64_t* d_ranges = reinterpret_cast<uint64_t*>(extra);
+        uint32_t* d_slot = reinterpret_cast<uint32_t*>(extra + n * 16);
+        for (int which = 0, at = 0; which < 2; at += (int)range_slot[which++].size()) {
+            if (range_slot[which].empty()) continue;
+            CU(cudaMemcpyAsync(d_ranges + 2 * at, ranges[which].data(), range_slot[which].size() * 16, cudaMemcpyHostToDevice, stream));
+            CU(cudaMemcpyAsync(d_slot + at, range_slot[which].data(), range_slot[which].size() * 4, cudaMemcpyHostToDevice, stream));
+        }
+        prefilter_scatter_kernel<<<(unsigned)n, 256, 0, stream>>>(s->inv[NIDX_INV_LABELS].d_post.p, s->inv[NIDX_INV_FIELDS].d_post.p, (uint32_t)n0, nullptr,
+                                                                   0, nullptr, d_ranges, d_slot, 0, bits, words);
+        LAUNCHED();
+        return 0;
+    }
+};
+
+static PrefilterArgs paragraph_args(const nidx_vec_segment* s) {
+    PrefilterArgs A{};
+    A.n_docs = (uint32_t)s->n_par; A.words = ((size_t)s->n_par + 63) / 64; A.alive = s->d_alive;
+    return A;
+}
+
+// filter ∧ alive (segment.rs:516-534) into w.filter ([words] bits | its match count), returned in *bits.  With h_count, the number of
 // set bits is copied back to it (the caller synchronises).
-static int filter_and_alive(nidx_vec_segment* s, Workspace& w, const uint64_t* filter, uint64_t* out, unsigned long long* h_count, cudaStream_t stream,
+static int filter_and_alive(nidx_vec_segment* s, Workspace& w, const uint64_t* filter, unsigned long long* h_count, cudaStream_t stream,
                             const uint64_t** bits) {
-    FilterBufs f;
-    int r = filter_bufs(s, w, 0, 0, f);
-    if (r) return r;
-    if (!out) out = f.bits;
-    CU(cudaMemsetAsync(f.count, 0, 8, stream));
-    and_bits_kernel<<<std::min<size_t>((f.words + 255) / 256, 1024), 256, 0, stream>>>(filter, s->d_alive, out, f.words, f.count);
+    const size_t words = ((size_t)s->n_par + 63) / 64;
+    ENSURE(w.filter, (words + 8) * 8);
+    uint64_t* out = w.filter.as<uint64_t>();
+    unsigned long long* count = reinterpret_cast<unsigned long long*>(out + words);
+    CU(cudaMemsetAsync(count, 0, 8, stream));
+    and_bits_kernel<<<std::min<size_t>((words + 255) / 256, 1024), 256, 0, stream>>>(filter, s->d_alive, out, words, count);
     LAUNCHED();
-    if (h_count) CU(cudaMemcpyAsync(h_count, f.count, 8, cudaMemcpyDeviceToHost, stream));
+    if (h_count) CU(cudaMemcpyAsync(h_count, count, 8, cudaMemcpyDeviceToHost, stream));
     *bits = out;
     return 0;
 }
 
-// ParagraphInvertedIndexes::filter on the device: nodes (pre-order; several top-level nodes are not allowed: wrap them in an AND /
-// OR node) -> bitset among the node buffers of `w.filter`, returns the device pointer in *out
-static int filter_formula_device(nidx_vec_segment* s, Workspace& w, const nidx_filter_node* nodes, int n_nodes, cudaStream_t stream, uint64_t** out) {
-    if (!nodes || n_nodes <= 0) return fail(NIDX_EINVAL, "empty filter formula");
-    size_t words = ((size_t)s->n_par + 63) / 64;
-    for (int i = 0; i < n_nodes; ++i) {
-        int kd = nodes[i].kind;
-        if (kd < NIDX_F_LABEL || kd > NIDX_F_NOT || nodes[i].n < 0) return fail(NIDX_EINVAL, "filter node %d: bad kind / count", i);
-        if ((kd == NIDX_F_LABEL || kd == NIDX_F_KEYS) && nodes[i].n > 0 && (!nodes[i].keys || !nodes[i].key_len)) return fail(NIDX_EINVAL, "filter node %d: null keys", i);
-        if ((kd == NIDX_F_AND || kd == NIDX_F_OR || kd == NIDX_F_NOT) && nodes[i].n < 1) return fail(NIDX_EINVAL, "filter node %d: a compound clause needs operands", i);
-    }
-    FilterEval ev;
-    ev.s = s; ev.nodes = nodes; ev.n_nodes = n_nodes; ev.words = words; ev.stream = stream;
-    ev.atom_ranges.assign(n_nodes, {0, 0});
-    if (ev.collect(0) != n_nodes) return fail(NIDX_EINVAL, "malformed filter formula (operand counts do not add up to %d nodes)", n_nodes);
-    size_t range_bytes = ev.ranges.size() * 8;
-    FilterBufs f;
-    int r = filter_bufs(s, w, n_nodes, range_bytes, f);
+// ParagraphInvertedIndexes::filter ∧ alive on the device (segment.rs:516-531): nodes (pre-order; several top-level nodes are not
+// allowed: wrap them in an AND / OR node) -> out, the number of matches -> *h_count.  Returns with the stream synchronised.
+static int filter_formula(nidx_vec_segment* s, Workspace& w, const nidx_filter_node* nodes, int n_nodes, cudaStream_t stream, uint64_t* out,
+                          unsigned long long* h_count) {
+    FormulaPlan P;
+    int r = P.compile(s, nodes, n_nodes);
     if (r) return r;
-    ev.bufs = f.nodes;
-    ev.d_ranges = f.ranges;
-    if (range_bytes) CU(cudaMemcpyAsync(ev.d_ranges, ev.ranges.data(), range_bytes, cudaMemcpyHostToDevice, stream));
-    int next = 0;
-    uint64_t* res = ev.eval(0, &next);
-    CU(cudaGetLastError());
-    if (range_bytes) CU(cudaStreamSynchronize(stream));   // `ranges` is a host temporary
-    *out = res;
+    const PrefilterArgs A = paragraph_args(s);
+    r = run_program(w, stream, s->sm_count, P.prog, P.slots, A, P.extra_bytes(),
+                    [&](uint64_t* bits, unsigned char* extra) { return P.scatter(bits, extra, A.words, stream); }, out, h_count);
+    if (r) return r;
+    CU(cudaStreamSynchronize(stream));   // the program and the ranges are host temporaries
     return 0;
 }
 
@@ -1381,16 +1404,17 @@ static int vec_search_impl(nidx_vec_segment* s, const float* queries, int32_t nq
     // filter ∧ alive (segment.rs:516-534)
     c.bits = s->d_alive;
     uint64_t matching = s->d_alive ? s->alive_count : s->n_par;
-    if (d_filter || formula) {
-        if (formula) {   // the formula is evaluated on the device (inverted_index/paragraph.rs:124-186): no host bitset, no copy
-            uint64_t* fdev = nullptr;
-            r = filter_formula_device(s, w, formula, n_formula, stream, &fdev);
-            if (r) return r;
-            d_filter = fdev;
-        }
-        matching = formula ? 0 : p->filter_matching;
+    if (formula) {   // the formula is evaluated on the device (inverted_index/paragraph.rs:124-186): no host bitset, no copy
+        ENSURE(w.filter, ((size_t)s->n_par + 63) / 64 * 8);
         unsigned long long h = 0;   // segment.rs:531: the reference counts the matches of every filtered request (8 bytes back, one sync)
-        r = filter_and_alive(s, w, d_filter, nullptr, matching ? nullptr : &h, stream, &c.bits);
+        r = filter_formula(s, w, formula, n_formula, stream, w.filter.as<uint64_t>(), &h);
+        if (r) return r;
+        c.bits = w.filter.as<uint64_t>();
+        matching = h;
+    } else if (d_filter) {
+        matching = p->filter_matching;
+        unsigned long long h = 0;
+        r = filter_and_alive(s, w, d_filter, matching ? nullptr : &h, stream, &c.bits);
         if (r) return r;
         if (matching == 0) {
             CU(cudaStreamSynchronize(stream));
@@ -1435,7 +1459,7 @@ int nidx_vec_set_inverted_index(nidx_vec_segment* s, int32_t which, uint32_t n_k
     nidx_vec_segment::InvIndex ix;
     if (!n_keys) { ix.key_off.assign(1, 0); ix.post_off.assign(1, 0); s->inv[which] = std::move(ix); return 0; }
     for (uint32_t i = 0; i + 1 < n_keys; ++i)
-        if (FilterEval::cmp_key(key_bytes + key_off[i], key_off[i + 1] - key_off[i], key_bytes + key_off[i + 1], key_off[i + 2] - key_off[i + 1]) >= 0)
+        if (cmp_key(key_bytes + key_off[i], key_off[i + 1] - key_off[i], key_bytes + key_off[i + 1], key_off[i + 2] - key_off[i + 1]) >= 0)
             return fail(NIDX_EINVAL, "inverted index keys must be strictly ascending (key %u)", i + 1);
     uint64_t np = post_off[n_keys];
     for (uint64_t i = 0; i < np; ++i) if (postings[i] >= s->n_par) return fail(NIDX_EINVAL, "posting %llu: paragraph %u out of range", (unsigned long long)i, postings[i]);
@@ -1462,11 +1486,8 @@ int nidx_vec_filter(nidx_vec_segment* s, const nidx_filter_node* nodes, int32_t 
     uint64_t* d_bits;
     st.out(out_bits, ((size_t)s->n_par + 63) / 64, &d_bits);
     int r = st.place(w.stage);
-    uint64_t* fdev = nullptr;
-    if (!r) r = filter_formula_device(s, w, nodes, n_nodes, stream, &fdev);
     unsigned long long h = 0;
-    const uint64_t* bits;
-    if (!r) r = filter_and_alive(s, w, fdev, d_bits, &h, stream, &bits);   // segment.rs:523-526: intersect with the alive set
+    if (!r) r = filter_formula(s, w, nodes, n_nodes, stream, d_bits, &h);   // segment.rs:523-526: intersect with the alive set
     if (!r) r = st.finish(true);
     if (r) return r;
     if (out_matching) *out_matching = h;
@@ -2665,7 +2686,6 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
     r = P.compile(nodes, n_nodes, at, 1);
     if (r) return r;
     if (at != n_nodes) return fail(NIDX_EINVAL, "malformed prefilter expression (operand counts do not add up to %d nodes)", n_nodes);
-    if (P.prog.size() > (size_t)PF_MAX_PROGRAM) return fail(NIDX_EINVAL, "the prefilter program has more than %d instructions", PF_MAX_PROGRAM);
     if (P.facets && !t->d_fdoc_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
     if (P.columns && !t->d_res_ord) return fail(NIDX_ESTATE, "the segment has no document columns (nidx_txt_set_doc_columns)");
     if ((P.dates[0] && !t->d_secs[0]) || (P.dates[1] && !t->d_secs[1])) return fail(NIDX_ESTATE, "the segment has no dates (nidx_txt_set_dates)");
@@ -2684,53 +2704,37 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
     st.out(out_bits, words, &d_out);
     r = st.place(w.stage);
     if (r) return r;
-    // w.prefilter: [slots][words] keyword bitsets | match count | program | term leaves
-    const size_t o_count = (slots * words * 8 + 15) & ~(size_t)15, o_prog = o_count + 16, o_terms = o_prog + P.prog.size() * sizeof(PfOp);
-    ENSURE(w.prefilter, o_terms + std::max<size_t>(n_terms, 1) * 4);
-    unsigned char* base = w.prefilter.p;
-    uint64_t* kw = reinterpret_cast<uint64_t*>(base);
-    unsigned long long* d_count = reinterpret_cast<unsigned long long*>(base + o_count);
-    PfOp* d_prog = reinterpret_cast<PfOp*>(base + o_prog);
-    uint32_t* d_terms = reinterpret_cast<uint32_t*>(base + o_terms);
-    CU(cudaMemsetAsync(d_count, 0, 8, stream));
-    CU(cudaMemcpyAsync(d_prog, P.prog.data(), P.prog.size() * sizeof(PfOp), cudaMemcpyHostToDevice, stream));
-    if (slots && words) CU(cudaMemsetAsync(kw, 0, slots * words * 8, stream));
-    if (n_terms && words) {
-        CU(cudaMemcpyAsync(d_terms, P.terms.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice, stream));
-        prefilter_scatter_kernel<<<n_terms, 256, 0, stream>>>(t->d_post, t->d_term_off, t->n_terms, d_terms, nullptr, 0, kw, words);
-        LAUNCHED();
-    }
-    PhrasePlan pp;
-    if (nv && words) {   // the phrases' virtual lists (phrase.cuh), as the keyword search makes them, then scattered like terms
-        const int32_t nq = (int32_t)((nv + BM_MAX_TERMS - 1) / BM_MAX_TERMS);
-        const std::vector<uint32_t> no_terms(nq + 1, 0);
-        const nidx_txt_phrases ph{P.ph_terms.data(), P.ph_off.data(), P.ph_query.data(), (int32_t)nv};
-        r = phrase_plan(t, &ph, nq, no_terms, pp);
-        if (r) return r;
-        TxtDev T;
-        T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
-        T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
-        Bm25Args a{};
-        r = phrase_pass(t, pp, T, w, stream, a);
-        if (r) return r;
-        prefilter_scatter_kernel<<<nv, 256, 0, stream>>>(a.ph_post, nullptr, 0, nullptr, a.ph_range, n_terms, kw, words);
-        LAUNCHED();
-    }
-    PrefilterArgs A;
+    PrefilterArgs A{};
     A.n_docs = t->n_docs; A.res_ord = t->d_res_ord; A.field_ord = t->d_field_ord; A.fdoc_off = t->d_fdoc_off; A.ford = t->d_ford;
-    A.secs0 = t->d_secs[0]; A.secs1 = t->d_secs[1]; A.kw_bits = kw; A.words = words; A.alive = t->d_alive;
-    A.prog = d_prog; A.n_prog = (uint32_t)P.prog.size(); A.out = reinterpret_cast<uint32_t*>(d_out); A.count = d_count;
-    const size_t smem = P.prog.size() * sizeof(PfOp);
-    CU(cudaFuncSetAttribute(prefilter_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)t->sm_count * 8, (2 * words * 32 + PF_THREADS - 1) / PF_THREADS));
-    CU(cudaEventRecord(t->ev_k0, stream));
-    prefilter_eval_kernel<<<blocks, PF_THREADS, smem, stream>>>(A);
-    CU(cudaEventRecord(t->ev_k1, stream));
-    LAUNCHED();
-    CU(cudaGetLastError());
+    A.secs0 = t->d_secs[0]; A.secs1 = t->d_secs[1]; A.words = words; A.alive = t->d_alive;
+    PhrasePlan pp;
+    auto scatter = [&](uint64_t* kw, unsigned char* extra) -> int {   // keyword leaves: terms first, then phrases
+        if (n_terms) {
+            uint32_t* d_terms = reinterpret_cast<uint32_t*>(extra);
+            CU(cudaMemcpyAsync(d_terms, P.terms.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice, stream));
+            prefilter_scatter_kernel<<<n_terms, 256, 0, stream>>>(t->d_post.p, t->d_post.p, n_terms, t->d_term_off, t->n_terms, d_terms, nullptr, nullptr, 0, kw, words);
+            LAUNCHED();
+        }
+        if (nv) {   // the phrases' virtual lists (phrase.cuh), as the keyword search makes them, then scattered like terms
+            const int32_t nq = (int32_t)((nv + BM_MAX_TERMS - 1) / BM_MAX_TERMS);
+            const std::vector<uint32_t> no_terms(nq + 1, 0);
+            const nidx_txt_phrases ph{P.ph_terms.data(), P.ph_off.data(), P.ph_query.data(), (int32_t)nv};
+            int r = phrase_plan(t, &ph, nq, no_terms, pp);
+            if (r) return r;
+            TxtDev T;
+            T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
+            T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
+            Bm25Args a{};
+            r = phrase_pass(t, pp, T, w, stream, a);
+            if (r) return r;
+            prefilter_scatter_kernel<<<nv, 256, 0, stream>>>(a.ph_post, a.ph_post, nv, nullptr, 0, nullptr, a.ph_range, nullptr, n_terms, kw, words);
+            LAUNCHED();
+        }
+        return 0;
+    };
     unsigned long long h = 0;
-    CU(cudaMemcpyAsync(&h, d_count, 8, cudaMemcpyDeviceToHost, stream));
-    r = st.finish(true);   // the program and the plans are host temporaries, and the count is read back
+    r = run_program(w, stream, t->sm_count, P.prog, slots, A, (size_t)n_terms * 4, scatter, d_out, &h, t->ev_k0, t->ev_k1);
+    if (!r) r = st.finish(true);   // the program and the plans are host temporaries, and the count is read back
     if (r) return r;
     if (out_matching) *out_matching = h;
     return 0;
@@ -2758,27 +2762,27 @@ int nidx_vec_prefilter_bits(nidx_vec_segment* s, const uint64_t* doc_bits, uint6
     st.out(out_bits, words, &d_out);
     r = st.place(w.stage);
     if (r) return r;
-    ENSURE(w.prefilter, std::max<size_t>(words, 1) * 8);
-    uint64_t* acc = w.prefilter.as<uint64_t>();
-    if (words) CU(cudaMemsetAsync(acc, 0, words * 8, stream));
-    const nidx_vec_segment::InvIndex& ix = s->inv[NIDX_INV_FIELDS];
-    if (n_docs && ix.n_keys) {
-        const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_docs + 255) / 256));
-        prefilter_join_kernel<<<blocks, 256, 0, stream>>>(d_doc, d_join, n_docs, ix.n_keys, ix.d_post_off, ix.d_post, acc);
-        LAUNCHED();
-    }
+    // the program: slot 0 (the matched documents' paragraphs), combined with the formula under op
+    FormulaPlan P;
+    P.slots = 1;
     if (n_nodes) {   // the paragraph formula (segment.rs:516-534), combined as the reference combines its clauses
-        uint64_t* fdev = nullptr;
-        r = filter_formula_device(s, w, nodes, n_nodes, stream, &fdev);
+        r = P.compile(s, nodes, n_nodes);
         if (r) return r;
-        bits_combine_kernel<<<(unsigned)std::min<size_t>(std::max<size_t>((words + 255) / 256, 1), 1024), 256, 0, stream>>>(acc, fdev, words, s->n_par,
-                                                                                                                        op == NIDX_F_OR ? 1 : 0);
-        LAUNCHED();
     }
+    P.prog.insert(P.prog.begin(), FormulaPlan::leaf(0));
+    if (n_nodes) { PfOp b{}; b.op = op == NIDX_F_OR ? PF_OR : PF_AND; P.prog.push_back(b); }
+    const nidx_vec_segment::InvIndex& ix = s->inv[NIDX_INV_FIELDS];
+    auto scatter = [&](uint64_t* bits, unsigned char* extra) -> int {
+        if (n_docs && ix.n_keys) {
+            const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_docs + 255) / 256));
+            prefilter_join_kernel<<<blocks, 256, 0, stream>>>(d_doc, d_join, n_docs, ix.n_keys, ix.d_post_off, ix.d_post, bits);
+            LAUNCHED();
+        }
+        return P.scatter(bits, extra, words, stream);
+    };
     unsigned long long h = 0;
-    const uint64_t* bits;
-    r = words ? filter_and_alive(s, w, acc, d_out, &h, stream, &bits) : 0;   // an empty segment: no words, nothing matches
-    if (!r) r = st.finish(true);
+    r = run_program(w, stream, s->sm_count, P.prog, P.slots, paragraph_args(s), P.extra_bytes(), scatter, d_out, &h);
+    if (!r) r = st.finish(true);   // the program and the ranges are host temporaries, and the count is read back
     if (r) return r;
     if (out_matching) *out_matching = h;
     return 0;

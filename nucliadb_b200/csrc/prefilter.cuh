@@ -1,16 +1,24 @@
-// nidx_b200 — the prefilter of a filtered search on the device (sm_90a).
+// nidx_b200 — boolean filters on the device (sm_90a): one evaluator, two front ends.
 //
-// Replaces nidx_text's TextReaderService::prefilter (nidx_text/src/reader.rs:147-180: filter_to_query over every document, the
-// FieldUuidCollector) and the host key set it hands to the vector search (nidx_vector/src/searcher.rs:300-314).
-//   prefilter_scatter_kernel  keyword leaves, before the pass: one CTA per leaf sets the bits of a posting list (a term's, or a
-//                             phrase's virtual list from phrase.cuh) in the leaf's document bitset;
-//   prefilter_eval_kernel     one pass over the documents: a warp covers 32 consecutive documents, every lane runs the program (the
-//                             expression in post-order, in shared memory) for its own document on a bit stack held in a register;
-//                             the warp's ballot is one 32-bit word of the result, ANDed with the alive bits, and counted;
+// A filter is a program: its leaves and binary AND / OR in post-order, NOT flipping the top of the bit stack (PfOp).  Two front ends
+// compile into it (api.cu):
+//   the prefilter      nidx_txt_prefilter, an expression over a text segment's documents (nidx_text/src/reader.rs:147-180:
+//                      filter_to_query over every document, the FieldUuidCollector); its leaves read the document columns or, for
+//                      keywords, a bitset slot;
+//   paragraph formulas nidx_vec_filter / nidx_vec_search_formula / nidx_vec_prefilter_bits, a formula over a vector segment's
+//                      paragraphs (inverted_index/paragraph.rs:124-186); its leaves are bitset slots set from the label and field
+//                      postings, looked up on the host.
+// One run: the slots are zeroed, set by the scatter kernels, and the program is evaluated over the documents, ANDed with the alive
+// set and counted.
+//   prefilter_scatter_kernel  before the pass: one CTA per posting range (a term's list, a phrase's virtual list from phrase.cuh,
+//                             or a paragraph leaf's range) sets its documents in the range's slot;
+//   prefilter_eval_kernel     one pass over the documents: a warp covers 32 consecutive documents, every lane runs the program (in
+//                             shared memory) for its own document on a bit stack held in a register; the warp's ballot is one 32-bit
+//                             word of the result, ANDed with the alive bits, and counted;
 //   prefilter_join_kernel     text documents -> paragraphs of one vector segment: every matched document with a join entry sets the
 //                             paragraphs of that field key (the NIDX_INV_FIELDS postings).
 // HBM traffic of the pass = per document the columns the program reads (4 B per ord column, 8 B per date column, the facet CSR
-// entry and ords) + 1/8 B of alive bits + 1/8 B per keyword leaf + 1/8 B of output.
+// entry and ords) + 1/8 B of alive bits + 1/8 B per bitset leaf + 1/8 B of output.
 #pragma once
 #include <cstdint>
 
@@ -98,10 +106,16 @@ __global__ void __launch_bounds__(PF_THREADS) prefilter_eval_kernel(PrefilterArg
     if (lane == 0 && local) atomicAdd(A.count, local);
 }
 
-// One CTA per keyword leaf (slot0 + blockIdx.x): terms != NULL -> the posting list of terms[blockIdx.x] (none when the id is not a
-// term of the segment), else the range ranges[2 blockIdx.x .. +1] of `post` (a phrase's compacted virtual list).
-__global__ void prefilter_scatter_kernel(const uint2* __restrict__ post, const uint64_t* __restrict__ term_off, uint32_t n_terms,
-                                         const uint32_t* __restrict__ terms, const uint64_t* __restrict__ ranges, uint32_t slot0,
+__device__ __forceinline__ uint32_t pf_doc(const uint2* p) { return __ldg(&p->x); }   // a text posting: (doc, tf)
+__device__ __forceinline__ uint32_t pf_doc(const uint32_t* p) { return __ldg(p); }   // a paragraph posting
+
+// One CTA per posting range, which sets slot (slot ? slot[blockIdx.x] : slot0 + blockIdx.x): terms != NULL -> the posting list of
+// terms[blockIdx.x] in `post` (none when the id is not a term of the segment), else the range ranges[2 blockIdx.x .. +1] of `post`
+// for the first n_post ranges and of `post1` for the rest.
+template <typename Post>
+__global__ void prefilter_scatter_kernel(const Post* __restrict__ post, const Post* __restrict__ post1, uint32_t n_post,
+                                         const uint64_t* __restrict__ term_off, uint32_t n_terms, const uint32_t* __restrict__ terms,
+                                         const uint64_t* __restrict__ ranges, const uint32_t* __restrict__ slot, uint32_t slot0,
                                          uint64_t* __restrict__ bits, size_t words) {
     uint64_t b, e;
     if (terms) {
@@ -111,9 +125,11 @@ __global__ void prefilter_scatter_kernel(const uint2* __restrict__ post, const u
     } else {
         b = ranges[2 * blockIdx.x]; e = ranges[2 * blockIdx.x + 1];
     }
-    unsigned long long* out = reinterpret_cast<unsigned long long*>(bits + (size_t)(slot0 + blockIdx.x) * words);
+    if (blockIdx.x >= n_post) post = post1;
+    const uint32_t sl = slot ? slot[blockIdx.x] : slot0 + blockIdx.x;
+    unsigned long long* out = reinterpret_cast<unsigned long long*>(bits + (size_t)sl * words);
     for (uint64_t i = b + threadIdx.x; i < e; i += blockDim.x) {
-        const uint32_t doc = __ldg(&post[i].x);
+        const uint32_t doc = pf_doc(post + i);
         atomicOr(out + (doc >> 6), 1ull << (doc & 63));
     }
 }

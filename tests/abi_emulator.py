@@ -201,7 +201,7 @@ class EmulatedLib:
         s.g = O.hnsw_extend(s.v, g0, sim=s.sim, efC=s.efc, seed=_v(seed), max_batch=mb, nthreads=4)
         return 0
 
-    # ---- filters on the "device" (api.cu filter_formula_device restated with numpy) --------------------------------------------
+    # ---- filters on the "device" (api.cu filter_formula restated with numpy) --------------------------------------------
     def nidx_vec_set_inverted_index(self, h, which, n_keys, key_bytes, key_off, post_off, postings):
         s, which, n = self._get(h), _v(which), _v(n_keys)
         ko = _arr(key_off, np.uint64, n + 1) if n else np.zeros(1, np.uint64)
