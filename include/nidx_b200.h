@@ -262,7 +262,19 @@ int nidx_txt_create(int32_t device, uint32_t n_docs, uint32_t n_terms, const uin
  * doc_freq[n_terms].  Defaults to the segment's own statistics. */
 int nidx_txt_set_stats(nidx_txt_segment* seg, uint64_t total_docs, uint64_t total_tokens, const uint64_t* doc_freq);
 int nidx_txt_set_alive(nidx_txt_segment* seg, const uint64_t* alive_bits);
+/* Closes a segment or a view.  Closing a view frees only its alive bits. */
 void nidx_txt_close(nidx_txt_segment* seg);
+
+/* A view of seg under a document mask: a handle whose alive set is seg's alive set AND mask_bits ((n_docs + 63) / 64 words, `mem`;
+ * on the device path typically nidx_txt_prefilter's output, which never leaves HBM).  Every search entry point of a text segment
+ * (nidx_txt_search*, nidx_txt_list_ordered, nidx_txt_facet_count_all, nidx_txt_prefilter, ...) accepts the view and runs over the
+ * masked set only: matches, totals, facet counts and listings are those of a copy of seg whose alive bits were set to alive AND mask.
+ * Scores keep seg's statistics (nidx_txt_set_stats): masked-out documents still count in N, document frequencies and the average
+ * length, as under a filter in the reference.  The view shares every other array of seg read-only and owns only its
+ * (n_docs + 63) / 64 alive words, computed on `stream` (a call on another stream must be ordered after it by the caller).  Setters on
+ * a view are NIDX_EINVAL.  seg must outlive the view, and must not be changed while the view is in use; close the view with
+ * nidx_txt_close. */
+int nidx_txt_view(nidx_txt_segment* seg, const uint64_t* mask_bits, int mem, nidx_txt_segment** out_view, void* stream);
 
 typedef struct nidx_txt_search_params {
     int32_t k;       /* result_per_page + 1 in the reference (reader.rs:386-387) */
@@ -408,6 +420,14 @@ int nidx_txt_list_ordered(nidx_txt_segment* seg, const nidx_txt_order* order, in
  * and field paths.  The columns live in HBM (8 bytes per document).  A call that fails leaves the previous columns in place. */
 int nidx_txt_set_doc_columns(nidx_txt_segment* seg, const uint32_t* resource_ord, const uint32_t* field_ord);
 
+/* Every document's access groups (reference: Resource.security, nidx_text/src/resource_indexer.rs:49-62), in the shape of
+ * nidx_txt_set_facets: n_groups keys strictly ascending in facet order (each a group id with a leading '/' added when it lacks one,
+ * encoded as a facet), document d carries the ords doc_ords[doc_off[d] .. doc_off[d + 1]) (strictly ascending).  A document without
+ * ords is public.  The ords live in HBM; host pointers.  A call that fails (rejected input included) leaves the previous groups in
+ * place. */
+int nidx_txt_set_doc_groups(nidx_txt_segment* seg, uint32_t n_groups, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
+                            const uint32_t* doc_ords);
+
 #define NIDX_P_FACET 0     /* the document carries a facet ord in [lo, hi) */
 #define NIDX_P_FIELD 1     /* the document's field ord is in [lo, hi) */
 #define NIDX_P_RESOURCE 2  /* the document's resource ord is in [lo, hi) */
@@ -418,6 +438,10 @@ int nidx_txt_set_doc_columns(nidx_txt_segment* seg, const uint32_t* resource_ord
 #define NIDX_P_AND 6       /* intersection of the n operand subtrees that follow; n = 0 matches nothing */
 #define NIDX_P_OR 7        /* union of the n operand subtrees that follow; n = 0 matches nothing */
 #define NIDX_P_NOT 8       /* n = 1: every document that the operand does not match */
+#define NIDX_P_PUBLIC 9    /* the document has no access group (nidx_txt_set_doc_groups) */
+#define NIDX_P_GROUP 10    /* the document carries an access group ord in [lo, hi): a group and its descendants are one range, so a
+                              requested group grants the resources of its descendant groups (SearchRequest.security is
+                              OR(PUBLIC, GROUP of each requested group)) */
 #define NIDX_PREFILTER_MAX_DEPTH 64   /* levels of nesting: a leaf is one level, each AND / OR / NOT adds one */
 typedef struct nidx_prefilter_node {   /* an expression in pre-order */
     int32_t kind;                      /* NIDX_P_* */
@@ -429,8 +453,8 @@ typedef struct nidx_prefilter_node {   /* an expression in pre-order */
 /* The expression AND the alive set over the segment's documents -> out_bits ((n_docs + 63) / 64 words, `mem`, bits past n_docs
  * zero; may be NULL) and *out_matching (host) = the number of set bits.  The call returns when both are in place.  The program
  * (at most 4096 instructions: one per leaf and per operand after an operand's first) runs in one pass over the columns; FACET
- * needs nidx_txt_set_facets, FIELD / RESOURCE nidx_txt_set_doc_columns, DATE nidx_txt_set_dates, a phrase nidx_txt_set_positions
- * (else NIDX_ESTATE).  A malformed expression, one deeper than NIDX_PREFILTER_MAX_DEPTH or a longer program is NIDX_EINVAL. */
+ * needs nidx_txt_set_facets, FIELD / RESOURCE nidx_txt_set_doc_columns, DATE nidx_txt_set_dates, a phrase nidx_txt_set_positions,
+ * PUBLIC / GROUP nidx_txt_set_doc_groups (else NIDX_ESTATE).  A malformed expression, one deeper than NIDX_PREFILTER_MAX_DEPTH or a longer program is NIDX_EINVAL. */
 int nidx_txt_prefilter(nidx_txt_segment* seg, const nidx_prefilter_node* nodes, int32_t n_nodes, uint64_t* out_bits, int mem, uint64_t* out_matching,
                        void* stream);
 

@@ -58,7 +58,7 @@ class PrefilterNode(C.Structure):
     _fields_ = [("kind", C.c_int32), ("n", C.c_int32), ("lo", C.c_int64), ("hi", C.c_int64), ("terms", C.c_void_p)]
 
 
-NIDX_P_FACET, NIDX_P_FIELD, NIDX_P_RESOURCE, NIDX_P_DATE, NIDX_P_KEYWORD, NIDX_P_ALL, NIDX_P_AND, NIDX_P_OR, NIDX_P_NOT = range(9)
+NIDX_P_FACET, NIDX_P_FIELD, NIDX_P_RESOURCE, NIDX_P_DATE, NIDX_P_KEYWORD, NIDX_P_ALL, NIDX_P_AND, NIDX_P_OR, NIDX_P_NOT, NIDX_P_PUBLIC, NIDX_P_GROUP = range(11)
 NIDX_PREFILTER_MAX_DEPTH = 64
 
 
@@ -138,6 +138,7 @@ SIGNATURES = {
     "nidx_txt_set_stats": (i32, [P, u64, u64, P]),
     "nidx_txt_set_alive": (i32, [P, P]),
     "nidx_txt_close": (None, [P]),
+    "nidx_txt_view": (i32, [P, P, i32, P, P]),
     "nidx_txt_search": (i32, [P, P, P, i32, i32, TSP, P, P, P, P, P]),
     "nidx_txt_last_kernel_ms": (i32, [P, P]),
     "nidx_txt_set_facets": (i32, [P, u32, P, P, P, P]),
@@ -150,6 +151,7 @@ SIGNATURES = {
     "nidx_txt_set_positions": (i32, [P, P, u64]),
     "nidx_txt_search_phrases": (i32, [P, P, P, i32, i32, TSP, P, ORDER, REQ, P, P, P, P, P, P, P]),
     "nidx_txt_set_doc_columns": (i32, [P, P, P]),
+    "nidx_txt_set_doc_groups": (i32, [P, u32, P, P, P, P]),
     "nidx_txt_prefilter": (i32, [P, P, i32, P, i32, P, P]),   # nodes: an array of PrefilterNode
     "nidx_vec_prefilter_bits": (i32, [P, P, u64, P, NODES, i32, i32, P, i32, P, P]),
     "nidx_shard_unique_id": (i32, [P]),

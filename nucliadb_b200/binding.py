@@ -11,6 +11,7 @@ Reference:
   nidx/nidx_vector/src/indexer.rs:96-146                          Resource -> vector Elems (key = sentence id, labels = paragraph labels)
   nidx/nidx_text/src/resource_indexer.rs:22-91                    Resource.texts -> one document per field
   nidx/nidx_paragraph/src/resource_indexer.rs:33-131              Resource.paragraphs -> one document per paragraph (text[start:end])
+  nidx/nidx_text/src/resource_indexer.rs:49-62                    Resource.security -> the access groups of its documents
 
 What is kept of the reference's machinery is the INTERFACE: metadata lives in memory (no PostgreSQL), every index message
 becomes one immutable segment per index (as in the reference), deletions are (key, seq) pairs applied to older segments, and
@@ -215,9 +216,12 @@ class NidxBinding:
         meta = res.metadata if res.HasField("metadata") else None
         created = meta.created.seconds if meta is not None and meta.HasField("created") else None
         modified = meta.modified.seconds if meta is not None and meta.HasField("modified") else None
+        # access groups (nidx_text/src/resource_indexer.rs:49-62): every document of the resource carries them, its paragraphs too,
+        # so that each keyword index evaluates SearchRequest.security over its own documents
+        groups = tuple(res.security.access_groups) if res.HasField("security") else ()
         if not res.skip_texts:
-            docs = [T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, ti.text, tuple(list(res.labels) + list(ti.labels)), created, modified)
-                    for fid, ti in res.texts.items()]
+            docs = [T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, ti.text, tuple(list(res.labels) + list(ti.labels)), created, modified,
+                              groups) for fid, ti in res.texts.items()]
             if docs:
                 shard.text_segments.append((docs, seq))
         if not res.skip_paragraphs:
@@ -226,7 +230,7 @@ class NidxBinding:
                 text = res.texts[fid].text if fid in res.texts else ""
                 for pid, par in paragraphs.paragraphs.items():
                     labels = tuple(list(res.labels) + list(res.texts[fid].labels if fid in res.texts else ()) + list(par.labels))
-                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels, created, modified))
+                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels, created, modified, groups))
                     shard.paragraph_meta[(rid, "/" + fid if not fid.startswith("/") else fid, len(pdocs) - 1, seq)] = (pid, par)
             if pdocs:
                 shard.paragraph_segments.append((pdocs, seq))
@@ -282,11 +286,16 @@ class NidxBinding:
         k = int(req.result_per_page)
         out = {}
         order = T.OrderBy(sort_by=int(req.order.sort_by), type=int(req.order.type)) if req.HasField("order") else None
-        # prefilter (shard_search.rs:108-137): field_filter evaluated on the device over the documents -> the fields that may answer
+        # prefilter (shard_search.rs:108-137, query_planner/prefilter.rs:106-160): field_filter and security evaluated on the device
+        # over the documents -> the fields that may answer
+        security = list(req.security.access_groups) if req.HasField("security") else None
+        field_filter = req.field_filter if req.HasField("field_filter") else None
         prefilter = V.PrefilterResult.all()
-        if req.HasField("field_filter") and shard.text_searcher is not None:
-            if hasattr(V._lib.load(), "nidx_txt_prefilter"):
-                prefilter = shard.text_searcher.prefilter(req.field_filter)
+        if security is not None and shard.text_searcher is None:   # no document to grant access through
+            prefilter = V.PrefilterResult.none()
+        elif (field_filter is not None or security is not None) and shard.text_searcher is not None:
+            if security is not None or hasattr(V._lib.load(), "nidx_txt_prefilter"):
+                prefilter = shard.text_searcher.prefilter(field_filter, security=security)
             else:   # a stand-in for libnidx_b200.so without the prefilter (the ABI emulator of the host-logic tests): the host loop
                 fields = [V.FieldId(_uuid.UUID(d.uuid), d.field) for seg in shard.text_searcher.segments for d in seg.docs if _doc_matches(req.field_filter, d)]
                 prefilter = V.PrefilterResult.some(fields) if fields else V.PrefilterResult.none()
@@ -302,13 +311,15 @@ class NidxBinding:
             out["vector"] = vi.searcher.search(vreq, prefilter).documents if vi.searcher is not None else []
         if req.document and shard.text_searcher is not None:
             out["document"] = shard.text_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25),
-                                                                                 faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order))
+                                                                                 faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order,
+                                                                                 security=security))
         if req.paragraph and shard.paragraph_searcher is not None:
             after = None
             if req.HasField("search_after"):
                 after = T.SearchAfter(score=req.search_after.score, tie_break="keep_after", docaddr=int(req.search_after.docaddr))
             out["paragraph"] = shard.paragraph_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25), search_after=after,
-                                                                                       faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order))
+                                                                                       faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order,
+                                                                                       security=security))
         return out
 
     def _merge(self, req, parts):

@@ -851,7 +851,7 @@ __global__ void and_bits_kernel(const uint64_t* a, const uint64_t* b, uint64_t* 
         local += __popcll(v);
     }
     for (int off = 16; off >= 1; off >>= 1) local += __shfl_xor_sync(0xFFFFFFFFu, local, off);
-    if ((threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
+    if (count && (threadIdx.x & 31) == 0 && local) atomicAdd(count, local);
 }
 
 // Shared-memory plans of the two walks, used by AUTO's choice and by the launch alike.  Each returns false when the plan does not
@@ -1913,7 +1913,17 @@ int nidx_vec_save(nidx_vec_segment* s, const char* dir) {
 }
 
 // ---- text ---------------------------------------------------------------------------------------
-struct nidx_txt_segment {
+// A dictionary of path keys on the host (in facet order) and every document's ords of it as CSR in HBM: the facets
+// (nidx_txt_set_facets) and the access groups (nidx_txt_set_doc_groups).
+struct OrdColumn {
+    std::vector<std::string> keys;
+    DevArray<uint32_t> d_off;         // [n_docs + 1]
+    DevArray<uint32_t> d_ord;         // [n_ords]
+    uint64_t n_ords = 0;
+};
+
+// What a text segment and its views share: everything but the alive bits.
+struct TxtIndex {
     int device = 0, sm_count = 0;
     uint32_t n_docs = 0, n_terms = 0;
     uint64_t n_post = 0;
@@ -1922,18 +1932,14 @@ struct nidx_txt_segment {
     DevArray<uint32_t> d_skip_row;    // [n_terms]
     DevArray<uint32_t> d_skip;        // [rows][n_fine + 1]
     uint32_t n_fine = 0;
-    DevArray<uint64_t> d_alive;
     DevArray<float> d_weight;         // [n_terms]
     DevArray<float> d_norm_cache;     // [256]
     DevArray<uint64_t> d_doc_keys;    // [n_docs] caller keys of the documents (paragraph ids) for rank fusion (nidx_txt_set_doc_keys)
     std::vector<uint64_t> own_df;
     uint64_t own_tokens = 0;
     cudaEvent_t ev_k0 = nullptr, ev_k1 = nullptr;  // around bm25_kernel of the last search (bench roofline)
-    // facets (nidx_txt_set_facets): the dictionary on the host in facet order, every document's ords (CSR) in HBM
-    std::vector<std::string> facet_keys;
-    DevArray<uint32_t> d_fdoc_off;    // [n_docs + 1]
-    DevArray<uint32_t> d_ford;        // [n_facet_ords]
-    uint64_t n_facet_ords = 0;
+    OrdColumn facets;                 // nidx_txt_set_facets
+    OrdColumn groups;                 // nidx_txt_set_doc_groups: a document without ords is public
     // dates (nidx_txt_set_dates), per field (NIDX_ORDER_CREATED, NIDX_ORDER_MODIFIED): the seconds and every document's dense rank
     DevArray<int64_t> d_secs[2];      // [n_docs]
     DevArray<uint32_t> d_rank[2];     // [n_docs rounded up to 8], 0 = no date
@@ -1946,10 +1952,17 @@ struct nidx_txt_segment {
     DevArray<uint32_t> d_res_ord, d_field_ord;
     WorkspacePool pool;
 
-    ~nidx_txt_segment() {
+    ~TxtIndex() {
         if (ev_k0) cudaEventDestroy(ev_k0);
         if (ev_k1) cudaEventDestroy(ev_k1);
     }
+};
+
+// A segment owns its index; a view (nidx_txt_view) shares its parent's and owns only its alive bits.
+struct nidx_txt_segment {
+    std::unique_ptr<TxtIndex> own;    // NULL for a view
+    TxtIndex* ix = nullptr;
+    DevArray<uint64_t> d_alive;
 };
 
 // tantivy fieldnorm code -> token count (Lucene SmallFloat.byte4ToInt) [recalled]
@@ -1964,15 +1977,15 @@ static int txt_upload_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t t
     float avg = (float)total_tokens / (float)total_docs;
     float cache[256];
     for (int i = 0; i < 256; ++i) cache[i] = K1 * (1.0f - B + B * (float)fieldnorm_id_to_value(i) / avg);
-    std::vector<float> weight(t->n_terms), idf(t->n_terms);
-    for (uint32_t i = 0; i < t->n_terms; ++i) {
+    std::vector<float> weight(t->ix->n_terms), idf(t->ix->n_terms);
+    for (uint32_t i = 0; i < t->ix->n_terms; ++i) {
         float x = ((float)(total_docs - df[i]) + 0.5f) / ((float)df[i] + 0.5f);
         idf[i] = logf(1.0f + x);
         weight[i] = idf[i] * (1.0f + K1);
     }
-    CU(cudaMemcpy(t->d_norm_cache, cache, sizeof(cache), cudaMemcpyHostToDevice));
-    if (t->n_terms) CU(cudaMemcpy(t->d_weight, weight.data(), (size_t)t->n_terms * 4, cudaMemcpyHostToDevice));
-    t->idf = std::move(idf);
+    CU(cudaMemcpy(t->ix->d_norm_cache, cache, sizeof(cache), cudaMemcpyHostToDevice));
+    if (t->ix->n_terms) CU(cudaMemcpy(t->ix->d_weight, weight.data(), (size_t)t->ix->n_terms * 4, cudaMemcpyHostToDevice));
+    t->ix->idf = std::move(idf);
     return 0;
 }
 
@@ -1983,32 +1996,34 @@ int nidx_txt_create(int32_t device, uint32_t n_docs, uint32_t n_terms, const uin
     if (r) return r;
     if (n_docs >= (1u << 31)) return fail(NIDX_EINVAL, "at most 2^31-1 documents per segment");
     std::unique_ptr<nidx_txt_segment> t(new nidx_txt_segment());   // freed with everything it holds unless the call succeeds
-    t->device = device; t->n_docs = n_docs; t->n_terms = n_terms; t->n_post = term_off[n_terms];
+    t->own.reset(new TxtIndex());
+    t->ix = t->own.get();
+    t->ix->device = device; t->ix->n_docs = n_docs; t->ix->n_terms = n_terms; t->ix->n_post = term_off[n_terms];
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
-    t->sm_count = prop.multiProcessorCount;
-    t->n_fine = (n_docs + BM_FINE - 1) / BM_FINE;
-    ALLOC(t->d_term_off, ((size_t)n_terms + 1) * 8);
-    ALLOC(t->d_post, std::max<uint64_t>(t->n_post, 1) * 8);
-    ALLOC(t->d_weight, std::max<uint32_t>(n_terms, 1) * 4);
-    ALLOC(t->d_norm_cache, 1024);
-    ALLOC(t->d_skip_row, std::max<uint32_t>(n_terms, 1) * 4);
-    CU(cudaEventCreate(&t->ev_k0));
-    CU(cudaEventCreate(&t->ev_k1));
-    CU(cudaMemcpy(t->d_term_off, term_off, ((size_t)n_terms + 1) * 8, cudaMemcpyHostToDevice));
-    if (t->n_post) {
+    t->ix->sm_count = prop.multiProcessorCount;
+    t->ix->n_fine = (n_docs + BM_FINE - 1) / BM_FINE;
+    ALLOC(t->ix->d_term_off, ((size_t)n_terms + 1) * 8);
+    ALLOC(t->ix->d_post, std::max<uint64_t>(t->ix->n_post, 1) * 8);
+    ALLOC(t->ix->d_weight, std::max<uint32_t>(n_terms, 1) * 4);
+    ALLOC(t->ix->d_norm_cache, 1024);
+    ALLOC(t->ix->d_skip_row, std::max<uint32_t>(n_terms, 1) * 4);
+    CU(cudaEventCreate(&t->ix->ev_k0));
+    CU(cudaEventCreate(&t->ix->ev_k1));
+    CU(cudaMemcpy(t->ix->d_term_off, term_off, ((size_t)n_terms + 1) * 8, cudaMemcpyHostToDevice));
+    if (t->ix->n_post) {
         // staged only to be packed into the 8-byte posting records
         DevArray<uint32_t> d_doc, d_tf;
         DevArray<unsigned char> d_fn;
-        ALLOC(d_doc, t->n_post * 4);
+        ALLOC(d_doc, t->ix->n_post * 4);
         ALLOC(d_fn, std::max<uint32_t>(n_docs, 1));
-        CU(cudaMemcpy(d_doc, post_doc, t->n_post * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(d_doc, post_doc, t->ix->n_post * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(d_fn, fieldnorm_id, n_docs, cudaMemcpyHostToDevice));
         if (post_tf) {
-            ALLOC(d_tf, t->n_post * 4);
-            CU(cudaMemcpy(d_tf, post_tf, t->n_post * 4, cudaMemcpyHostToDevice));
+            ALLOC(d_tf, t->ix->n_post * 4);
+            CU(cudaMemcpy(d_tf, post_tf, t->ix->n_post * 4, cudaMemcpyHostToDevice));
         }
-        bm25_pack_kernel<<<t->sm_count * 8, 256>>>(d_doc, d_tf, d_fn, t->n_post, t->d_post);
+        bm25_pack_kernel<<<t->ix->sm_count * 8, 256>>>(d_doc, d_tf, d_fn, t->ix->n_post, t->ix->d_post);
         LAUNCHED();
         CU(cudaGetLastError());
         CU(cudaDeviceSynchronize());
@@ -2017,93 +2032,146 @@ int nidx_txt_create(int32_t device, uint32_t n_docs, uint32_t n_terms, const uin
     std::vector<uint32_t> skip_row(n_terms, NIDX_NIL), row_term;
     for (uint32_t i = 0; i < n_terms; ++i)
         if (term_off[i + 1] - term_off[i] >= (uint64_t)BM_SKIP_DF) { skip_row[i] = (uint32_t)row_term.size(); row_term.push_back(i); }
-    if (n_terms) CU(cudaMemcpy(t->d_skip_row, skip_row.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice));
-    size_t skip_words = std::max<size_t>(row_term.size(), 1) * ((size_t)t->n_fine + 1);
-    ALLOC(t->d_skip, skip_words * 4);
+    if (n_terms) CU(cudaMemcpy(t->ix->d_skip_row, skip_row.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice));
+    size_t skip_words = std::max<size_t>(row_term.size(), 1) * ((size_t)t->ix->n_fine + 1);
+    ALLOC(t->ix->d_skip, skip_words * 4);
     if (!row_term.empty()) {
         DevArray<uint32_t> d_row_term;
         ALLOC(d_row_term, row_term.size() * 4);
         CU(cudaMemcpy(d_row_term, row_term.data(), row_term.size() * 4, cudaMemcpyHostToDevice));
-        bm25_build_skip_kernel<<<t->sm_count * 8, 256>>>(t->d_term_off, t->d_post, d_row_term, (uint32_t)row_term.size(), t->n_fine, t->d_skip);
+        bm25_build_skip_kernel<<<t->ix->sm_count * 8, 256>>>(t->ix->d_term_off, t->ix->d_post, d_row_term, (uint32_t)row_term.size(), t->ix->n_fine, t->ix->d_skip);
         LAUNCHED();
         CU(cudaGetLastError());
         CU(cudaDeviceSynchronize());
     }
-    t->own_df.resize(n_terms);
-    for (uint32_t i = 0; i < n_terms; ++i) t->own_df[i] = term_off[i + 1] - term_off[i];
+    t->ix->own_df.resize(n_terms);
+    for (uint32_t i = 0; i < n_terms; ++i) t->ix->own_df[i] = term_off[i + 1] - term_off[i];
     // a segment alone only knows the quantised lengths; the exact token total comes with set_stats
     uint64_t tokens = 0;
     for (uint32_t i = 0; i < n_docs; ++i) tokens += fieldnorm_id_to_value(fieldnorm_id[i]);
-    t->own_tokens = tokens;
-    r = txt_upload_stats(t.get(), std::max<uint32_t>(n_docs, 1), std::max<uint64_t>(tokens, 1), t->own_df.data());
+    t->ix->own_tokens = tokens;
+    r = txt_upload_stats(t.get(), std::max<uint32_t>(n_docs, 1), std::max<uint64_t>(tokens, 1), t->ix->own_df.data());
     if (r) return r;
     *out = t.release();
     return 0;
 }
 
+// The setters change what a segment's views share: a view has none.
+static int require_owner(const nidx_txt_segment* t) {
+    if (!t) return fail(NIDX_EINVAL, "null segment");
+    return t->own ? 0 : fail(NIDX_EINVAL, "a view (nidx_txt_view) cannot be changed");
+}
+
 int nidx_txt_set_stats(nidx_txt_segment* t, uint64_t total_docs, uint64_t total_tokens, const uint64_t* doc_freq) {
-    if (!t || !total_docs) return fail(NIDX_EINVAL, "bad argument");
-    CU(cudaSetDevice(t->device));
-    return txt_upload_stats(t, total_docs, total_tokens, doc_freq ? doc_freq : t->own_df.data());
+    int r = require_owner(t);
+    if (r) return r;
+    if (!total_docs) return fail(NIDX_EINVAL, "bad argument");
+    CU(cudaSetDevice(t->ix->device));
+    return txt_upload_stats(t, total_docs, total_tokens, doc_freq ? doc_freq : t->ix->own_df.data());
 }
 
 int nidx_txt_set_alive(nidx_txt_segment* t, const uint64_t* alive_bits) {
-    if (!t) return fail(NIDX_EINVAL, "null segment");
-    return set_rows(t->device, t->d_alive, alive_bits, ((size_t)t->n_docs + 63) / 64);
+    int r = require_owner(t);
+    if (r) return r;
+    return set_rows(t->ix->device, t->d_alive, alive_bits, ((size_t)t->ix->n_docs + 63) / 64);
 }
 
 void nidx_txt_close(nidx_txt_segment* t) {
     if (!t) return;
-    cudaSetDevice(t->device);
+    cudaSetDevice(t->ix->device);
     cudaDeviceSynchronize();
     delete t;
 }
 
-int nidx_txt_last_kernel_ms(nidx_txt_segment* t, float* ms) {
-    if (!t || !ms) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(t->device));
-    CU(cudaEventSynchronize(t->ev_k1));
-    CU(cudaEventElapsedTime(ms, t->ev_k0, t->ev_k1));
+int nidx_txt_view(nidx_txt_segment* t, const uint64_t* mask_bits, int mem, nidx_txt_segment** out, void* stream_) {
+    if (!t || !mask_bits || !out) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->ix->device));
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const size_t words = ((size_t)t->ix->n_docs + 63) / 64;
+    std::unique_ptr<nidx_txt_segment> v(new nidx_txt_segment());
+    v->ix = t->ix;
+    ALLOC(v->d_alive, std::max<size_t>(words, 1) * 8);
+    const uint64_t* d_mask = mask_bits;
+    if (mem == NIDX_MEM_HOST && words) {
+        CU(cudaMemcpyAsync(v->d_alive, mask_bits, words * 8, cudaMemcpyHostToDevice, stream));
+        d_mask = v->d_alive;
+    }
+    if (words) {   // the parent's alive set AND the mask: one pass over the words, on the caller's stream
+        and_bits_kernel<<<(unsigned)std::min<size_t>((words + 255) / 256, 1024), 256, 0, stream>>>(d_mask, t->d_alive, v->d_alive, words, nullptr);
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    *out = v.release();
     return 0;
 }
 
-int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
-                        const uint32_t* doc_ords) {
-    if (!t || !doc_off || (n_facets && (!key_bytes || !key_off))) return fail(NIDX_EINVAL, "null argument");
-    std::vector<std::string> keys(n_facets);
-    for (uint32_t i = 0; i < n_facets; ++i) {
+int nidx_txt_last_kernel_ms(nidx_txt_segment* t, float* ms) {
+    if (!t || !ms) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->ix->device));
+    CU(cudaEventSynchronize(t->ix->ev_k1));
+    CU(cudaEventElapsedTime(ms, t->ix->ev_k0, t->ix->ev_k1));
+    return 0;
+}
+
+}  // extern "C"
+
+// nidx_txt_set_facets / nidx_txt_set_doc_groups: checks the dictionary and the CSR, uploads them and only then replaces `col`, so a
+// rejected or failed call leaves the previous column in place.  `what` names the column in errors.
+static int set_ord_column(nidx_txt_segment* t, OrdColumn TxtIndex::*column, const char* what, uint32_t n_keys, const uint8_t* key_bytes, const uint64_t* key_off,
+                          const uint64_t* doc_off, const uint32_t* doc_ords) {
+    int r = require_owner(t);
+    if (r) return r;
+    if (!doc_off || (n_keys && (!key_bytes || !key_off))) return fail(NIDX_EINVAL, "null argument");
+    std::vector<std::string> keys(n_keys);
+    for (uint32_t i = 0; i < n_keys; ++i) {
         keys[i].assign(reinterpret_cast<const char*>(key_bytes) + key_off[i], key_off[i + 1] - key_off[i]);
-        if (i && !(keys[i - 1] < keys[i])) return fail(NIDX_EINVAL, "facet keys must be strictly ascending (facet order)");
+        if (i && !(keys[i - 1] < keys[i])) return fail(NIDX_EINVAL, "%s keys must be strictly ascending (facet order)", what);
     }
-    const uint64_t nnz = doc_off[t->n_docs];
-    if (nnz >= (1ull << 32)) return fail(NIDX_EINVAL, "at most 2^32-1 facet ords per segment");
+    const uint32_t n_docs = t->ix->n_docs;
+    const uint64_t nnz = doc_off[n_docs];
+    if (nnz >= (1ull << 32)) return fail(NIDX_EINVAL, "at most 2^32-1 %s ords per segment", what);
     if (nnz && !doc_ords) return fail(NIDX_EINVAL, "null argument");
-    std::vector<uint32_t> off(t->n_docs + 1);
-    for (uint32_t d = 0; d <= t->n_docs; ++d) {
+    std::vector<uint32_t> off(n_docs + 1);
+    for (uint32_t d = 0; d <= n_docs; ++d) {
         if (d && doc_off[d] < doc_off[d - 1]) return fail(NIDX_EINVAL, "doc_off must be non-decreasing");
         off[d] = (uint32_t)doc_off[d];
     }
-    for (uint32_t d = 0; d < t->n_docs; ++d)
+    for (uint32_t d = 0; d < n_docs; ++d)
         for (uint64_t i = doc_off[d]; i < doc_off[d + 1]; ++i)
-            if (doc_ords[i] >= n_facets || (i > doc_off[d] && doc_ords[i] <= doc_ords[i - 1]))
-                return fail(NIDX_EINVAL, "document %u: facet ords must be < n_facets and strictly ascending", d);
-    CU(cudaSetDevice(t->device));
-    DevArray<uint32_t> fdoc_off, ford;
-    ALLOC(fdoc_off, ((size_t)t->n_docs + 1) * 4);
-    ALLOC(ford, std::max<uint64_t>(nnz, 1) * 4);
-    CU(cudaMemcpy(fdoc_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
-    if (nnz) CU(cudaMemcpy(ford, doc_ords, nnz * 4, cudaMemcpyHostToDevice));
-    t->d_fdoc_off = std::move(fdoc_off);   // only now: a rejected or failed call leaves the previous facets in place
-    t->d_ford = std::move(ford);
-    t->facet_keys = std::move(keys);
-    t->n_facet_ords = nnz;
+            if (doc_ords[i] >= n_keys || (i > doc_off[d] && doc_ords[i] <= doc_ords[i - 1]))
+                return fail(NIDX_EINVAL, "document %u: %s ords must be < n_%ss and strictly ascending", d, what, what);
+    CU(cudaSetDevice(t->ix->device));
+    DevArray<uint32_t> d_off, d_ord;
+    ALLOC(d_off, ((size_t)n_docs + 1) * 4);
+    ALLOC(d_ord, std::max<uint64_t>(nnz, 1) * 4);
+    CU(cudaMemcpy(d_off, off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+    if (nnz) CU(cudaMemcpy(d_ord, doc_ords, nnz * 4, cudaMemcpyHostToDevice));
+    OrdColumn& col = t->ix->*column;
+    col.d_off = std::move(d_off);
+    col.d_ord = std::move(d_ord);
+    col.keys = std::move(keys);
+    col.n_ords = nnz;
     return 0;
+}
+
+extern "C" {
+
+int nidx_txt_set_facets(nidx_txt_segment* t, uint32_t n_facets, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
+                        const uint32_t* doc_ords) {
+    return set_ord_column(t, &TxtIndex::facets, "facet", n_facets, key_bytes, key_off, doc_off, doc_ords);
+}
+
+int nidx_txt_set_doc_groups(nidx_txt_segment* t, uint32_t n_groups, const uint8_t* key_bytes, const uint64_t* key_off, const uint64_t* doc_off,
+                            const uint32_t* doc_ords) {
+    return set_ord_column(t, &TxtIndex::groups, "group", n_groups, key_bytes, key_off, doc_off, doc_ords);
 }
 
 int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_t* modified) {
     if (!t || !created || !modified) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(t->device));
-    const uint32_t n = t->n_docs;
+    int r = require_owner(t);
+    if (r) return r;
+    CU(cudaSetDevice(t->ix->device));
+    const uint32_t n = t->ix->n_docs;
     const size_t padded = std::max<size_t>(((size_t)n + 7) & ~(size_t)7, 8);
     // ranks: sort (seconds, doc) on the device, flag the first document of every distinct date, inclusive prefix sum, scatter
     DevArray<int64_t> d_sorted, secs[2];
@@ -2124,7 +2192,7 @@ int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_
         CU(cub::DeviceScan::InclusiveSum(nullptr, scan_bytes, d_flag.p, d_incl.p, (int)n));
         ALLOC(d_cub, std::max(sort_bytes, scan_bytes));
     }
-    const int blocks = std::max(1, std::min<int>(t->sm_count * 8, (int)((n + 255) / 256)));
+    const int blocks = std::max(1, std::min<int>(t->ix->sm_count * 8, (int)((n + 255) / 256)));
     for (int f = 0; f < 2; ++f) {
         ALLOC(secs[f], std::max<size_t>(n, 1) * 8);
         ALLOC(rank[f], padded * 4);
@@ -2146,17 +2214,19 @@ int nidx_txt_set_dates(nidx_txt_segment* t, const int64_t* created, const int64_
     }
     CU(cudaDeviceSynchronize());
     for (int f = 0; f < 2; ++f) {   // only now: a failed call leaves the previous dates in place
-        t->d_secs[f] = std::move(secs[f]);
-        t->d_rank[f] = std::move(rank[f]);
-        t->n_ranks[f] = n_ranks[f];
+        t->ix->d_secs[f] = std::move(secs[f]);
+        t->ix->d_rank[f] = std::move(rank[f]);
+        t->ix->n_ranks[f] = n_ranks[f];
     }
     return 0;
 }
 
 int nidx_txt_set_positions(nidx_txt_segment* t, const uint32_t* positions, uint64_t n_positions) {
     if (!t || (n_positions && !positions)) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(t->device));
-    const uint64_t n = t->n_post;
+    int r = require_owner(t);
+    if (r) return r;
+    CU(cudaSetDevice(t->ix->device));
+    const uint64_t n = t->ix->n_post;
     DevArray<uint64_t> tf, pos_off;
     DevArray<uint32_t> pos;
     DevArray<unsigned int> flags;   // [0] a tf was clamped when packed, [1] positions not strictly ascending
@@ -2166,8 +2236,8 @@ int nidx_txt_set_positions(nidx_txt_segment* t, const uint32_t* positions, uint6
     ALLOC(pos, std::max<uint64_t>(n_positions, 1) * 4);
     ALLOC(flags, 8);
     CU(cudaMemset(flags, 0, 8));
-    const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)t->sm_count * 8, (n + 256) / 256));
-    pos_tf_kernel<<<blocks, 256>>>(t->d_post, n, tf, flags);
+    const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)t->ix->sm_count * 8, (n + 256) / 256));
+    pos_tf_kernel<<<blocks, 256>>>(t->ix->d_post, n, tf, flags);
     LAUNCHED();
     size_t scan_bytes = 0;
     CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, tf.p, pos_off.p, n + 1));
@@ -2187,8 +2257,8 @@ int nidx_txt_set_positions(nidx_txt_segment* t, const uint32_t* positions, uint6
     CU(cudaGetLastError());
     CU(cudaMemcpy(h_flags, flags, 8, cudaMemcpyDeviceToHost));
     if (h_flags[1]) return fail(NIDX_EINVAL, "the positions of every posting must be strictly ascending");
-    t->d_pos_off = std::move(pos_off);   // only now: a rejected or failed call leaves the previous positions in place
-    t->d_pos = std::move(pos);
+    t->ix->d_pos_off = std::move(pos_off);   // only now: a rejected or failed call leaves the previous positions in place
+    t->ix->d_pos = std::move(pos);
     return 0;
 }
 
@@ -2206,7 +2276,7 @@ struct PhrasePlan {
 
 static int phrase_plan(const nidx_txt_segment* t, const nidx_txt_phrases* ph, int32_t nq, const std::vector<uint32_t>& h_off, PhrasePlan& P) {
     if (ph->n < 0 || (ph->n && (!ph->terms || !ph->off || !ph->query))) return fail(NIDX_EINVAL, "bad phrases");
-    if (!t->d_pos) return fail(NIDX_EINVAL, "the segment has no positions (nidx_txt_set_positions)");
+    if (!t->ix->d_pos) return fail(NIDX_EINVAL, "the segment has no positions (nidx_txt_set_positions)");
     const uint32_t nv = (uint32_t)ph->n;
     std::vector<uint32_t> per_q(nq + 1, 0);
     for (uint32_t i = 0; i < nv; ++i) {
@@ -2237,9 +2307,9 @@ static int phrase_plan(const nidx_txt_segment* t, const nidx_txt_phrases* ph, in
         for (uint32_t j = ph->off[i]; j < ph->off[i + 1]; ++j) {
             const uint32_t term = ph->terms[j];
             terms.push_back(term);
-            if (term >= t->n_terms) { known = false; continue; }
-            idf += t->idf[term];
-            if (t->own_df[term] < cap) { cap = t->own_df[term]; dv = j - ph->off[i]; }
+            if (term >= t->ix->n_terms) { known = false; continue; }
+            idf += t->ix->idf[term];
+            if (t->ix->own_df[term] < cap) { cap = t->ix->own_df[term]; dv = j - ph->off[i]; }
         }
         if (!known) cap = 0;   // a term the segment's dictionary lacks: the phrase matches nothing and weighs 0, like the term alone
         off[v + 1] = (uint32_t)terms.size();
@@ -2261,7 +2331,7 @@ static int phrase_plan(const nidx_txt_segment* t, const nidx_txt_phrases* ph, in
     const size_t in_bytes = P.bytes;
     take(P.o_range, std::max<size_t>(nv, 1) * 16);
     take(P.o_post, std::max<uint64_t>(cap_off[nv], 1) * 8);
-    take(P.o_skip, std::max<size_t>(row_term.size(), 1) * ((size_t)t->n_fine + 1) * 4);
+    take(P.o_skip, std::max<size_t>(row_term.size(), 1) * ((size_t)t->ix->n_fine + 1) * 4);
     P.buf.assign(in_bytes, 0);
     auto put = [&](size_t o, const auto& v) { if (!v.empty()) memcpy(P.buf.data() + o, v.data(), v.size() * sizeof(v[0])); };
     put(P.o_qoff, per_q); put(P.o_terms, terms); put(P.o_off, off); put(P.o_driver, driver); put(P.o_skip_row, skip_row);
@@ -2276,19 +2346,19 @@ static int phrase_pass(nidx_txt_segment* t, const PhrasePlan& P, const TxtDev& T
     unsigned char* d = w.phrases.p;
     CU(cudaMemcpyAsync(d, P.buf.data(), P.buf.size(), cudaMemcpyHostToDevice, stream));
     PhraseArgs A;
-    A.pos_off = t->d_pos_off; A.pos = t->d_pos;
+    A.pos_off = t->ix->d_pos_off; A.pos = t->ix->d_pos;
     A.terms = reinterpret_cast<const uint32_t*>(d + P.o_terms); A.off = reinterpret_cast<const uint32_t*>(d + P.o_off);
     A.driver = reinterpret_cast<const uint32_t*>(d + P.o_driver); A.cap_off = reinterpret_cast<const uint64_t*>(d + P.o_cap_off);
     A.nv = P.nv; A.out = reinterpret_cast<uint2*>(d + P.o_post); A.range = reinterpret_cast<uint64_t*>(d + P.o_range);
     if (P.slots) {
-        const int blocks = (int)std::min<uint64_t>((uint64_t)t->sm_count * 8, (P.slots + 255) / 256);
+        const int blocks = (int)std::min<uint64_t>((uint64_t)t->ix->sm_count * 8, (P.slots + 255) / 256);
         phrase_match_kernel<<<blocks, 256, 0, stream>>>(T, A);
         LAUNCHED();
     }
     phrase_compact_kernel<<<P.nv, PHRASE_COMPACT_THREADS, 0, stream>>>(A);
     LAUNCHED();
     if (P.n_rows) {
-        bm25_build_skip_kernel<<<t->sm_count * 8, 256, 0, stream>>>(A.range, A.out, reinterpret_cast<const uint32_t*>(d + P.o_row_term), P.n_rows, t->n_fine,
+        bm25_build_skip_kernel<<<t->ix->sm_count * 8, 256, 0, stream>>>(A.range, A.out, reinterpret_cast<const uint32_t*>(d + P.o_row_term), P.n_rows, t->ix->n_fine,
                                                                     reinterpret_cast<uint32_t*>(d + P.o_skip));
         LAUNCHED();
     }
@@ -2302,10 +2372,10 @@ static int phrase_pass(nidx_txt_segment* t, const PhrasePlan& P, const TxtDev& T
 static int order_args(const nidx_txt_segment* t, const nidx_txt_order* order, OrderArgs& O) {
     if (!order || (order->field != NIDX_ORDER_CREATED && order->field != NIDX_ORDER_MODIFIED) || (order->type != NIDX_ORDER_DESC && order->type != NIDX_ORDER_ASC))
         return fail(NIDX_EINVAL, "bad order");
-    if (!t->d_rank[order->field]) return fail(NIDX_EINVAL, "the segment has no dates (nidx_txt_set_dates)");
-    O.rank = t->d_rank[order->field];
-    O.secs = t->d_secs[order->field];
-    O.n_ranks = t->n_ranks[order->field];
+    if (!t->ix->d_rank[order->field]) return fail(NIDX_EINVAL, "the segment has no dates (nidx_txt_set_dates)");
+    O.rank = t->ix->d_rank[order->field];
+    O.secs = t->ix->d_secs[order->field];
+    O.n_ranks = t->ix->n_ranks[order->field];
     O.asc = order->type == NIDX_ORDER_ASC;
     return 0;
 }
@@ -2319,7 +2389,7 @@ struct FacetPlan {
 
 static int facet_plan(const nidx_txt_segment* t, const nidx_txt_facet_request* r, FacetPlan& P) {
     if (!r || r->n < 0 || (r->n && (!r->key_bytes || !r->key_off))) return fail(NIDX_EINVAL, "bad facet request");
-    if (!t->d_fdoc_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
+    if (!t->ix->facets.d_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
     std::vector<std::pair<std::string, int>> req;
     for (int i = 0; i < r->n; ++i) req.emplace_back(std::string(reinterpret_cast<const char*>(r->key_bytes) + r->key_off[i], r->key_off[i + 1] - r->key_off[i]), i);
     std::sort(req.begin(), req.end());
@@ -2331,7 +2401,7 @@ static int facet_plan(const nidx_txt_segment* t, const nidx_txt_facet_request* r
         if (a.empty() || (b.size() > a.size() && b.compare(0, a.size(), a) == 0 && b[a.size()] == '\0'))
             return fail(NIDX_EINVAL, "a requested facet is an ancestor of another requested facet");
     }
-    const std::vector<std::string>& K = t->facet_keys;
+    const std::vector<std::string>& K = t->ix->facets.keys;
     P.bucket.assign(K.size(), NIDX_NIL);
     P.b_req.clear(); P.b_ord.clear();
     for (const auto& [f, idx] : req) {
@@ -2353,7 +2423,7 @@ static int facet_plan(const nidx_txt_segment* t, const nidx_txt_facet_request* r
 static int facet_args(const nidx_txt_segment* t, const FacetPlan& P, Workspace& w, uint32_t* d_out, cudaStream_t stream, FacetArgs& F) {
     ENSURE(w.facets, std::max<size_t>(P.bucket.size(), 1) * 4);
     if (!P.bucket.empty()) CU(cudaMemcpyAsync(w.facets.p, P.bucket.data(), P.bucket.size() * 4, cudaMemcpyHostToDevice, stream));
-    F.doc_off = t->d_fdoc_off; F.ords = t->d_ford; F.bucket = w.facets.as<uint32_t>();
+    F.doc_off = t->ix->facets.d_off; F.ords = t->ix->facets.d_ord; F.bucket = w.facets.as<uint32_t>();
     F.n_buckets = (uint32_t)P.b_req.size();
     F.smem = F.n_buckets <= FACET_SMEM_BUCKETS;
     F.out = d_out;
@@ -2381,8 +2451,8 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     if (nq <= 0) return 0;
     int k = p->k;
     if (k <= 0 || k > 1024) return fail(NIDX_EINVAL, "k must be in 1..1024");
-    CU(cudaSetDevice(t->device));
-    WsGuard g(t->pool, stream);
+    CU(cudaSetDevice(t->ix->device));
+    WsGuard g(t->ix->pool, stream);
     Workspace& w = *g.w;
     // query offsets are needed on the host to size things
     std::vector<uint32_t> h_off(nq + 1);
@@ -2421,11 +2491,11 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     int r = st.place(w.stage);
     if (r) return r;
     TxtDev T;
-    T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
-    T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
+    T.n_docs = t->ix->n_docs; T.n_terms = t->ix->n_terms; T.n_fine = t->ix->n_fine; T.term_off = t->ix->d_term_off; T.post = t->ix->d_post;
+    T.skip_row = t->ix->d_skip_row; T.skip = t->ix->d_skip; T.alive = t->d_alive;
     Bm25Args a;
     a.query_terms = d_qt; a.query_off = d_qo; a.nq = nq; a.k = k; a.cap = cap;
-    a.term_weight = t->d_weight; a.norm_cache = t->d_norm_cache;
+    a.term_weight = t->ix->d_weight; a.norm_cache = t->ix->d_norm_cache;
     a.after_mode = p->after_mode; a.after_score = p->after_score; a.after_docaddr = p->after_docaddr; a.docaddr_base = p->docaddr_base;
     a.out_keys = w.partial.as<uint64_t>(); a.out_total = reinterpret_cast<unsigned long long*>(d_total);
     if (order) a.after_mode = 0;   // TopDocs::order_by_fast_field: no search-after
@@ -2439,9 +2509,9 @@ static int txt_search_impl(nidx_txt_segment* t, const uint32_t* query_terms, con
     }
     auto launch = [&](auto kern, size_t bytes, auto... extra) -> int {   // the BM25 pass, between the roofline events
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        CU(cudaEventRecord(t->ev_k0, stream));
+        CU(cudaEventRecord(t->ix->ev_k0, stream));
         kern<<<nq, BM_THREADS, bytes, stream>>>(T, a, extra...);
-        CU(cudaEventRecord(t->ev_k1, stream));
+        CU(cudaEventRecord(t->ix->ev_k1, stream));
         LAUNCHED();
         return 0;
     };
@@ -2509,8 +2579,8 @@ int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* 
     if (!nb) return 0;
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const bool host = mem == NIDX_MEM_HOST;
-    CU(cudaSetDevice(t->device));
-    WsGuard g(t->pool, stream);
+    CU(cudaSetDevice(t->ix->device));
+    WsGuard g(t->ix->pool, stream);
     Workspace& w = *g.w;
     Stage st(stream, host, host);
     uint32_t* d_fc;
@@ -2521,10 +2591,10 @@ int nidx_txt_facet_count_all(nidx_txt_segment* t, const nidx_txt_facet_request* 
     if (r) return r;
     CU(cudaMemsetAsync(d_fc, 0, nb * 4, stream));
     const int threads = 256;
-    const int blocks = std::max(1, std::min<int>(t->sm_count * (2048 / threads), (int)((t->n_docs + threads - 1) / threads)));
-    CU(cudaEventRecord(t->ev_k0, stream));
-    facet_count_all_kernel<<<blocks, threads, F.smem ? nb * 4 : 0, stream>>>(t->n_docs, t->d_alive, F);
-    CU(cudaEventRecord(t->ev_k1, stream));
+    const int blocks = std::max(1, std::min<int>(t->ix->sm_count * (2048 / threads), (int)((t->ix->n_docs + threads - 1) / threads)));
+    CU(cudaEventRecord(t->ix->ev_k0, stream));
+    facet_count_all_kernel<<<blocks, threads, F.smem ? nb * 4 : 0, stream>>>(t->ix->n_docs, t->d_alive, F);
+    CU(cudaEventRecord(t->ix->ev_k1, stream));
     LAUNCHED();
     CU(cudaGetLastError());
     return st.finish();
@@ -2557,12 +2627,12 @@ int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int3
     if (k <= 0 || k > 1024) return fail(NIDX_EINVAL, "k must be in 1..1024");
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const bool host = mem == NIDX_MEM_HOST;
-    CU(cudaSetDevice(t->device));
-    WsGuard g(t->pool, stream);
+    CU(cudaSetDevice(t->ix->device));
+    WsGuard g(t->ix->pool, stream);
     Workspace& w = *g.w;
     // per-CTA top-k over a grid-stride slice, then one merge (the scan_select / topk_merge pattern)
     const int threads = 512;
-    const int blocks = std::max(1, std::min<int>(t->sm_count * 2, (int)(((size_t)t->n_docs + threads * DATE_PT - 1) / (threads * DATE_PT))));
+    const int blocks = std::max(1, std::min<int>(t->ix->sm_count * 2, (int)(((size_t)t->ix->n_docs + threads * DATE_PT - 1) / (threads * DATE_PT))));
     const int cap = topk_cap(k, threads);
     ENSURE(w.partial, (size_t)blocks * k * 8);
     Stage st(stream, host, host);
@@ -2579,13 +2649,13 @@ int nidx_txt_list_ordered(nidx_txt_segment* t, const nidx_txt_order* order, int3
     CU(cudaFuncSetAttribute(date_topk_all_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
     CU(cudaFuncSetAttribute(date_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
     CU(cudaMemsetAsync(d_total, 0, 8, stream));
-    CU(cudaEventRecord(t->ev_k0, stream));
-    date_topk_all_kernel<<<blocks, threads, (size_t)cap * 8, stream>>>(t->n_docs, t->d_alive, O, k, cap, w.partial.as<uint64_t>(),
+    CU(cudaEventRecord(t->ix->ev_k0, stream));
+    date_topk_all_kernel<<<blocks, threads, (size_t)cap * 8, stream>>>(t->ix->n_docs, t->d_alive, O, k, cap, w.partial.as<uint64_t>(),
                                                                       reinterpret_cast<unsigned long long*>(d_total));
     LAUNCHED();
     date_merge_kernel<<<1, threads, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), blocks * k, k, cap, O.secs, d_docs, d_dates, d_cnt);
     LAUNCHED();
-    CU(cudaEventRecord(t->ev_k1, stream));
+    CU(cudaEventRecord(t->ix->ev_k1, stream));
     CU(cudaGetLastError());
     return st.finish();
 }
@@ -2599,19 +2669,20 @@ static int require_handle(const void* h) {
 
 int nidx_txt_set_doc_columns(nidx_txt_segment* t, const uint32_t* resource_ord, const uint32_t* field_ord) {
     int r = require_handle(t);
+    if (!r) r = require_owner(t);
     if (r) return r;
-    if (t->n_docs && (!resource_ord || !field_ord)) return fail(NIDX_EINVAL, "null argument");
-    CU(cudaSetDevice(t->device));
+    if (t->ix->n_docs && (!resource_ord || !field_ord)) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(t->ix->device));
     DevArray<uint32_t> res, fld;
-    const size_t n = t->n_docs;
+    const size_t n = t->ix->n_docs;
     ALLOC(res, std::max<size_t>(n, 1) * 4);
     ALLOC(fld, std::max<size_t>(n, 1) * 4);
     if (n) {
         CU(cudaMemcpy(res, resource_ord, n * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(fld, field_ord, n * 4, cudaMemcpyHostToDevice));
     }
-    t->d_res_ord = std::move(res);   // only now: a failed call leaves the previous columns in place
-    t->d_field_ord = std::move(fld);
+    t->ix->d_res_ord = std::move(res);   // only now: a failed call leaves the previous columns in place
+    t->ix->d_field_ord = std::move(fld);
     return 0;
 }
 
@@ -2623,7 +2694,7 @@ struct PrefilterPlan {
     std::vector<PfOp> prog;
     std::vector<uint32_t> terms;                       // term leaves, slot = index
     std::vector<uint32_t> ph_terms, ph_off{0}, ph_query;   // phrase leaves, slot = terms.size() + index
-    bool facets = false, columns = false, dates[2] = {false, false};
+    bool facets = false, columns = false, groups = false, dates[2] = {false, false};
 
     int compile(const nidx_prefilter_node* nodes, int n_nodes, int& i, int depth) {
         if (i >= n_nodes) return fail(NIDX_EINVAL, "malformed prefilter expression (operand counts do not add up to %d nodes)", n_nodes);
@@ -2633,6 +2704,8 @@ struct PrefilterPlan {
         o.lo = nd.lo; o.hi = nd.hi;
         switch (nd.kind) {
             case NIDX_P_FACET: o.op = PF_FACET; facets = true; break;
+            case NIDX_P_GROUP: o.op = PF_FACET; o.arg = 1; groups = true; break;
+            case NIDX_P_PUBLIC: o.op = PF_PUBLIC; o.arg = 1; groups = true; break;
             case NIDX_P_FIELD: o.op = PF_FIELD; columns = true; break;
             case NIDX_P_RESOURCE: o.op = PF_RESOURCE; columns = true; break;
             case NIDX_P_DATE:
@@ -2686,33 +2759,35 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
     r = P.compile(nodes, n_nodes, at, 1);
     if (r) return r;
     if (at != n_nodes) return fail(NIDX_EINVAL, "malformed prefilter expression (operand counts do not add up to %d nodes)", n_nodes);
-    if (P.facets && !t->d_fdoc_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
-    if (P.columns && !t->d_res_ord) return fail(NIDX_ESTATE, "the segment has no document columns (nidx_txt_set_doc_columns)");
-    if ((P.dates[0] && !t->d_secs[0]) || (P.dates[1] && !t->d_secs[1])) return fail(NIDX_ESTATE, "the segment has no dates (nidx_txt_set_dates)");
-    if (!P.ph_query.empty() && !t->d_pos) return fail(NIDX_ESTATE, "the segment has no positions (nidx_txt_set_positions)");
+    if (P.facets && !t->ix->facets.d_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
+    if (P.columns && !t->ix->d_res_ord) return fail(NIDX_ESTATE, "the segment has no document columns (nidx_txt_set_doc_columns)");
+    if (P.groups && !t->ix->groups.d_off) return fail(NIDX_ESTATE, "the segment has no access groups (nidx_txt_set_doc_groups)");
+    if ((P.dates[0] && !t->ix->d_secs[0]) || (P.dates[1] && !t->ix->d_secs[1])) return fail(NIDX_ESTATE, "the segment has no dates (nidx_txt_set_dates)");
+    if (!P.ph_query.empty() && !t->ix->d_pos) return fail(NIDX_ESTATE, "the segment has no positions (nidx_txt_set_positions)");
     const uint32_t n_terms = (uint32_t)P.terms.size(), nv = (uint32_t)P.ph_query.size();
     for (PfOp& o : P.prog)
         if (o.op == PF_BITS && (o.arg & 0x80000000u)) o.arg = n_terms + (o.arg & 0x7FFFFFFFu);
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const bool host = mem == NIDX_MEM_HOST;
-    CU(cudaSetDevice(t->device));
-    WsGuard g(t->pool, stream);
+    CU(cudaSetDevice(t->ix->device));
+    WsGuard g(t->ix->pool, stream);
     Workspace& w = *g.w;
-    const size_t words = ((size_t)t->n_docs + 63) / 64, slots = (size_t)n_terms + nv;
+    const size_t words = ((size_t)t->ix->n_docs + 63) / 64, slots = (size_t)n_terms + nv;
     Stage st(stream, host, host);
     uint64_t* d_out;
     st.out(out_bits, words, &d_out);
     r = st.place(w.stage);
     if (r) return r;
     PrefilterArgs A{};
-    A.n_docs = t->n_docs; A.res_ord = t->d_res_ord; A.field_ord = t->d_field_ord; A.fdoc_off = t->d_fdoc_off; A.ford = t->d_ford;
-    A.secs0 = t->d_secs[0]; A.secs1 = t->d_secs[1]; A.words = words; A.alive = t->d_alive;
+    A.n_docs = t->ix->n_docs; A.res_ord = t->ix->d_res_ord; A.field_ord = t->ix->d_field_ord; A.fdoc_off = t->ix->facets.d_off; A.ford = t->ix->facets.d_ord;
+    A.gdoc_off = t->ix->groups.d_off; A.gord = t->ix->groups.d_ord;
+    A.secs0 = t->ix->d_secs[0]; A.secs1 = t->ix->d_secs[1]; A.words = words; A.alive = t->d_alive;
     PhrasePlan pp;
     auto scatter = [&](uint64_t* kw, unsigned char* extra) -> int {   // keyword leaves: terms first, then phrases
         if (n_terms) {
             uint32_t* d_terms = reinterpret_cast<uint32_t*>(extra);
             CU(cudaMemcpyAsync(d_terms, P.terms.data(), (size_t)n_terms * 4, cudaMemcpyHostToDevice, stream));
-            prefilter_scatter_kernel<<<n_terms, 256, 0, stream>>>(t->d_post.p, t->d_post.p, n_terms, t->d_term_off, t->n_terms, d_terms, nullptr, nullptr, 0, kw, words);
+            prefilter_scatter_kernel<<<n_terms, 256, 0, stream>>>(t->ix->d_post.p, t->ix->d_post.p, n_terms, t->ix->d_term_off, t->ix->n_terms, d_terms, nullptr, nullptr, 0, kw, words);
             LAUNCHED();
         }
         if (nv) {   // the phrases' virtual lists (phrase.cuh), as the keyword search makes them, then scattered like terms
@@ -2722,8 +2797,8 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
             int r = phrase_plan(t, &ph, nq, no_terms, pp);
             if (r) return r;
             TxtDev T;
-            T.n_docs = t->n_docs; T.n_terms = t->n_terms; T.n_fine = t->n_fine; T.term_off = t->d_term_off; T.post = t->d_post;
-            T.skip_row = t->d_skip_row; T.skip = t->d_skip; T.alive = t->d_alive;
+            T.n_docs = t->ix->n_docs; T.n_terms = t->ix->n_terms; T.n_fine = t->ix->n_fine; T.term_off = t->ix->d_term_off; T.post = t->ix->d_post;
+            T.skip_row = t->ix->d_skip_row; T.skip = t->ix->d_skip; T.alive = t->d_alive;
             Bm25Args a{};
             r = phrase_pass(t, pp, T, w, stream, a);
             if (r) return r;
@@ -2733,7 +2808,7 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
         return 0;
     };
     unsigned long long h = 0;
-    r = run_program(w, stream, t->sm_count, P.prog, slots, A, (size_t)n_terms * 4, scatter, d_out, &h, t->ev_k0, t->ev_k1);
+    r = run_program(w, stream, t->ix->sm_count, P.prog, slots, A, (size_t)n_terms * 4, scatter, d_out, &h, t->ix->ev_k0, t->ix->ev_k1);
     if (!r) r = st.finish(true);   // the program and the plans are host temporaries, and the count is read back
     if (r) return r;
     if (out_matching) *out_matching = h;
@@ -2987,7 +3062,7 @@ int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uin
                             void* stream_) {
     if (!c || !seg || !p || !out_docs || !out_scores) return fail(NIDX_EINVAL, "null argument");
     if (nq <= 0) return 0;
-    if (seg->device != c->device) return fail(NIDX_EINVAL, "segment on device %d, communicator on device %d", seg->device, c->device);
+    if (seg->ix->device != c->device) return fail(NIDX_EINVAL, "segment on device %d, communicator on device %d", seg->ix->device, c->device);
     int k = p->k;
     CU(cudaSetDevice(c->device));
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
@@ -3018,8 +3093,9 @@ int nidx_txt_search_sharded(nidx_shard_comm* c, nidx_txt_segment* seg, const uin
 
 // ---- rank fusion + the fused shard search (SURVEY 8f rank 4) --------------------------------------------------------------
 int nidx_txt_set_doc_keys(nidx_txt_segment* t, const uint64_t* keys) {
-    if (!t) return fail(NIDX_EINVAL, "null segment");
-    return set_rows(t->device, t->d_doc_keys, keys, t->n_docs);
+    int r = require_owner(t);
+    if (r) return r;
+    return set_rows(t->ix->device, t->ix->d_doc_keys, keys, t->ix->n_docs);
 }
 
 }  // extern "C"
@@ -3107,8 +3183,8 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
     const int nq = rq->nq;
     if (nq <= 0) return 0;
     if (!rq->vec && !rq->par && !rq->doc) return fail(NIDX_EINVAL, "shard search without any index request");
-    int device = rq->vec ? rq->vec->cfg.device : (rq->par ? rq->par->device : rq->doc->device);
-    if ((rq->vec && rq->vec->cfg.device != device) || (rq->par && rq->par->device != device) || (rq->doc && rq->doc->device != device))
+    int device = rq->vec ? rq->vec->cfg.device : (rq->par ? rq->par->ix->device : rq->doc->ix->device);
+    if ((rq->vec && rq->vec->cfg.device != device) || (rq->par && rq->par->ix->device != device) || (rq->doc && rq->doc->ix->device != device))
         return fail(NIDX_EINVAL, "the indexes of one shard search must live on one device");
     if (rq->vec && (!rq->vec_params || !rs->vec_ids || !rs->vec_scores || !rs->vec_counts)) return fail(NIDX_EINVAL, "vector request: params and outputs are required");
     if (rq->par && (!rq->par_params || !rs->par_docs || !rs->par_scores || !rs->par_counts)) return fail(NIDX_EINVAL, "paragraph request: params and outputs are required");
@@ -3172,7 +3248,7 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
     if (fuse) {
         ids_to_keys_kernel<<<std::min<size_t>((nv + 255) / 256, 1024), 256, 0, stream>>>(d_vid, nv, rq->vec->d_par_of, rq->vec->d_par_keys, d_vkey);
         LAUNCHED();
-        ids_to_keys_kernel<<<std::min<size_t>((np + 255) / 256, 1024), 256, 0, stream>>>(d_pdoc, np, nullptr, rq->par->d_doc_keys, d_pkey);
+        ids_to_keys_kernel<<<std::min<size_t>((np + 255) / 256, 1024), 256, 0, stream>>>(d_pdoc, np, nullptr, rq->par->ix->d_doc_keys, d_pkey);
         LAUNCHED();
         RrfSourceDev src[2];
         RrfSourceDev kw{d_pkey, d_psc, d_pcnt, kp, rq->weight_keyword}, sem{d_vkey, d_vsc, d_vcnt, kv, rq->weight_semantic};

@@ -17,8 +17,8 @@
 //                             word of the result, ANDed with the alive bits, and counted;
 //   prefilter_join_kernel     text documents -> paragraphs of one vector segment: every matched document with a join entry sets the
 //                             paragraphs of that field key (the NIDX_INV_FIELDS postings).
-// HBM traffic of the pass = per document the columns the program reads (4 B per ord column, 8 B per date column, the facet CSR
-// entry and ords) + 1/8 B of alive bits + 1/8 B per bitset leaf + 1/8 B of output.
+// HBM traffic of the pass = per document the columns the program reads (4 B per ord column, 8 B per date column, the facet or
+// access group CSR entry and ords) + 1/8 B of alive bits + 1/8 B per bitset leaf + 1/8 B of output.
 #pragma once
 #include <cstdint>
 
@@ -30,12 +30,13 @@ constexpr int PF_MAX_DEPTH = 64;        // the bit stack is one 64-bit register:
 constexpr int PF_MAX_PROGRAM = 4096;    // instructions (32 B each) in shared memory
 constexpr int PF_THREADS = 256;
 
-enum PfOpcode : uint32_t { PF_FACET, PF_FIELD, PF_RESOURCE, PF_DATE, PF_BITS, PF_CONST, PF_AND, PF_OR, PF_NOT };
+enum PfOpcode : uint32_t { PF_FACET, PF_FIELD, PF_RESOURCE, PF_DATE, PF_BITS, PF_CONST, PF_AND, PF_OR, PF_NOT, PF_PUBLIC };
 
 struct PfOp {          // one instruction: leaves push a bit, AND / OR pop two and push one, NOT flips the top
     int64_t lo, hi;    // FACET / FIELD / RESOURCE: ord range [lo, hi); DATE: since, until (inclusive)
     uint32_t op;       // PfOpcode
-    uint32_t arg;      // DATE: the seconds column (0 created, 1 modified); BITS: the keyword leaf's slot; CONST: the bit
+    uint32_t arg;      // FACET / PUBLIC: the CSR column (0 facets, 1 access groups); DATE: the seconds column (0 created, 1 modified);
+                       // BITS: the keyword leaf's slot; CONST: the bit
     uint32_t pad[2];
 };
 
@@ -45,6 +46,8 @@ struct PrefilterArgs {
     const uint32_t* field_ord;   // [n_docs]
     const uint32_t* fdoc_off;    // [n_docs + 1] facet CSR (nidx_txt_set_facets)
     const uint32_t* ford;
+    const uint32_t* gdoc_off;    // [n_docs + 1] access group CSR (nidx_txt_set_doc_groups)
+    const uint32_t* gord;
     const int64_t* secs0;        // [n_docs] created, modified seconds (nidx_txt_set_dates); INT64_MIN = no date
     const int64_t* secs1;
     const uint64_t* kw_bits;     // [slots][words] keyword leaves
@@ -75,13 +78,16 @@ __global__ void __launch_bounds__(PF_THREADS) prefilter_eval_kernel(PrefilterArg
                 uint64_t b;
                 switch (o.op) {
                     case PF_FACET: {   // ords ascend: the first one >= lo decides
+                        const uint32_t* off = o.arg ? A.gdoc_off : A.fdoc_off;
+                        const uint32_t* ords = o.arg ? A.gord : A.ford;
                         b = 0;
-                        for (uint32_t j = __ldg(A.fdoc_off + d), e = __ldg(A.fdoc_off + d + 1); j < e; ++j) {
-                            const int64_t u = __ldg(A.ford + j);
+                        for (uint32_t j = __ldg(off + d), e = __ldg(off + d + 1); j < e; ++j) {
+                            const int64_t u = __ldg(ords + j);
                             if (u >= o.lo) { b = u < o.hi; break; }
                         }
                         break;
                     }
+                    case PF_PUBLIC: { const uint32_t* off = o.arg ? A.gdoc_off : A.fdoc_off; b = __ldg(off + d) == __ldg(off + d + 1); break; }
                     case PF_FIELD: { const int64_t u = __ldg(A.field_ord + d); b = u >= o.lo && u < o.hi; break; }
                     case PF_RESOURCE: { const int64_t u = __ldg(A.res_ord + d); b = u >= o.lo && u < o.hi; break; }
                     case PF_DATE: {

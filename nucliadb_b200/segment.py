@@ -443,6 +443,25 @@ class TextSegment:
         assert len(resource_ord) == self.n_docs and len(field_ord) == self.n_docs
         check(_lib.load().nidx_txt_set_doc_columns(self._h, ptr(resource_ord), ptr(field_ord)))
 
+    def set_doc_groups(self, keys, doc_off, doc_ords):
+        """The access group dictionary (encoded facet keys, strictly ascending) and every document's group ords (as set_facets);
+        a document without ords is public."""
+        kb, ko = _pack_keys(keys)
+        doc_off = np.ascontiguousarray(doc_off, dtype=np.uint64)
+        doc_ords = np.ascontiguousarray(doc_ords, dtype=np.uint32)
+        check(_lib.load().nidx_txt_set_doc_groups(self._h, len(keys), ptr(kb), ptr(ko), ptr(doc_off), ptr(doc_ords)))
+
+    def view(self, mask) -> "TextSegment":
+        """This segment under a document mask (nidx_txt_view): every search of the returned segment runs over alive AND mask, with
+        this segment's statistics.  mask: uint64 words [(n_docs + 63) // 64], numpy (host) or a torch CUDA int64 tensor (device
+        path, current torch stream).  The view keeps this segment open; close it when done."""
+        mem, stream, _ = _stage(self.device, _is_torch(mask))
+        h = C.c_void_p()
+        check(_lib.load().nidx_txt_view(self._h, ptr(mask), mem, C.byref(h), stream))
+        v = TextSegment(h, self.n_docs, self.n_terms, self.device)
+        v._parent = self
+        return v
+
     def prefilter(self, nodes, out=None):
         """The expression (a PrefilterNode array in pre-order) AND alive -> (bits, matching): bits = uint64 words [(n_docs + 63) // 64]
         in a new numpy array, or written into `out` (a torch CUDA int64 tensor of that many words: device path)."""

@@ -27,6 +27,12 @@ the top-k with its date (``bm25_order_kernel``), and an empty body lists every a
 seconds, results carry ``date`` instead of ``score``, ``min_score`` and search-after do not apply, and ``next_page = total > k``.
 Segments are merged by (date in the requested direction, undated documents last, segment ord, doc): the tie order and the place of
 undated documents are fixed here, not taken from the reference.
+
+Security (``SearchRequest.security``: ``security_query``, nidx_text/src/search_query.rs:63-87) is a document mask: a resource's access
+groups are indexed as a facet column (a group id gets a leading '/' when it lacks one; a resource without groups is public), the
+request's groups compile to OR(public, each group's facet range) and run on the prefilter's evaluator, and the keyword passes run on
+``nidx_txt_view``s of the segments under the resulting bits: totals, next page, facet counts and date listings all come from the masked
+passes.  It filters only: BM25 scores are the body's (the reference also adds the security clause's own score).
 """
 from __future__ import annotations
 
@@ -182,6 +188,7 @@ class DocumentSearchRequest:  # nidx_text/src/request_types.rs:17-28
     faceted: Sequence[str] = ()               # Faceted.labels: the facets to count children of (SearchRequest.faceted)
     search_after: Optional[SearchAfter] = None  # ParagraphSearchRequest.search_after (nidx_paragraph only)
     order: Optional[OrderBy] = None            # SearchRequest.order: results by date instead of score
+    security: Optional[Sequence[str]] = None   # SearchRequest.security.access_groups: only public resources and those of these groups
 
 
 @dataclass
@@ -217,6 +224,12 @@ def facet_key(path: str) -> Optional[bytes]:
     return b"" if path == "/" else path[1:].encode("utf-8").replace(b"/", b"\0")
 
 
+def group_key(group: str) -> bytes:
+    """An access group id as the group column holds it: a facet, with a leading '/' added when the id lacks one
+    (nidx_text/src/resource_indexer.rs:49-62, search_query.rs:63-87)."""
+    return facet_key(group if group.startswith("/") else "/" + group)
+
+
 def facet_path(key: bytes) -> str:
     return "/" + key.replace(b"\0", b"/").decode("utf-8")
 
@@ -238,6 +251,7 @@ class TextDoc:
     labels: Sequence[str] = ()
     created: Optional[int] = None    # IndexMetadata.created / .modified, seconds
     modified: Optional[int] = None
+    groups: Sequence[str] = ()       # Resource.security.access_groups; none = public
 
 
 class TextIndexSegment:
@@ -307,6 +321,7 @@ class TextSearcher:
         for s in self.segments:  # union statistics on every segment (index_reader.rs:39-77)
             s.upload(n_terms).set_stats(max(total_docs, 1), max(total_tokens, 1), df)
         self.facet_keys: Optional[list] = None   # built on the first faceted request
+        self.group_keys: Optional[list] = None   # built on the first request with security
         self._dates = False                        # uploaded on the first ordered request
         self._prefilter: Optional[_PrefilterIndex] = None   # built on the first prefilter
         self._positions = False                    # uploaded on the first phrase (query or keyword filter)
@@ -325,6 +340,46 @@ class TextSearcher:
             s._gpu.set_facets(keys, off, np.asarray([o for r in rows for o in r], dtype=np.uint32))
         self.facet_keys = keys
 
+    def _ensure_groups(self):
+        """The index's access group dictionary (group_key of every document's groups, in facet order) and each segment's
+        per-document group ords, uploaded once."""
+        if self.group_keys is not None:
+            return
+        keys = sorted({group_key(g) for s in self.segments for d in s.docs for g in d.groups})
+        ord_of = {k: i for i, k in enumerate(keys)}
+        for s in self.segments:
+            rows = [sorted({ord_of[group_key(g)] for g in d.groups}) for d in s.docs]
+            off = np.zeros(len(rows) + 1, dtype=np.uint64)
+            off[1:] = np.cumsum([len(r) for r in rows])
+            s._gpu.set_doc_groups(keys, off, np.asarray([o for r in rows for o in r], dtype=np.uint32))
+        self.group_keys = keys
+
+    def security_nodes(self, access_groups: Sequence[str]) -> list:
+        """security_query (nidx_text/src/search_query.rs:63-87) as flat pre-order prefilter nodes (kind, n, lo, hi, terms): OR of
+        PUBLIC and, per requested group, the GROUP range of that group and its descendants.  No groups: public resources only."""
+        self._ensure_groups()
+        flat = [(_lib.NIDX_P_OR, 1 + len(access_groups), 0, 0, None), (_lib.NIDX_P_PUBLIC, 0, 0, 0, None)]
+        for g in access_groups:
+            flat.append((_lib.NIDX_P_GROUP, 0, *_prefix_range(self.group_keys, group_key(g), facet=True), None))
+        return flat
+
+    def _security_views(self, access_groups: Sequence[str]) -> list:
+        """Every segment as a view (nidx_txt_view) under the security expression's bits, which stay on the device."""
+        import torch
+
+        nodes = _node_array(self.security_nodes(access_groups))
+        views = []
+        try:
+            for s in self.segments:
+                bits = torch.empty((s.n_docs + 63) // 64, dtype=torch.int64, device=torch.device("cuda", s.device))
+                s._gpu.prefilter(nodes, out=bits)
+                views.append(s._gpu.view(bits))
+        except BaseException:
+            for v in views:
+                v.close()
+            raise
+        return views
+
     def _ensure_dates(self):
         """Every segment's created / modified seconds, uploaded once."""
         if self._dates:
@@ -341,8 +396,9 @@ class TextSearcher:
                 s._gpu.set_positions(s.positions)
             self._positions = True
 
-    def prefilter(self, expr):
-        """TextReaderService::prefilter (nidx_text/src/reader.rs:147-180) for a nodereader.FilterExpression: evaluated on the device
+    def prefilter(self, expr, security: Optional[Sequence[str]] = None):
+        """TextReaderService::prefilter (nidx_text/src/reader.rs:147-180) for a nodereader.FilterExpression and / or the access groups
+        of SearchRequest.security (both given: their intersection, in one program; expr may then be None): evaluated on the device
         over every segment -> vector.PrefilterResult: none (nothing matched), all (every alive document matched) or some, whose
         matched documents stay in HBM as a bitset (handed to VectorSearcher.search as they are; `fields` lists them on demand).
         A malformed expression, an invalid facet or resource UUID, or one the device cannot run (deeper than
@@ -357,7 +413,7 @@ class TextSearcher:
         if self._prefilter is None:
             self._prefilter = _PrefilterIndex(self)
         ix = self._prefilter
-        nodes, keep, phrases = ix.compile(expr)
+        nodes, keep, phrases = ix.compile(expr, None if security is None else self.security_nodes(security))
         if phrases:
             self._ensure_positions()
         bits = torch.empty(ix.words_total, dtype=torch.int64, device=torch.device("cuda", self.segments[0].device))
@@ -375,7 +431,7 @@ class TextSearcher:
             return V.PrefilterResult.all()
         return V.PrefilterResult.from_device(ix, bits, matching)
 
-    def _facets(self, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None, phrases=()):
+    def _facets(self, handles: list, faceted: Sequence[str], terms, k: int, params: dict, order: Optional[OrderBy] = None, phrases=()):
         """Counts of the request's facets over the matched set of every segment, summed, then grouped and cut to the top 50.
         With terms: the faceted BM25 search, ordered by date when `order` is given (returns its per-segment (docs, scores or
         dates, counts, total) too); without: every alive document (AllQuery)."""
@@ -392,20 +448,20 @@ class TextSearcher:
             raise
         counts = np.zeros(len(b_req), dtype=np.int64)
         hits = []
-        for ord_, seg in enumerate(self.segments):
+        for ord_, seg in enumerate(handles):
             if terms or phrases:
                 qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
                 if phrases:
-                    docs, scores, cnt, total, fc = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k, docaddr_base=ord_ << 32, facets=keys,
+                    docs, scores, cnt, total, fc = seg.search_phrases(qt, qo, [(0, p) for p in phrases], k, docaddr_base=ord_ << 32, facets=keys,
                                                                            order=None if order is None else (order.sort_by, order.type), **params)
                 elif order is not None:
-                    docs, scores, cnt, total, fc = seg._gpu.search_ordered(qt, qo, k, order.sort_by, order.type, params["mode"], facets=keys)
+                    docs, scores, cnt, total, fc = seg.search_ordered(qt, qo, k, order.sort_by, order.type, params["mode"], facets=keys)
                 else:
-                    docs, scores, cnt, total, fc = seg._gpu.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
+                    docs, scores, cnt, total, fc = seg.search_faceted(qt, qo, k, keys, docaddr_base=ord_ << 32, **params)
                 hits.append((docs, scores, cnt, total))
                 counts += fc[0]
             else:
-                counts += seg._gpu.facet_count_all(keys)
+                counts += seg.facet_count_all(keys)
         groups: dict = {}
         for b, (r, o) in enumerate(zip(b_req, b_ord)):
             if counts[b]:
@@ -434,6 +490,17 @@ class TextSearcher:
         return self._terms(body), []
 
     def search(self, request: DocumentSearchRequest) -> DocumentSearchResponse:
+        if request.security is None:
+            return self._search(request, [s._gpu for s in self.segments])
+        views = self._security_views(request.security)
+        try:
+            return self._search(request, views)
+        finally:
+            for v in views:
+                v.close()
+
+    def _search(self, request: DocumentSearchRequest, handles: list) -> DocumentSearchResponse:
+        """search() over one handle per segment: the segments themselves, or their views under a security mask."""
         terms, phrases = self._clauses(request.body)
         k = request.result_per_page
         resp = DocumentSearchResponse(query=request.body)
@@ -443,10 +510,10 @@ class TextSearcher:
             after = (sa.score, {"drop": 1, "keep_after": 2, "keep": 3}[sa.tie_break], sa.docaddr)
         params = dict(mode=_lib.NIDX_BM25_AND if self.conjunction else _lib.NIDX_BM25_OR, use_tf=self.use_tf, min_score=0.0, after=after)
         if request.order is not None and not request.only_faceted:   # only_faceted comes first (nidx_text/src/reader.rs:405-414)
-            return self._search_ordered(request, terms, params, phrases)
+            return self._search_ordered(request, handles, terms, params, phrases)
         hits = None
         if _facet_request(request.faceted):
-            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, phrases=phrases)
+            resp.facets, hits = self._facets(handles, request.faceted, terms, max(k, 0) + 1, params, phrases=phrases)
         if request.only_faceted:   # only the facets: no results, total 0 (nidx_text/src/reader.rs:407-414, search_response.rs:111-124)
             return DocumentSearchResponse(facets=resp.facets)
         if not (terms or phrases) or k <= 0:
@@ -454,13 +521,13 @@ class TextSearcher:
         qt = np.asarray(terms, dtype=np.uint32)
         qo = np.asarray([0, len(terms)], dtype=np.uint32)
         merged = []
-        for ord_, seg in enumerate(self.segments):
+        for ord_, seg in enumerate(handles):
             if hits is not None:   # the faceted pass already returned this segment's top-k and Count
                 docs, scores, counts, total = hits[ord_]
             elif phrases:
-                docs, scores, counts, total = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, docaddr_base=ord_ << 32, **params)
+                docs, scores, counts, total = seg.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, docaddr_base=ord_ << 32, **params)
             else:
-                docs, scores, counts, total = seg._gpu.search(qt, qo, k + 1, docaddr_base=ord_ << 32, **params)
+                docs, scores, counts, total = seg.search(qt, qo, k + 1, docaddr_base=ord_ << 32, **params)
             resp.total += int(total[0])
             merged += [(-float(scores[0, i]), ord_, int(docs[0, i])) for i in range(int(counts[0]))]
         merged.sort()  # score desc, then segment_ord, then doc: lower docaddr first
@@ -474,7 +541,7 @@ class TextSearcher:
         return resp
 
 
-    def _search_ordered(self, request: DocumentSearchRequest, terms, params: dict, phrases=()) -> DocumentSearchResponse:
+    def _search_ordered(self, request: DocumentSearchRequest, handles: list, terms, params: dict, phrases=()) -> DocumentSearchResponse:
         """TopDocs(k + 1) ordered by date beside Count (and the FacetCollector) in one pass per segment; an empty body lists every
         alive document.  convert_int_order (nidx_text/src/reader.rs:226-287): no min_score, next_page = total > k."""
         order, k = request.order, request.result_per_page
@@ -482,21 +549,21 @@ class TextSearcher:
         self._ensure_dates()
         hits = None
         if _facet_request(request.faceted):
-            resp.facets, hits = self._facets(request.faceted, terms, max(k, 0) + 1, params, order=order, phrases=phrases)
+            resp.facets, hits = self._facets(handles, request.faceted, terms, max(k, 0) + 1, params, order=order, phrases=phrases)
         if k <= 0:
             return resp
         qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
         rows = []
-        for ord_, seg in enumerate(self.segments):
+        for ord_, seg in enumerate(handles):
             if not (terms or phrases):
-                docs, dates, count, total = seg._gpu.list_ordered(k + 1, order.sort_by, order.type)
+                docs, dates, count, total = seg.list_ordered(k + 1, order.sort_by, order.type)
             else:
                 if hits is not None:
                     d2, t2, c2, tot2 = hits[ord_]
                 elif phrases:
-                    d2, t2, c2, tot2 = seg._gpu.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, mode=params["mode"], order=(order.sort_by, order.type))
+                    d2, t2, c2, tot2 = seg.search_phrases(qt, qo, [(0, p) for p in phrases], k + 1, mode=params["mode"], order=(order.sort_by, order.type))
                 else:
-                    d2, t2, c2, tot2 = seg._gpu.search_ordered(qt, qo, k + 1, order.sort_by, order.type, params["mode"])
+                    d2, t2, c2, tot2 = seg.search_ordered(qt, qo, k + 1, order.sort_by, order.type, params["mode"])
                 docs, dates, count, total = d2[0], t2[0], int(c2[0]), int(tot2[0])
             resp.total += int(total)
             rows += [(date_sort_key(int(dates[i]), order.type), ord_, int(docs[i]), int(dates[i])) for i in range(count)]
@@ -521,6 +588,14 @@ def _prefix_range(keys: list, prefix: bytes, facet: bool):
         return lo, bisect.bisect_left(keys, prefix + b"\x01")
     stem = prefix.rstrip(b"\xff")   # the least byte string above every key that starts with `prefix`
     return lo, bisect.bisect_left(keys, stem[:-1] + bytes([stem[-1] + 1])) if stem else len(keys)
+
+
+def _node_array(flat: list):
+    """Flat pre-order nodes (kind, n, lo, hi, terms) -> the ctypes nidx_prefilter_node array."""
+    nodes = (_lib.PrefilterNode * len(flat))()
+    for i, (kind, n, lo, hi, terms) in enumerate(flat):
+        nodes[i].kind, nodes[i].n, nodes[i].lo, nodes[i].hi, nodes[i].terms = kind, n, lo, hi, terms
+    return nodes
 
 
 class _PrefilterIndex:
@@ -560,9 +635,14 @@ class _PrefilterIndex:
         self._joins = weakref.WeakKeyDictionary()
 
     # ---- filter_to_query (nidx_text/src/search_query.rs:156-217) -> nidx_prefilter_node, pre-order ---------------------------------
-    def compile(self, expr):
-        """-> (ctypes PrefilterNode array, keep-alive list, whether a phrase is used)."""
+    def compile(self, expr, security: Optional[list] = None):
+        """-> (ctypes PrefilterNode array, keep-alive list, whether a phrase is used).  security: flat nodes
+        (TextSearcher.security_nodes) ANDed with expr; expr may then be None."""
         flat, keep = [], []
+        if security is not None:
+            if expr is not None:
+                flat.append((_lib.NIDX_P_AND, 2, 0, 0, None))
+            flat += security
         phrases = False
         vocab = self.searcher.vocab
 
@@ -626,11 +706,9 @@ class _PrefilterIndex:
             else:
                 raise ValueError(f"filter expression without a known expression: {kind!r}")
 
-        walk(expr)
-        nodes = (_lib.PrefilterNode * len(flat))()
-        for i, (kind, n, lo, hi, terms) in enumerate(flat):
-            nodes[i].kind, nodes[i].n, nodes[i].lo, nodes[i].hi, nodes[i].terms = kind, n, lo, hi, terms
-        return nodes, keep, phrases
+        if expr is not None:
+            walk(expr)
+        return _node_array(flat), keep, phrases
 
     # ---- hand-off to the vector index ---------------------------------------------------------------------------------------
     def n_docs_total(self) -> int:
