@@ -892,8 +892,9 @@ static auto pick_ng(int ld, F inst) {
 }
 
 typedef void (*hs_kernel_t)(VecDev, GraphDev, SearchArgs);
-static hs_kernel_t pick_search_kernel(int ld) {
-    return pick_ng<1, 2, 3, 4, 6, 8>(ld, [](auto ng) -> hs_kernel_t { return hnsw_search_kernel<ng>; });
+// defer: closest_up_nodes may settle neighbours on the kept layer-0 set (hnsw_search_kernel's DEFER)
+static hs_kernel_t pick_search_kernel(int ld, bool defer = false) {
+    return pick_ng<1, 2, 3, 4, 6, 8>(ld, [defer](auto ng) -> hs_kernel_t { return defer ? hnsw_search_kernel<ng, true> : hnsw_search_kernel<ng>; });
 }
 
 // w4: the 4-warp CTA shape (quantised_walk)
@@ -1334,7 +1335,9 @@ struct VecCall {
             return fail(NIDX_EINVAL, "HNSW search needs %zu bytes of shared memory (ef=%d, k=%d, dim=%d): too large", smem, ef0, k, s->d);
         VecDev Vh = V;   // with the screening copy attached
         int r = attach_half_copy(s, &Vh);
-        hs_kernel_t kern = pick_search_kernel(s->ld);
+        // deferral needs the fp16 copy's walk and pops that are never rejected (hs_can_defer)
+        const bool defer = Vh.hvecs != nullptr && !bits && p->with_duplicates && !s->cfg.multi_vector;
+        hs_kernel_t kern = pick_search_kernel(s->ld, defer);
         int grid = 0;
         if (!r) r = walk_grid(kern, HS_THREADS, smem, &grid);
         if (r) return r;

@@ -89,6 +89,23 @@ struct VisitedSet {
             if (old == y) return false;
         }
     }
+
+    // closest_up_nodes on top of the layer-0 walk's set (hs_closest_up<DEFER>): the ids it has reached carry MARK (ids < 2^31 - 1,
+    // so y | MARK != NIL).  0 if y was reached before (or the table is full, as insert), 1 if y was not in the table, 2 if only
+    // the layer-0 walk had visited it.
+    static constexpr uint32_t MARK = 0x80000000u;
+    __device__ int mark(uint32_t y, int count, bool& overflow) const {
+        if (count >= limit) { overflow = true; return 0; }
+        for (uint32_t h = slot(y);; h = (h + 1) & mask) {
+            uint32_t old = atomicCAS(&slots[h], NIL, y | MARK);
+            if (old == NIL) return 1;
+            if (old == y) {
+                old = atomicCAS(&slots[h], y, y | MARK);
+                if (old == y) return 2;
+            }
+            if (old == (y | MARK)) return 0;
+        }
+    }
 };
 
 // What one expansion leaves for hs_merge and for the code after it.  There are two records, used by alternate hops (the parity of
@@ -202,10 +219,11 @@ __device__ inline void hs_flush_counters(const SearchCtx& c, unsigned long long*
 }
 
 // Start a layer search (or closest_up_nodes) on the list in c.A: every entry unexpanded, the visited set `vis` = the list's ids,
-// both hop records reset.
-__device__ inline void hs_reseed(SearchCtx& c, const VisitedSet& vis) {
+// both hop records reset.  MARKED: the list's ids are marked (VisitedSet::mark), in the table as it stands when `keep`.
+template <bool MARKED = false>
+__device__ inline void hs_reseed(SearchCtx& c, const VisitedSet& vis, bool keep = false) {
     __syncthreads();
-    vis.clear();
+    if (!(MARKED && keep)) vis.clear();
     if (threadIdx.x == 0) {
         *c.s_hash_count = 0; *c.s_best = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL;
         c.hops[0].clear(); c.hops[1].clear();
@@ -216,7 +234,8 @@ __device__ inline void hs_reseed(SearchCtx& c, const VisitedSet& vis) {
     for (int i = threadIdx.x; i < len; i += blockDim.x) {
         uint64_t key = c.A[i] | 1ull;
         c.A[i] = key;
-        vis.insert(key_id(key), 0, ov);
+        if (MARKED) vis.mark(key_id(key), 0, ov);
+        else vis.insert(key_id(key), 0, ov);
     }
     __syncthreads();
     if (threadIdx.x == 0) *c.s_hash_count = len;
@@ -259,7 +278,9 @@ __device__ inline int hs_prefetch_next(const GraphDev& G, SearchCtx& c, int laye
 // The hop's record: warp 0 resets it before the first barrier, the scoring after it adds the admitted keys.
 // LEAN (the layer search's hot loop): the list length arrives in a register, so that hs_merge needs no barrier after thread 0 has
 // published the new length -- three barriers per expansion instead of four.
-template <bool CU, int NG, int W = HS_WARPS, bool LEAN = false>
+// DEFER (CU, hs_closest_up<.., true>): visits are marked (VisitedSet::mark), and a neighbour only the layer-0 walk had visited is
+// settled without its row.
+template <bool CU, int NG, int W = HS_WARPS, bool LEAN = false, bool DEFER = false>
 __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& c, uint32_t node, int layer, int ef, float min_score, int best, int len_in = -1) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int stride = G.stride(layer);
@@ -275,7 +296,12 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
         for (int e0 = 0; e0 < stride; e0 += 32) {
             uint32_t y = NIL;
             if (e0 + lane < stride) y = hit ? prow[e0 + lane] : __ldg(row + e0 + lane);
-            bool fresh = (y != NIL) && c.vis.insert(y, visited, ov);
+            bool fresh;
+            if (DEFER) {   // todo_id carries MARK for a neighbour to settle without its row
+                const int m = y != NIL ? c.vis.mark(y, visited, ov) : 0;
+                fresh = m != 0;
+                if (m == 2) y |= VisitedSet::MARK;
+            } else fresh = (y != NIL) && c.vis.insert(y, visited, ov);
             unsigned mask = __ballot_sync(0xFFFFFFFFu, fresh);
             if (fresh) c.todo_id[ntodo + __popc(mask & ((1u << lane) - 1))] = y;
             ntodo += __popc(mask);
@@ -316,11 +342,13 @@ __device__ inline void hs_expand(const VecDev& V, const GraphDev& G, SearchCtx& 
     // each; no registers held, unlike a second row in flight).  Under the screen the row read first is the fp16 one.
     const int lines = screen ? (V.ldh * 2 + 127) >> 7 : (V.ld * 4 + 127) >> 7;
     for (int j = warp + W; j < ntodo; j += W) {
+        if (DEFER && (c.todo_id[j] & VisitedSet::MARK)) continue;
         const char* rowp = screen ? reinterpret_cast<const char*>(hrow(c.todo_id[j])) : reinterpret_cast<const char*>(frow(c.todo_id[j]));
         for (int l = lane; l < lines; l += 32) prefetch_l2(rowp + (size_t)l * 128);
     }
     for (int j = warp; j < ntodo; j += W) {
         uint32_t y = c.todo_id[j];
+        if (DEFER && (y & VisitedSet::MARK)) { if (lane == 0) skip(j); continue; }
         float vnorm;
         if (screen) {
             float4 r = __ldg(V.hrec + y);
@@ -436,11 +464,37 @@ __device__ inline bool hs_passes(const VecDev& V, const SearchArgs& a, uint32_t 
     return true;
 }
 
+// Whether closest_up_nodes may run on the kept layer-0 set (DEFER below), for the list the dense layer-0 walk left in c.A and
+// its visited set in c.vis; every thread, before hs_reseed's barrier.  Only hnsw_search_kernel<NG, true> asks, which the host
+// launches only when every pop is accepted (dense_walk) and the fp16 copy is attached.
+//   The walk ends only when every list entry has been expanded, so every neighbour of a list entry is in its set, and one outside
+//   the final list was refused (s <= worst, a float comparison), screened out or evicted: its key is at most make_key(b, y) with
+//   b = s_w, the last entry's score (the worst only improves), or +0 when s_w = -0 (a float refusal lets +0 pass a worst of -0).
+//   When every pop is accepted (no filter, duplicates allowed, one vector per paragraph, no NaN in the list; a NaN score is
+//   never admitted) closest_up_nodes pops at most k entries and expands at most k - 1.  When moreover A[k-1] scores above b, one
+//   of A[0, k) outranks every such neighbour at each pop, so none is ever popped or affects a pop: it can be settled without its
+//   row.  Each expansion adds at most s0 ids to the table and s0 - 1 entries to the list, so the last two tests keep the table
+//   below its insert limit and the list within cu_cap: no overflow, and no truncation that could differ from the f32 walk's.
+__device__ inline bool hs_can_defer(const VecDev& V, const GraphDev& G, const SearchCtx& c, const SearchArgs& a) {
+    const int len = *c.s_len;
+    if (len != a.ef0) return false;
+    const float top = key_score(c.A[0]), sw = key_score(c.A[len - 1]);
+    if (top != top || sw != sw) return false;
+    const float b = __float_as_uint(sw) == 0x80000000u ? 0.0f : sw;
+    const int grow = (a.k - 1) * G.s0;
+    return (uint32_t)(c.A[a.k - 1] >> 32) > ordered_bits(b) && *c.s_hash_count + grow <= c.vis.limit && len + grow <= a.cu_cap;
+}
+
 // hnsw/search.rs:188-240.  Results go straight to out_ids/out_scores (already descending).
-template <int NG, int W = HS_WARPS>
-__device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, uint32_t* out_ids, float* out_scores) {
+// DEFER: closest_up_nodes' visits are marked in the table, and `keep` (hs_can_defer) keeps the layer-0 walk's set under them, so a
+// neighbour is new exactly when the reference's BitSet says so, and a new neighbour the layer-0 walk had visited is counted as a
+// similarity settled without its row (as the screen's) and not listed.  Without `keep` the table is cleared first and no
+// neighbour is settled, as without DEFER: one walk serves both cases, so the kernel carries one copy of it.
+template <int NG, int W = HS_WARPS, bool DEFER = false>
+__device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, uint32_t* out_ids, float* out_scores,
+                                    bool keep = false) {
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    hs_reseed(c, c.vis);
+    hs_reseed<DEFER>(c, c.vis, keep);
     int nacc = 0;
     while (true) {
         int len = *c.s_len;
@@ -460,19 +514,19 @@ __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCt
         __syncthreads();
         nacc += *c.s_flag;
         if (nacc == a.k) break;  // 214
-        hs_expand<true, NG, W>(V, G, c, node, 0, 0, a.min_score, 0);
+        hs_expand<true, NG, W, false, DEFER>(V, G, c, node, 0, 0, a.min_score, 0);
         hs_merge<true>(c, a.cu_cap, 0, c.last_hop().ntodo);
     }
     return nacc;
 }
 
 // The tail of HnswSearcher::search for query q: closest_up_nodes on the list in c.A (search.rs:369-375), the final stable sort
-// (search.rs:381) and the NIL padding of the outputs.
-template <int NG, int W = HS_WARPS>
+// (search.rs:381) and the NIL padding of the outputs.  L0: closest_up_nodes may defer (hnsw_search_kernel<NG, true>).
+template <int NG, int W = HS_WARPS, bool L0 = false>
 __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, SearchCtx& c, const SearchArgs& a, unsigned int q) {
     uint32_t* oi = a.out_ids + (size_t)q * a.k;
     float* os = a.out_scores + (size_t)q * a.k;
-    int nacc = hs_closest_up<NG, W>(V, G, c, a, oi, os);
+    int nacc = hs_closest_up<NG, W, L0>(V, G, c, a, oi, os, L0 && hs_can_defer(V, G, c, a));
     __syncthreads();
     // search.rs:381 `filtered_result.sort_by(|a, b| b.1.total_cmp(&a.1))`: stable, descending.
     // (closest_up_nodes can accept a late-found neighbour that outranks earlier results.)
@@ -498,7 +552,10 @@ __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, Searc
 }
 
 // HS_WARPS = 8 warps per CTA, one row per warp in flight, 4 CTAs per SM (528 queries resident on 132 SMs).
-template <int NG>
+// DEFER: closest_up_nodes may settle neighbours on the kept layer-0 set (hs_can_defer).  The host launches it only for queries
+// whose pops are all accepted (no filter, duplicates allowed, one vector per paragraph) with the fp16 copy attached; every other
+// walk, and the build, runs the kernel without it.
+template <int NG, bool DEFER = false>
 __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, GraphDev G, SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
     SearchCtx c;
@@ -553,7 +610,7 @@ __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, Gr
         if (a.mode == 1 && threadIdx.x == 0)
             for (int layer = (int)G.entry_layer + 1; layer <= top && layer < HS_MAX_LAYERS; ++layer) a.found_count[(size_t)q * HS_MAX_LAYERS + layer] = 0;
 
-        if (a.mode == 0) hs_emit_results<NG>(V, G, c, a, q);
+        if (a.mode == 0) hs_emit_results<NG, HS_WARPS, DEFER>(V, G, c, a, q);
     }
     hs_flush_counters(c, a.counters);
     // [6] = f32 rows read for a similarity (n_skip lives in lane 0 of every warp, as n_dist)
