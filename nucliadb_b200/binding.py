@@ -12,11 +12,13 @@ Reference:
   nidx/nidx_text/src/resource_indexer.rs:22-91                    Resource.texts -> one document per field
   nidx/nidx_paragraph/src/resource_indexer.rs:33-131              Resource.paragraphs -> one document per paragraph (text[start:end])
   nidx/nidx_text/src/resource_indexer.rs:49-62                    Resource.security -> the access groups of its documents
+  nidx/nidx_json/src/resource_indexer.rs, lib.rs                  Resource.json_fields -> one JSON document per resource
+  nidx/src/searcher/query_planner/prefilter.rs:24-72              SearchRequest.json_filter, combined with the text prefilter
 
 What is kept of the reference's machinery is the INTERFACE: metadata lives in memory (no PostgreSQL), every index message
 becomes one immutable segment per index (as in the reference), deletions are (key, seq) pairs applied to older segments, and
 "sync" re-opens the searchers (index_cache.rs:180-200).  Scheduler, worker, merges-in-the-background, NATS, object stores other
-than the local file store, relations / JSON / graph / suggest are outside the hot path (SURVEY 8) and answer UNIMPLEMENTED.
+than the local file store, relations / graph / suggest are outside the hot path (SURVEY 8) and answer UNIMPLEMENTED.
 """
 from __future__ import annotations
 
@@ -30,6 +32,7 @@ from typing import Optional
 
 import numpy as np
 
+from . import json_index as J
 from . import nidx_protos as P
 from . import text as T
 from . import vector as V
@@ -52,6 +55,10 @@ class _Shard:
     paragraph_segments: list = field(default_factory=list)   # [[TextDoc]] (+ paragraph positions in .field / extra)
     paragraph_meta: dict = field(default_factory=dict)       # paragraph id -> (field, start, end, index, split, labels, metadata bytes)
     deleted_resources: set = field(default_factory=set)
+    json_docs: list = field(default_factory=list)            # [(resource id, [(path, kind, value)], seq)]
+    resource_groups: dict = field(default_factory=dict)      # resource id -> access groups of its latest index message
+    json_deletions: list = field(default_factory=list)       # [(deletion key, seq)]: json_fields_to_delete and resource deletions
+    json_index: Optional[J.JsonIndex] = None
     text_searcher: Optional[T.TextSearcher] = None
     paragraph_searcher: Optional[T.ParagraphSearcher] = None
 
@@ -90,6 +97,17 @@ def _doc_matches(e, doc: T.TextDoc) -> bool:
     if kind == "bool_or":
         return any(_doc_matches(o, doc) for o in e.bool_or.operands)
     return True
+
+
+def _json_deletes(key: str, rid: str) -> bool:
+    """JsonDeletionQueryBuilder (nidx_json/src/lib.rs): a key's first 32 characters (the whole key when shorter) are a resource
+    UUID, and every JSON document of that resource id goes; a key that does not parse as a UUID deletes nothing."""
+    raw = key[:32] if len(key) > 32 else key
+    try:
+        _uuid.UUID(raw)
+    except ValueError:
+        return False
+    return raw == rid
 
 
 def merge_facets(shards_facets) -> dict:
@@ -190,9 +208,13 @@ class NidxBinding:
             for vi in shard.vectorsets.values():
                 vi.deletions.append((msg.resource, seq))
             shard.deleted_resources.add((msg.resource, seq))
+            shard.json_deletions.append((msg.resource, seq))
             return
         res = self._load_resource(msg.storage_key)
         rid = res.resource.uuid
+        # the JSON document (nidx_json/src/resource_indexer.rs), flattened first: invalid JSON fails the message before any index
+        # changes.  Its deletions are json_fields_to_delete only (JsonIndexer::deletions_for_resource), not the re-index itself
+        json_entries = J.flatten({k: v.value for k, v in res.json_fields.items()}) if res.json_fields and not res.skip_json else None
         # a re-indexed resource replaces its older copies: prefixes to delete, applied to OLDER segments only (seq rule, lib.rs:188-199)
         for vi in shard.vectorsets.values():
             for key in list(res.vectors_to_delete_in_all_vectorsets) or [rid]:
@@ -234,6 +256,10 @@ class NidxBinding:
                     shard.paragraph_meta[(rid, "/" + fid if not fid.startswith("/") else fid, len(pdocs) - 1, seq)] = (pid, par)
             if pdocs:
                 shard.paragraph_segments.append((pdocs, seq))
+        shard.json_deletions.extend((key, seq) for key in res.json_fields_to_delete)
+        if json_entries is not None:
+            shard.json_docs.append((rid, json_entries, seq))
+        shard.resource_groups[rid] = groups
 
     # ---- sync (lib.rs:113-126; searcher/sync.rs + index_cache.rs:180-200: searchers are re-opened, never mutated) --------------
     def wait_for_sync(self) -> None:
@@ -257,6 +283,13 @@ class NidxBinding:
         ps = self._alive(shard.paragraph_segments, shard.deleted_resources)
         shard.text_searcher = T.TextSearcher.open(ts, device=self.device) if ts else None
         shard.paragraph_searcher = T.ParagraphSearcher.open(ps, device=self.device) if ps else None
+        # a JSON document carries its resource's groups of the latest message, which may have changed security without touching
+        # the JSON document (skip_json, or no json_fields): the JSON pass must never see groups the text documents no longer have
+        jd = [(rid, entries, shard.resource_groups.get(rid, ())) for rid, entries, seq in shard.json_docs
+              if not any(dseq > seq and _json_deletes(key, rid) for key, dseq in shard.json_deletions)]
+        if shard.json_index is not None:
+            shard.json_index.close()
+        shard.json_index = J.JsonIndex(jd, device=self.device) if jd else None
 
     # ---- NidxSearcher.Search (shard_search.rs:60-241 + shard_merge.rs) ---------------------------------------------------------
     def search(self, request):
@@ -299,6 +332,35 @@ class NidxBinding:
             else:   # a stand-in for libnidx_b200.so without the prefilter (the ABI emulator of the host-logic tests): the host loop
                 fields = [V.FieldId(_uuid.UUID(d.uuid), d.field) for seg in shard.text_searcher.segments for d in seg.docs if _doc_matches(req.field_filter, d)]
                 prefilter = V.PrefilterResult.some(fields) if fields else V.PrefilterResult.none()
+        # the JSON prefilter (query_planner/prefilter.rs:24-72): the JSON resource set, ANDed on the device with security, combined
+        # with the text result under filter_operator (PrefilterResult::combine).  Security is applied outside the combination:
+        # AND(security, op(field_filter, json)), so a security filter is never widened (DESIGN 7)
+        masks = None
+        if req.HasField("json_filter"):
+            J.validate(req.json_filter)
+            op_or = req.filter_operator == P.FILTER_OR
+            jx = shard.json_index
+            res_bits, found = None, 0
+            if jx is not None:
+                _, found, res_bits = jx.prefilter(req.json_filter, security)
+            text = prefilter.device_bits if prefilter.kind == "some" else None
+            if prefilter.kind == "some" and text is None:
+                raise ValueError("json_filter needs the device prefilter")
+            if found == 0:   # combine(text, {}, op): the text result under OR, None under AND
+                if not op_or:
+                    prefilter = V.PrefilterResult.none()
+                elif text is not None and req.paragraph and shard.paragraph_searcher is not None:
+                    masks = shard.paragraph_searcher.json_masks(security, text[1], text[0], None, None, True)
+            elif (prefilter.kind == "none" and not op_or) or (prefilter.kind == "all" and op_or):
+                pass
+            else:
+                # text None under OR is the JSON set alone; text All under AND is the JSON set ANDed with every field
+                prefilter = V.PrefilterResult.from_json(text, jx, res_bits, op_or and text is not None)
+                if req.paragraph and shard.paragraph_searcher is not None:
+                    masks = shard.paragraph_searcher.json_masks(security, text[1] if text else None, text[0] if text else None, jx, res_bits,
+                                                                op_or and text is not None)
+            if prefilter.kind == "none":   # IndexQueries::apply_prefilter: the sections are absent
+                return out
         if len(req.vector):
             name = req.vectorset
             if name not in shard.vectorsets:
@@ -319,7 +381,7 @@ class NidxBinding:
                 after = T.SearchAfter(score=req.search_after.score, tie_break="keep_after", docaddr=int(req.search_after.docaddr))
             out["paragraph"] = shard.paragraph_searcher.search(T.DocumentSearchRequest(body=req.body, result_per_page=k, min_score=float(req.min_score_bm25), search_after=after,
                                                                                        faceted=list(req.faceted.labels), only_faceted=bool(req.only_faceted), order=order,
-                                                                                       security=security))
+                                                                                       security=security), masks=masks)
         return out
 
     def _merge(self, req, parts):
@@ -385,6 +447,9 @@ class NidxBinding:
                             if seg._gpu is not None:
                                 seg._gpu.close()
                 shard.text_searcher = shard.paragraph_searcher = None
+                if shard.json_index is not None:
+                    shard.json_index.close()
+                    shard.json_index = None
             self._shards.clear()
 
     def __del__(self):   # lib.rs Drop: the cancellation token

@@ -155,4 +155,58 @@ __global__ void prefilter_join_kernel(const uint64_t* __restrict__ doc_bits, con
     }
 }
 
+// JSON filters (nidx_txt_resource_bits, nidx_vec_prefilter_resources, nidx_txt_join_mask): a JSON document's result is a resource.
+// doc_bits [n_docs] -> out (resource bits, zeroed by the caller): res_ord[d] = the document's resource ord (>= n_res: none).
+__global__ void prefilter_resource_kernel(const uint64_t* __restrict__ doc_bits, const uint32_t* __restrict__ res_ord, uint64_t n_docs, uint64_t n_res,
+                                          uint64_t* __restrict__ out) {
+    for (uint64_t d = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; d < n_docs; d += (uint64_t)gridDim.x * blockDim.x) {
+        if (!((__ldg(doc_bits + (d >> 6)) >> (d & 63)) & 1ull)) continue;
+        const uint64_t r = __ldg(res_ord + d);
+        if (r < n_res) atomicOr(reinterpret_cast<unsigned long long*>(out) + (r >> 6), 1ull << (r & 63));
+    }
+}
+
+// res_bits [n_res] -> out (paragraph bits, zeroed by the caller): resource r's paragraphs are post[ranges[2 r] .. ranges[2 r + 1]) (the
+// postings of the field index keys that start with its 16 uuid bytes: one contiguous run of keys).
+__global__ void prefilter_res_join_kernel(const uint64_t* __restrict__ res_bits, uint64_t n_res, const uint64_t* __restrict__ ranges,
+                                          const uint32_t* __restrict__ post, uint64_t* __restrict__ out) {
+    for (uint64_t r = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; r < n_res; r += (uint64_t)gridDim.x * blockDim.x) {
+        if (!((__ldg(res_bits + (r >> 6)) >> (r & 63)) & 1ull)) continue;
+        for (uint64_t i = __ldg(ranges + 2 * r), e = __ldg(ranges + 2 * r + 1); i < e; ++i) {
+            const uint32_t p = __ldg(post + i);
+            atomicOr(reinterpret_cast<unsigned long long*>(out) + (p >> 6), 1ull << (p & 63));
+        }
+    }
+}
+
+// One mask over n documents: bit d = and_bits[d] (NULL: 1) AND op(doc_bits[doc_join[d]] (doc_bits NULL: 1), res_bits[res_join[d]]),
+// a join entry of NIDX_NIL (or >= the bitset's length) reading 0; op: 0 AND, 1 OR.  out: [2 * words] 32-bit words, padding bits zero;
+// *count += set bits.  A warp writes one 32-bit word by ballot, as prefilter_eval_kernel does.
+__global__ void __launch_bounds__(PF_THREADS) join_mask_kernel(uint64_t n, const uint64_t* __restrict__ and_bits, const uint64_t* __restrict__ doc_bits,
+                                                               uint64_t n_doc_bits, const uint32_t* __restrict__ doc_join,
+                                                               const uint64_t* __restrict__ res_bits, uint64_t n_res, const uint32_t* __restrict__ res_join,
+                                                               int op, uint32_t* __restrict__ out, uint64_t n32, unsigned long long* count) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    unsigned long long local = 0;
+    for (uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < n32; w += n_warps) {
+        const uint64_t d = w * 32 + lane;
+        uint32_t bit = 0;
+        if (d < n) {
+            uint32_t t = 1;
+            if (doc_bits) {
+                const uint64_t j = __ldg(doc_join + d);
+                t = j < n_doc_bits ? (uint32_t)((__ldg(doc_bits + (j >> 6)) >> (j & 63)) & 1ull) : 0u;
+            }
+            const uint64_t r = __ldg(res_join + d);
+            const uint32_t j = r < n_res ? (uint32_t)((__ldg(res_bits + (r >> 6)) >> (r & 63)) & 1ull) : 0u;
+            bit = op ? (t | j) : (t & j);
+            if (and_bits) bit &= (uint32_t)((__ldg(and_bits + (d >> 6)) >> (d & 63)) & 1ull);
+        }
+        const uint32_t word = __ballot_sync(0xFFFFFFFFu, bit);
+        if (lane == 0) { out[w] = word; local += __popc(word); }
+    }
+    if (lane == 0 && local) atomicAdd(count, local);
+}
+
 }  // namespace nidx

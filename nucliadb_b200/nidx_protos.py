@@ -15,6 +15,8 @@ serialised by the reference's clients (``nidx_protos`` / ``nucliadb_protos``) de
     Resource, IndexParagraph(s), VectorSentence, ...       noderesources.proto:8-180
     IndexMetadata                                          noderesources.proto:17-20 (google.protobuf.Timestamp)
     Security (Resource.security, SearchRequest.security)   nucliadb_protos utils.proto: repeated string access_groups = 1
+    JsonFieldValue, Resource.json_fields / skip_json       noderesources.proto:13-15, 169-176
+    JsonFilterExpression, JsonFieldPathFilter              nodereader.proto:338-380 (SearchRequest.json_filter = 32)
 """
 from __future__ import annotations
 
@@ -22,7 +24,7 @@ from google.protobuf import descriptor_pb2, descriptor_pool, message_factory, ti
 
 _F = descriptor_pb2.FieldDescriptorProto
 _T = {"string": _F.TYPE_STRING, "bytes": _F.TYPE_BYTES, "int32": _F.TYPE_INT32, "int64": _F.TYPE_INT64, "uint32": _F.TYPE_UINT32, "uint64": _F.TYPE_UINT64,
-      "float": _F.TYPE_FLOAT, "bool": _F.TYPE_BOOL}
+      "float": _F.TYPE_FLOAT, "double": _F.TYPE_DOUBLE, "bool": _F.TYPE_BOOL}
 
 
 def _field(msg, name, number, typ, repeated=False, oneof=None, optional=False):
@@ -71,6 +73,8 @@ def _build():
                                             dependency=["google/protobuf/timestamp.proto", "nucliadb_protos/utils.proto"])
     m = fd.message_type.add(name="TextInformation")           # :8-11
     _field(m, "text", 1, "string"); _field(m, "labels", 2, "string", repeated=True)
+    m = fd.message_type.add(name="JsonFieldValue")            # :13-15: a JSON-encoded value
+    _field(m, "value", 1, "string")
     m = fd.message_type.add(name="ResourceID")                # :36-39
     _field(m, "shard_id", 1, "string"); _field(m, "uuid", 2, "string")
     m = fd.message_type.add(name="IndexMetadata")             # :17-20
@@ -105,6 +109,8 @@ def _build():
     _field(m, "shard_id", 11, "string"); _field(m, "security", 14, ".utils.Security", optional=True)
     _field(m, "texts_to_delete", 17, "string", repeated=True)
     _field(m, "skip_texts", 18, "bool"); _field(m, "skip_paragraphs", 19, "bool")
+    _map(m, ".noderesources.Resource", "json_fields", 22, "string", ".noderesources.JsonFieldValue")
+    _field(m, "json_fields_to_delete", 23, "string", repeated=True); _field(m, "skip_json", 24, "bool")
     pool.Add(fd)
 
     # ---- nodereader.proto ------------------------------------------------------------------------------------------------
@@ -171,6 +177,25 @@ def _build():
     _field(m, "date", 7, ".nodereader.FilterExpression.DateRangeFilter", oneof=0)
     _field(m, "facet", 8, ".nodereader.FilterExpression.FacetFilter", oneof=0)
     _field(m, "resource_field_prefix", 9, ".nodereader.FilterExpression.ResourceFieldPrefixFilter", oneof=0)
+    m = fd.message_type.add(name="JsonFieldPathFilter")       # :338-367
+    _field(m, "field_id", 1, "string"); _field(m, "json_path", 2, "string")
+    ir = m.nested_type.add(name="IntegerRangePredicate"); _field(ir, "lower", 1, "int64", optional=True); _field(ir, "upper", 2, "int64", optional=True)
+    fr = m.nested_type.add(name="FloatRangePredicate"); _field(fr, "lower", 1, "double", optional=True); _field(fr, "upper", 2, "double", optional=True)
+    dr = m.nested_type.add(name="DateRangePredicate")
+    _field(dr, "lower", 1, ".google.protobuf.Timestamp", optional=True); _field(dr, "upper", 2, ".google.protobuf.Timestamp", optional=True)
+    m.oneof_decl.add().name = "predicate"
+    _field(m, "text", 3, "string", oneof=0); _field(m, "boolean", 6, "bool", oneof=0); _field(m, "int", 8, "int64", oneof=0)
+    _field(m, "float", 9, "double", oneof=0); _field(m, "date", 10, ".google.protobuf.Timestamp", oneof=0)
+    _field(m, "int_range", 4, ".nodereader.JsonFieldPathFilter.IntegerRangePredicate", oneof=0)
+    _field(m, "float_range", 5, ".nodereader.JsonFieldPathFilter.FloatRangePredicate", oneof=0)
+    _field(m, "date_range", 7, ".nodereader.JsonFieldPathFilter.DateRangePredicate", oneof=0)
+    m = fd.message_type.add(name="JsonFilterExpression")      # :369-380
+    lst = m.nested_type.add(name="List"); _field(lst, "operands", 1, ".nodereader.JsonFilterExpression", repeated=True)
+    m.oneof_decl.add().name = "expr"
+    _field(m, "bool_and", 1, ".nodereader.JsonFilterExpression.List", oneof=0)
+    _field(m, "bool_or", 2, ".nodereader.JsonFilterExpression.List", oneof=0)
+    _field(m, "bool_not", 3, ".nodereader.JsonFilterExpression", oneof=0)
+    _field(m, "path", 4, ".nodereader.JsonFieldPathFilter", oneof=0)
     m = fd.message_type.add(name="SearchAfter")               # :382-386
     _field(m, "score", 1, "float"); _field(m, "shard_id", 2, "bytes"); _field(m, "docaddr", 3, "uint64")
     m = fd.message_type.add(name="SearchRequest")             # :388-437
@@ -182,6 +207,7 @@ def _build():
     _field(m, "min_score_semantic", 23, "float"); _field(m, "security", 24, ".utils.Security", optional=True); _field(m, "min_score_bm25", 25, "float")
     _field(m, "field_filter", 26, ".nodereader.FilterExpression", optional=True); _field(m, "paragraph_filter", 27, ".nodereader.FilterExpression", optional=True)
     _field(m, "filter_operator", 28, "enum:.nodereader.FilterOperator"); _field(m, "search_after", 35, ".nodereader.SearchAfter", optional=True)
+    _field(m, "json_filter", 32, ".nodereader.JsonFilterExpression", optional=True)
     m = fd.message_type.add(name="SearchResponse")            # :476-488
     _field(m, "document", 1, ".nodereader.DocumentSearchResponse"); _field(m, "paragraph", 2, ".nodereader.ParagraphSearchResponse")
     _field(m, "vector", 3, ".nodereader.VectorSearchResponse"); _field(m, "shard_ids", 6, "string", repeated=True)
@@ -235,6 +261,9 @@ VectorSearchResponse = _cls("nodereader.VectorSearchResponse")
 SentenceMetadata = _cls("noderesources.SentenceMetadata")
 Resource = _cls("noderesources.Resource")
 Security = _cls("utils.Security")
+JsonFieldValue = _cls("noderesources.JsonFieldValue")
+JsonFilterExpression = _cls("nodereader.JsonFilterExpression")
+JsonFieldPathFilter = _cls("nodereader.JsonFieldPathFilter")
 IndexMessage = _cls("nodewriter.IndexMessage")
 NewShardRequest = _cls("nodewriter.NewShardRequest")
 ShardCreated = _cls("noderesources.ShardCreated")

@@ -185,6 +185,26 @@ class VectorSegment:
                                                   C.byref(matching), stream))
         return out, matching.value
 
+    def prefilter_resources(self, doc_bits, join, n_docs: int, doc_op, res_bits, res_ranges, n_res: int, n_paragraphs: int, formula=None,
+                            op=_lib.NIDX_F_AND):
+        """nidx_vec_prefilter_resources: the paragraphs of the resources in res_bits (res_ranges: uint64 [n_res][2], each resource's
+        postings in the field index) combined under doc_op with those of the text documents in doc_bits (None: no text part), then
+        with `formula` under `op`, AND alive -> (paragraph bits, matching).  torch CUDA res_bits -> device path, numpy -> host path."""
+        on_device = _is_torch(res_bits)
+        mem, stream, alloc = _stage(self.cfg.device, on_device)
+        if not on_device:
+            res_bits = np.ascontiguousarray(res_bits, dtype=np.uint64)
+            res_ranges = np.ascontiguousarray(res_ranges, dtype=np.uint64)
+            if doc_bits is not None:
+                doc_bits = np.ascontiguousarray(doc_bits, dtype=np.uint64)
+                join = np.ascontiguousarray(join, dtype=np.uint32)
+        out = alloc((n_paragraphs + 63) // 64, np.uint64)
+        matching = C.c_uint64()
+        check(_lib.load().nidx_vec_prefilter_resources(self._h, ptr(doc_bits), n_docs if doc_bits is not None else 0, ptr(join), doc_op, ptr(res_bits),
+                                                       n_res, ptr(res_ranges), formula, 0 if formula is None else len(formula), op, ptr(out), mem,
+                                                       C.byref(matching), stream))
+        return out, matching.value
+
     # ---- search ----------------------------------------------------------------------------------------
     def search(self, queries, k: int, ef: int = 0, min_score: float = -1.0, with_duplicates=True, method=_lib.NIDX_METHOD_AUTO,
                filter_bits=None, filter_matching: int = 0, formula=None, out=None, stream: Optional[int] = None):
@@ -471,6 +491,34 @@ class TextSegment:
             out = alloc((self.n_docs + 63) // 64, np.uint64)
         matching = C.c_uint64()
         check(_lib.load().nidx_txt_prefilter(self._h, C.addressof(nodes), len(nodes), ptr(out), mem, C.byref(matching), stream))
+        return out, matching.value
+
+    def resource_bits(self, doc_bits, n_resources: int):
+        """nidx_txt_resource_bits: document bits -> the bits of their resource ords (uint64 words [(n_resources + 63) // 64]); a torch
+        CUDA tensor in -> a torch int64 tensor out (device path), numpy -> numpy."""
+        on_device = _is_torch(doc_bits)
+        mem, stream, alloc = _stage(self.device, on_device)
+        if not on_device:
+            doc_bits = np.ascontiguousarray(doc_bits, dtype=np.uint64)
+        out = alloc(max((n_resources + 63) // 64, 1), np.uint64)
+        check(_lib.load().nidx_txt_resource_bits(self._h, ptr(doc_bits), n_resources, ptr(out), mem, stream))
+        return out
+
+    def join_mask(self, and_bits, doc_bits, n_doc_bits: int, doc_join, res_bits, n_res: int, res_join, op=_lib.NIDX_F_AND):
+        """nidx_txt_join_mask: bit d = and_bits[d] AND op(doc_bits[doc_join[d]], res_bits[res_join[d]]) (and_bits / doc_bits None:
+        all set) -> (mask words, matching).  torch CUDA res_bits -> device path (every input a device tensor), numpy -> host path."""
+        on_device = _is_torch(res_bits)
+        mem, stream, alloc = _stage(self.device, on_device)
+        if not on_device:
+            res_bits, res_join = np.ascontiguousarray(res_bits, dtype=np.uint64), np.ascontiguousarray(res_join, dtype=np.uint32)
+            if and_bits is not None:
+                and_bits = np.ascontiguousarray(and_bits, dtype=np.uint64)
+            if doc_bits is not None:
+                doc_bits, doc_join = np.ascontiguousarray(doc_bits, dtype=np.uint64), np.ascontiguousarray(doc_join, dtype=np.uint32)
+        out = alloc(max((self.n_docs + 63) // 64, 1), np.uint64)
+        matching = C.c_uint64()
+        check(_lib.load().nidx_txt_join_mask(self._h, ptr(and_bits), ptr(doc_bits), n_doc_bits if doc_bits is not None else 0, ptr(doc_join),
+                                             ptr(res_bits), n_res, ptr(res_join), op, ptr(out), mem, C.byref(matching), stream))
         return out, matching.value
 
     def set_doc_keys(self, keys: Optional[np.ndarray]):

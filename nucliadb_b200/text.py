@@ -489,10 +489,61 @@ class TextSearcher:
         """-> (term ids, phrases as term-id lists).  nidx_text's QueryParser grammar is not restated: no phrases."""
         return self._terms(body), []
 
-    def search(self, request: DocumentSearchRequest) -> DocumentSearchResponse:
-        if request.security is None:
+    def _json_joins(self, text_index, json_index) -> list:
+        """Per segment, on the device: (doc_join, res_join), each document's bit in the text prefilter's output (text_index: the
+        shard's text _PrefilterIndex; NIL without a text document of its field) and its resource's ord in json_index.resource_ids
+        (NIL: none).  Each half is built once per (this searcher, text_index / json_index), vectorised, and kept in HBM."""
+        import torch
+
+        def lookup(keys_sorted, values, queries):
+            if len(keys_sorted) == 0:
+                return np.full(len(queries), _lib.NIL, dtype=np.uint32)
+            at = np.minimum(np.searchsorted(keys_sorted, queries), len(keys_sorted) - 1)
+            return np.where(keys_sorted[at] == queries, values[at], _lib.NIL).astype(np.uint32)
+
+        dev = torch.device("cuda", self.segments[0].device)
+        up = lambda a: torch.from_numpy(a.view(np.int32)).to(dev)   # noqa: E731
+        if getattr(self, "_res_join", None) is None or self._res_join[0] is not json_index:
+            rids = np.asarray(json_index.resource_ids if json_index is not None else [], dtype=str)
+            self._res_join = (json_index, [up(lookup(rids, np.arange(len(rids), dtype=np.uint32), np.asarray([d.uuid for d in s.docs], dtype=str)))
+                                           for s in self.segments])
+        if text_index is not None and (getattr(self, "_doc_join", None) is None or self._doc_join[0] is not text_index):
+            keys = np.concatenate([np.asarray([d.uuid + "\x01" + d.field for d in ts.docs], dtype=str) for ts in text_index.searcher.segments])
+            pos = np.concatenate([64 * off + np.arange(ts.n_docs, dtype=np.uint64) for ts, off in zip(text_index.searcher.segments, text_index.word_off)])
+            keys, first = np.unique(keys, return_index=True)   # a field's first document, as a dict's setdefault would keep
+            self._doc_join = (text_index, [up(lookup(keys, pos[first].astype(np.uint32), np.asarray([d.uuid + "\x01" + d.field for d in s.docs], dtype=str)))
+                                           for s in self.segments])
+        return [(self._doc_join[1][i] if text_index is not None else None, self._res_join[1][i]) for i in range(len(self.segments))]
+
+    def json_masks(self, security: Optional[Sequence[str]], text_bits, text_index, json_index, res_bits, op_or: bool) -> list:
+        """The per-segment masks of a search under SearchRequest.json_filter (nidx_txt_join_mask, on the device): bit d = the
+        security bits (when `security` is given) AND op(the text prefilter's bit of the document's field (text_bits None: every
+        field), the JSON prefilter's bit of its resource (res_bits over json_index.resource_ids; json_index None: no resource)),
+        op OR when op_or."""
+        import torch
+
+        sec = _node_array(self.security_nodes(security)) if security is not None else None
+        n_res = len(json_index.resource_ids) if json_index is not None else 0
+        dev = torch.device("cuda", self.segments[0].device)
+        if res_bits is None:
+            res_bits = torch.zeros(1, dtype=torch.int64, device=dev)
+        masks = []
+        for s, (doc_join, res_join) in zip(self.segments, self._json_joins(text_index if text_bits is not None else None, json_index)):
+            and_bits = None
+            if sec is not None:
+                and_bits = torch.empty(max((s.n_docs + 63) // 64, 1), dtype=torch.int64, device=dev)
+                s._gpu.prefilter(sec, out=and_bits)
+            mask, _ = s._gpu.join_mask(and_bits, text_bits, 0 if text_bits is None else text_bits.numel() * 64, doc_join, res_bits, n_res, res_join,
+                                       _lib.NIDX_F_OR if op_or else _lib.NIDX_F_AND)
+            masks.append(mask)
+        return masks
+
+    def search(self, request: DocumentSearchRequest, masks: Optional[list] = None) -> DocumentSearchResponse:
+        """masks (one device bitset per segment, as json_masks makes them) replace the security mask: the search runs on views
+        under them."""
+        if request.security is None and masks is None:
             return self._search(request, [s._gpu for s in self.segments])
-        views = self._security_views(request.security)
+        views = self._security_views(request.security) if masks is None else [s._gpu.view(m) for s, m in zip(self.segments, masks)]
         try:
             return self._search(request, views)
         finally:

@@ -99,9 +99,9 @@ class PrefilterResult:
     text documents as a bitset in HBM (`device_bits`: (the text index's prefilter state, the bits, the match count)); its `fields`
     are listed only when read, and VectorSearcher.search hands the bits to the vector segments without leaving the device."""
 
-    def __init__(self, kind: str, fields: Sequence[FieldId] = (), device_bits=None):
-        self.kind, self.device_bits = kind, device_bits
-        self._fields = None if device_bits is not None else list(fields)
+    def __init__(self, kind: str, fields: Sequence[FieldId] = (), device_bits=None, json=None):
+        self.kind, self.device_bits, self.json = kind, device_bits, json
+        self._fields = None if device_bits is not None or json is not None else list(fields)
 
     @property
     def fields(self) -> list:
@@ -117,6 +117,13 @@ class PrefilterResult:
     @classmethod
     def from_device(cls, index, bits, matching: int):
         return cls("some", device_bits=(index, bits, matching))
+
+    @classmethod
+    def from_json(cls, text, json_index, res_bits, op_or: bool):
+        """PrefilterResult::combine of a text result (`text`: its device_bits, or None for All) with the non-empty resource set of
+        a JSON prefilter (res_bits over json_index.resource_ids, in HBM) under AND (op_or False) or OR, kept on the device: the
+        hand-offs combine the bitsets themselves (OpenSegment.search_json, TextSearcher.json_masks)."""
+        return cls("some", json=(text, json_index, res_bits, op_or))
 
     @classmethod
     def all(cls):
@@ -415,6 +422,55 @@ class OpenSegment:
         c = int(counts[0].item())
         return ids[0, :c].cpu().numpy().view(np.uint32), scores[0, :c].cpu().numpy()
 
+    def json_ranges(self, json_index):
+        """uint64 [n_res][2] on the device: the postings of the field index keys that start with each JSON resource's 16 uuid bytes
+        (one contiguous run of the sorted keys), cached per JSON index."""
+        import bisect
+
+        import torch
+
+        cached = getattr(self, "_json_ranges", None)
+        if cached is not None and cached[0] is json_index:
+            return cached[1]
+        keys = sorted(self._field_index)
+        post_off = np.zeros(len(keys) + 1, dtype=np.uint64)
+        post_off[1:] = np.cumsum([len(self._field_index[k]) for k in keys])
+        ranges = np.zeros((max(len(json_index.resource_ids), 1), 2), dtype=np.uint64)
+        for r, rid in enumerate(json_index.resource_ids):
+            try:
+                prefix = _uuid.UUID(rid).bytes
+            except ValueError:
+                continue
+            lo = bisect.bisect_left(keys, prefix)
+            hi = bisect.bisect_left(keys, (int.from_bytes(prefix, "big") + 1).to_bytes(16, "big")) if prefix != b"\xff" * 16 else len(keys)
+            ranges[r] = post_off[lo], post_off[hi]
+        t = torch.from_numpy(ranges.view(np.int64)).to(torch.device("cuda", self.config.device))
+        self._json_ranges = (json_index, t)
+        return t
+
+    def search_json(self, query, json, formula, operator_and, with_duplicates, top_k, min_score, method=_lib.NIDX_METHOD_AUTO, ef=0):
+        """search() restricted by a prefilter combined with a JSON resource set (PrefilterResult.json): the paragraphs of the matched
+        resources (every field of theirs, with or without a text document) and those of the text prefilter's documents, combined
+        under its operator, then with `formula` (nidx_vec_prefilter_resources), all on the device."""
+        import torch
+
+        text, json_index, res_bits, op_or = json
+        nodes, _, keep = self.formula_nodes([formula]) if formula is not None else (None, 0, None)
+        doc_bits = join = None
+        n_docs = 0
+        if text is not None:
+            index, doc_bits, _ = text
+            join, n_docs = index.join(self), index.n_docs_total()
+        bits, matching = self.segment.prefilter_resources(doc_bits, join, n_docs, _lib.NIDX_F_OR if op_or else _lib.NIDX_F_AND, res_bits,
+                                                          self.json_ranges(json_index), len(json_index.resource_ids), self.records, nodes,
+                                                          _lib.NIDX_F_AND if operator_and else _lib.NIDX_F_OR)
+        if matching == 0:
+            return np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.float32)
+        q = torch.as_tensor(np.asarray(query, dtype=np.float32)[None, :]).to(torch.device("cuda", self.config.device))
+        ids, scores, counts = self.segment.search(q, top_k, ef, min_score, with_duplicates, method, filter_bits=bits, filter_matching=matching)
+        c = int(counts[0].item())
+        return ids[0, :c].cpu().numpy().view(np.uint32), scores[0, :c].cpu().numpy()
+
     def _raw_search(self, queries, k, filter_bits):
         """exact scan restricted to a paragraph bitset, no min_score: per (query, paragraph) the best vector's similarity."""
         return self.segment.search(queries, k, 0, float(np.finfo(np.float32).min), True, _lib.NIDX_METHOD_BRUTE, filter_bits=filter_bits)
@@ -481,7 +537,7 @@ class VectorSearcher:
         multi = self.config.vector_cardinality == VectorCardinality.Multi
         on_device = prefilter.device_bits if prefilter.kind == "some" and not multi else None
         clauses = []
-        if prefilter.kind == "some" and on_device is None:  # searcher.rs:300-314
+        if prefilter.kind == "some" and on_device is None and prefilter.json is None:  # searcher.rs:300-314
             clauses.append(_KeyPrefixSet(frozenset(f"{f.resource_id.hex}{f.field_id}" if f.field_id else f.resource_id.hex for f in prefilter.fields)))
         if request.filtering_formula is not None:
             clauses.append(_map_expression(request.filtering_formula))
@@ -493,13 +549,18 @@ class VectorSearcher:
             raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {len(query)}")
         k = request.result_per_page
         if self.config.vector_cardinality == VectorCardinality.Multi:
+            if prefilter.json is not None:
+                raise ValueError("json_filter is not supported on a multi-vector vectorset")
             return self._search_multi_vector(request, clauses, operator_and, prefilter, method, ef)
         fssc = _Fssc(k, request.with_duplicates)
         if k > 0 and prefilter.kind != "none":
             for seg in self.open_segments:
                 if request.segment_filtering_formula is not None and not _segment_matches(request.segment_filtering_formula, seg.tags):
                     continue
-                if on_device is not None:
+                if prefilter.json is not None:
+                    addrs, scores = seg.search_json(query, prefilter.json, request.filtering_formula, operator_and, request.with_duplicates, k,
+                                                    request.min_score, method, ef)
+                elif on_device is not None:
                     addrs, scores = seg.search_prefiltered(query, on_device, request.filtering_formula, operator_and, request.with_duplicates, k,
                                                            request.min_score, method, ef)
                 else:
