@@ -870,6 +870,14 @@ static bool hnsw_search_smem(const nidx_vec_segment* s, int ef0, int k, int* lis
     return *bytes <= 200 * 1024;
 }
 
+// log2 of the smallest visited table whose insert limit (VisitedSet::init) stays above n nodes: a walk on it never overflows.
+// At most 28: VisitedSet::init computes the limit in 32 bits (a 2^28-slot table already holds 251 M nodes, 1 GiB per CTA).
+static int rq_table_bits(uint64_t n) {
+    int b = 1;
+    while (b < 28 && ((15ull << b) >> 4) < n + 1 + HS_MAX_ROW) ++b;
+    return b;
+}
+
 static bool rq_walk_smem(const nidx_vec_segment* s, int k, int* last_k, int* cu_cap, int* list_cap, int* hash_bits, size_t* bytes) {
     *last_k = (int)std::min<size_t>((size_t)k * 100, 2000);              // rabitq.rs:34-36 RERANKING_FACTOR / RERANKING_LIMIT
     *cu_cap = std::min(std::max(k + k * s->s0, 2 * k), 4096);
@@ -1302,8 +1310,13 @@ struct VecCall {
         size_t smem;
         if (!rq_walk_smem(s, k, &last_k, &cu_cap, &list_cap, &hash_bits, &smem))
             return fail(NIDX_EINVAL, "quantised HNSW search needs %zu bytes of shared memory (k=%d, dim=%d): too large", smem, k, s->d);
-        int gv_bits = 16;                                                       // 64 k slots: layer 0 visits ~10-20 k nodes at k = 10
-        while ((1 << gv_bits) < 24 * last_k) ++gv_bits;
+        // Layer 0's visited set is a table in global memory, one slice per resident CTA.  A walk estimates about 0.5 x last_k x s0
+        // nodes, up to 0.6 x on hard data (500 000 x 64 Dot rows, M0 = 60, k = 20: 74 391 of last_k x s0 = 128 000), so the table has
+        // 1.5 x last_k x s0 slots and at least 2^16, as the dense walk sizes its shared one -- and no more than the smallest table whose
+        // insert limit holds every node of the segment, which cannot overflow.
+        const int all_bits = rq_table_bits(s->n);
+        int gv_bits = std::min(ilog2(next_pow2(std::max(1 << 16, last_k * s->s0 * 3 / 2))), all_bits);
+        if (const char* eg = getenv("NIDX_B200_RQ_GV_BITS")) gv_bits = std::min(all_bits, std::max(8, atoi(eg)));   // tests: a smaller table
         // CTA shape: the walk is bound by the ~1 000 dependent hops of a query, so what counts is how many queries are resident.
         // 8 warps per query: 4 CTAs per SM; 4 warps: 7 per SM.  The 4-warp shape is taken when the batch does not fit one wave of the
         // 8-warp shape (NIDX_B200_RQ_W = 4 / 8 forces one).
@@ -1322,6 +1335,20 @@ struct VecCall {
         SearchArgs a = walk_args(last_k, list_cap, cu_cap, hash_bits);
         a.codes = s->d_quant; a.code_stride = s->quant_stride; a.planes = planes; a.qparams = params;
         a.gvisited = w.scores.as<uint32_t>(); a.gv_bits = gv_bits; a.last_k = last_k;
+        r = launch_walk(kern, grid, threads, smem, V, a);
+        if (r || gv_bits == all_bits) return r;
+        // A full table reports its new nodes as visited, and the walk would skip neighbours the reference scores.  When a query
+        // overflowed the layer-0 table (counters[7]; the shared-memory sets count in [2] only), the batch runs again with the table
+        // that holds every node, on as many CTAs as fit the workspace the first run used (at least 1 GiB).
+        unsigned long long overflows = 0;
+        CU(cudaMemcpyAsync(&overflows, counters + 7, sizeof(overflows), cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+        if (!overflows) return 0;
+        const size_t budget = std::max(((size_t)grid << gv_bits) * 4, (size_t)1 << 30);
+        grid = (int)std::max<size_t>(1, std::min<size_t>((size_t)grid, budget / (((size_t)4) << all_bits)));
+        ENSURE(w.scores, ((size_t)grid << all_bits) * 4);
+        CU(cudaMemsetAsync(w.sched.p, 0, 128, stream));              // the work counter and this call's counters
+        a.gvisited = w.scores.as<uint32_t>(); a.gv_bits = all_bits;
         return launch_walk(kern, grid, threads, smem, V, a);
     }
 

@@ -39,6 +39,7 @@ struct RqCtx {
     uint32_t sum_quantized;
     VisitedSet gvis;          // layer 0: this CTA's slice of the global visited table
     unsigned long long n_quant, n_rerank;
+    unsigned long long n_gvis_overflow;   // hops whose insert the full global table refused
 };
 
 // rabitq.rs:166-218: the float tail of QueryVector::similarity from the integer dot product -> (estimate, error bound)
@@ -219,7 +220,7 @@ __device__ inline void rq_expand(const GraphDev& G, SearchCtx& c, const SearchAr
         *c.s_hash_count = visited + h.nfresh;
         c.n_expand++;
         r.n_quant += h.nfresh;
-        if (h.overflow) c.n_overflow++;
+        if (h.overflow) { c.n_overflow++; if (GLOBAL_VIS) r.n_gvis_overflow++; }
         c.hops[cur ^ 1u].clear();
     }
 }
@@ -266,7 +267,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
     float* surv_real = reinterpret_cast<float*>(p);
     r.planes = planes; r.planes_t = planes_t; r.nw = V.d / 32; r.root_dim = __fsqrt_rn((float)V.d);
     r.gvis.init(a.gvisited + ((size_t)blockIdx.x << a.gv_bits), a.gv_bits);
-    r.n_quant = r.n_rerank = 0;
+    r.n_quant = r.n_rerank = r.n_gvis_overflow = 0;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int ng = V.ld >> 2;
     const RabitqQueryParams* qparams = reinterpret_cast<const RabitqQueryParams*>(a.qparams);
@@ -373,6 +374,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
     if (threadIdx.x == 0) {
         if (r.n_quant) atomicAdd(&a.counters[4], r.n_quant);
         if (r.n_rerank) atomicAdd(&a.counters[5], r.n_rerank);
+        if (r.n_gvis_overflow) atomicAdd(&a.counters[7], r.n_gvis_overflow);
     }
 }
 

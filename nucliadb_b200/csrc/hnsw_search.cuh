@@ -132,6 +132,7 @@ struct SearchCtx {
     uint32_t* pref_row;   // [2][HS_MAX_ROW] speculatively prefetched adjacency rows (double buffered by hop parity)
     uint32_t* pref_node;  // [2] node each buffer belongs to (NIL = none)
     int *s_len, *s_best, *s_hash_count, *s_flag;
+    unsigned long long* s_dropped;   // closest_up_nodes: the best key a full list has dropped (0: none)
     HopRec* hops;         // [2], by hop parity
     unsigned hop;         // expansions so far; hs_expand and rq_expand advance it at their end
     float qnorm;
@@ -182,6 +183,7 @@ __host__ __device__ __forceinline__ size_t hs_smem_bytes(int ld, int list_cap, i
 __device__ inline unsigned char* hs_setup(SearchCtx& c, const SearchArgs& a, unsigned char* p, int ld) {
     __shared__ int s_ints[4];
     __shared__ HopRec s_hops[2];
+    __shared__ unsigned long long s_drop;
     c.qvec = reinterpret_cast<float*>(p); p += (size_t)ld * 4;
     c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
     c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
@@ -192,6 +194,7 @@ __device__ inline unsigned char* hs_setup(SearchCtx& c, const SearchArgs& a, uns
     c.pref_node = reinterpret_cast<uint32_t*>(p); p += 16;
     c.s_len = &s_ints[0]; c.s_best = &s_ints[1]; c.s_hash_count = &s_ints[2]; c.s_flag = &s_ints[3];
     c.hops = s_hops;
+    c.s_dropped = &s_drop;
     c.hop = 0;
     c.qnorm = 0.0f;
     c.n_dist = c.n_expand = c.n_overflow = c.n_skip = 0;
@@ -225,7 +228,7 @@ __device__ inline void hs_reseed(SearchCtx& c, const VisitedSet& vis, bool keep 
     __syncthreads();
     if (!(MARKED && keep)) vis.clear();
     if (threadIdx.x == 0) {
-        *c.s_hash_count = 0; *c.s_best = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL;
+        *c.s_hash_count = 0; *c.s_best = 0; *c.s_dropped = 0; c.pref_node[0] = NIL; c.pref_node[1] = NIL;
         c.hops[0].clear(); c.hops[1].clear();
     }
     __syncthreads();
@@ -405,6 +408,8 @@ __device__ inline void hs_merge(SearchCtx& c, int cap, int best, int ntodo, int*
         if (p < cap) {
             c.B[p] = key;
             if (key & 1ull) my_best = min(my_best, p);
+        } else if (CU && p == cap && (key | 1ull) > *c.s_dropped) {
+            *c.s_dropped = key | 1ull;             // the best key the full list drops (one thread per merge)
         }
     }
     // first unexpanded entry of the merged list: one shared-memory atomic per warp, not per entry
@@ -416,7 +421,6 @@ __device__ inline void hs_merge(SearchCtx& c, int cap, int best, int ntodo, int*
     if (over) nl = cap;
     const int nb = *bn;
     if (threadIdx.x == 0) {
-        if (over && CU) c.n_overflow += (1ull << 32);
         *c.s_len = nl;
         *c.s_best = nb;
     }
@@ -496,8 +500,16 @@ __device__ inline int hs_closest_up(const VecDev& V, const GraphDev& G, SearchCt
     int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     hs_reseed<DEFER>(c, c.vis, keep);
     int nacc = 0;
+    bool lost = false;
     while (true) {
         int len = *c.s_len;
+        // The reference's candidate heap is unbounded; this list keeps its best cu_cap entries.  A dropped entry changes the result
+        // only if it would be popped: when it outranks the list's head (or the list is empty) and passes min_score.  Counted once.
+        const unsigned long long dropped = *c.s_dropped;
+        if (!lost && dropped && (len == 0 || (c.A[0] | 1ull) < dropped) && !(key_score(dropped) < a.min_score)) {
+            lost = true;
+            if (threadIdx.x == 0) c.n_overflow += 1ull << 32;
+        }
         if (len == 0) break;
         uint64_t ckey = c.A[0];
         float score = key_score(ckey);

@@ -125,6 +125,11 @@ struct Scored {
     float score;
 };
 static inline bool better(const Scored& a, const Scored& b) { return rank_key(a.score, a.id) > rank_key(b.score, b.id); }
+// search.rs:381 `filtered_result.sort_by(|a, b| b.1.total_cmp(&a.1))`: a STABLE sort on the score alone, so equal scores keep the
+// order closest_up_nodes accepted them in (a late-found neighbour can tie with an earlier result and carry a lower id).
+static inline void sort_by_score(std::vector<Scored>& r) {
+    std::stable_sort(r.begin(), r.end(), [](const Scored& a, const Scored& b) { return ordered_bits(a.score) > ordered_bits(b.score); });
+}
 
 struct alignas(64) Counters {  // one cache line per thread: these are bumped on every similarity
     uint64_t n_dist = 0, n_expand = 0, n_edges_read = 0;
@@ -284,7 +289,7 @@ static inline std::vector<Scored> hnsw_search(const Data& D, const GraphView& G,
     size_t last_k = std::max(k_neighbours, (size_t)ef);  // 338-345
     auto neighbours = layer_search(D, G, q, 0, last_k, eps, sc, cnt);
     auto filtered = closest_up_nodes(D, G, q, neighbours, k_neighbours, min_score, filter, sc, cnt);
-    std::sort(filtered.begin(), filtered.end(), better);  // 381
+    sort_by_score(filtered);  // 381
     return filtered;
 }
 

@@ -146,7 +146,7 @@ static inline std::vector<Scored> hnsw_search_rabitq(const Data& D, const GraphV
     }
     auto reranked = rerank_top(cand, k_neighbours, min_score, [&](uint32_t v) { return sim_to(D, q, v, cnt); });   // 355-361
     auto filtered = closest_up_nodes(D, G, q, reranked, k_neighbours, min_score, filter, sc, cnt);                  // 369-375, exact
-    std::sort(filtered.begin(), filtered.end(), better);
+    sort_by_score(filtered);   // 381
     return filtered;
 }
 

@@ -116,6 +116,12 @@ class _Key:
         return self.rank() < other.rank()
 
 
+def _total_cmp_key(score):
+    """f32::total_cmp as an integer."""
+    u = int(np.float32(score).view(np.uint32))
+    return (~u & 0xFFFFFFFF) if u & 0x80000000 else (u | 0x80000000)
+
+
 class _Max(_Key):                      # heapq is a min-heap: invert for BinaryHeap<Cnx>
     def __lt__(self, other):
         return self.rank() > other.rank()
@@ -179,7 +185,7 @@ def py_search(sim, g, vecs, k, ef, min_score, filter_bits, with_duplicates):
                 if s >= min_score:
                     candidates.append(_Key(y, s))
         candidates.sort(key=lambda x: x.rank())
-    return sorted(results, key=lambda x: x.rank(), reverse=True)
+    return sorted(results, key=lambda x: -_total_cmp_key(x.score))     # 381: stable, on the score alone
 
 
 def test_oracle_walk_equals_the_python_transcription():
@@ -199,6 +205,25 @@ def test_oracle_walk_equals_the_python_transcription():
             assert cnt[qi] == len(want)
             assert ids[qi, : cnt[qi]].tolist() == [x.id for x in want]
             assert sc[qi, : cnt[qi]].tolist() == [np.float32(x.score) for x in want]
+
+
+def test_oracle_walk_keeps_closest_up_order_on_score_ties():
+    """search.rs:381 sorts the results with a stable sort on the score alone: of two equal scores the one closest_up_nodes accepted
+    first stays first, even when a later-found neighbour carries a lower id.  Dot queries with one +-inf element make every
+    similarity +-inf, so nearly every result ties."""
+    v = make_vectors(1500, 32, seed=39)
+    g = O.hnsw_build(v, sim=O.SIM_DOT, M=6, M0=12, efC=30, max_batch=8, nthreads=4)
+    q = make_queries(v, 6, seed=40)
+    q[:3, 5] = np.inf
+    q[3:, 7] = -np.inf
+    moved = 0
+    for min_score, ef in ((-np.inf, 20), (-1.0, 20)):
+        ids, sc, cnt, _ = O.hnsw_search(v, g, q, 12, ef, sim=O.SIM_DOT, min_score=min_score)
+        for qi in range(len(q)):
+            want = py_search(lambda x: O.dot(v[x], q[qi]), g, v, 12, ef, min_score, None, True)
+            assert cnt[qi] == len(want) and ids[qi, : cnt[qi]].tolist() == [x.id for x in want]
+            moved += [x.id for x in want] != [x.id for x in sorted(want, key=lambda x: x.rank(), reverse=True)]
+    assert moved > 0                                                 # some tie is not in id order: the case tests the rule
 
 
 def py_select_neighbours(pair_sim, k, candidates):
