@@ -458,15 +458,22 @@ typedef struct nidx_prefilter_node {   /* an expression in pre-order */
 int nidx_txt_prefilter(nidx_txt_segment* seg, const nidx_prefilter_node* nodes, int32_t n_nodes, uint64_t* out_bits, int mem, uint64_t* out_matching,
                        void* stream);
 
-/* The hand-off to one vector segment (reference: nidx_vector/src/searcher.rs:300-314 with PrefilterResult::Some): doc_bits over
- * n_docs text documents and join[n_docs] (u32: the document's key in this segment's NIDX_INV_FIELDS index, or NIDX_NIL; both
- * `mem`) -> the paragraphs of the matched documents' keys; with a filter formula (nodes, n_nodes > 0; nidx_vec_filter's format)
- * combined with it under op (NIDX_F_AND | NIDX_F_OR: SearchRequest.filter_operator), then ANDed with the alive set -> out_bits
- * ((paragraphs + 63) / 64 words, `mem`; may be NULL) and *out_matching (host), to be passed to nidx_vec_search as filter_bits and
- * filter_matching.  The call returns when both are in place.  The formula has nidx_vec_filter's limit, less two instructions
- * (the documents' paragraphs and the combination under op). */
-int nidx_vec_prefilter_bits(nidx_vec_segment* seg, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, const nidx_filter_node* nodes,
-                            int32_t n_nodes, int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
+/* The hand-off to one vector segment (reference: nidx_vector/src/searcher.rs:300-314 with PrefilterResult::Some) of a text part,
+ * a resource part (SearchRequest.json_filter, below) or both:
+ *   text: doc_bits over n_docs text documents and join[n_docs] (u32: the document's key in this segment's NIDX_INV_FIELDS index, or
+ *     NIDX_NIL) -> the paragraphs of the matched documents' keys; doc_bits NULL = no text part;
+ *   resources: res_bits over n_res resources -> their paragraphs: resource r's are the postings res_ranges[2 r] .. res_ranges[2 r + 1]
+ *     of the NIDX_INV_FIELDS index (every key with r's 16 uuid bytes as prefix, one contiguous run of keys); res_bits NULL = no
+ *     resource part;
+ * combined under doc_op (NIDX_F_AND | NIDX_F_OR; read only when both parts are given), then with a filter formula (nodes, n_nodes > 0;
+ * nidx_vec_filter's format) under op (NIDX_F_AND | NIDX_F_OR: SearchRequest.filter_operator), then ANDed with the alive set ->
+ * out_bits ((paragraphs + 63) / 64 words; may be NULL) and *out_matching (host), to be passed to nidx_vec_search as filter_bits and
+ * filter_matching.  No part at all is NIDX_EINVAL; a part with no documents or resources is an empty set.  All buffers `mem`; the call
+ * returns when both outputs are in place.  The formula has nidx_vec_filter's limit, less one instruction per part, one for doc_op
+ * when both are given and one for op. */
+int nidx_vec_prefilter_bits(nidx_vec_segment* seg, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, int32_t doc_op,
+                            const uint64_t* res_bits, uint64_t n_res, const uint64_t* res_ranges, const nidx_filter_node* nodes, int32_t n_nodes,
+                            int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
 
 /* ---- JSON filters: SearchRequest.json_filter (reference: nidx_json, JsonSearcher::search -> a set of resources, combined with the
  * text prefilter by PrefilterResult::combine, nidx_types/src/prefilter.rs:49-92).  The JSON index is a text segment without terms:
@@ -474,22 +481,12 @@ int nidx_vec_prefilter_bits(nidx_vec_segment* seg, const uint64_t* doc_bits, uin
  * carried as a facet ord (nidx_txt_set_facets), the resource ord in the resource column (nidx_txt_set_doc_columns) and the resource's
  * access groups (nidx_txt_set_doc_groups).  A leaf is then one NIDX_P_FACET range, NOT ranges over the alive JSON documents, and the
  * expression runs in nidx_txt_prefilter's one pass.  The entry points below turn its output into a resource bitset and hand that to
- * the vector and paragraph searches; none of the bitsets leaves HBM on the device path. */
+ * the paragraph search; nidx_vec_prefilter_bits takes it as its resource part.  None of the bitsets leaves HBM on the device path. */
 
 /* doc_bits ((n_docs + 63) / 64 words: typically nidx_txt_prefilter's output) -> out_res_bits ((n_resources + 63) / 64 words, zeroed
  * first): bit r set when a set document's resource ord (nidx_txt_set_doc_columns) is r; ords >= n_resources are dropped.  `mem` applies
  * to both. */
 int nidx_txt_resource_bits(nidx_txt_segment* seg, const uint64_t* doc_bits, uint64_t n_resources, uint64_t* out_res_bits, int mem, void* stream);
-
-/* nidx_vec_prefilter_bits with a resource set: the paragraphs of the resources set in res_bits (n_res bits; resource r's paragraphs are
- * the postings res_ranges[2 r] .. res_ranges[2 r + 1] of this segment's NIDX_INV_FIELDS index, i.e. every key with r's 16 uuid bytes
- * as prefix, one contiguous run of keys), combined under doc_op (NIDX_F_AND | NIDX_F_OR) with the paragraphs of the text documents
- * (doc_bits / join as nidx_vec_prefilter_bits; doc_bits NULL = no text part: the resources' paragraphs alone), then with the formula
- * under op, then ANDed with alive -> out_bits, *out_matching.  All inputs `mem`.  The formula has nidx_vec_filter's limit less four
- * instructions. */
-int nidx_vec_prefilter_resources(nidx_vec_segment* seg, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, int32_t doc_op,
-                                 const uint64_t* res_bits, uint64_t n_res, const uint64_t* res_ranges, const nidx_filter_node* nodes, int32_t n_nodes,
-                                 int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
 
 /* One mask over seg's documents (for nidx_txt_view): bit d = and_bits[d] AND op(doc_bits[doc_join[d]], res_bits[res_join[d]]), op =
  * NIDX_F_AND | NIDX_F_OR.  and_bits NULL = every bit set; doc_bits NULL = every bit set (doc_join unread); a join entry of NIDX_NIL,

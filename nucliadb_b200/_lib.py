@@ -153,9 +153,8 @@ SIGNATURES = {
     "nidx_txt_set_doc_columns": (i32, [P, P, P]),
     "nidx_txt_set_doc_groups": (i32, [P, u32, P, P, P, P]),
     "nidx_txt_prefilter": (i32, [P, P, i32, P, i32, P, P]),   # nodes: an array of PrefilterNode
-    "nidx_vec_prefilter_bits": (i32, [P, P, u64, P, NODES, i32, i32, P, i32, P, P]),
+    "nidx_vec_prefilter_bits": (i32, [P, P, u64, P, i32, P, u64, P, NODES, i32, i32, P, i32, P, P]),
     "nidx_txt_resource_bits": (i32, [P, P, u64, P, i32, P]),
-    "nidx_vec_prefilter_resources": (i32, [P, P, u64, P, i32, P, u64, P, NODES, i32, i32, P, i32, P, P]),
     "nidx_txt_join_mask": (i32, [P, P, P, u64, P, P, u64, P, i32, P, i32, P, P]),
     "nidx_shard_unique_id": (i32, [P]),
     "nidx_shard_init": (i32, [P, i32, i32, i32, P]),

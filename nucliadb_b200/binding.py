@@ -338,29 +338,14 @@ class NidxBinding:
         masks = None
         if req.HasField("json_filter"):
             J.validate(req.json_filter)
-            op_or = req.filter_operator == P.FILTER_OR
-            jx = shard.json_index
             res_bits, found = None, 0
-            if jx is not None:
-                _, found, res_bits = jx.prefilter(req.json_filter, security)
-            text = prefilter.device_bits if prefilter.kind == "some" else None
-            if prefilter.kind == "some" and text is None:
-                raise ValueError("json_filter needs the device prefilter")
-            if found == 0:   # combine(text, {}, op): the text result under OR, None under AND
-                if not op_or:
-                    prefilter = V.PrefilterResult.none()
-                elif text is not None and req.paragraph and shard.paragraph_searcher is not None:
-                    masks = shard.paragraph_searcher.json_masks(security, text[1], text[0], None, None, True)
-            elif (prefilter.kind == "none" and not op_or) or (prefilter.kind == "all" and op_or):
-                pass
-            else:
-                # text None under OR is the JSON set alone; text All under AND is the JSON set ANDed with every field
-                prefilter = V.PrefilterResult.from_json(text, jx, res_bits, op_or and text is not None)
-                if req.paragraph and shard.paragraph_searcher is not None:
-                    masks = shard.paragraph_searcher.json_masks(security, text[1] if text else None, text[0] if text else None, jx, res_bits,
-                                                                op_or and text is not None)
+            if shard.json_index is not None:
+                _, found, res_bits = shard.json_index.prefilter(req.json_filter, security)
+            prefilter = prefilter.combine(shard.json_index, res_bits, found, req.filter_operator == P.FILTER_OR)
             if prefilter.kind == "none":   # IndexQueries::apply_prefilter: the sections are absent
                 return out
+            if prefilter.on_device and req.paragraph and shard.paragraph_searcher is not None:
+                masks = shard.paragraph_searcher.json_masks(security, prefilter)
         if len(req.vector):
             name = req.vectorset
             if name not in shard.vectorsets:

@@ -2845,12 +2845,18 @@ int nidx_txt_prefilter(nidx_txt_segment* t, const nidx_prefilter_node* nodes, in
     return 0;
 }
 
-int nidx_vec_prefilter_bits(nidx_vec_segment* s, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, const nidx_filter_node* nodes,
-                            int32_t n_nodes, int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream_) {
+int nidx_vec_prefilter_bits(nidx_vec_segment* s, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, int32_t doc_op,
+                            const uint64_t* res_bits, uint64_t n_res, const uint64_t* res_ranges, const nidx_filter_node* nodes, int32_t n_nodes,
+                            int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream_) {
     int r = require_handle(s);
     if (r) return r;
-    if (n_docs && (!doc_bits || !join)) return fail(NIDX_EINVAL, "null argument");
-    if (op != NIDX_F_AND && op != NIDX_F_OR) return fail(NIDX_EINVAL, "op must be NIDX_F_AND or NIDX_F_OR");
+    const bool text = doc_bits != nullptr, res = res_bits != nullptr;
+    if (!text && !res) return fail(NIDX_EINVAL, "neither a text part nor a resource part");
+    if (!text) n_docs = 0;
+    if (!res) n_res = 0;
+    if ((n_docs && !join) || (n_res && !res_ranges)) return fail(NIDX_EINVAL, "null argument");
+    if ((op != NIDX_F_AND && op != NIDX_F_OR) || (text && res && doc_op != NIDX_F_AND && doc_op != NIDX_F_OR))
+        return fail(NIDX_EINVAL, "op must be NIDX_F_AND or NIDX_F_OR");
     if (n_nodes < 0 || (n_nodes > 0 && !nodes)) return fail(NIDX_EINVAL, "bad filter formula");
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
     const bool host = mem == NIDX_MEM_HOST;
@@ -2859,28 +2865,41 @@ int nidx_vec_prefilter_bits(nidx_vec_segment* s, const uint64_t* doc_bits, uint6
     Workspace& w = *g.w;
     const size_t words = ((size_t)s->n_par + 63) / 64;
     Stage st(stream, host, host);
-    const uint64_t* d_doc;
+    const uint64_t *d_doc, *d_res, *d_ranges;
     const uint32_t* d_join;
     uint64_t* d_out;
     st.in(doc_bits, (size_t)((n_docs + 63) / 64), &d_doc);
-    st.in(join, (size_t)n_docs, &d_join);
+    st.in(text ? join : nullptr, (size_t)n_docs, &d_join);
+    st.in(res_bits, (size_t)((n_res + 63) / 64), &d_res);
+    st.in(res ? res_ranges : nullptr, (size_t)(2 * n_res), &d_ranges);
     st.out(out_bits, words, &d_out);
     r = st.place(w.stage);
     if (r) return r;
-    // the program: slot 0 (the matched documents' paragraphs), combined with the formula under op
+    // the program: [slot 0: the text documents' paragraphs] [slot rs: the resources' paragraphs] [doc_op when both], combined with
+    // the paragraph formula (segment.rs:516-534) under op, as the reference combines its clauses
+    const uint32_t rs = text ? 1 : 0;
     FormulaPlan P;
-    P.slots = 1;
-    if (n_nodes) {   // the paragraph formula (segment.rs:516-534), combined as the reference combines its clauses
+    P.slots = rs + (res ? 1 : 0);
+    if (n_nodes) {
         r = P.compile(s, nodes, n_nodes);
         if (r) return r;
     }
-    P.prog.insert(P.prog.begin(), FormulaPlan::leaf(0));
+    std::vector<PfOp> head;
+    if (text) head.push_back(FormulaPlan::leaf(0));
+    if (res) head.push_back(FormulaPlan::leaf((int)rs));
+    if (text && res) { PfOp b{}; b.op = doc_op == NIDX_F_OR ? PF_OR : PF_AND; head.push_back(b); }
+    P.prog.insert(P.prog.begin(), head.begin(), head.end());
     if (n_nodes) { PfOp b{}; b.op = op == NIDX_F_OR ? PF_OR : PF_AND; P.prog.push_back(b); }
     const nidx_vec_segment::InvIndex& ix = s->inv[NIDX_INV_FIELDS];
     auto scatter = [&](uint64_t* bits, unsigned char* extra) -> int {
         if (n_docs && ix.n_keys) {
             const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_docs + 255) / 256));
             prefilter_join_kernel<<<blocks, 256, 0, stream>>>(d_doc, d_join, n_docs, ix.n_keys, ix.d_post_off, ix.d_post, bits);
+            LAUNCHED();
+        }
+        if (n_res && ix.n_keys) {
+            const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_res + 255) / 256));
+            prefilter_res_join_kernel<<<blocks, 256, 0, stream>>>(d_res, n_res, d_ranges, ix.d_post, bits + (size_t)rs * words);
             LAUNCHED();
         }
         return P.scatter(bits, extra, words, stream);
@@ -2919,69 +2938,6 @@ int nidx_txt_resource_bits(nidx_txt_segment* t, const uint64_t* doc_bits, uint64
         CU(cudaGetLastError());
     }
     return st.finish();
-}
-
-int nidx_vec_prefilter_resources(nidx_vec_segment* s, const uint64_t* doc_bits, uint64_t n_docs, const uint32_t* join, int32_t doc_op,
-                                 const uint64_t* res_bits, uint64_t n_res, const uint64_t* res_ranges, const nidx_filter_node* nodes, int32_t n_nodes,
-                                 int32_t op, uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream_) {
-    int r = require_handle(s);
-    if (r) return r;
-    if ((doc_bits && n_docs && !join) || (n_res && (!res_bits || !res_ranges))) return fail(NIDX_EINVAL, "null argument");
-    if ((op != NIDX_F_AND && op != NIDX_F_OR) || (doc_op != NIDX_F_AND && doc_op != NIDX_F_OR)) return fail(NIDX_EINVAL, "op must be NIDX_F_AND or NIDX_F_OR");
-    if (n_nodes < 0 || (n_nodes > 0 && !nodes)) return fail(NIDX_EINVAL, "bad filter formula");
-    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-    const bool host = mem == NIDX_MEM_HOST;
-    CU(cudaSetDevice(s->cfg.device));
-    WsGuard g(s->pool, stream);
-    Workspace& w = *g.w;
-    const size_t words = ((size_t)s->n_par + 63) / 64;
-    Stage st(stream, host, host);
-    const uint64_t *d_doc, *d_res, *d_ranges;
-    const uint32_t* d_join;
-    uint64_t* d_out;
-    const bool text = doc_bits != nullptr;
-    st.in(doc_bits, (size_t)((n_docs + 63) / 64), &d_doc);
-    st.in(text ? join : nullptr, (size_t)n_docs, &d_join);
-    st.in(res_bits, (size_t)((n_res + 63) / 64), &d_res);
-    st.in(res_ranges, (size_t)(2 * n_res), &d_ranges);
-    st.out(out_bits, words, &d_out);
-    r = st.place(w.stage);
-    if (r) return r;
-    // the program: [slot 0 (the text documents' paragraphs)] slot t (the resources' paragraphs) [doc_op], combined with the formula
-    // under op
-    const uint32_t rs = text ? 1 : 0;
-    FormulaPlan P;
-    P.slots = rs + 1;
-    if (n_nodes) {
-        r = P.compile(s, nodes, n_nodes);
-        if (r) return r;
-    }
-    std::vector<PfOp> head;
-    if (text) head.push_back(FormulaPlan::leaf(0));
-    head.push_back(FormulaPlan::leaf((int)rs));
-    if (text) { PfOp b{}; b.op = doc_op == NIDX_F_OR ? PF_OR : PF_AND; head.push_back(b); }
-    P.prog.insert(P.prog.begin(), head.begin(), head.end());
-    if (n_nodes) { PfOp b{}; b.op = op == NIDX_F_OR ? PF_OR : PF_AND; P.prog.push_back(b); }
-    const nidx_vec_segment::InvIndex& ix = s->inv[NIDX_INV_FIELDS];
-    auto scatter = [&](uint64_t* bits, unsigned char* extra) -> int {
-        if (text && n_docs && ix.n_keys) {
-            const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_docs + 255) / 256));
-            prefilter_join_kernel<<<blocks, 256, 0, stream>>>(d_doc, d_join, n_docs, ix.n_keys, ix.d_post_off, ix.d_post, bits);
-            LAUNCHED();
-        }
-        if (n_res && ix.n_keys) {
-            const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)s->sm_count * 8, (n_res + 255) / 256));
-            prefilter_res_join_kernel<<<blocks, 256, 0, stream>>>(d_res, n_res, d_ranges, ix.d_post, bits + (size_t)rs * words);
-            LAUNCHED();
-        }
-        return P.scatter(bits, extra, words, stream);
-    };
-    unsigned long long h = 0;
-    r = run_program(w, stream, s->sm_count, P.prog, P.slots, paragraph_args(s), P.extra_bytes(), scatter, d_out, &h);
-    if (!r) r = st.finish(true);   // the program and the ranges are host temporaries, and the count is read back
-    if (r) return r;
-    if (out_matching) *out_matching = h;
-    return 0;
 }
 
 int nidx_txt_join_mask(nidx_txt_segment* t, const uint64_t* and_bits, const uint64_t* doc_bits, uint64_t n_doc_bits, const uint32_t* doc_join,

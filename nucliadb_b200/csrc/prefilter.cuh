@@ -155,7 +155,7 @@ __global__ void prefilter_join_kernel(const uint64_t* __restrict__ doc_bits, con
     }
 }
 
-// JSON filters (nidx_txt_resource_bits, nidx_vec_prefilter_resources, nidx_txt_join_mask): a JSON document's result is a resource.
+// JSON filters (nidx_txt_resource_bits, nidx_vec_prefilter_bits' resource part, nidx_txt_join_mask): a JSON document's result is a resource.
 // doc_bits [n_docs] -> out (resource bits, zeroed by the caller): res_ord[d] = the document's resource ord (>= n_res: none).
 __global__ void prefilter_resource_kernel(const uint64_t* __restrict__ doc_bits, const uint32_t* __restrict__ res_ord, uint64_t n_docs, uint64_t n_res,
                                           uint64_t* __restrict__ out) {

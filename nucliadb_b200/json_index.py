@@ -231,12 +231,11 @@ class JsonIndex:
                 for o in ops:
                     walk(o)
 
-        if security is not None:   # the resource's access groups, as TextSearcher.security_nodes over this index's dictionary
-            from .text import _prefix_range, group_key
+        if security is not None:   # the resource's access groups, over this index's dictionary
+            from .text import security_tree
 
             flat.append((_lib.NIDX_P_AND, 2, 0, 0, None))
-            flat += [(_lib.NIDX_P_OR, 1 + len(security), 0, 0, None), (_lib.NIDX_P_PUBLIC, 0, 0, 0, None)]
-            flat += [(_lib.NIDX_P_GROUP, 0, *_prefix_range(self.group_keys, group_key(g), facet=True), None) for g in security]
+            flat += security_tree(self.group_keys, security)
         walk(expr)
         return flat
 

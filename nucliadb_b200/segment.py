@@ -170,39 +170,22 @@ class VectorSegment:
         check(_lib.load().nidx_vec_filter(self._h, nodes, n, ptr(out_bits), _lib.NIDX_MEM_HOST, C.byref(matching), None))
         return matching.value
 
-    def prefilter_bits(self, doc_bits, join, n_docs: int, n_paragraphs: int, formula=None, op=_lib.NIDX_F_AND):
-        """nidx_vec_prefilter_bits: text-document bits (uint64 words) and the join table (uint32 [n_docs]: each document's key in the
-        field index, or NIL) -> (paragraph bits, matching): the matched documents' paragraphs, combined with `formula` (a FilterNode
-        array, or None) under `op`, AND alive.  numpy inputs -> numpy words; torch CUDA tensors -> a torch int64 tensor (device path)."""
-        on_device = _is_torch(doc_bits)
+    def prefilter_bits(self, doc_bits, join, n_docs: int, res_bits, res_ranges, n_res: int, n_paragraphs: int, formula=None, op=_lib.NIDX_F_AND,
+                       doc_op=_lib.NIDX_F_AND):
+        """nidx_vec_prefilter_bits -> (paragraph bits, matching): the paragraphs of the text documents in doc_bits (uint64 words; join:
+        uint32 [n_docs], each document's key in the field index, or NIL) and those of the resources in res_bits (res_ranges: uint64
+        [n_res][2], each resource's postings in the field index), combined under doc_op when both are given (None: no such part),
+        then with `formula` (a FilterNode array, or None) under `op`, AND alive.  numpy inputs -> numpy words; torch CUDA tensors ->
+        a torch int64 tensor (device path)."""
+        on_device = _is_torch(doc_bits if doc_bits is not None else res_bits)
         mem, stream, alloc = _stage(self.cfg.device, on_device)
         if not on_device:
-            doc_bits = np.ascontiguousarray(doc_bits, dtype=np.uint64)
-            join = np.ascontiguousarray(join, dtype=np.uint32)
+            host = lambda a, dtype: None if a is None else np.ascontiguousarray(a, dtype=dtype)   # noqa: E731
+            doc_bits, join, res_bits, res_ranges = host(doc_bits, np.uint64), host(join, np.uint32), host(res_bits, np.uint64), host(res_ranges, np.uint64)
         out = alloc((n_paragraphs + 63) // 64, np.uint64)
         matching = C.c_uint64()
-        check(_lib.load().nidx_vec_prefilter_bits(self._h, ptr(doc_bits), n_docs, ptr(join), formula, 0 if formula is None else len(formula), op, ptr(out), mem,
-                                                  C.byref(matching), stream))
-        return out, matching.value
-
-    def prefilter_resources(self, doc_bits, join, n_docs: int, doc_op, res_bits, res_ranges, n_res: int, n_paragraphs: int, formula=None,
-                            op=_lib.NIDX_F_AND):
-        """nidx_vec_prefilter_resources: the paragraphs of the resources in res_bits (res_ranges: uint64 [n_res][2], each resource's
-        postings in the field index) combined under doc_op with those of the text documents in doc_bits (None: no text part), then
-        with `formula` under `op`, AND alive -> (paragraph bits, matching).  torch CUDA res_bits -> device path, numpy -> host path."""
-        on_device = _is_torch(res_bits)
-        mem, stream, alloc = _stage(self.cfg.device, on_device)
-        if not on_device:
-            res_bits = np.ascontiguousarray(res_bits, dtype=np.uint64)
-            res_ranges = np.ascontiguousarray(res_ranges, dtype=np.uint64)
-            if doc_bits is not None:
-                doc_bits = np.ascontiguousarray(doc_bits, dtype=np.uint64)
-                join = np.ascontiguousarray(join, dtype=np.uint32)
-        out = alloc((n_paragraphs + 63) // 64, np.uint64)
-        matching = C.c_uint64()
-        check(_lib.load().nidx_vec_prefilter_resources(self._h, ptr(doc_bits), n_docs if doc_bits is not None else 0, ptr(join), doc_op, ptr(res_bits),
-                                                       n_res, ptr(res_ranges), formula, 0 if formula is None else len(formula), op, ptr(out), mem,
-                                                       C.byref(matching), stream))
+        check(_lib.load().nidx_vec_prefilter_bits(self._h, ptr(doc_bits), n_docs, ptr(join), doc_op, ptr(res_bits), n_res, ptr(res_ranges), formula,
+                                                  0 if formula is None else len(formula), op, ptr(out), mem, C.byref(matching), stream))
         return out, matching.value
 
     # ---- search ----------------------------------------------------------------------------------------

@@ -355,24 +355,26 @@ class TextSearcher:
         self.group_keys = keys
 
     def security_nodes(self, access_groups: Sequence[str]) -> list:
-        """security_query (nidx_text/src/search_query.rs:63-87) as flat pre-order prefilter nodes (kind, n, lo, hi, terms): OR of
-        PUBLIC and, per requested group, the GROUP range of that group and its descendants.  No groups: public resources only."""
+        """security_tree over this index's group dictionary."""
         self._ensure_groups()
-        flat = [(_lib.NIDX_P_OR, 1 + len(access_groups), 0, 0, None), (_lib.NIDX_P_PUBLIC, 0, 0, 0, None)]
-        for g in access_groups:
-            flat.append((_lib.NIDX_P_GROUP, 0, *_prefix_range(self.group_keys, group_key(g), facet=True), None))
-        return flat
+        return security_tree(self.group_keys, access_groups)
 
-    def _security_views(self, access_groups: Sequence[str]) -> list:
-        """Every segment as a view (nidx_txt_view) under the security expression's bits, which stay on the device."""
+    def _security_bits(self, access_groups: Sequence[str]) -> list:
+        """Per segment, the security expression's bits (nidx_txt_prefilter), in HBM."""
         import torch
 
         nodes = _node_array(self.security_nodes(access_groups))
+        out = []
+        for s in self.segments:
+            out.append(torch.empty(max((s.n_docs + 63) // 64, 1), dtype=torch.int64, device=torch.device("cuda", s.device)))
+            s._gpu.prefilter(nodes, out=out[-1])
+        return out
+
+    def _security_views(self, access_groups: Sequence[str]) -> list:
+        """Every segment as a view (nidx_txt_view) under the security expression's bits, which stay on the device."""
         views = []
         try:
-            for s in self.segments:
-                bits = torch.empty((s.n_docs + 63) // 64, dtype=torch.int64, device=torch.device("cuda", s.device))
-                s._gpu.prefilter(nodes, out=bits)
+            for s, bits in zip(self.segments, self._security_bits(access_groups)):
                 views.append(s._gpu.view(bits))
         except BaseException:
             for v in views:
@@ -515,26 +517,21 @@ class TextSearcher:
                                            for s in self.segments])
         return [(self._doc_join[1][i] if text_index is not None else None, self._res_join[1][i]) for i in range(len(self.segments))]
 
-    def json_masks(self, security: Optional[Sequence[str]], text_bits, text_index, json_index, res_bits, op_or: bool) -> list:
-        """The per-segment masks of a search under SearchRequest.json_filter (nidx_txt_join_mask, on the device): bit d = the
-        security bits (when `security` is given) AND op(the text prefilter's bit of the document's field (text_bits None: every
-        field), the JSON prefilter's bit of its resource (res_bits over json_index.resource_ids; json_index None: no resource)),
-        op OR when op_or."""
+    def json_masks(self, security: Optional[Sequence[str]], prefilter) -> list:
+        """The per-segment masks of a search under SearchRequest.json_filter (nidx_txt_join_mask, on the device) for a Some on the
+        device (vector.PrefilterResult): bit d = the security bits (when `security` is given) AND op(the text part's bit of the
+        document's field (no text part: every field), the resource part's bit of its resource (no resource part: none)), op OR when
+        the result's op_or or when it has no resource part."""
         import torch
 
-        sec = _node_array(self.security_nodes(security)) if security is not None else None
+        text_index, text_bits, _ = prefilter.device_bits or (None, None, 0)
+        json_index, res_bits = prefilter.resources or (None, torch.zeros(1, dtype=torch.int64, device=torch.device("cuda", self.segments[0].device)))
         n_res = len(json_index.resource_ids) if json_index is not None else 0
-        dev = torch.device("cuda", self.segments[0].device)
-        if res_bits is None:
-            res_bits = torch.zeros(1, dtype=torch.int64, device=dev)
+        op = _lib.NIDX_F_OR if prefilter.op_or or prefilter.resources is None else _lib.NIDX_F_AND
+        sec = self._security_bits(security) if security is not None else [None] * len(self.segments)
         masks = []
-        for s, (doc_join, res_join) in zip(self.segments, self._json_joins(text_index if text_bits is not None else None, json_index)):
-            and_bits = None
-            if sec is not None:
-                and_bits = torch.empty(max((s.n_docs + 63) // 64, 1), dtype=torch.int64, device=dev)
-                s._gpu.prefilter(sec, out=and_bits)
-            mask, _ = s._gpu.join_mask(and_bits, text_bits, 0 if text_bits is None else text_bits.numel() * 64, doc_join, res_bits, n_res, res_join,
-                                       _lib.NIDX_F_OR if op_or else _lib.NIDX_F_AND)
+        for s, and_bits, (doc_join, res_join) in zip(self.segments, sec, self._json_joins(text_index, json_index)):
+            mask, _ = s._gpu.join_mask(and_bits, text_bits, 0 if text_bits is None else text_bits.numel() * 64, doc_join, res_bits, n_res, res_join, op)
             masks.append(mask)
         return masks
 
@@ -639,6 +636,14 @@ def _prefix_range(keys: list, prefix: bytes, facet: bool):
         return lo, bisect.bisect_left(keys, prefix + b"\x01")
     stem = prefix.rstrip(b"\xff")   # the least byte string above every key that starts with `prefix`
     return lo, bisect.bisect_left(keys, stem[:-1] + bytes([stem[-1] + 1])) if stem else len(keys)
+
+
+def security_tree(group_keys: list, access_groups: Sequence[str]) -> list:
+    """security_query (nidx_text/src/search_query.rs:63-87) as flat pre-order prefilter nodes (kind, n, lo, hi, terms) over a group
+    dictionary (the sorted group_key of every group): OR of PUBLIC and, per requested group, the GROUP range of that group and its
+    descendants.  No groups: public resources only."""
+    flat = [(_lib.NIDX_P_OR, 1 + len(access_groups), 0, 0, None), (_lib.NIDX_P_PUBLIC, 0, 0, 0, None)]
+    return flat + [(_lib.NIDX_P_GROUP, 0, *_prefix_range(group_keys, group_key(g), facet=True), None) for g in access_groups]
 
 
 def _node_array(flat: list):

@@ -95,13 +95,15 @@ class FieldId:  # nidx_types/src/prefilter.rs
 
 
 class PrefilterResult:
-    """nidx_types/src/prefilter.rs: All | None | Some(fields).  A Some made on the device (TextSearcher.prefilter) keeps the matched
-    text documents as a bitset in HBM (`device_bits`: (the text index's prefilter state, the bits, the match count)); its `fields`
-    are listed only when read, and VectorSearcher.search hands the bits to the vector segments without leaving the device."""
+    """nidx_types/src/prefilter.rs: All | None | Some(fields).  A Some made on the device keeps its sets in HBM, in two parts: the
+    text part `device_bits` (TextSearcher.prefilter: (the text index's prefilter state, the bits, the match count), or None) and the
+    resource part `resources` (combine: (the JsonIndex, its resource bits), or None), combined under OR when `op_or`, else AND.
+    Its `fields` are listed only when read; VectorSearcher.search and TextSearcher.json_masks hand the parts on without leaving
+    the device."""
 
-    def __init__(self, kind: str, fields: Sequence[FieldId] = (), device_bits=None, json=None):
-        self.kind, self.device_bits, self.json = kind, device_bits, json
-        self._fields = None if device_bits is not None or json is not None else list(fields)
+    def __init__(self, kind: str, fields: Sequence[FieldId] = (), device_bits=None, resources=None, op_or: bool = False):
+        self.kind, self.device_bits, self.resources, self.op_or = kind, device_bits, resources, op_or
+        self._fields = None if device_bits is not None or resources is not None else list(fields)
 
     @property
     def fields(self) -> list:
@@ -110,20 +112,28 @@ class PrefilterResult:
             self._fields = index.fields(bits)
         return self._fields
 
-    @fields.setter
-    def fields(self, value):
-        self._fields, self.device_bits = list(value), None
+    @property
+    def on_device(self) -> bool:
+        """A Some whose sets are in HBM."""
+        return self.kind == "some" and (self.device_bits is not None or self.resources is not None)
 
     @classmethod
     def from_device(cls, index, bits, matching: int):
         return cls("some", device_bits=(index, bits, matching))
 
-    @classmethod
-    def from_json(cls, text, json_index, res_bits, op_or: bool):
-        """PrefilterResult::combine of a text result (`text`: its device_bits, or None for All) with the non-empty resource set of
-        a JSON prefilter (res_bits over json_index.resource_ids, in HBM) under AND (op_or False) or OR, kept on the device: the
-        hand-offs combine the bitsets themselves (OpenSegment.search_json, TextSearcher.json_masks)."""
-        return cls("some", json=(text, json_index, res_bits, op_or))
+    def combine(self, json_index, res_bits, found: int, op_or: bool) -> "PrefilterResult":
+        """PrefilterResult::combine (nidx_types/src/prefilter.rs:49-92) of this text result with the resource set of a JSON prefilter
+        (res_bits over json_index.resource_ids, in HBM, from `found` matched JSON documents) under OR (op_or) or AND.  A Some stays on
+        the device: its text part, if any, and the resource part, which the hand-offs combine."""
+        text = self.device_bits if self.kind == "some" else None
+        if self.kind == "some" and text is None:
+            raise ValueError("json_filter needs the device prefilter")
+        if found == 0:   # an empty set: the text result under OR, None under AND
+            return self if op_or else PrefilterResult.none()
+        if (self.kind == "none" and not op_or) or (self.kind == "all" and op_or):
+            return self
+        # None under OR is the resource set alone; All under AND is the resource set ANDed with every field
+        return PrefilterResult("some", device_bits=text, resources=(json_index, res_bits), op_or=op_or and text is not None)
 
     @classmethod
     def all(cls):
@@ -406,15 +416,25 @@ class OpenSegment:
         return self.segment.search(queries, top_k, ef, min_score, with_duplicates, method, formula=nodes)
 
     def search_prefiltered(self, query, prefilter, formula, operator_and, with_duplicates, top_k, min_score, method=_lib.NIDX_METHOD_AUTO, ef=0):
-        """search() restricted by a prefilter made on the device (PrefilterResult.device_bits) instead of a key set: the matched
-        documents' paragraphs (nidx_vec_prefilter_bits through the text index's join table), combined with `formula` under the
-        operator as search() combines its clauses, go to the search as a bitset that never leaves the device."""
+        """search() restricted by a prefilter made on the device (a PrefilterResult with device_bits and / or resources) instead of a
+        key set: the paragraphs of the text part's documents (through the text index's join table) and of the resource part's
+        resources (every field of theirs, with or without a text document), combined under the result's operator, then with
+        `formula` under the operator as search() combines its clauses (nidx_vec_prefilter_bits), go to the search as a bitset that
+        never leaves the device."""
         import torch
 
-        index, doc_bits, _ = prefilter
         nodes, _, keep = self.formula_nodes([formula]) if formula is not None else (None, 0, None)
-        bits, matching = self.segment.prefilter_bits(doc_bits, index.join(self), index.n_docs_total(), self.records, nodes,
-                                                     _lib.NIDX_F_AND if operator_and else _lib.NIDX_F_OR)
+        doc_bits = join = res_bits = ranges = None
+        n_docs = n_res = 0
+        if prefilter.device_bits is not None:
+            index, doc_bits, _ = prefilter.device_bits
+            join, n_docs = index.join(self), index.n_docs_total()
+        if prefilter.resources is not None:
+            json_index, res_bits = prefilter.resources
+            ranges, n_res = self.json_ranges(json_index), len(json_index.resource_ids)
+        bits, matching = self.segment.prefilter_bits(doc_bits, join, n_docs, res_bits, ranges, n_res, self.records, nodes,
+                                                     _lib.NIDX_F_AND if operator_and else _lib.NIDX_F_OR,
+                                                     _lib.NIDX_F_OR if prefilter.op_or else _lib.NIDX_F_AND)
         if matching == 0:   # segment.rs:532-534: nothing can match
             return np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.float32)
         q = torch.as_tensor(np.asarray(query, dtype=np.float32)[None, :]).to(torch.device("cuda", self.config.device))
@@ -447,29 +467,6 @@ class OpenSegment:
         t = torch.from_numpy(ranges.view(np.int64)).to(torch.device("cuda", self.config.device))
         self._json_ranges = (json_index, t)
         return t
-
-    def search_json(self, query, json, formula, operator_and, with_duplicates, top_k, min_score, method=_lib.NIDX_METHOD_AUTO, ef=0):
-        """search() restricted by a prefilter combined with a JSON resource set (PrefilterResult.json): the paragraphs of the matched
-        resources (every field of theirs, with or without a text document) and those of the text prefilter's documents, combined
-        under its operator, then with `formula` (nidx_vec_prefilter_resources), all on the device."""
-        import torch
-
-        text, json_index, res_bits, op_or = json
-        nodes, _, keep = self.formula_nodes([formula]) if formula is not None else (None, 0, None)
-        doc_bits = join = None
-        n_docs = 0
-        if text is not None:
-            index, doc_bits, _ = text
-            join, n_docs = index.join(self), index.n_docs_total()
-        bits, matching = self.segment.prefilter_resources(doc_bits, join, n_docs, _lib.NIDX_F_OR if op_or else _lib.NIDX_F_AND, res_bits,
-                                                          self.json_ranges(json_index), len(json_index.resource_ids), self.records, nodes,
-                                                          _lib.NIDX_F_AND if operator_and else _lib.NIDX_F_OR)
-        if matching == 0:
-            return np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.float32)
-        q = torch.as_tensor(np.asarray(query, dtype=np.float32)[None, :]).to(torch.device("cuda", self.config.device))
-        ids, scores, counts = self.segment.search(q, top_k, ef, min_score, with_duplicates, method, filter_bits=bits, filter_matching=matching)
-        c = int(counts[0].item())
-        return ids[0, :c].cpu().numpy().view(np.uint32), scores[0, :c].cpu().numpy()
 
     def _raw_search(self, queries, k, filter_bits):
         """exact scan restricted to a paragraph bitset, no min_score: per (query, paragraph) the best vector's similarity."""
@@ -535,9 +532,8 @@ class VectorSearcher:
     def search(self, request: VectorSearchRequest, prefilter: PrefilterResult = None, method=_lib.NIDX_METHOD_AUTO, ef=0) -> VectorSearchResponse:
         prefilter = prefilter or PrefilterResult.all()
         multi = self.config.vector_cardinality == VectorCardinality.Multi
-        on_device = prefilter.device_bits if prefilter.kind == "some" and not multi else None
         clauses = []
-        if prefilter.kind == "some" and on_device is None and prefilter.json is None:  # searcher.rs:300-314
+        if prefilter.kind == "some" and prefilter.resources is None and (multi or prefilter.device_bits is None):  # searcher.rs:300-314
             clauses.append(_KeyPrefixSet(frozenset(f"{f.resource_id.hex}{f.field_id}" if f.field_id else f.resource_id.hex for f in prefilter.fields)))
         if request.filtering_formula is not None:
             clauses.append(_map_expression(request.filtering_formula))
@@ -549,7 +545,7 @@ class VectorSearcher:
             raise NidxError(-1, f"InconsistentDimensions: index_config {self.config.dimension}, vector {len(query)}")
         k = request.result_per_page
         if self.config.vector_cardinality == VectorCardinality.Multi:
-            if prefilter.json is not None:
+            if prefilter.resources is not None:
                 raise ValueError("json_filter is not supported on a multi-vector vectorset")
             return self._search_multi_vector(request, clauses, operator_and, prefilter, method, ef)
         fssc = _Fssc(k, request.with_duplicates)
@@ -557,11 +553,8 @@ class VectorSearcher:
             for seg in self.open_segments:
                 if request.segment_filtering_formula is not None and not _segment_matches(request.segment_filtering_formula, seg.tags):
                     continue
-                if prefilter.json is not None:
-                    addrs, scores = seg.search_json(query, prefilter.json, request.filtering_formula, operator_and, request.with_duplicates, k,
-                                                    request.min_score, method, ef)
-                elif on_device is not None:
-                    addrs, scores = seg.search_prefiltered(query, on_device, request.filtering_formula, operator_and, request.with_duplicates, k,
+                if prefilter.on_device:
+                    addrs, scores = seg.search_prefiltered(query, prefilter, request.filtering_formula, operator_and, request.with_duplicates, k,
                                                            request.min_score, method, ef)
                 else:
                     addrs, scores = seg.search(query, clauses, operator_and, request.with_duplicates, k, request.min_score, method, ef)

@@ -165,8 +165,8 @@ def worker(a):
         doc_bits = np.packbits(rng.random(((n_docs + 63) // 64) * 64) < 0.3, bitorder="little").view(np.uint64).copy()
         join = np.arange(n_docs, dtype=np.uint32)
         for name, (f, nf) in (("no_formula", (None, 0)), ("formula", (mixed, nm))):
-            fn = lambda: _lib.check(L.nidx_vec_prefilter_bits(seg._h, _lib.ptr(doc_bits), n_docs, _lib.ptr(join), f, nf, _lib.NIDX_F_AND,   # noqa: E731
-                                                              _lib.ptr(out), _lib.NIDX_MEM_HOST, C.byref(m), None))
+            fn = lambda: _lib.check(L.nidx_vec_prefilter_bits(seg._h, _lib.ptr(doc_bits), n_docs, _lib.ptr(join), _lib.NIDX_F_AND, None, 0, None,   # noqa: E731
+                                                              f, nf, _lib.NIDX_F_AND, _lib.ptr(out), _lib.NIDX_MEM_HOST, C.byref(m), None))
             times[f"{n}/prefilter_bits/{name}"] = timed(fn, a.warmup, a.steps)
             digests[f"{n}/prefilter_bits/{name}"] = hashlib.sha256(out.tobytes() + bytes(m)).hexdigest()
         seg.close()

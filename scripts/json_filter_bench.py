@@ -5,7 +5,7 @@ resources in one of 100 access groups; one paragraph per resource in a vector se
 timed) and in a paragraph segment.  Timed, each as the whole call (they end in a synchronise, as the search path calls them):
   json_pass         JsonIndex.prefilter: the host compile, nidx_txt_prefilter and nidx_txt_resource_bits, for
                     AND(price range, OR(cat, NOT ok)) ANDed with a two-group security tree;
-  vector_json       nidx_vec_prefilter_resources with the resources alone (text All under AND);
+  vector_json       nidx_vec_prefilter_bits with the resources alone (text All under AND);
   vector_json_text  the same under OR with a text result of 30 % of the fields;
   paragraph_mask    nidx_txt_join_mask with the security bits, the text bits and the resource bits under OR.
 Medians of --steps calls after --warmup, with min and max; the card's name and power limit are read in the same process.  One
@@ -86,10 +86,10 @@ def one_size(n, steps, warmup):
     text_words[: len(packed)] = packed
     text_bits = torch.from_numpy(text_words.view(np.int64)).to(dev)
     join = torch.from_numpy(np.arange(n, dtype=np.int32)).to(dev)
-    out["vector_json"] = timed(lambda: vec.prefilter_resources(None, None, 0, _lib.NIDX_F_AND, res_bits, ranges, n, n), steps, warmup)
-    out["vector_json_text"] = timed(lambda: vec.prefilter_resources(text_bits, join, n, _lib.NIDX_F_OR, res_bits, ranges, n, n), steps, warmup)
-    _, m1 = vec.prefilter_resources(None, None, 0, _lib.NIDX_F_AND, res_bits, ranges, n, n)
-    _, m2 = vec.prefilter_resources(text_bits, join, n, _lib.NIDX_F_OR, res_bits, ranges, n, n)
+    out["vector_json"] = timed(lambda: vec.prefilter_bits(None, None, 0, res_bits, ranges, n, n), steps, warmup)
+    out["vector_json_text"] = timed(lambda: vec.prefilter_bits(text_bits, join, n, res_bits, ranges, n, n, doc_op=_lib.NIDX_F_OR), steps, warmup)
+    _, m1 = vec.prefilter_bits(None, None, 0, res_bits, ranges, n, n)
+    _, m2 = vec.prefilter_bits(text_bits, join, n, res_bits, ranges, n, n, doc_op=_lib.NIDX_F_OR)
     out["vector_matching"] = [int(m1), int(m2)]
 
     par = TextSegment.create(n, 0, np.zeros(1, dtype=np.uint64), np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.uint32), np.zeros(n, dtype=np.uint8))

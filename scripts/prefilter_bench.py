@@ -119,11 +119,11 @@ def main():
     nodes, _keep = node_array(shapes["facet"][0])
     _, doc_matching = ts.prefilter(nodes, out=bits)
     for _ in range(a.warmup):
-        vs.prefilter_bits(bits, join, n, 2 * n_keys)
+        vs.prefilter_bits(bits, join, n, None, None, 0, 2 * n_keys)
     j_ms = []
     for _ in range(a.steps):
         t0 = time.perf_counter()
-        _, par_matching = vs.prefilter_bits(bits, join, n, 2 * n_keys)
+        _, par_matching = vs.prefilter_bits(bits, join, n, None, None, 0, 2 * n_keys)
         j_ms.append((time.perf_counter() - t0) * 1e3)
     out["join"] = dict(call_ms=round(float(np.median(j_ms)), 3), docs_matched=int(doc_matching), paragraphs_matched=int(par_matching))
     # the host loop it replaced, on the same documents (facet AND field), as the binding ran it

@@ -215,7 +215,15 @@ def test_launches_per_call_do_not_grow_with_the_formula():
         assert L_.nidx_launch_count() - before <= 2, t[0]
 
 
-def test_prefilter_bits_with_and_without_a_formula():
+def has_postings(ix, t):
+    kind, arg = t
+    return bool(ix.model(t).any()) if kind in ("label", "keys") else any(has_postings(ix, c) for c in arg)
+
+
+def test_prefilter_bits_text_and_resource_parts_with_and_without_a_formula():
+    """The hand-off's text part (documents joined to field keys), resource part (runs of field keys) or both under doc_op, with and
+    without a formula under op, against the host model; and its launches: one per part, one to scatter the formula's postings, and
+    and_bits_kernel or the program's pass."""
     ix = Index(4097)
     rng = np.random.default_rng(8)
     ix.set_alive("random", rng)
@@ -231,19 +239,41 @@ def test_prefilter_bits_with_and_without_a_formula():
     for d in np.flatnonzero(doc):
         if join[d] < N_FIELDS:
             joined[ix.fields[keys[join[d]]]] = True
-    for t in (None, L(4), chain(9, rng), ("or", [L(i) for i in range(40)])):
-        for op in (_lib.NIDX_F_AND, _lib.NIDX_F_OR):
-            nodes = None if t is None else nodes_of(t)
-            bits, matching = ix.seg.prefilter_bits(doc_words.view(np.uint64), join, n_docs, ix.n, None if t is None else nodes[0], op)
-            want = joined.copy()
-            if t is not None:
-                want = want & ix.model(t) if op == _lib.NIDX_F_AND else want | ix.model(t)
-            want &= ix.alive
-            ww = np.zeros((ix.n + 63) // 64 * 8, dtype=np.uint8)
-            pw = np.packbits(want, bitorder="little")
-            ww[: len(pw)] = pw
-            assert np.array_equal(bits, ww.view(np.uint64)), (t, op)
-            assert matching == int(want.sum())
+    # resource r's paragraphs: the postings of the field keys [lo, hi) (a resource's fields are one run of keys; some runs are empty)
+    n_res = 300
+    runs = np.sort(rng.integers(0, N_FIELDS + 1, (n_res, 2)), axis=1)
+    post_off = np.concatenate([[0], np.cumsum([len(ix.fields[k]) for k in keys])]).astype(np.uint64)
+    res = rng.random(n_res) < 0.2
+    res_words = np.zeros((n_res + 63) // 64 * 8, dtype=np.uint8)
+    pr = np.packbits(res, bitorder="little")
+    res_words[: len(pr)] = pr
+    res_joined = np.zeros(ix.n, dtype=bool)
+    for r in np.flatnonzero(res):
+        for j in range(*runs[r]):
+            res_joined[ix.fields[keys[j]]] = True
+    L_ = _lib.load()
+    for text, resources, doc_op in ((True, False, _lib.NIDX_F_AND), (False, True, _lib.NIDX_F_AND), (True, True, _lib.NIDX_F_AND),
+                                    (True, True, _lib.NIDX_F_OR)):
+        parts = dict(doc_bits=doc_words.view(np.uint64) if text else None, join=join if text else None, n_docs=n_docs if text else 0,
+                     res_bits=res_words.view(np.uint64) if resources else None, res_ranges=post_off[runs] if resources else None,
+                     n_res=n_res if resources else 0)
+        matched = joined if not resources else res_joined if not text else joined & res_joined if doc_op == _lib.NIDX_F_AND else joined | res_joined
+        for t in (None, L(4), chain(9, rng), ("or", [L(i) for i in range(40)])):
+            for op in (_lib.NIDX_F_AND, _lib.NIDX_F_OR):
+                nodes = None if t is None else nodes_of(t)
+                before = L_.nidx_launch_count()
+                bits, matching = ix.seg.prefilter_bits(**parts, n_paragraphs=ix.n, formula=None if t is None else nodes[0], op=op, doc_op=doc_op)
+                launches = L_.nidx_launch_count() - before
+                want = matched.copy()
+                if t is not None:
+                    want = want & ix.model(t) if op == _lib.NIDX_F_AND else want | ix.model(t)
+                want &= ix.alive
+                ww = np.zeros((ix.n + 63) // 64 * 8, dtype=np.uint8)
+                pw = np.packbits(want, bitorder="little")
+                ww[: len(pw)] = pw
+                assert np.array_equal(bits, ww.view(np.uint64)), (t, op, text, resources, doc_op)
+                assert matching == int(want.sum())
+                assert launches == text + resources + (t is not None and has_postings(ix, t)) + 1, (t, op, text, resources)
 
 
 def _open_segment():

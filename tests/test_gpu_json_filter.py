@@ -86,7 +86,7 @@ def test_json_prefilter_matches_the_model(n):
     ix.close()
 
 
-def test_vector_hand_off_and_paragraph_mask_match_host_restatements():
+def test_combined_result_hand_off_and_paragraph_mask_match_host_restatements():
     """A resource whose vectors belong to a field with no text document still passes at resource level."""
     import torch
 
@@ -109,7 +109,7 @@ def test_vector_hand_off_and_paragraph_mask_match_host_restatements():
     ix, keep = _index(jdocs, [True] * len(jdocs))
     for e in (path("t/p", "v", int_range=(1, 2)), op("not", path("t/p", "v", int=1))):
         res = M.resources(keep, e)
-        _, _, res_bits = ix.prefilter(e)
+        _, found, res_bits = ix.prefilter(e)
         for ff, op_or in (("/l/x1", False), ("/l/x1", True), (None, False), ("/l/none", True)):
             expr = None
             if ff is not None:
@@ -120,13 +120,13 @@ def test_vector_hand_off_and_paragraph_mask_match_host_restatements():
             tset = text.kind if text.kind in ("all", "none") else {(uuid.UUID(str(f.resource_id)).hex, f.field_id) for f in text.fields}
             want = M.combine(tset, res, op_or)
             assert want not in ("all", "none")
-            pf = V.PrefilterResult.from_json(text.device_bits if text.kind == "some" else None, ix, res_bits, op_or and text.kind == "some")
+            pf = text.combine(ix, res_bits, found, op_or)
             got = V.VectorSearcher(seg.config, [seg]).search(V.VectorSearchRequest(vector=[0.1] * 8, result_per_page=len(elems), min_score=-1e9,
                                                                                     with_duplicates=True), pf)
             got_keys = {d.doc_id for d in got.documents}
             want_keys = {k.key for k in elems if M.admits(want, k.key.split("/")[0], "/" + "/".join(k.key.split("/")[1:3]))}
             assert got_keys == want_keys, (e, ff, op_or)
-            masks = ps.json_masks(None, pf.json[0][1] if pf.json[0] else None, pf.json[0][0] if pf.json[0] else None, ix, res_bits, pf.json[3])
+            masks = ps.json_masks(None, pf)
             m = masks[0].cpu().numpy().view(np.uint64)
             want_m = [M.admits(want, d.uuid, d.field) for d in ps.segments[0].docs]
             assert np.array_equal(m, _words(want_m)), (e, ff, op_or)

@@ -129,6 +129,18 @@ def test_combine_cases():
     assert M.combine("none", {"a"}, True) == {("a", None)} and M.combine("none", {"a"}, False) == "none"
     assert M.combine(t, {"a"}, True) == {("a", None), ("b", "/t/y")}
     assert M.combine(t, {"a"}, False) == {("a", "/t/x")} and M.combine(t, {"c"}, False) == "none"
+    # PrefilterResult.combine gives the model's All and None; a Some keeps the text part and the non-empty resource set as parts
+    from nucliadb_b200 import vector as V
+
+    text = V.PrefilterResult.from_device("text index", "text bits", len(t))
+    for model, pf in (("all", V.PrefilterResult.all()), ("none", V.PrefilterResult.none()), (t, text)):
+        for res in (set(), {"a"}):
+            for op_or in (False, True):
+                got, want = pf.combine("json index", "res bits" if res else None, len(res), op_or), M.combine(model, res, op_or)
+                assert got.kind == (want if want in ("all", "none") else "some"), (model, res, op_or)
+                if got.kind == "some":
+                    assert got.device_bits == pf.device_bits and got.resources == (("json index", "res bits") if res else None)
+                    assert got.op_or == (op_or and pf is text and bool(res))
 
 
 def test_empty_expression_and_missing_predicate_are_invalid():
