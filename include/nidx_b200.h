@@ -497,6 +497,89 @@ int nidx_txt_join_mask(nidx_txt_segment* seg, const uint64_t* and_bits, const ui
                        const uint64_t* res_bits, uint64_t n_res, const uint32_t* res_join, int32_t op, uint64_t* out_bits, int mem,
                        uint64_t* out_matching, void* stream);
 
+/* ---- Graph search: NidxSearcher.GraphSearch (reference: nidx_relation).  One document per relation, in a text segment without
+ * terms: its facets (nidx_txt_set_facets), resource / field ords (nidx_txt_set_doc_columns) and alive bits, so the prefilter mask
+ * is nidx_txt_join_mask's.  The graph columns live in a handle that borrows that segment: the segment must outlive it. */
+typedef struct nidx_graph nidx_graph;
+
+#define NIDX_G_SRC_VALUE 0    /* per-document u32 ord columns: the source / target normalised value (values dictionary) */
+#define NIDX_G_DST_VALUE 1
+#define NIDX_G_SRC_TYPE 2     /* node types (0..3) */
+#define NIDX_G_DST_TYPE 3
+#define NIDX_G_SRC_SUBTYPE 4  /* subtype ords */
+#define NIDX_G_DST_SUBTYPE 5
+#define NIDX_G_REL_TYPE 6     /* relation type (0..5) */
+#define NIDX_G_LABEL 7        /* label ord */
+#define NIDX_G_SRC_NODE 8     /* node key ords (value, type, subtype) */
+#define NIDX_G_DST_NODE 9
+#define NIDX_G_REL_KEY 10     /* relation key ord (type, label) */
+#define NIDX_G_COLUMNS 11
+
+typedef struct nidx_graph_columns {   /* host pointers */
+    const uint32_t* col[NIDX_G_COLUMNS];   /* [n_docs] each */
+    const uint64_t* tok_off[2];            /* [n_docs + 1]: source (0) / target (1) default tokens as ords of the token dictionary */
+    const uint32_t* tok_ord[2];
+    uint32_t n_values;                     /* the values dictionary: entry e is value_cp[value_off[e] .. value_off[e + 1]) (code points) */
+    const uint32_t* value_cp;
+    const uint64_t* value_off;
+    uint32_t n_tokens;                     /* the token dictionary, as the values' */
+    const uint32_t* token_cp;
+    const uint64_t* token_off;
+    uint32_t n_node_keys, n_rel_keys;      /* NODE columns are < n_node_keys, REL_KEY < n_rel_keys */
+} nidx_graph_columns;
+
+/* A graph handle over seg (which must outlive it), without columns. */
+int nidx_graph_create(nidx_txt_segment* seg, nidx_graph** out);
+/* Checks and uploads the columns and dictionaries to HBM; a rejected or failed call leaves the previous ones in place. */
+int nidx_graph_set_columns(nidx_graph* g, const nidx_graph_columns* cols);
+void nidx_graph_close(nidx_graph* g);
+
+#define NIDX_G_EQ 0          /* column arg == lo; score w */
+#define NIDX_G_COLBITS 1     /* column arg (a value column) has an ord matched by automaton term lo; score w */
+#define NIDX_G_TOKBITS 2     /* some token of side arg (0 source, 1 target) is matched by automaton term lo; score w */
+#define NIDX_G_TOKSET 3      /* some token of side arg is one of the n ords `ords` (host pointer); score w */
+#define NIDX_G_FACET 4       /* a facet ord in [lo, hi); score w */
+#define NIDX_G_CONST 5       /* every document (lo = 1) or none (lo = 0); score w */
+#define NIDX_G_AND 6         /* n >= 1 operands: all match; score = their sum, in order */
+#define NIDX_G_OR 7          /* n >= 1 operands: any matches; score = the sum of the matched ones, in order */
+#define NIDX_G_NOT 8         /* n = 1: the operand does not match; score 0 */
+#define NIDX_G_CONST_SCORE 9 /* n = 1: the operand, scored w where it matches */
+typedef struct nidx_graph_node {      /* an expression in pre-order */
+    int32_t kind;                     /* NIDX_G_* */
+    int32_t n;                        /* AND / OR / NOT / CONST_SCORE: operands; TOKSET: ords */
+    int32_t arg;                      /* EQ / COLBITS: the column; TOKBITS / TOKSET: the side */
+    float w;
+    int64_t lo, hi;
+    const uint32_t* ords;
+} nidx_graph_node;
+
+#define NIDX_G_TERMS_VALUES 0   /* an automaton term over the values dictionary */
+#define NIDX_G_TERMS_TOKENS 1   /* over the token dictionary */
+#define NIDX_G_MAX_TERMS 64     /* automaton terms per search, 4096 code points in all */
+typedef struct nidx_graph_term {
+    int32_t dict;                     /* NIDX_G_TERMS_* */
+    int32_t distance;                 /* 0..2: restricted Damerau-Levenshtein on code points */
+    int32_t prefix;                   /* 1: some prefix of the entry is within distance */
+    int32_t n_cp;
+    const uint32_t* cp;               /* host pointer */
+} nidx_graph_term;
+
+#define NIDX_G_PATH 0        /* ids: documents (ties: lower document first) */
+#define NIDX_G_NODES 1       /* two expressions follow each other in nodes: the source side and the destination side; ids: node key
+                                ords, each scored with the max over both sides' matched documents (ties: lower ord first) */
+#define NIDX_G_RELATIONS 2   /* ids: relation key ords, the max over the matched documents (ties: lower ord first) */
+#define NIDX_G_MAX_K 1024
+/* The scored expression(s) over the documents alive AND mask (n_docs bits, `mem`; NULL: alive) -> the best k (1..NIDX_G_MAX_K) ids by
+ * score descending: out_ids [k] (NIDX_NIL padded), out_scores [k], *out_count (all `mem`).  An expression deeper than
+ * NIDX_PREFILTER_MAX_DEPTH or longer than 4096 instructions, more automaton terms or code points than above, a distance > 2 and a k
+ * out of range, and a node whose w is negative, NaN or infinite are NIDX_EINVAL (sums of finite scores >= 0 order as their bits);
+ * a handle without columns is NIDX_ESTATE.  The call returns when the outputs are in place (host) or
+ * are enqueued on `stream` (device). */
+int nidx_graph_search(nidx_graph* g, const nidx_graph_node* nodes, int32_t n_nodes, const nidx_graph_term* terms, int32_t n_terms, int32_t kind,
+                      int32_t k, const uint64_t* mask, int mem, uint32_t* out_ids, float* out_scores, int32_t* out_count, void* stream);
+/* The times (ms) of the last search's dictionary pass, scored pass(es), collection (unique max + top-k) and whole call. */
+int nidx_graph_last_times(nidx_graph* g, float* ms4);
+
 /* ------------------------------------------------------------------------------------------
  * Segments sharded over the GPUs of one node: one process (or thread) per GPU, one segment each
  * (reference: the searcher's scatter-gather, nidx/src/searcher/grpc.rs:253-431, merged by

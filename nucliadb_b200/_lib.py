@@ -62,6 +62,26 @@ NIDX_P_FACET, NIDX_P_FIELD, NIDX_P_RESOURCE, NIDX_P_DATE, NIDX_P_KEYWORD, NIDX_P
 NIDX_PREFILTER_MAX_DEPTH = 64
 
 
+class GraphColumns(C.Structure):
+    _fields_ = [("col", C.c_void_p * 11), ("tok_off", C.c_void_p * 2), ("tok_ord", C.c_void_p * 2), ("n_values", C.c_uint32), ("value_cp", C.c_void_p),
+                ("value_off", C.c_void_p), ("n_tokens", C.c_uint32), ("token_cp", C.c_void_p), ("token_off", C.c_void_p), ("n_node_keys", C.c_uint32),
+                ("n_rel_keys", C.c_uint32)]
+
+
+class GraphNode(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("n", C.c_int32), ("arg", C.c_int32), ("w", C.c_float), ("lo", C.c_int64), ("hi", C.c_int64), ("ords", C.c_void_p)]
+
+
+class GraphTerm(C.Structure):
+    _fields_ = [("dict", C.c_int32), ("distance", C.c_int32), ("prefix", C.c_int32), ("n_cp", C.c_int32), ("cp", C.c_void_p)]
+
+
+(NIDX_G_EQ, NIDX_G_COLBITS, NIDX_G_TOKBITS, NIDX_G_TOKSET, NIDX_G_FACET, NIDX_G_CONST, NIDX_G_AND, NIDX_G_OR, NIDX_G_NOT,
+ NIDX_G_CONST_SCORE) = range(10)
+NIDX_G_TERMS_VALUES, NIDX_G_TERMS_TOKENS = 0, 1
+NIDX_G_PATH, NIDX_G_NODES, NIDX_G_RELATIONS = 0, 1, 2
+
+
 class TxtSearchParams(C.Structure):
     _fields_ = [("k", C.c_int32), ("mode", C.c_int32), ("use_tf", C.c_int32), ("min_score", C.c_float), ("after_mode", C.c_int32),
                 ("after_score", C.c_float), ("after_docaddr", C.c_uint64), ("docaddr_base", C.c_uint64)]
@@ -156,6 +176,11 @@ SIGNATURES = {
     "nidx_vec_prefilter_bits": (i32, [P, P, u64, P, i32, P, u64, P, NODES, i32, i32, P, i32, P, P]),
     "nidx_txt_resource_bits": (i32, [P, P, u64, P, i32, P]),
     "nidx_txt_join_mask": (i32, [P, P, P, u64, P, P, u64, P, i32, P, i32, P, P]),
+    "nidx_graph_create": (i32, [P, P]),
+    "nidx_graph_set_columns": (i32, [P, P]),   # cols: a GraphColumns
+    "nidx_graph_close": (None, [P]),
+    "nidx_graph_search": (i32, [P, P, i32, P, i32, i32, i32, P, i32, P, P, P, P]),
+    "nidx_graph_last_times": (i32, [P, P]),
     "nidx_shard_unique_id": (i32, [P]),
     "nidx_shard_init": (i32, [P, i32, i32, i32, P]),
     "nidx_shard_destroy": (None, [P]),

@@ -14,11 +14,13 @@ Reference:
   nidx/nidx_text/src/resource_indexer.rs:49-62                    Resource.security -> the access groups of its documents
   nidx/nidx_json/src/resource_indexer.rs, lib.rs                  Resource.json_fields -> one JSON document per resource
   nidx/src/searcher/query_planner/prefilter.rs:24-72              SearchRequest.json_filter, combined with the text prefilter
+  nidx/nidx_relation/src/resource_indexer.rs, reader.rs           Resource.field_relations -> one relation document each; GraphSearch
+  nidx/src/searcher/shard_search.rs:290-362, shard_merge.rs:350-375   NidxSearcher.GraphSearch: prefilter, search, concatenation
 
 What is kept of the reference's machinery is the INTERFACE: metadata lives in memory (no PostgreSQL), every index message
 becomes one immutable segment per index (as in the reference), deletions are (key, seq) pairs applied to older segments, and
 "sync" re-opens the searchers (index_cache.rs:180-200).  Scheduler, worker, merges-in-the-background, NATS, object stores other
-than the local file store, relations / graph / suggest are outside the hot path (SURVEY 8) and answer UNIMPLEMENTED.
+than the local file store, relation prefix search / suggest are outside the hot path (SURVEY 8) and answer UNIMPLEMENTED.
 """
 from __future__ import annotations
 
@@ -32,6 +34,7 @@ from typing import Optional
 
 import numpy as np
 
+from . import graph as Gr
 from . import json_index as J
 from . import nidx_protos as P
 from . import text as T
@@ -59,6 +62,8 @@ class _Shard:
     resource_groups: dict = field(default_factory=dict)      # resource id -> access groups of its latest index message
     json_deletions: list = field(default_factory=list)       # [(deletion key, seq)]: json_fields_to_delete and resource deletions
     json_index: Optional[J.JsonIndex] = None
+    graph_docs: list = field(default_factory=list)           # [([GraphDoc], seq)] one list per index message
+    graph_index: Optional[Gr.GraphIndex] = None
     text_searcher: Optional[T.TextSearcher] = None
     paragraph_searcher: Optional[T.ParagraphSearcher] = None
 
@@ -110,6 +115,26 @@ def _json_deletes(key: str, rid: str) -> bool:
     return raw == rid
 
 
+def _uuid_hex(rid: str) -> str:
+    try:
+        return _uuid.UUID(rid).hex
+    except ValueError:
+        return rid
+
+
+def merge_graph(into, part):
+    """shard_merge.rs:350-375: a shard's GraphSearchResponse appended to the merged one, its paths' node and relation indices offset
+    by what is already there."""
+    n_nodes, n_rels = len(into.nodes), len(into.relations)
+    into.nodes.extend(part.nodes)
+    into.relations.extend(part.relations)
+    into.scores.extend(part.scores)
+    for p in part.graph:
+        q = into.graph.add()
+        q.CopyFrom(p)
+        q.source, q.relation, q.destination = p.source + n_nodes, p.relation + n_rels, p.destination + n_nodes
+
+
 def merge_facets(shards_facets) -> dict:
     """shard_merge.rs:380-414: the counts of equal (group, tag) pairs of the shards' facet maps ({group: [(tag, total)]}) are
     summed; the merged lists are not cut again.  The reference lists them in a HashMap's order; here count descending, then tag
@@ -151,7 +176,9 @@ class NidxBinding:
         self._searcher = grpc.server(futures.ThreadPoolExecutor(max_workers=8))
         self._searcher.add_generic_rpc_handlers((grpc.method_handlers_generic_handler("nidx.NidxSearcher", {
             "Search": grpc.unary_unary_rpc_method_handler(self._grpc_search, request_deserializer=P.SearchRequest.FromString,
-                                                          response_serializer=lambda m: m.SerializeToString())}),))
+                                                          response_serializer=lambda m: m.SerializeToString()),
+            "GraphSearch": grpc.unary_unary_rpc_method_handler(self._grpc_graph_search, request_deserializer=P.GraphSearchRequest.FromString,
+                                                               response_serializer=lambda m: m.SerializeToString())}),))
         self.searcher_port = self._searcher.add_insecure_port("127.0.0.1:0")
         self._api = grpc.server(futures.ThreadPoolExecutor(max_workers=2))
         self._api.add_generic_rpc_handlers((grpc.method_handlers_generic_handler("nidx.NidxApi", {
@@ -215,6 +242,7 @@ class NidxBinding:
         # the JSON document (nidx_json/src/resource_indexer.rs), flattened first: invalid JSON fails the message before any index
         # changes.  Its deletions are json_fields_to_delete only (JsonIndexer::deletions_for_resource), not the re-index itself
         json_entries = J.flatten({k: v.value for k, v in res.json_fields.items()}) if res.json_fields and not res.skip_json else None
+        graph_docs = Gr.docs_from_resource(res) if res.field_relations else []   # a relation without source or target fails the message
         # a re-indexed resource replaces its older copies: prefixes to delete, applied to OLDER segments only (seq rule, lib.rs:188-199)
         for vi in shard.vectorsets.values():
             for key in list(res.vectors_to_delete_in_all_vectorsets) or [rid]:
@@ -256,6 +284,8 @@ class NidxBinding:
                     shard.paragraph_meta[(rid, "/" + fid if not fid.startswith("/") else fid, len(pdocs) - 1, seq)] = (pid, par)
             if pdocs:
                 shard.paragraph_segments.append((pdocs, seq))
+        if graph_docs:
+            shard.graph_docs.append((graph_docs, seq))
         shard.json_deletions.extend((key, seq) for key in res.json_fields_to_delete)
         if json_entries is not None:
             shard.json_docs.append((rid, json_entries, seq))
@@ -290,6 +320,15 @@ class NidxBinding:
         if shard.json_index is not None:
             shard.json_index.close()
         shard.json_index = J.JsonIndex(jd, device=self.device) if jd else None
+        # relations (nidx_relation): a newer message replaces a resource's relations, a deletion hides the older ones
+        last_del: dict = {}   # resource -> its latest deletion (or replacement) seq
+        for rid, dseq in shard.deleted_resources:
+            r = _uuid_hex(rid)
+            last_del[r] = max(last_del.get(r, 0), dseq)
+        gd = [d for docs, seq in shard.graph_docs for d in docs if last_del.get(d.rid, 0) <= seq]
+        if shard.graph_index is not None:
+            shard.graph_index.close()
+        shard.graph_index = Gr.GraphIndex(gd, device=self.device) if gd else None
 
     # ---- NidxSearcher.Search (shard_search.rs:60-241 + shard_merge.rs) ---------------------------------------------------------
     def search(self, request):
@@ -315,6 +354,47 @@ class NidxBinding:
         except ValueError as e:
             context.abort(grpc.StatusCode.INVALID_ARGUMENT, str(e))
 
+    # ---- NidxSearcher.GraphSearch (shard_search.rs:290-362, shard_merge.rs:350-375) ---------------------------------------------
+    def graph_search(self, request):
+        """nodereader.GraphSearchRequest -> nodereader.GraphSearchResponse: each shard's answer, concatenated in request order with its
+        node and relation indices offset.  A VectorMatch leaf is NotImplementedError (semantic node / edge matches)."""
+        resp = P.GraphSearchResponse()
+        with self._lock:
+            for sid in request.shard_ids:
+                shard = self._shards.get(sid)
+                if shard is None:
+                    raise KeyError(f"shard {sid} not found")
+                security = list(request.security.access_groups) if request.HasField("security") else None
+                field_filter = request.field_filter if request.HasField("field_filter") else None
+                merge_graph(resp, self._graph_shard(shard, request, field_filter, security))
+        resp.shard_ids.extend(request.shard_ids)
+        return resp
+
+    def _graph_shard(self, shard: _Shard, request, field_filter, security):
+        """Prefilter::parse_graph (field_filter and security only): no text index or a None result answers nothing."""
+        if shard.graph_index is None:
+            return P.GraphSearchResponse()
+        prefilter = None
+        if field_filter is not None or security is not None:
+            if shard.text_searcher is None:
+                return P.GraphSearchResponse()
+            prefilter = shard.text_searcher.prefilter(field_filter, security=security)
+        return Gr.GraphSearcher(shard.graph_index).search(request, prefilter)
+
+    def _grpc_graph_search(self, request, context):
+        import grpc
+
+        try:
+            return self.graph_search(request)
+        except KeyError as e:
+            context.abort(grpc.StatusCode.NOT_FOUND, str(e))
+        except NotImplementedError as e:
+            context.abort(grpc.StatusCode.UNIMPLEMENTED, str(e))
+        except V.NidxError as e:
+            context.abort(grpc.StatusCode.INTERNAL, str(e))
+        except ValueError as e:
+            context.abort(grpc.StatusCode.INVALID_ARGUMENT, str(e))
+
     def _search_shard(self, shard: _Shard, req):
         k = int(req.result_per_page)
         out = {}
@@ -332,6 +412,11 @@ class NidxBinding:
             else:   # a stand-in for libnidx_b200.so without the prefilter (the ABI emulator of the host-logic tests): the host loop
                 fields = [V.FieldId(_uuid.UUID(d.uuid), d.field) for seg in shard.text_searcher.segments for d in seg.docs if _doc_matches(req.field_filter, d)]
                 prefilter = V.PrefilterResult.some(fields) if fields else V.PrefilterResult.none()
+        # SearchRequest.graph_search (query_planner.rs:291-300): a PATH search with top_k = max(result_per_page, 20), prefiltered as
+        # GraphSearch is (_graph_shard: field_filter and security; json_filter does not apply to relations, DESIGN 9)
+        if req.HasField("graph_search"):
+            greq = P.GraphSearchRequest(query=req.graph_search.query, kind=Gr.PATH, top_k=max(k, 20))
+            out["graph"] = self._graph_shard(shard, greq, field_filter, security)
         # the JSON prefilter (query_planner/prefilter.rs:24-72): the JSON resource set, ANDed on the device with security, combined
         # with the text result under filter_operator (PrefilterResult::combine).  Security is applied outside the combination:
         # AND(security, op(field_filter, json)), so a security filter is never widened (DESIGN 7)
@@ -373,6 +458,10 @@ class NidxBinding:
         k = int(req.result_per_page)
         resp = P.SearchResponse()
         resp.shard_ids.extend(sid for sid, _ in parts)
+        if req.HasField("graph_search"):
+            for _, p in parts:
+                if "graph" in p:
+                    merge_graph(resp.graph, p["graph"])
         # vectors: kmerge_by(score >=), take(k) (shard_merge.rs:332-348), shards in request order standing for the reference's
         # `responses` order; equal scores come out in the order itertools' heap gives them, not first shard first
         merged = kmerge_by([p.get("vector", []) for _, p in parts], lambda a, b: a.score >= b.score)
@@ -435,6 +524,9 @@ class NidxBinding:
                 if shard.json_index is not None:
                     shard.json_index.close()
                     shard.json_index = None
+                if shard.graph_index is not None:
+                    shard.graph_index.close()
+                    shard.graph_index = None
             self._shards.clear()
 
     def __del__(self):   # lib.rs Drop: the cancellation token

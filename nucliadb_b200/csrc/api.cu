@@ -18,6 +18,7 @@
 
 #include "../../include/nidx_b200.h"
 #include "bm25.cuh"
+#include "graph.cuh"
 #include "phrase.cuh"
 #include "prefilter.cuh"
 #include "common.cuh"
@@ -3379,6 +3380,322 @@ int nidx_shard_search(const nidx_shard_search_request* rq, nidx_shard_search_res
         if (r) return r;
     }
     return st.finish();
+}
+
+}  // extern "C"
+
+// ---- graph search (graph.cuh) ---------------------------------------------------------------------------------------------------
+struct nidx_graph {
+    nidx_txt_segment* seg = nullptr;   // borrowed: alive bits, facets
+    bool ready = false;
+    DevArray<uint32_t> d_col[GF_COLS], d_tok_off[2], d_tok[2], d_value_cp, d_token_cp;
+    DevArray<uint64_t> d_value_off, d_token_off;
+    uint32_t n_values = 0, n_tokens = 0, n_node_keys = 0, n_rel_keys = 0;
+    cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // call start, dictionary pass, scored pass, collection
+    ~nidx_graph() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
+// An expression (pre-order nidx_graph_node) as graph_eval_kernel runs it: post-order, with the deepest stack it reaches.
+struct GraphPlan {
+    std::vector<PfOp> prog;
+    std::vector<uint32_t> ords;        // TOKSET lists
+    bool val_bits = false, tok_bits = false;
+    uint32_t level = 0, depth = 0;
+
+    void push(const PfOp& o, int pops) { prog.push_back(o); level = level - pops + 1; depth = std::max(depth, level); }
+    int compile(const nidx_graph_node* nodes, int n_nodes, int& i, int lvl, uint32_t n_terms, const std::vector<int>& term_dict) {
+        if (i >= n_nodes) return fail(NIDX_EINVAL, "malformed graph expression (operand counts do not add up to %d nodes)", n_nodes);
+        if (lvl > NIDX_PREFILTER_MAX_DEPTH) return fail(NIDX_EINVAL, "the graph expression nests deeper than %d levels", NIDX_PREFILTER_MAX_DEPTH);
+        const nidx_graph_node& nd = nodes[i++];
+        const int at = i - 1;
+        PfOp o{};
+        o.lo = nd.lo; o.hi = nd.hi; o.w = nd.w;
+        // the per-key max (atomicMax on the bits) and the top-k keys (score bits << 32) order scores as unsigned integers: only
+        // finite scores >= 0 (and -0, which is +0 there) keep their order
+        if (!(nd.w >= 0.f) || !std::isfinite(nd.w)) return fail(NIDX_EINVAL, "graph node %d: the score must be finite and >= 0", at);
+        if (nd.w == 0.f) o.w = 0.f;
+        switch (nd.kind) {
+            case NIDX_G_EQ:
+                if (nd.arg < 0 || nd.arg >= GF_COLS) return fail(NIDX_EINVAL, "graph node %d: bad column", at);
+                o.op = GF_EQ; o.arg = (uint32_t)nd.arg; break;
+            case NIDX_G_COLBITS:
+                if (nd.arg != NIDX_G_SRC_VALUE && nd.arg != NIDX_G_DST_VALUE) return fail(NIDX_EINVAL, "graph node %d: automaton leaves read a value column", at);
+                if (nd.lo < 0 || nd.lo >= n_terms || term_dict[nd.lo] != NIDX_G_TERMS_VALUES) return fail(NIDX_EINVAL, "graph node %d: bad values term", at);
+                o.op = GF_COLBITS; o.arg = (uint32_t)nd.arg; val_bits = true; break;
+            case NIDX_G_TOKBITS:
+                if (nd.arg != 0 && nd.arg != 1) return fail(NIDX_EINVAL, "graph node %d: bad side", at);
+                if (nd.lo < 0 || nd.lo >= n_terms || term_dict[nd.lo] != NIDX_G_TERMS_TOKENS) return fail(NIDX_EINVAL, "graph node %d: bad tokens term", at);
+                o.op = GF_TOKBITS; o.arg = (uint32_t)nd.arg; tok_bits = true; break;
+            case NIDX_G_TOKSET:
+                if ((nd.arg != 0 && nd.arg != 1) || nd.n < 0 || (nd.n && !nd.ords)) return fail(NIDX_EINVAL, "graph node %d: bad token set", at);
+                o.op = GF_TOKSET; o.arg = (uint32_t)nd.arg; o.lo = (int64_t)ords.size();
+                ords.insert(ords.end(), nd.ords, nd.ords + nd.n);
+                o.hi = (int64_t)ords.size();
+                break;
+            case NIDX_G_FACET: o.op = GF_FACET; break;
+            case NIDX_G_CONST: o.op = GF_CONST; o.arg = nd.lo ? 1u : 0u; break;
+            case NIDX_G_AND: case NIDX_G_OR: {
+                if (nd.n < 1) return fail(NIDX_EINVAL, "graph node %d: AND / OR take at least one operand", at);
+                for (int c = 0; c < nd.n; ++c) {
+                    int r = compile(nodes, n_nodes, i, lvl + 1, n_terms, term_dict);
+                    if (r) return r;
+                    if (c) { PfOp b{}; b.op = nd.kind == NIDX_G_AND ? GF_AND : GF_OR; push(b, 2); }
+                }
+                return 0;
+            }
+            case NIDX_G_NOT: case NIDX_G_CONST_SCORE: {
+                if (nd.n != 1) return fail(NIDX_EINVAL, "graph node %d: NOT / CONST_SCORE take one operand", at);
+                int r = compile(nodes, n_nodes, i, lvl + 1, n_terms, term_dict);
+                if (r) return r;
+                o.op = nd.kind == NIDX_G_NOT ? GF_NOT : GF_CONST_SCORE;
+                push(o, 1);
+                return 0;
+            }
+            default: return fail(NIDX_EINVAL, "graph node %d: bad kind %d", at, nd.kind);
+        }
+        push(o, 0);
+        return 0;
+    }
+};
+
+extern "C" {
+
+int nidx_graph_create(nidx_txt_segment* seg, nidx_graph** out) {
+    int r = require_handle(seg);
+    if (r) return r;
+    if (!out) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(seg->ix->device));
+    std::unique_ptr<nidx_graph> g(new nidx_graph());
+    g->seg = seg;
+    for (cudaEvent_t& e : g->ev) CU(cudaEventCreate(&e));
+    *out = g.release();
+    return 0;
+}
+
+void nidx_graph_close(nidx_graph* g) {
+    if (!g) return;
+    cudaSetDevice(g->seg->ix->device);
+    cudaDeviceSynchronize();
+    delete g;
+}
+
+int nidx_graph_set_columns(nidx_graph* g, const nidx_graph_columns* c) {
+    int r = require_handle(g);
+    if (r) return r;
+    if (!c) return fail(NIDX_EINVAL, "null argument");
+    const uint32_t n = g->seg->ix->n_docs;
+    if (n && std::any_of(c->col, c->col + GF_COLS, [](const uint32_t* p) { return !p; })) return fail(NIDX_EINVAL, "null column");
+    if (!c->tok_off[0] || !c->tok_off[1] || !c->value_off || !c->token_off) return fail(NIDX_EINVAL, "null argument");
+    if ((c->value_off[c->n_values] && !c->value_cp) || (c->token_off[c->n_tokens] && !c->token_cp)) return fail(NIDX_EINVAL, "null dictionary");
+    const uint32_t limit[GF_COLS] = {c->n_values, c->n_values, 4, 4, NIDX_NIL, NIDX_NIL, 6, NIDX_NIL, c->n_node_keys, c->n_node_keys, c->n_rel_keys};
+    for (int k = 0; k < GF_COLS; ++k)
+        for (uint32_t d = 0; d < n; ++d)
+            if (c->col[k][d] >= limit[k]) return fail(NIDX_EINVAL, "column %d, document %u: ord out of range", k, d);
+    for (int s = 0; s < 2; ++s) {
+        if (c->tok_off[s][n] >= (1ull << 32)) return fail(NIDX_EINVAL, "at most 2^32-1 tokens per side");
+        if (c->tok_off[s][n] && !c->tok_ord[s]) return fail(NIDX_EINVAL, "null token ords");
+        for (uint32_t d = 0; d < n; ++d) {
+            if (c->tok_off[s][d + 1] < c->tok_off[s][d]) return fail(NIDX_EINVAL, "tok_off must be non-decreasing");
+            for (uint64_t j = c->tok_off[s][d]; j < c->tok_off[s][d + 1]; ++j)
+                if (c->tok_ord[s][j] >= c->n_tokens) return fail(NIDX_EINVAL, "document %u: token ord out of range", d);
+        }
+    }
+    CU(cudaSetDevice(g->seg->ix->device));
+    DevArray<uint32_t> col[GF_COLS], tok_off[2], tok[2], value_cp, token_cp;
+    DevArray<uint64_t> value_off, token_off;
+    for (int k = 0; k < GF_COLS; ++k) {
+        ALLOC(col[k], std::max<size_t>(n, 1) * 4);
+        if (n) CU(cudaMemcpy(col[k], c->col[k], (size_t)n * 4, cudaMemcpyHostToDevice));
+    }
+    for (int s = 0; s < 2; ++s) {
+        const uint64_t nnz = c->tok_off[s][n];
+        std::vector<uint32_t> off(n + 1);
+        for (uint32_t d = 0; d <= n; ++d) off[d] = (uint32_t)c->tok_off[s][d];
+        ALLOC(tok_off[s], ((size_t)n + 1) * 4);
+        ALLOC(tok[s], std::max<uint64_t>(nnz, 1) * 4);
+        CU(cudaMemcpy(tok_off[s], off.data(), off.size() * 4, cudaMemcpyHostToDevice));
+        if (nnz) CU(cudaMemcpy(tok[s], c->tok_ord[s], nnz * 4, cudaMemcpyHostToDevice));
+    }
+    auto dict = [&](uint32_t nd, const uint32_t* cp, const uint64_t* off, DevArray<uint32_t>& dcp, DevArray<uint64_t>& doff) -> int {
+        for (uint32_t e = 0; e < nd; ++e)
+            if (off[e + 1] < off[e]) return fail(NIDX_EINVAL, "dictionary offsets must be non-decreasing");
+        ALLOC(dcp, std::max<uint64_t>(off[nd], 1) * 4);
+        ALLOC(doff, ((size_t)nd + 1) * 8);
+        if (off[nd]) CU(cudaMemcpy(dcp, cp, off[nd] * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(doff, off, ((size_t)nd + 1) * 8, cudaMemcpyHostToDevice));
+        return 0;
+    };
+    r = dict(c->n_values, c->value_cp, c->value_off, value_cp, value_off);
+    if (!r) r = dict(c->n_tokens, c->token_cp, c->token_off, token_cp, token_off);
+    if (r) return r;
+    for (int k = 0; k < GF_COLS; ++k) g->d_col[k] = std::move(col[k]);   // only now: a failed call leaves the previous columns
+    for (int s = 0; s < 2; ++s) { g->d_tok_off[s] = std::move(tok_off[s]); g->d_tok[s] = std::move(tok[s]); }
+    g->d_value_cp = std::move(value_cp); g->d_value_off = std::move(value_off);
+    g->d_token_cp = std::move(token_cp); g->d_token_off = std::move(token_off);
+    g->n_values = c->n_values; g->n_tokens = c->n_tokens; g->n_node_keys = c->n_node_keys; g->n_rel_keys = c->n_rel_keys;
+    g->ready = true;
+    return 0;
+}
+
+int nidx_graph_search(nidx_graph* g, const nidx_graph_node* nodes, int32_t n_nodes, const nidx_graph_term* terms, int32_t n_terms, int32_t kind,
+                      int32_t k, const uint64_t* mask, int mem, uint32_t* out_ids, float* out_scores, int32_t* out_count, void* stream_) {
+    int r = require_handle(g);
+    if (r) return r;
+    if (!nodes || n_nodes <= 0 || !out_ids || !out_scores || !out_count) return fail(NIDX_EINVAL, "null argument");
+    if (kind != NIDX_G_PATH && kind != NIDX_G_NODES && kind != NIDX_G_RELATIONS) return fail(NIDX_EINVAL, "bad kind %d", kind);
+    if (k < 1 || k > NIDX_G_MAX_K) return fail(NIDX_EINVAL, "k must be in 1..%d", NIDX_G_MAX_K);
+    if (n_terms < 0 || n_terms > GF_MAX_TERMS || (n_terms && !terms)) return fail(NIDX_EINVAL, "at most %d automaton terms", GF_MAX_TERMS);
+    if (!g->ready) return fail(NIDX_ESTATE, "the graph has no columns (nidx_graph_set_columns)");
+    TxtIndex* ix = g->seg->ix;
+    // the automaton terms, grouped by dictionary: each dictionary's bitsets are [its terms][words]
+    std::vector<int> term_dict(n_terms);
+    std::vector<uint32_t> slot(n_terms), term_cp;
+    std::vector<GraphTerm> dterms[2];
+    for (int t = 0; t < n_terms; ++t) {
+        const nidx_graph_term& T = terms[t];
+        if (T.dict != NIDX_G_TERMS_VALUES && T.dict != NIDX_G_TERMS_TOKENS) return fail(NIDX_EINVAL, "term %d: bad dictionary", t);
+        if (T.distance < 0 || T.distance > GF_MAX_DIST) return fail(NIDX_EINVAL, "term %d: the distance must be in 0..%d", t, GF_MAX_DIST);
+        if (T.n_cp < 0 || (T.n_cp && !T.cp)) return fail(NIDX_EINVAL, "term %d: bad code points", t);
+        term_dict[t] = T.dict;
+        slot[t] = (uint32_t)dterms[T.dict].size();
+        dterms[T.dict].push_back(GraphTerm{(uint32_t)term_cp.size(), (uint32_t)T.n_cp, (uint32_t)T.distance, T.prefix ? 1u : 0u});
+        term_cp.insert(term_cp.end(), T.cp, T.cp + T.n_cp);
+        if (term_cp.size() > (size_t)GF_MAX_TERM_CPS) return fail(NIDX_EINVAL, "the automaton terms have more than %d code points", GF_MAX_TERM_CPS);
+    }
+    GraphPlan P[2];
+    const int n_prog = kind == NIDX_G_NODES ? 2 : 1;
+    int at = 0;
+    for (int p = 0; p < n_prog; ++p) {
+        r = P[p].compile(nodes, n_nodes, at, 1, (uint32_t)n_terms, term_dict);
+        if (r) return r;
+        if (P[p].prog.size() > (size_t)PF_MAX_PROGRAM) return fail(NIDX_EINVAL, "the graph program has more than %d instructions", PF_MAX_PROGRAM);
+        for (PfOp& o : P[p].prog)   // automaton leaves name their dictionary's bitset
+            if (o.op == GF_COLBITS || o.op == GF_TOKBITS) o.lo = slot[o.lo];
+    }
+    if (at != n_nodes) return fail(NIDX_EINVAL, "malformed graph expression (operand counts do not add up to %d nodes)", n_nodes);
+    for (int p = 0; p < n_prog; ++p)
+        for (const PfOp& o : P[p].prog)
+            if (o.op == GF_FACET && !ix->facets.d_off) return fail(NIDX_ESTATE, "the segment has no facets (nidx_txt_set_facets)");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(ix->device));
+    WsGuard wg(ix->pool, stream);
+    Workspace& w = *wg.w;
+    const uint32_t n = ix->n_docs;
+    const size_t words = ((size_t)n + 63) / 64;
+    Stage st(stream, host, host);
+    const uint64_t* d_mask;
+    uint32_t* d_ids; float* d_sc; int32_t* d_cnt;
+    st.in(mask, words, &d_mask);
+    st.out(out_ids, (size_t)k, &d_ids);
+    st.out(out_scores, (size_t)k, &d_sc);
+    st.out(out_count, 1, &d_cnt);
+    r = st.place(w.stage);
+    if (r) return r;
+    CU(cudaEventRecord(g->ev[0], stream));
+    // scratch (w.prefilter): [values bitsets][token bitsets][term code points][terms][TOKSET ords][programs]
+    const size_t vw = ((size_t)g->n_values + 63) / 64, tw = ((size_t)g->n_tokens + 63) / 64;
+    const size_t nv = dterms[0].size(), nt = dterms[1].size();
+    auto al = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t o_tb = al(nv * vw * 8), o_cp = o_tb + al(nt * tw * 8), o_terms = o_cp + al(term_cp.size() * 4),
+                 o_ords = o_terms + al((nv + nt) * sizeof(GraphTerm)), o_prog0 = o_ords + al((P[0].ords.size() + P[1].ords.size()) * 4),
+                 o_prog1 = o_prog0 + al(P[0].prog.size() * sizeof(PfOp)), o_end = o_prog1 + al(P[1].prog.size() * sizeof(PfOp));
+    ENSURE(w.prefilter, o_end + 16);
+    unsigned char* base = w.prefilter.p;
+    uint64_t* val_bits = reinterpret_cast<uint64_t*>(base);
+    uint64_t* tok_bits = reinterpret_cast<uint64_t*>(base + o_tb);
+    uint32_t* d_term_cp = reinterpret_cast<uint32_t*>(base + o_cp);
+    GraphTerm* d_terms = reinterpret_cast<GraphTerm*>(base + o_terms);
+    uint32_t* d_ords = reinterpret_cast<uint32_t*>(base + o_ords);
+    // the host temporaries are staged in one pinned-free copy each; the call synchronises before they go
+    std::vector<GraphTerm> all_terms(dterms[0]);
+    all_terms.insert(all_terms.end(), dterms[1].begin(), dterms[1].end());
+    std::vector<uint32_t> all_ords(P[0].ords);
+    for (PfOp& o : P[1].prog)
+        if (o.op == GF_TOKSET) { o.lo += (int64_t)P[0].ords.size(); o.hi += (int64_t)P[0].ords.size(); }
+    all_ords.insert(all_ords.end(), P[1].ords.begin(), P[1].ords.end());
+    if (!term_cp.empty()) CU(cudaMemcpyAsync(d_term_cp, term_cp.data(), term_cp.size() * 4, cudaMemcpyHostToDevice, stream));
+    if (!all_terms.empty()) CU(cudaMemcpyAsync(d_terms, all_terms.data(), all_terms.size() * sizeof(GraphTerm), cudaMemcpyHostToDevice, stream));
+    if (!all_ords.empty()) CU(cudaMemcpyAsync(d_ords, all_ords.data(), all_ords.size() * 4, cudaMemcpyHostToDevice, stream));
+    for (int p = 0; p < n_prog; ++p)
+        CU(cudaMemcpyAsync(base + (p ? o_prog1 : o_prog0), P[p].prog.data(), P[p].prog.size() * sizeof(PfOp), cudaMemcpyHostToDevice, stream));
+    const size_t cp_smem = term_cp.size() * 4;
+    const int dict_threads = GF_THREADS;
+    for (int dct = 0; dct < 2; ++dct) {
+        const size_t nterm = dct ? nt : nv, dw = dct ? tw : vw;
+        const uint32_t nd = dct ? g->n_tokens : g->n_values;
+        if (!nterm || !dw) continue;
+        uint64_t* outb = dct ? tok_bits : val_bits;
+        CU(cudaMemsetAsync(outb, 0, nterm * dw * 8, stream));
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ix->sm_count * 8, (nd + dict_threads - 1) / dict_threads));
+        graph_dict_match_kernel<<<blocks, dict_threads, cp_smem, stream>>>(dct ? g->d_token_cp : g->d_value_cp, dct ? g->d_token_off : g->d_value_off, nd,
+                                                                           d_terms + (dct ? nv : 0), (uint32_t)nterm, d_term_cp, (uint32_t)term_cp.size(), outb, dw);
+        LAUNCHED();
+    }
+    CU(cudaEventRecord(g->ev[1], stream));
+    // scores and bits per program, then the per-key max (NODES / RELATIONS)
+    const uint32_t n_keys = kind == NIDX_G_PATH ? n : (kind == NIDX_G_NODES ? g->n_node_keys : g->n_rel_keys);
+    ENSURE(w.scores, (size_t)std::max<uint32_t>(n, 1) * 4 + 2 * std::max<size_t>(words, 1) * 8 + (size_t)std::max<uint32_t>(n_keys, 1) * 4);
+    float* d_score = w.scores.as<float>();
+    uint32_t* d_bits = reinterpret_cast<uint32_t*>(w.scores.p + (size_t)std::max<uint32_t>(n, 1) * 4);
+    uint32_t* d_kmax = reinterpret_cast<uint32_t*>(w.scores.p + (size_t)std::max<uint32_t>(n, 1) * 4 + 2 * std::max<size_t>(words, 1) * 8);
+    if (kind != NIDX_G_PATH && n_keys) CU(cudaMemsetAsync(d_kmax, 0, (size_t)n_keys * 4, stream));
+    GraphEvalArgs A{};
+    A.G.n_docs = n;
+    for (int c = 0; c < GF_COLS; ++c) A.G.col[c] = g->d_col[c];
+    for (int s = 0; s < 2; ++s) { A.G.tok_off[s] = g->d_tok_off[s]; A.G.tok[s] = g->d_tok[s]; }
+    A.G.fdoc_off = ix->facets.d_off; A.G.ford = ix->facets.d_ord;
+    A.alive = g->seg->d_alive; A.mask = d_mask; A.val_bits = val_bits; A.tok_bits = tok_bits; A.val_words = vw; A.tok_words = tw; A.ords = d_ords;
+    A.score = d_score; A.bits = d_bits;
+    const int eval_blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ix->sm_count * 8, (2 * words * 32 + GF_THREADS - 1) / GF_THREADS));
+    const int uniq_blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ix->sm_count * 8, ((size_t)n + 255) / 256));
+    const uint32_t key_col[3] = {0, NIDX_G_SRC_NODE, NIDX_G_REL_KEY};
+    for (int p = 0; p < n_prog; ++p) {
+        if (!words) break;
+        A.prog = reinterpret_cast<const PfOp*>(base + (p ? o_prog1 : o_prog0));
+        A.n_prog = (uint32_t)P[p].prog.size();
+        A.depth = P[p].depth;
+        const size_t smem = P[p].prog.size() * sizeof(PfOp) + (size_t)P[p].depth * GF_THREADS * 4;
+        CU(cudaFuncSetAttribute(graph_eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        graph_eval_kernel<<<eval_blocks, GF_THREADS, smem, stream>>>(A);
+        LAUNCHED();
+        if (kind != NIDX_G_PATH) {
+            graph_unique_kernel<<<uniq_blocks, 256, 0, stream>>>(n, d_bits, d_score, g->d_col[p ? NIDX_G_DST_NODE : key_col[kind]], d_kmax);
+            LAUNCHED();
+        }
+    }
+    CU(cudaEventRecord(g->ev[2], stream));
+    // the best k: per CTA, then one merge
+    const int cap = topk_cap(k, GF_THREADS);
+    const int tk_blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)ix->sm_count * 2, ((size_t)n_keys + GF_THREADS * 16 - 1) / (GF_THREADS * 16)));
+    ENSURE(w.partial, (size_t)tk_blocks * k * 8);
+    CU(cudaFuncSetAttribute(graph_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    CU(cudaFuncSetAttribute(graph_topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    if (n_keys && words) {
+        graph_topk_kernel<<<tk_blocks, GF_THREADS, (size_t)cap * 8, stream>>>(n_keys, d_bits, d_score, kind == NIDX_G_PATH ? nullptr : d_kmax, k, cap,
+                                                                             w.partial.as<uint64_t>());
+        LAUNCHED();
+    } else {
+        CU(cudaMemsetAsync(w.partial, 0, (size_t)tk_blocks * k * 8, stream));
+    }
+    graph_topk_merge_kernel<<<1, GF_THREADS, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), tk_blocks * k, k, cap, d_ids, d_sc, d_cnt);
+    LAUNCHED();
+    CU(cudaEventRecord(g->ev[3], stream));
+    CU(cudaGetLastError());
+    return st.finish(true);   // the programs, terms and lists are host temporaries
+}
+
+int nidx_graph_last_times(nidx_graph* g, float* ms4) {
+    int r = require_handle(g);
+    if (r) return r;
+    if (!ms4) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(g->seg->ix->device));
+    CU(cudaEventSynchronize(g->ev[3]));
+    CU(cudaEventElapsedTime(ms4 + 0, g->ev[0], g->ev[1]));
+    CU(cudaEventElapsedTime(ms4 + 1, g->ev[1], g->ev[2]));
+    CU(cudaEventElapsedTime(ms4 + 2, g->ev[2], g->ev[3]));
+    CU(cudaEventElapsedTime(ms4 + 3, g->ev[0], g->ev[3]));
+    return 0;
 }
 
 }  // extern "C"

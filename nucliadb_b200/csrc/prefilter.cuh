@@ -37,7 +37,8 @@ struct PfOp {          // one instruction: leaves push a bit, AND / OR pop two a
     uint32_t op;       // PfOpcode
     uint32_t arg;      // FACET / PUBLIC: the CSR column (0 facets, 1 access groups); DATE: the seconds column (0 created, 1 modified);
                        // BITS: the keyword leaf's slot; CONST: the bit
-    uint32_t pad[2];
+    float w;           // graph.cuh's scored leaves and CONST_SCORE: the score (unread here)
+    uint32_t pad;
 };
 
 struct PrefilterArgs {

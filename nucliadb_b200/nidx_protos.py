@@ -17,6 +17,8 @@ serialised by the reference's clients (``nidx_protos`` / ``nucliadb_protos``) de
     Security (Resource.security, SearchRequest.security)   nucliadb_protos utils.proto: repeated string access_groups = 1
     JsonFieldValue, Resource.json_fields / skip_json       noderesources.proto:13-15, 169-176
     JsonFilterExpression, JsonFieldPathFilter              nodereader.proto:338-380 (SearchRequest.json_filter = 32)
+    GraphQuery, GraphSearchRequest / Response              nodereader.proto:148-290 (SearchRequest.graph_search = 29, SearchResponse.graph = 5)
+    Relation, RelationNode, RelationMetadata, IndexRelation(s), Resource.field_relations   utils.proto, noderesources.proto
 """
 from __future__ import annotations
 
@@ -66,6 +68,21 @@ def _build():
     fd = descriptor_pb2.FileDescriptorProto(name="nucliadb_protos/utils.proto", package="utils", syntax="proto3")
     m = fd.message_type.add(name="Security")
     _field(m, "access_groups", 1, "string", repeated=True)
+    m = fd.message_type.add(name="RelationNode")                   # utils.proto: RelationNode
+    e = m.enum_type.add(name="NodeType")
+    for i, n in enumerate(("ENTITY", "LABEL", "RESOURCE", "USER")):
+        e.value.add(name=n, number=i)
+    _field(m, "value", 4, "string"); _field(m, "ntype", 5, "enum:.utils.RelationNode.NodeType"); _field(m, "subtype", 6, "string")
+    m = fd.message_type.add(name="RelationMetadata")
+    _field(m, "paragraph_id", 1, "string", optional=True); _field(m, "source_start", 2, "int32", optional=True)
+    _field(m, "source_end", 3, "int32", optional=True); _field(m, "to_start", 4, "int32", optional=True); _field(m, "to_end", 5, "int32", optional=True)
+    _field(m, "data_augmentation_task_id", 6, "string", optional=True)
+    m = fd.message_type.add(name="Relation")
+    e = m.enum_type.add(name="RelationType")
+    for i, n in enumerate(("CHILD", "ABOUT", "ENTITY", "COLAB", "SYNONYM", "OTHER")):
+        e.value.add(name=n, number=i)
+    _field(m, "relation", 5, "enum:.utils.Relation.RelationType"); _field(m, "source", 6, ".utils.RelationNode"); _field(m, "to", 7, ".utils.RelationNode")
+    _field(m, "relation_label", 8, "string"); _field(m, "metadata", 9, ".utils.RelationMetadata")
     pool.Add(fd)
 
     # ---- noderesources.proto ---------------------------------------------------------------------------------------------
@@ -99,6 +116,10 @@ def _build():
     _map(m, ".noderesources.IndexParagraph", "vectorsets_sentences", 10, "string", ".noderesources.VectorsetSentences")
     m = fd.message_type.add(name="IndexParagraphs")           # :118-121
     _map(m, ".noderesources.IndexParagraphs", "paragraphs", 1, "string", ".noderesources.IndexParagraph")
+    m = fd.message_type.add(name="IndexRelation")             # IndexRelation / IndexRelations
+    _field(m, "relation", 1, ".utils.Relation"); _field(m, "resource_field_id", 2, "string"); _field(m, "facets", 3, "string", repeated=True)
+    m = fd.message_type.add(name="IndexRelations")
+    _field(m, "relations", 1, ".noderesources.IndexRelation", repeated=True)
     m = fd.message_type.add(name="Resource")                  # :123-180
     _field(m, "resource", 1, ".noderesources.ResourceID"); _field(m, "metadata", 2, ".noderesources.IndexMetadata")
     _map(m, ".noderesources.Resource", "texts", 3, "string", ".noderesources.TextInformation")
@@ -111,6 +132,7 @@ def _build():
     _field(m, "skip_texts", 18, "bool"); _field(m, "skip_paragraphs", 19, "bool")
     _map(m, ".noderesources.Resource", "json_fields", 22, "string", ".noderesources.JsonFieldValue")
     _field(m, "json_fields_to_delete", 23, "string", repeated=True); _field(m, "skip_json", 24, "bool")
+    _map(m, ".noderesources.Resource", "field_relations", 10, "string", ".noderesources.IndexRelations")
     pool.Add(fd)
 
     # ---- nodereader.proto ------------------------------------------------------------------------------------------------
@@ -198,6 +220,52 @@ def _build():
     _field(m, "path", 4, ".nodereader.JsonFieldPathFilter", oneof=0)
     m = fd.message_type.add(name="SearchAfter")               # :382-386
     _field(m, "score", 1, "float"); _field(m, "shard_id", 2, "bytes"); _field(m, "docaddr", 3, "uint64")
+    m = fd.message_type.add(name="GraphQuery")                # :148-231
+    nd = m.nested_type.add(name="Node")
+    e = nd.enum_type.add(name="MatchLocation")
+    for i, n in enumerate(("FULL", "PREFIX", "WORDS", "PREFIX_WORDS")):
+        e.value.add(name=n, number=i)
+    em = nd.nested_type.add(name="ExactMatch"); _field(em, "kind", 1, "enum:.nodereader.GraphQuery.Node.MatchLocation")
+    fm = nd.nested_type.add(name="FuzzyMatch"); _field(fm, "kind", 1, "enum:.nodereader.GraphQuery.Node.MatchLocation"); _field(fm, "distance", 2, "uint32")
+    vm = nd.nested_type.add(name="VectorMatch"); _field(vm, "vector", 1, "float", repeated=True)
+    nd.oneof_decl.add().name = "match_kind"
+    _field(nd, "exact", 5, ".nodereader.GraphQuery.Node.ExactMatch", oneof=0); _field(nd, "fuzzy", 6, ".nodereader.GraphQuery.Node.FuzzyMatch", oneof=0)
+    _field(nd, "vector", 7, ".nodereader.GraphQuery.Node.VectorMatch", oneof=0)
+    _field(nd, "value", 1, "string", optional=True); _field(nd, "node_type", 2, "enum:.utils.RelationNode.NodeType", optional=True)
+    _field(nd, "node_subtype", 3, "string", optional=True)
+    rl = m.nested_type.add(name="Relation")
+    rl.nested_type.add(name="ExactMatch")
+    vm = rl.nested_type.add(name="VectorMatch"); _field(vm, "vector", 1, "float", repeated=True)
+    rl.oneof_decl.add().name = "match_kind"
+    _field(rl, "exact", 3, ".nodereader.GraphQuery.Relation.ExactMatch", oneof=0); _field(rl, "vector", 4, ".nodereader.GraphQuery.Relation.VectorMatch", oneof=0)
+    _field(rl, "value", 1, "string", optional=True); _field(rl, "relation_type", 2, "enum:.utils.Relation.RelationType", optional=True)
+    pa = m.nested_type.add(name="Path")
+    _field(pa, "source", 1, ".nodereader.GraphQuery.Node"); _field(pa, "relation", 2, ".nodereader.GraphQuery.Relation")
+    _field(pa, "destination", 3, ".nodereader.GraphQuery.Node"); _field(pa, "undirected", 4, "bool")
+    bq = m.nested_type.add(name="BoolQuery"); _field(bq, "operands", 1, ".nodereader.GraphQuery.PathQuery", repeated=True)
+    ff = m.nested_type.add(name="FacetFilter"); _field(ff, "facet", 1, "string")
+    pq = m.nested_type.add(name="PathQuery")
+    pq.oneof_decl.add().name = "query"
+    _field(pq, "path", 1, ".nodereader.GraphQuery.Path", oneof=0); _field(pq, "bool_not", 2, ".nodereader.GraphQuery.PathQuery", oneof=0)
+    _field(pq, "bool_and", 3, ".nodereader.GraphQuery.BoolQuery", oneof=0); _field(pq, "bool_or", 4, ".nodereader.GraphQuery.BoolQuery", oneof=0)
+    _field(pq, "facet", 5, ".nodereader.GraphQuery.FacetFilter", oneof=0)
+    _field(m, "path", 1, ".nodereader.GraphQuery.PathQuery")
+    m = fd.message_type.add(name="GraphSearchRequest")        # :233-262
+    e = m.enum_type.add(name="QueryKind"); e.value.add(name="PATH", number=0); e.value.add(name="NODES", number=1); e.value.add(name="RELATIONS", number=2)
+    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "query", 2, ".nodereader.GraphQuery")
+    _field(m, "kind", 3, "enum:.nodereader.GraphSearchRequest.QueryKind"); _field(m, "top_k", 4, "uint32")
+    _field(m, "security", 5, ".utils.Security", optional=True); _field(m, "field_filter", 6, ".nodereader.FilterExpression", optional=True)
+    _field(m, "graph_node_vectorset", 7, "string"); _field(m, "graph_edge_vectorset", 8, "string")
+    _field(m, "min_score_node_semantic", 9, "float"); _field(m, "min_score_edge_semantic", 10, "float")
+    m = fd.message_type.add(name="GraphSearchResponse")       # :264-290
+    rl = m.nested_type.add(name="Relation"); _field(rl, "relation_type", 1, "enum:.utils.Relation.RelationType"); _field(rl, "label", 2, "string")
+    pa = m.nested_type.add(name="Path")
+    _field(pa, "source", 1, "uint32"); _field(pa, "relation", 2, "uint32"); _field(pa, "destination", 3, "uint32")
+    _field(pa, "metadata", 4, ".utils.RelationMetadata", optional=True); _field(pa, "resource_field_id", 5, "string", optional=True)
+    _field(pa, "facets", 6, "string", repeated=True)
+    _field(m, "nodes", 1, ".utils.RelationNode", repeated=True); _field(m, "relations", 2, ".nodereader.GraphSearchResponse.Relation", repeated=True)
+    _field(m, "graph", 3, ".nodereader.GraphSearchResponse.Path", repeated=True); _field(m, "scores", 4, "float", repeated=True)
+    _field(m, "shard_ids", 5, "string", repeated=True)
     m = fd.message_type.add(name="SearchRequest")             # :388-437
     _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 3, "string"); _field(m, "order", 5, ".nodereader.OrderBy")
     _field(m, "faceted", 6, ".nodereader.Faceted")
@@ -208,9 +276,12 @@ def _build():
     _field(m, "field_filter", 26, ".nodereader.FilterExpression", optional=True); _field(m, "paragraph_filter", 27, ".nodereader.FilterExpression", optional=True)
     _field(m, "filter_operator", 28, "enum:.nodereader.FilterOperator"); _field(m, "search_after", 35, ".nodereader.SearchAfter", optional=True)
     _field(m, "json_filter", 32, ".nodereader.JsonFilterExpression", optional=True)
+    gs = m.nested_type.add(name="GraphSearch"); _field(gs, "query", 1, ".nodereader.GraphQuery")
+    _field(m, "graph_search", 29, ".nodereader.SearchRequest.GraphSearch", optional=True)
     m = fd.message_type.add(name="SearchResponse")            # :476-488
     _field(m, "document", 1, ".nodereader.DocumentSearchResponse"); _field(m, "paragraph", 2, ".nodereader.ParagraphSearchResponse")
     _field(m, "vector", 3, ".nodereader.VectorSearchResponse"); _field(m, "shard_ids", 6, "string", repeated=True)
+    _field(m, "graph", 5, ".nodereader.GraphSearchResponse")
     pool.Add(fd)
 
     # ---- nodewriter.proto ------------------------------------------------------------------------------------------------
@@ -264,9 +335,18 @@ Security = _cls("utils.Security")
 JsonFieldValue = _cls("noderesources.JsonFieldValue")
 JsonFilterExpression = _cls("nodereader.JsonFilterExpression")
 JsonFieldPathFilter = _cls("nodereader.JsonFieldPathFilter")
+GraphQuery = _cls("nodereader.GraphQuery")
+GraphSearchRequest = _cls("nodereader.GraphSearchRequest")
+GraphSearchResponse = _cls("nodereader.GraphSearchResponse")
+Relation = _cls("utils.Relation")
+RelationNode = _cls("utils.RelationNode")
+RelationMetadata = _cls("utils.RelationMetadata")
+IndexRelation = _cls("noderesources.IndexRelation")
+IndexRelations = _cls("noderesources.IndexRelations")
 IndexMessage = _cls("nodewriter.IndexMessage")
 NewShardRequest = _cls("nodewriter.NewShardRequest")
 ShardCreated = _cls("noderesources.ShardCreated")
 NEW_SHARD_METHOD = "/nidx.NidxApi/NewShard"           # nidx.proto:9
 FILTER_AND, FILTER_OR = 0, 1
+GRAPH_SEARCH_METHOD = "/nidx.NidxSearcher/GraphSearch"   # nidx.proto: rpc GraphSearch
 SEARCH_METHOD = "/nidx.NidxSearcher/Search"   # nidx.proto:20-21: package nidx, service NidxSearcher, rpc Search
