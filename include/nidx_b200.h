@@ -580,6 +580,59 @@ int nidx_graph_search(nidx_graph* g, const nidx_graph_node* nodes, int32_t n_nod
 /* The times (ms) of the last search's dictionary pass, scored pass(es), collection (unique max + top-k) and whole call. */
 int nidx_graph_last_times(nidx_graph* g, float* ms4);
 
+/* ---- Suggest: the paragraph pass of NidxSearcher.Suggest (reference: nidx_paragraph/src/reader.rs:58-90, search_query.rs:87-183,
+ * query_parser/fuzzy_parser.rs, fuzzy_query.rs:88-116).  The keyword pass is nidx_txt_search(_phrases) on views (nidx_txt_view) under
+ * the suggest mask below; when it finds nothing, the fuzzy pass runs over the same views: every fuzzy literal is expanded over the
+ * paragraph index's vocabulary (one dictionary per index, shared by its segments) and each clause becomes a constant-score union of
+ * the postings of the terms it accepts. */
+typedef struct nidx_suggest_dict nidx_suggest_dict;
+
+/* The vocabulary as code points: term id e is cp[off[e] .. off[e + 1]) (host pointers, copied to HBM). */
+int nidx_suggest_dict_create(int32_t device, uint32_t n_terms, const uint32_t* cp, const uint64_t* off, nidx_suggest_dict** out);
+void nidx_suggest_dict_close(nidx_suggest_dict* d);
+/* The n (0..NIDX_G_MAX_TERMS) automaton terms (nidx_graph_term, host; `dict` is not read) -> out_bits [n][(n_terms + 63) / 64]
+ * (a DEVICE pointer): bit e of row i when term e is within row i's distance (prefix: some prefix of term e is).  out_counts (host,
+ * may be NULL) = the set bits of each row.  The call returns when the bits are in place. */
+int nidx_suggest_expand(nidx_suggest_dict* d, const nidx_graph_term* terms, int32_t n, uint64_t* out_bits, uint64_t* out_counts, void* stream);
+/* The time (ms) of the last nidx_suggest_expand's dictionary pass. */
+int nidx_suggest_last_ms(nidx_suggest_dict* d, float* ms);
+
+/* The paragraphs repeated in their field (IndexParagraph.repeated_in_field): (n_docs + 63) / 64 words (host); NULL = none. */
+int nidx_txt_set_repeated(nidx_txt_segment* seg, const uint64_t* bits);
+/* The suggest mask over seg's documents: bit d = NOT repeated AND sec_bits AND op(pf_bits, joined_bits), op = NIDX_F_AND | NIDX_F_OR; a
+ * NULL operand is dropped (not read as "all": op applies only when both pf_bits and joined_bits are given).  Every bitset has
+ * (n_docs + 63) / 64 words -> out_bits (padding bits zero) and *out_matching = its set bits (the alive set is not applied: the view
+ * does that).  All buffers `mem`; the call returns when both are in place. */
+int nidx_txt_suggest_mask(nidx_txt_segment* seg, const uint64_t* sec_bits, const uint64_t* pf_bits, const uint64_t* joined_bits, int32_t op,
+                          uint64_t* out_bits, int mem, uint64_t* out_matching, void* stream);
+
+#define NIDX_SG_FUZZY 0        /* arg = a row of the expansion bitsets: the union of its terms' postings, scored 1.0 */
+#define NIDX_SG_TERM 1         /* arg = a term id (>= n_terms: matches nothing): BM25 at tf = 1 */
+#define NIDX_SG_PHRASE 2       /* arg = a phrase of `phrases` (slop 0): BM25 at the phrase frequency */
+#define NIDX_SG_MAX_CLAUSES 64
+#define NIDX_SG_MAX_HITS 16
+typedef struct nidx_suggest_clause {
+    int32_t kind;              /* NIDX_SG_* */
+    uint32_t arg;
+} nidx_suggest_clause;
+
+/* The fuzzy pass over seg's alive documents (a view: under its mask).  A document matches when a clause does, and scores
+ * 0.5 * (the f32 sum, in clause order, of 1.0 per matched FUZZY clause, w_t * (1 / (1 + norm)) per matched TERM and
+ * w_p * (freq / (freq + norm)) per matched PHRASE), with the weights and norms of nidx_txt_set_stats and of nidx_txt_search_phrases.
+ * exp_bits: n_exp_rows rows over the n_dict terms of the dictionary (<= the segment's terms), a DEVICE pointer (nidx_suggest_expand's
+ * output); phrases: as nidx_txt_search_phrases (`query` unread; NULL = none; the segment needs positions when there are some).
+ * -> out_ids [k] (1..NIDX_G_MAX_K; score descending, ties to the lower document; NIDX_NIL padded), out_scores [k], *out_count, and
+ * for the first min(count, match_hits) hits (match_hits 0..NIDX_SG_MAX_HITS) every (hit, FUZZY clause, expanded term) whose term
+ * occurs in the hit, packed as hit << 40 | clause << 32 | term id, in no fixed order: the first match_cap of them in out_matches,
+ * their number in *out_n_matches (larger than match_cap when some did not fit).  Outputs `mem`; the call returns when they are in
+ * place (host) or enqueued on `stream` (device). */
+int nidx_txt_suggest_fuzzy(nidx_txt_segment* seg, const nidx_suggest_clause* clauses, int32_t n_clauses, const uint64_t* exp_bits, int32_t n_exp_rows,
+                           uint64_t n_dict, const nidx_txt_phrases* phrases, int32_t k, int32_t match_hits, int mem, uint32_t* out_ids, float* out_scores,
+                           int32_t* out_count, uint64_t* out_matches, uint32_t match_cap, uint32_t* out_n_matches, void* stream);
+/* The times (ms) of the last fuzzy pass on seg (or on a view of it): clause bitsets (phrase lists included), scored pass, top-k,
+ * matches. */
+int nidx_txt_suggest_last_times(nidx_txt_segment* seg, float* ms4);
+
 /* ------------------------------------------------------------------------------------------
  * Segments sharded over the GPUs of one node: one process (or thread) per GPU, one segment each
  * (reference: the searcher's scatter-gather, nidx/src/searcher/grpc.rs:253-431, merged by

@@ -82,6 +82,14 @@ NIDX_G_TERMS_VALUES, NIDX_G_TERMS_TOKENS = 0, 1
 NIDX_G_PATH, NIDX_G_NODES, NIDX_G_RELATIONS = 0, 1, 2
 
 
+class SuggestClause(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("arg", C.c_uint32)]
+
+
+NIDX_SG_FUZZY, NIDX_SG_TERM, NIDX_SG_PHRASE = 0, 1, 2
+NIDX_SG_MAX_CLAUSES, NIDX_SG_MAX_HITS = 64, 16
+
+
 class TxtSearchParams(C.Structure):
     _fields_ = [("k", C.c_int32), ("mode", C.c_int32), ("use_tf", C.c_int32), ("min_score", C.c_float), ("after_mode", C.c_int32),
                 ("after_score", C.c_float), ("after_docaddr", C.c_uint64), ("docaddr_base", C.c_uint64)]
@@ -181,6 +189,14 @@ SIGNATURES = {
     "nidx_graph_close": (None, [P]),
     "nidx_graph_search": (i32, [P, P, i32, P, i32, i32, i32, P, i32, P, P, P, P]),
     "nidx_graph_last_times": (i32, [P, P]),
+    "nidx_suggest_dict_create": (i32, [i32, u32, P, P, P]),
+    "nidx_suggest_dict_close": (None, [P]),
+    "nidx_suggest_expand": (i32, [P, P, i32, P, P, P]),   # terms: an array of GraphTerm
+    "nidx_suggest_last_ms": (i32, [P, P]),
+    "nidx_txt_set_repeated": (i32, [P, P]),
+    "nidx_txt_suggest_mask": (i32, [P, P, P, P, i32, P, i32, P, P]),
+    "nidx_txt_suggest_fuzzy": (i32, [P, P, i32, P, i32, u64, P, i32, i32, i32, P, P, P, P, u32, P, P]),   # clauses: SuggestClause, phrases: TxtPhrases
+    "nidx_txt_suggest_last_times": (i32, [P, P]),
     "nidx_shard_unique_id": (i32, [P]),
     "nidx_shard_init": (i32, [P, i32, i32, i32, P]),
     "nidx_shard_destroy": (None, [P]),

@@ -16,11 +16,12 @@ Reference:
   nidx/src/searcher/query_planner/prefilter.rs:24-72              SearchRequest.json_filter, combined with the text prefilter
   nidx/nidx_relation/src/resource_indexer.rs, reader.rs           Resource.field_relations -> one relation document each; GraphSearch
   nidx/src/searcher/shard_search.rs:290-362, shard_merge.rs:350-375   NidxSearcher.GraphSearch: prefilter, search, concatenation
+  nidx/src/searcher/shard_suggest.rs:94-161, shard_merge.rs:101-151    NidxSearcher.Suggest: prefilter, paragraphs, entities, merge
 
 What is kept of the reference's machinery is the INTERFACE: metadata lives in memory (no PostgreSQL), every index message
 becomes one immutable segment per index (as in the reference), deletions are (key, seq) pairs applied to older segments, and
 "sync" re-opens the searchers (index_cache.rs:180-200).  Scheduler, worker, merges-in-the-background, NATS, object stores other
-than the local file store, relation prefix search / suggest are outside the hot path (SURVEY 8) and answer UNIMPLEMENTED.
+than the local file store are outside the hot path (SURVEY 8); the RPCs served are Search, GraphSearch and Suggest.
 """
 from __future__ import annotations
 
@@ -37,6 +38,7 @@ import numpy as np
 from . import graph as Gr
 from . import json_index as J
 from . import nidx_protos as P
+from . import suggest as S
 from . import text as T
 from . import vector as V
 from .shard_merge import bm25_order_key, kmerge_by
@@ -56,7 +58,6 @@ class _Shard:
     vectorsets: dict = field(default_factory=dict)   # name -> _VectorIndex
     text_segments: list = field(default_factory=list)        # [[TextDoc]] one list per index message
     paragraph_segments: list = field(default_factory=list)   # [[TextDoc]] (+ paragraph positions in .field / extra)
-    paragraph_meta: dict = field(default_factory=dict)       # paragraph id -> (field, start, end, index, split, labels, metadata bytes)
     deleted_resources: set = field(default_factory=set)
     json_docs: list = field(default_factory=list)            # [(resource id, [(path, kind, value)], seq)]
     resource_groups: dict = field(default_factory=dict)      # resource id -> access groups of its latest index message
@@ -178,7 +179,9 @@ class NidxBinding:
             "Search": grpc.unary_unary_rpc_method_handler(self._grpc_search, request_deserializer=P.SearchRequest.FromString,
                                                           response_serializer=lambda m: m.SerializeToString()),
             "GraphSearch": grpc.unary_unary_rpc_method_handler(self._grpc_graph_search, request_deserializer=P.GraphSearchRequest.FromString,
-                                                               response_serializer=lambda m: m.SerializeToString())}),))
+                                                               response_serializer=lambda m: m.SerializeToString()),
+            "Suggest": grpc.unary_unary_rpc_method_handler(self._grpc_suggest, request_deserializer=P.SuggestRequest.FromString,
+                                                           response_serializer=lambda m: m.SerializeToString())}),))
         self.searcher_port = self._searcher.add_insecure_port("127.0.0.1:0")
         self._api = grpc.server(futures.ThreadPoolExecutor(max_workers=2))
         self._api.add_generic_rpc_handlers((grpc.method_handlers_generic_handler("nidx.NidxApi", {
@@ -280,8 +283,8 @@ class NidxBinding:
                 text = res.texts[fid].text if fid in res.texts else ""
                 for pid, par in paragraphs.paragraphs.items():
                     labels = tuple(list(res.labels) + list(res.texts[fid].labels if fid in res.texts else ()) + list(par.labels))
-                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels, created, modified, groups))
-                    shard.paragraph_meta[(rid, "/" + fid if not fid.startswith("/") else fid, len(pdocs) - 1, seq)] = (pid, par)
+                    pdocs.append(T.TextDoc(rid, "/" + fid if not fid.startswith("/") else fid, text[par.start:par.end], labels, created, modified, groups,
+                                           repeated=bool(par.repeated_in_field), paragraph=(pid, par)))
             if pdocs:
                 shard.paragraph_segments.append((pdocs, seq))
         if graph_docs:
@@ -390,6 +393,84 @@ class NidxBinding:
             context.abort(grpc.StatusCode.NOT_FOUND, str(e))
         except NotImplementedError as e:
             context.abort(grpc.StatusCode.UNIMPLEMENTED, str(e))
+        except V.NidxError as e:
+            context.abort(grpc.StatusCode.INTERNAL, str(e))
+        except ValueError as e:
+            context.abort(grpc.StatusCode.INVALID_ARGUMENT, str(e))
+
+    # ---- NidxSearcher.Suggest (shard_suggest.rs:94-161, shard_merge.rs:101-151) --------------------------------------------------
+    def suggest(self, request):
+        """nodereader.SuggestRequest -> nodereader.SuggestResponse: each shard's paragraph and entity suggestions (nucliadb_b200/suggest.py),
+        merged.  An unknown shard is a KeyError, a top_k above 1024 or a filter the device cannot run a ValueError."""
+        parts = []
+        with self._lock:
+            for sid in request.shard_ids:
+                shard = self._shards.get(sid)
+                if shard is None:
+                    raise KeyError(f"shard {sid} not found")
+                parts.append((sid, self._suggest_shard(shard, request, sid)))
+        return S.merge_suggest(parts, int(request.top_k))
+
+    def _suggest_shard(self, shard: _Shard, req, sid: str):
+        """SuggestPlan::build + blocking_suggest: nothing for top_k == 0 or without a feature; the prefilter of Prefilter::parse_suggest
+        (field_filter and security on the text index, json_filter combined under filter_operator), whose None empties the answer; the
+        paragraph pass under the suggest mask; the entity NODES search under the text part of the prefilter (json_filter does not apply
+        to relations, DESIGN 9)."""
+        resp = P.SuggestResponse(shard_ids=[sid])
+        k = int(req.top_k)
+        paragraphs, entities = P.SUGGEST_PARAGRAPHS in req.features, P.SUGGEST_ENTITIES in req.features
+        if k == 0 or not (paragraphs or entities):
+            return resp
+        if k > S.MAX_TOP_K:
+            raise ValueError(f"top_k must be at most {S.MAX_TOP_K}")
+        security = list(req.security.access_groups) if req.HasField("security") else None
+        field_filter = req.field_filter if req.HasField("field_filter") else None
+        text_pf = None   # All
+        if field_filter is not None or security is not None:
+            text_pf = shard.text_searcher.prefilter(field_filter, security=security) if shard.text_searcher is not None else V.PrefilterResult.none()
+        prefilter = text_pf
+        if req.HasField("json_filter"):
+            J.validate(req.json_filter)
+            res_bits, found = None, 0
+            if shard.json_index is not None:
+                _, found, res_bits = shard.json_index.prefilter(req.json_filter, security)
+            prefilter = (text_pf or V.PrefilterResult.all()).combine(shard.json_index, res_bits, found, req.filter_operator == P.FILTER_OR)
+        if prefilter is not None and prefilter.kind == "none":
+            return resp
+        if paragraphs:
+            resp.query = req.body
+            ps = shard.paragraph_searcher
+            if ps is None:
+                resp.ematches.extend(S.ematches(T.paragraph_query_tokens(req.body)))
+            else:
+                pfilter = req.paragraph_filter if req.HasField("paragraph_filter") else None
+                masks = ps.suggest_masks(security, pfilter, prefilter, req.filter_operator == P.FILTER_OR)
+                r = ps.suggest(req.body, k, masks)
+                resp.total = len(r.hits)
+                resp.ematches.extend(r.ematches)
+                for h in r.hits[: S.RESULTS_PER_PAGE]:
+                    d = ps.segments[h.segment].docs[h.doc]
+                    pid, par = d.paragraph
+                    o = resp.results.add(uuid=d.uuid, field=d.field, start=par.start, end=par.end, paragraph=pid, split=par.split, index=par.index)
+                    o.labels.extend(S.extract_labels(d.labels))
+                    if par.HasField("metadata"):
+                        o.metadata.CopyFrom(par.metadata)
+                    o.score.bm25, o.score.docaddr = h.score, (h.segment << 32) + h.doc
+                    o.matches.extend(h.matches)
+        if entities:
+            resp.entity_results.SetInParent()
+            greq = S.entity_request(req.body, k)
+            if greq is not None and shard.graph_index is not None:
+                resp.entity_results.nodes.extend(Gr.GraphSearcher(shard.graph_index).search(greq, text_pf).nodes)
+        return resp
+
+    def _grpc_suggest(self, request, context):
+        import grpc
+
+        try:
+            return self.suggest(request)
+        except KeyError as e:
+            context.abort(grpc.StatusCode.NOT_FOUND, str(e))
         except V.NidxError as e:
             context.abort(grpc.StatusCode.INTERNAL, str(e))
         except ValueError as e:

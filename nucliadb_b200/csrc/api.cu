@@ -31,6 +31,7 @@
 #include "scan_tc2.cuh"
 #include "segment_io.hpp"
 #include "shard.cuh"
+#include "suggest.cuh"
 #include "topk.cuh"
 
 using namespace nidx;
@@ -1981,11 +1982,14 @@ struct TxtIndex {
     std::vector<float> idf;           // [n_terms] of the statistics set last: a phrase's weight sums its terms'
     // prefilter columns (nidx_txt_set_doc_columns): every document's resource and field ord
     DevArray<uint32_t> d_res_ord, d_field_ord;
+    DevArray<uint64_t> d_repeated;    // nidx_txt_set_repeated: paragraphs repeated in their field (NULL: none)
+    cudaEvent_t ev_sg[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // the last fuzzy suggest pass (created on its first call)
     WorkspacePool pool;
 
     ~TxtIndex() {
         if (ev_k0) cudaEventDestroy(ev_k0);
         if (ev_k1) cudaEventDestroy(ev_k1);
+        for (cudaEvent_t e : ev_sg) if (e) cudaEventDestroy(e);
     }
 };
 
@@ -3695,6 +3699,324 @@ int nidx_graph_last_times(nidx_graph* g, float* ms4) {
     CU(cudaEventElapsedTime(ms4 + 1, g->ev[1], g->ev[2]));
     CU(cudaEventElapsedTime(ms4 + 2, g->ev[2], g->ev[3]));
     CU(cudaEventElapsedTime(ms4 + 3, g->ev[0], g->ev[3]));
+    return 0;
+}
+
+}  // extern "C"
+
+// ---- suggest (suggest.cuh) -------------------------------------------------------------------------------------------------------
+struct nidx_suggest_dict {
+    int device = 0, sm_count = 0;
+    uint32_t n_terms = 0;
+    DevArray<uint32_t> d_cp;
+    DevArray<uint64_t> d_off;
+    cudaEvent_t ev[2] = {nullptr, nullptr};   // around the last dictionary pass
+    WorkspacePool pool;
+    ~nidx_suggest_dict() { for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+};
+
+extern "C" {
+
+int nidx_suggest_dict_create(int32_t device, uint32_t n_terms, const uint32_t* cp, const uint64_t* off, nidx_suggest_dict** out) {
+    if (!off || !out || (off[n_terms] && !cp)) return fail(NIDX_EINVAL, "null argument");
+    int r = check_device(device);
+    if (r) return r;
+    for (uint32_t e = 0; e < n_terms; ++e)
+        if (off[e + 1] < off[e]) return fail(NIDX_EINVAL, "dictionary offsets must be non-decreasing");
+    CU(cudaSetDevice(device));
+    std::unique_ptr<nidx_suggest_dict> d(new nidx_suggest_dict());
+    d->device = device;
+    d->n_terms = n_terms;
+    cudaDeviceProp prop;
+    CU(cudaGetDeviceProperties(&prop, device));
+    d->sm_count = prop.multiProcessorCount;
+    ALLOC(d->d_cp, std::max<uint64_t>(off[n_terms], 1) * 4);
+    ALLOC(d->d_off, ((size_t)n_terms + 1) * 8);
+    if (off[n_terms]) CU(cudaMemcpy(d->d_cp, cp, off[n_terms] * 4, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(d->d_off, off, ((size_t)n_terms + 1) * 8, cudaMemcpyHostToDevice));
+    for (cudaEvent_t& e : d->ev) CU(cudaEventCreate(&e));
+    *out = d.release();
+    return 0;
+}
+
+void nidx_suggest_dict_close(nidx_suggest_dict* d) {
+    if (!d) return;
+    cudaSetDevice(d->device);
+    cudaDeviceSynchronize();
+    delete d;
+}
+
+int nidx_suggest_expand(nidx_suggest_dict* d, const nidx_graph_term* terms, int32_t n, uint64_t* out_bits, uint64_t* out_counts, void* stream_) {
+    int r = require_handle(d);
+    if (r) return r;
+    if (n < 0 || n > GF_MAX_TERMS || (n && (!terms || !out_bits))) return fail(NIDX_EINVAL, "at most %d automaton terms", GF_MAX_TERMS);
+    std::vector<GraphTerm> h_terms;
+    std::vector<uint32_t> term_cp;
+    for (int t = 0; t < n; ++t) {
+        const nidx_graph_term& T = terms[t];
+        if (T.distance < 0 || T.distance > GF_MAX_DIST) return fail(NIDX_EINVAL, "term %d: the distance must be in 0..%d", t, GF_MAX_DIST);
+        if (T.n_cp < 0 || (T.n_cp && !T.cp)) return fail(NIDX_EINVAL, "term %d: bad code points", t);
+        h_terms.push_back(GraphTerm{(uint32_t)term_cp.size(), (uint32_t)T.n_cp, (uint32_t)T.distance, T.prefix ? 1u : 0u});
+        term_cp.insert(term_cp.end(), T.cp, T.cp + T.n_cp);
+        if (term_cp.size() > (size_t)GF_MAX_TERM_CPS) return fail(NIDX_EINVAL, "the automaton terms have more than %d code points", GF_MAX_TERM_CPS);
+    }
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    CU(cudaSetDevice(d->device));
+    WsGuard g(d->pool, stream);
+    Workspace& w = *g.w;
+    const size_t words = ((size_t)d->n_terms + 63) / 64;
+    const size_t o_terms = (term_cp.size() * 4 + 15) & ~(size_t)15, o_counts = o_terms + ((h_terms.size() * sizeof(GraphTerm) + 15) & ~(size_t)15);
+    ENSURE(w.prefilter, o_counts + std::max<size_t>(n, 1) * 8);
+    uint32_t* d_cp = w.prefilter.as<uint32_t>();
+    GraphTerm* d_terms = reinterpret_cast<GraphTerm*>(w.prefilter.p + o_terms);
+    unsigned long long* d_counts = reinterpret_cast<unsigned long long*>(w.prefilter.p + o_counts);
+    CU(cudaEventRecord(d->ev[0], stream));
+    if (n && words) {
+        if (!term_cp.empty()) CU(cudaMemcpyAsync(d_cp, term_cp.data(), term_cp.size() * 4, cudaMemcpyHostToDevice, stream));
+        CU(cudaMemcpyAsync(d_terms, h_terms.data(), h_terms.size() * sizeof(GraphTerm), cudaMemcpyHostToDevice, stream));
+        CU(cudaMemsetAsync(out_bits, 0, (size_t)n * words * 8, stream));
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)d->sm_count * 8, ((size_t)d->n_terms + GF_THREADS - 1) / GF_THREADS));
+        graph_dict_match_kernel<<<blocks, GF_THREADS, term_cp.size() * 4, stream>>>(d->d_cp, d->d_off, d->n_terms, d_terms, (uint32_t)n, d_cp,
+                                                                                   (uint32_t)term_cp.size(), out_bits, words);
+        LAUNCHED();
+    }
+    CU(cudaEventRecord(d->ev[1], stream));
+    if (out_counts && n) {
+        CU(cudaMemsetAsync(d_counts, 0, (size_t)n * 8, stream));
+        if (words) {
+            suggest_popc_kernel<<<(unsigned)std::max<size_t>(1, std::min<size_t>((size_t)d->sm_count * 4, (n * words + 255) / 256)), 256, 0, stream>>>(
+                out_bits, words, (uint32_t)n, d_counts);
+            LAUNCHED();
+        }
+        CU(cudaMemcpyAsync(out_counts, d_counts, (size_t)n * 8, cudaMemcpyDeviceToHost, stream));
+        CU(cudaStreamSynchronize(stream));
+    } else {
+        CU(cudaStreamSynchronize(stream));   // the terms are host temporaries
+    }
+    CU(cudaGetLastError());
+    return 0;
+}
+
+int nidx_suggest_last_ms(nidx_suggest_dict* d, float* ms) {
+    int r = require_handle(d);
+    if (r) return r;
+    if (!ms) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(d->device));
+    CU(cudaEventSynchronize(d->ev[1]));
+    CU(cudaEventElapsedTime(ms, d->ev[0], d->ev[1]));
+    return 0;
+}
+
+int nidx_txt_set_repeated(nidx_txt_segment* t, const uint64_t* bits) {
+    int r = require_handle(t);
+    if (!r) r = require_owner(t);
+    if (r) return r;
+    if (!bits) { t->ix->d_repeated.release(); return 0; }
+    return set_rows(t->ix->device, t->ix->d_repeated, bits, ((size_t)t->ix->n_docs + 63) / 64);
+}
+
+int nidx_txt_suggest_mask(nidx_txt_segment* t, const uint64_t* sec_bits, const uint64_t* pf_bits, const uint64_t* joined_bits, int32_t op, uint64_t* out_bits,
+                          int mem, uint64_t* out_matching, void* stream_) {
+    int r = require_handle(t);
+    if (r) return r;
+    if (!out_bits) return fail(NIDX_EINVAL, "null argument");
+    if (op != NIDX_F_AND && op != NIDX_F_OR) return fail(NIDX_EINVAL, "op must be NIDX_F_AND or NIDX_F_OR");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(t->ix->device));
+    WsGuard g(t->ix->pool, stream);
+    Workspace& w = *g.w;
+    const size_t words = ((size_t)t->ix->n_docs + 63) / 64;
+    Stage st(stream, host, host);
+    const uint64_t *d_sec, *d_pf, *d_joined;
+    uint64_t* d_out;
+    st.in(sec_bits, words, &d_sec);
+    st.in(pf_bits, words, &d_pf);
+    st.in(joined_bits, words, &d_joined);
+    st.out(out_bits, words, &d_out);
+    r = st.place(w.stage);
+    if (r) return r;
+    ENSURE(w.misc, 16);
+    unsigned long long* d_count = w.misc.as<unsigned long long>();
+    CU(cudaMemsetAsync(d_count, 0, 8, stream));
+    if (words) {
+        suggest_mask_kernel<<<(unsigned)std::max<size_t>(1, std::min<size_t>((words + 255) / 256, 1024)), 256, 0, stream>>>(
+            t->ix->n_docs, t->ix->d_repeated, d_sec, d_pf, d_joined, op == NIDX_F_OR, d_out, d_count);
+        LAUNCHED();
+        CU(cudaGetLastError());
+    }
+    unsigned long long h = 0;
+    CU(cudaMemcpyAsync(&h, d_count, 8, cudaMemcpyDeviceToHost, stream));
+    r = st.finish(true);
+    if (r) return r;
+    if (out_matching) *out_matching = h;
+    return 0;
+}
+
+int nidx_txt_suggest_fuzzy(nidx_txt_segment* t, const nidx_suggest_clause* clauses, int32_t n_clauses, const uint64_t* exp_bits, int32_t n_exp_rows,
+                           uint64_t n_dict, const nidx_txt_phrases* phrases, int32_t k, int32_t match_hits, int mem, uint32_t* out_ids, float* out_scores,
+                           int32_t* out_count, uint64_t* out_matches, uint32_t match_cap, uint32_t* out_n_matches, void* stream_) {
+    int r = require_handle(t);
+    if (r) return r;
+    if (!clauses || !out_ids || !out_scores || !out_count || !out_n_matches || (match_cap && !out_matches)) return fail(NIDX_EINVAL, "null argument");
+    if (n_clauses < 1 || n_clauses > SG_MAX_CLAUSES) return fail(NIDX_EINVAL, "a fuzzy pass has 1 to %d clauses", SG_MAX_CLAUSES);
+    if (k < 1 || k > NIDX_G_MAX_K) return fail(NIDX_EINVAL, "k must be in 1..%d", NIDX_G_MAX_K);
+    if (match_hits < 0 || match_hits > SG_MAX_HITS) return fail(NIDX_EINVAL, "match_hits must be in 0..%d", SG_MAX_HITS);
+    if (n_exp_rows < 0 || (n_exp_rows && !exp_bits)) return fail(NIDX_EINVAL, "bad expansion bitsets");
+    if (n_dict > t->ix->n_terms) return fail(NIDX_EINVAL, "the dictionary has more terms (%llu) than the segment (%u)", (unsigned long long)n_dict, t->ix->n_terms);
+    const uint32_t n_ph = phrases ? (uint32_t)std::max(phrases->n, 0) : 0u;
+    int n_exact = 0;
+    for (int c = 0; c < n_clauses; ++c) {
+        const nidx_suggest_clause& C = clauses[c];
+        if (C.kind == NIDX_SG_FUZZY && C.arg >= (uint32_t)n_exp_rows) return fail(NIDX_EINVAL, "clause %d: no expansion row %u", c, C.arg);
+        else if (C.kind == NIDX_SG_TERM) ++n_exact;
+        else if (C.kind == NIDX_SG_PHRASE && C.arg >= n_ph) return fail(NIDX_EINVAL, "clause %d: no phrase %u", c, C.arg);
+        else if (C.kind != NIDX_SG_FUZZY && C.kind != NIDX_SG_TERM && C.kind != NIDX_SG_PHRASE) return fail(NIDX_EINVAL, "clause %d: bad kind %d", c, C.kind);
+    }
+    PhrasePlan pp;
+    if (n_ph) {
+        nidx_txt_phrases one = *phrases;
+        std::vector<uint32_t> query(n_ph, 0), h_off = {0, (uint32_t)n_exact};
+        one.query = query.data();   // one query: the plan keeps the phrases in the caller's order
+        r = phrase_plan(t, &one, 1, h_off, pp);
+        if (r) return r;
+    }
+    // the clauses as the kernels read them: weights resolved here, warp tasks laid out clause by clause
+    const float K1 = 1.2f;
+    const size_t exp_words = (n_dict + 63) / 64;
+    std::vector<SgClause> sc(n_clauses + 1);
+    std::vector<uint32_t> fz_clause;
+    uint64_t tasks = 0;
+    const float* ph_w = n_ph ? reinterpret_cast<const float*>(pp.buf.data() + pp.o_weight) : nullptr;
+    const uint64_t* ph_cap = n_ph ? reinterpret_cast<const uint64_t*>(pp.buf.data() + pp.o_cap_off) : nullptr;
+    for (int c = 0; c < n_clauses; ++c) {
+        const nidx_suggest_clause& C = clauses[c];
+        SgClause& S = sc[c];
+        S.task0 = (uint32_t)tasks;
+        S.arg = C.arg;
+        S.w = 0.f;
+        uint64_t postings = 0;
+        if (C.kind == NIDX_SG_FUZZY) {
+            S.kind = SG_FUZZY;   // its chunks are counted on the device (suggest_chunk_count_kernel)
+            fz_clause.push_back((uint32_t)c);
+        } else if (C.kind == NIDX_SG_TERM) {
+            S.kind = SG_TERM;
+            if (C.arg < t->ix->n_terms) { postings = t->ix->own_df[C.arg]; S.w = t->ix->idf[C.arg] * (1.0f + K1); }   // txt_upload_stats' weight
+            else S.arg = NIDX_NIL;
+        } else {
+            S.kind = SG_PHRASE;
+            postings = ph_cap[C.arg + 1] - ph_cap[C.arg];
+            S.w = ph_w[C.arg];
+        }
+        tasks += (postings + SG_CHUNK - 1) / SG_CHUNK;
+        if (tasks >= (1ull << 32)) return fail(NIDX_EINVAL, "the fuzzy pass has too many posting chunks");
+    }
+    sc[n_clauses].task0 = (uint32_t)tasks;
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+    const bool host = mem == NIDX_MEM_HOST;
+    CU(cudaSetDevice(t->ix->device));
+    TxtIndex* ix = t->ix;
+    for (cudaEvent_t& e : ix->ev_sg)
+        if (!e) CU(cudaEventCreate(&e));
+    WsGuard g(ix->pool, stream);
+    Workspace& w = *g.w;
+    const uint32_t n = ix->n_docs;
+    const size_t words = ((size_t)n + 63) / 64;
+    Stage st(stream, false, host);
+    uint32_t* d_ids; float* d_sc; int32_t* d_cnt; uint64_t* d_matches; uint32_t* d_nm;
+    st.out(out_ids, (size_t)k, &d_ids);
+    st.out(out_scores, (size_t)k, &d_sc);
+    st.out(out_count, 1, &d_cnt);
+    st.out(out_matches, std::max<size_t>(match_cap, 1), &d_matches);
+    st.out(out_n_matches, 1, &d_nm);
+    r = st.place(w.stage);
+    if (r) return r;
+    CU(cudaEventRecord(ix->ev_sg[0], stream));
+    TxtDev T;
+    T.n_docs = n; T.n_terms = ix->n_terms; T.n_fine = ix->n_fine; T.term_off = ix->d_term_off; T.post = ix->d_post;
+    T.skip_row = ix->d_skip_row; T.skip = ix->d_skip; T.alive = t->d_alive;
+    Bm25Args a{};
+    if (pp.nv) {
+        r = phrase_pass(t, pp, T, w, stream, a);
+        if (r) return r;
+    }
+    // scratch (w.scores): [clauses][words] bitsets, [n] scores, [2 words] hit bits, the clauses, the fuzzy clauses' indices;
+    // (w.sched): the chunk counts per (fuzzy clause, word), their exclusive prefix sum and the scan's temporary storage
+    const size_t o_score = (size_t)n_clauses * std::max<size_t>(words, 1) * 8, o_hits = o_score + ((std::max<size_t>(n, 1) * 4 + 15) & ~(size_t)15),
+                 o_cl = o_hits + std::max<size_t>(words, 1) * 8, o_fz = o_cl + ((sc.size() * sizeof(SgClause) + 15) & ~(size_t)15);
+    ENSURE(w.scores, o_fz + std::max<size_t>(fz_clause.size(), 1) * 4);
+    const size_t n_fw = fz_clause.size() * exp_words;
+    if (n_fw + 1 > (size_t)INT32_MAX) return fail(NIDX_EINVAL, "the expansion is too large");
+    size_t scan_bytes = 0;
+    if (n_fw) CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr, (int)(n_fw + 1), stream));
+    const size_t o_off = ((n_fw + 1) * 8 + 15) & ~(size_t)15, o_tmp = 2 * o_off;
+    ENSURE(w.sched, o_tmp + scan_bytes + 16);
+    SgArgs A{};
+    A.term_off = ix->d_term_off; A.post = ix->d_post; A.ph_range = a.ph_range; A.ph_post = a.ph_post; A.norm_cache = ix->d_norm_cache;
+    A.exp_bits = exp_bits; A.exp_words = exp_words; A.n_dict = (uint32_t)n_dict;
+    A.clauses = reinterpret_cast<const SgClause*>(w.scores.p + o_cl); A.n_clauses = (uint32_t)n_clauses;
+    A.fz_clause = reinterpret_cast<const uint32_t*>(w.scores.p + o_fz); A.n_fuzzy = (uint32_t)fz_clause.size();
+    A.fz_off = reinterpret_cast<const uint64_t*>(w.sched.p + o_off);
+    A.n_docs = n; A.words = words; A.bits = w.scores.as<uint64_t>(); A.alive = t->d_alive;
+    A.score = reinterpret_cast<float*>(w.scores.p + o_score); A.hit_bits = reinterpret_cast<uint32_t*>(w.scores.p + o_hits);
+    CU(cudaMemcpyAsync(w.scores.p + o_cl, sc.data(), sc.size() * sizeof(SgClause), cudaMemcpyHostToDevice, stream));
+    if (!fz_clause.empty()) CU(cudaMemcpyAsync(w.scores.p + o_fz, fz_clause.data(), fz_clause.size() * 4, cudaMemcpyHostToDevice, stream));
+    if (words) CU(cudaMemsetAsync(A.bits, 0, (size_t)n_clauses * words * 8, stream));
+    const int sm = ix->sm_count;
+    if (n_fw && words) {   // every expanded term's chunks: counted per word, then laid out by an exclusive prefix sum
+        uint64_t* cnt = w.sched.as<uint64_t>();
+        CU(cudaMemsetAsync(cnt + n_fw, 0, 8, stream));
+        suggest_chunk_count_kernel<<<(unsigned)std::max<size_t>(1, std::min<size_t>((size_t)sm * 8, (n_fw + 255) / 256)), 256, 0, stream>>>(A, cnt);
+        LAUNCHED();
+        CU(cub::DeviceScan::ExclusiveSum(w.sched.p + o_tmp, scan_bytes, cnt, reinterpret_cast<uint64_t*>(w.sched.p + o_off), (int)(n_fw + 1), stream));
+    }
+    if ((n_fw || tasks) && words) {   // the fuzzy chunk count stays on the device: a full grid strides over the tasks
+        const int blocks = n_fw ? sm * 8 : (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)sm * 8, (tasks * 32 + SG_THREADS - 1) / SG_THREADS));
+        suggest_scatter_kernel<<<blocks, SG_THREADS, 0, stream>>>(A);
+        LAUNCHED();
+    }
+    CU(cudaEventRecord(ix->ev_sg[1], stream));
+    if (words) {
+        const int blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)sm * 8, (2 * words * 32 + SG_THREADS - 1) / SG_THREADS));
+        suggest_score_kernel<<<blocks, SG_THREADS, 0, stream>>>(A);
+        LAUNCHED();
+    }
+    CU(cudaEventRecord(ix->ev_sg[2], stream));
+    const int cap = topk_cap(k, GF_THREADS);
+    const int tk_blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)sm * 2, ((size_t)n + GF_THREADS * 16 - 1) / (GF_THREADS * 16)));
+    ENSURE(w.partial, (size_t)tk_blocks * k * 8);
+    CU(cudaFuncSetAttribute(graph_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    CU(cudaFuncSetAttribute(graph_topk_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cap * 8));
+    if (n) {
+        graph_topk_kernel<<<tk_blocks, GF_THREADS, (size_t)cap * 8, stream>>>(n, A.hit_bits, A.score, nullptr, k, cap, w.partial.as<uint64_t>());
+        LAUNCHED();
+    } else {
+        CU(cudaMemsetAsync(w.partial, 0, (size_t)tk_blocks * k * 8, stream));
+    }
+    graph_topk_merge_kernel<<<1, GF_THREADS, (size_t)cap * 8, stream>>>(w.partial.as<uint64_t>(), tk_blocks * k, k, cap, d_ids, d_sc, d_cnt);
+    LAUNCHED();
+    CU(cudaEventRecord(ix->ev_sg[3], stream));
+    CU(cudaMemsetAsync(d_nm, 0, 4, stream));
+    uint64_t fuzzy_tasks = 0;
+    for (int c = 0; c < n_clauses; ++c) fuzzy_tasks += sc[c].kind == SG_FUZZY ? exp_words : 0;
+    if (match_hits && fuzzy_tasks) {
+        const int blocks = (int)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)sm * 8, (fuzzy_tasks * 32 + SG_THREADS - 1) / SG_THREADS));
+        suggest_matches_kernel<<<blocks, SG_THREADS, 0, stream>>>(A, d_ids, d_cnt, match_hits, d_matches, match_cap, d_nm);
+        LAUNCHED();
+    }
+    CU(cudaEventRecord(ix->ev_sg[4], stream));
+    CU(cudaGetLastError());
+    return st.finish(true);   // the phrase plan and the clauses are host temporaries
+}
+
+int nidx_txt_suggest_last_times(nidx_txt_segment* t, float* ms4) {
+    int r = require_handle(t);
+    if (r) return r;
+    if (!ms4) return fail(NIDX_EINVAL, "null argument");
+    if (!t->ix->ev_sg[4]) return fail(NIDX_ESTATE, "no fuzzy suggest pass has run on this segment");
+    CU(cudaSetDevice(t->ix->device));
+    CU(cudaEventSynchronize(t->ix->ev_sg[4]));
+    for (int i = 0; i < 4; ++i) CU(cudaEventElapsedTime(ms4 + i, t->ix->ev_sg[i], t->ix->ev_sg[i + 1]));
     return 0;
 }
 

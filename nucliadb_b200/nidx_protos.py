@@ -19,6 +19,7 @@ serialised by the reference's clients (``nidx_protos`` / ``nucliadb_protos``) de
     JsonFilterExpression, JsonFieldPathFilter              nodereader.proto:338-380 (SearchRequest.json_filter = 32)
     GraphQuery, GraphSearchRequest / Response              nodereader.proto:148-290 (SearchRequest.graph_search = 29, SearchResponse.graph = 5)
     Relation, RelationNode, RelationMetadata, IndexRelation(s), Resource.field_relations   utils.proto, noderesources.proto
+    SuggestFeatures, SuggestRequest / Response, RelationPrefixSearchResponse   nodereader.proto (NidxSearcher.Suggest)
 """
 from __future__ import annotations
 
@@ -282,6 +283,20 @@ def _build():
     _field(m, "document", 1, ".nodereader.DocumentSearchResponse"); _field(m, "paragraph", 2, ".nodereader.ParagraphSearchResponse")
     _field(m, "vector", 3, ".nodereader.VectorSearchResponse"); _field(m, "shard_ids", 6, "string", repeated=True)
     _field(m, "graph", 5, ".nodereader.GraphSearchResponse")
+    e = fd.enum_type.add(name="SuggestFeatures")              # :439-442
+    e.value.add(name="ENTITIES", number=0); e.value.add(name="PARAGRAPHS", number=1)
+    m = fd.message_type.add(name="SuggestRequest")            # :444-457
+    _field(m, "shard_ids", 1, "string", repeated=True); _field(m, "body", 2, "string")
+    _field(m, "features", 6, "enum:.nodereader.SuggestFeatures", repeated=True)
+    _field(m, "field_filter", 7, ".nodereader.FilterExpression", optional=True); _field(m, "paragraph_filter", 8, ".nodereader.FilterExpression", optional=True)
+    _field(m, "filter_operator", 9, "enum:.nodereader.FilterOperator"); _field(m, "security", 10, ".utils.Security", optional=True)
+    _field(m, "top_k", 11, "uint32"); _field(m, "json_filter", 12, ".nodereader.JsonFilterExpression", optional=True)
+    m = fd.message_type.add(name="RelationPrefixSearchResponse")   # :144-146
+    _field(m, "nodes", 1, ".utils.RelationNode", repeated=True)
+    m = fd.message_type.add(name="SuggestResponse")           # :468-474
+    _field(m, "total", 1, "int32"); _field(m, "results", 2, ".nodereader.ParagraphResult", repeated=True); _field(m, "query", 3, "string")
+    _field(m, "ematches", 4, "string", repeated=True)
+    _field(m, "entity_results", 6, ".nodereader.RelationPrefixSearchResponse"); _field(m, "shard_ids", 7, "string", repeated=True)
     pool.Add(fd)
 
     # ---- nodewriter.proto ------------------------------------------------------------------------------------------------
@@ -338,6 +353,10 @@ JsonFieldPathFilter = _cls("nodereader.JsonFieldPathFilter")
 GraphQuery = _cls("nodereader.GraphQuery")
 GraphSearchRequest = _cls("nodereader.GraphSearchRequest")
 GraphSearchResponse = _cls("nodereader.GraphSearchResponse")
+SuggestRequest = _cls("nodereader.SuggestRequest")
+SuggestResponse = _cls("nodereader.SuggestResponse")
+RelationPrefixSearchResponse = _cls("nodereader.RelationPrefixSearchResponse")
+SUGGEST_ENTITIES, SUGGEST_PARAGRAPHS = 0, 1   # SuggestFeatures
 Relation = _cls("utils.Relation")
 RelationNode = _cls("utils.RelationNode")
 RelationMetadata = _cls("utils.RelationMetadata")
@@ -349,4 +368,5 @@ ShardCreated = _cls("noderesources.ShardCreated")
 NEW_SHARD_METHOD = "/nidx.NidxApi/NewShard"           # nidx.proto:9
 FILTER_AND, FILTER_OR = 0, 1
 GRAPH_SEARCH_METHOD = "/nidx.NidxSearcher/GraphSearch"   # nidx.proto: rpc GraphSearch
+SUGGEST_METHOD = "/nidx.NidxSearcher/Suggest"            # nidx.proto: rpc Suggest
 SEARCH_METHOD = "/nidx.NidxSearcher/Search"   # nidx.proto:20-21: package nidx, service NidxSearcher, rpc Search

@@ -504,6 +504,60 @@ class TextSegment:
                                              ptr(res_bits), n_res, ptr(res_join), op, ptr(out), mem, C.byref(matching), stream))
         return out, matching.value
 
+    # ---- suggest (include/nidx_b200.h nidx_txt_set_repeated / nidx_txt_suggest_mask / nidx_txt_suggest_fuzzy) -----------------
+    def set_repeated(self, repeated: Optional[np.ndarray]):
+        """The paragraphs repeated in their field: a bool per document (None: none)."""
+        words = None
+        if repeated is not None:
+            words = np.zeros((self.n_docs + 63) // 64 * 8, dtype=np.uint8)
+            packed = np.packbits(np.asarray(repeated, dtype=bool), bitorder="little")
+            words[: len(packed)] = packed
+            words = words.view(np.uint64)
+        check(_lib.load().nidx_txt_set_repeated(self._h, ptr(words)))
+
+    def suggest_mask(self, sec_bits, pf_bits, joined_bits, op=_lib.NIDX_F_AND):
+        """NOT repeated AND sec_bits AND op(pf_bits, joined_bits), a None operand dropped -> (mask words, matching).  Torch CUDA operands
+        -> device path (a torch int64 mask), numpy or all None -> host path."""
+        ops = [b for b in (sec_bits, pf_bits, joined_bits) if b is not None]
+        on_device = any(_is_torch(b) for b in ops)
+        mem, stream, alloc = _stage(self.device, on_device)
+        if not on_device:
+            sec_bits, pf_bits, joined_bits = (None if b is None else np.ascontiguousarray(b, dtype=np.uint64) for b in (sec_bits, pf_bits, joined_bits))
+        out = alloc(max((self.n_docs + 63) // 64, 1), np.uint64)
+        matching = C.c_uint64()
+        check(_lib.load().nidx_txt_suggest_mask(self._h, ptr(sec_bits), ptr(pf_bits), ptr(joined_bits), op, ptr(out), mem, C.byref(matching), stream))
+        return out, matching.value
+
+    def suggest_fuzzy(self, clauses, exp_bits, n_exp_rows: int, n_dict: int, phrases, k: int, match_hits: int = 10, match_cap: int = 4096):
+        """The fuzzy pass: clauses = [(NIDX_SG_* kind, arg)], exp_bits = SuggestDict.expand's torch tensor (None without fuzzy
+        clauses), phrases = [[term ids]] -> (ids, scores, count, matches) with matches = sorted (hit, clause, term id) triples (host
+        path: the call returns when they are in place)."""
+        cl = (_lib.SuggestClause * len(clauses))(*[_lib.SuggestClause(kind, arg) for kind, arg in clauses])
+        terms = np.asarray([t for p in phrases for t in p], dtype=np.uint32)
+        poff = np.zeros(len(phrases) + 1, dtype=np.uint32)
+        poff[1:] = np.cumsum([len(p) for p in phrases])
+        pq = np.zeros(len(phrases), dtype=np.uint32)
+        ph = _lib.TxtPhrases(ptr(terms), ptr(poff), ptr(pq), len(phrases))
+        while True:
+            ids, scores, count = np.empty(k, np.uint32), np.empty(k, np.float32), np.zeros(1, np.int32)
+            matches, n_matches = np.empty(max(match_cap, 1), np.uint64), np.zeros(1, np.uint32)
+            check(_lib.load().nidx_txt_suggest_fuzzy(self._h, C.addressof(cl), len(clauses), ptr(exp_bits), n_exp_rows, n_dict,
+                                                     C.addressof(ph) if phrases else None, k, match_hits, _lib.NIDX_MEM_HOST, ptr(ids), ptr(scores),
+                                                     ptr(count), ptr(matches), match_cap, ptr(n_matches), None))
+            if int(n_matches[0]) <= match_cap:
+                break
+            match_cap = int(n_matches[0])   # a larger list than expected: run again with room for all of it
+        m = np.sort(matches[: int(n_matches[0])])
+        trip = [(int(x >> 40), int((x >> 32) & 0xFF), int(x & 0xFFFFFFFF)) for x in m]
+        c = int(count[0])
+        return ids[:c], scores[:c], c, trip
+
+    def suggest_last_times(self):
+        """(bitsets, scored pass, top-k, matches) ms of the last fuzzy pass."""
+        ms = (C.c_float * 4)()
+        check(_lib.load().nidx_txt_suggest_last_times(self._h, ms))
+        return list(ms)
+
     def set_doc_keys(self, keys: Optional[np.ndarray]):
         """Caller keys of the documents (paragraph ids) for rank fusion; None = the document number."""
         k = None if keys is None else np.ascontiguousarray(keys, dtype=np.uint64)
@@ -517,6 +571,48 @@ class TextSegment:
     def close(self):
         if self._h is not None:
             _lib.load().nidx_txt_close(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class SuggestDict:
+    """nidx_suggest_dict: a paragraph index's vocabulary as code points in HBM, for the fuzzy expansion of NidxSearcher.Suggest."""
+
+    def __init__(self, terms, device=0):
+        L = _lib.require_device()
+        cps = [np.frombuffer(t.encode("utf-32-le"), dtype=np.uint32) for t in terms]
+        off = np.zeros(len(terms) + 1, dtype=np.uint64)
+        off[1:] = np.cumsum([len(c) for c in cps]) if terms else []
+        cp = np.concatenate(cps).astype(np.uint32) if cps else np.zeros(1, dtype=np.uint32)
+        self.n_terms, self.device, self._h = len(terms), device, None
+        h = C.c_void_p()
+        check(L.nidx_suggest_dict_create(device, len(terms), ptr(cp), ptr(off), C.byref(h)))
+        self._h = h
+
+    def expand(self, terms):
+        """[(term, distance, prefix)] -> (torch CUDA int64 bitsets [len(terms)][(n_terms + 63) // 64], expanded terms per row)."""
+        import torch
+
+        cps = [np.frombuffer(t.encode("utf-32-le"), dtype=np.uint32).copy() for t, _, _ in terms]
+        arr = (_lib.GraphTerm * max(len(terms), 1))(*[_lib.GraphTerm(0, int(d), int(p), len(c), ptr(c)) for c, (_, d, p) in zip(cps, terms)])
+        bits = torch.empty((max(len(terms), 1), max((self.n_terms + 63) // 64, 1)), dtype=torch.int64, device=torch.device("cuda", self.device))
+        counts = np.zeros(max(len(terms), 1), dtype=np.uint64)
+        check(_lib.load().nidx_suggest_expand(self._h, arr, len(terms), ptr(bits), ptr(counts), _torch_stream(self.device)))
+        return bits, counts[: len(terms)]
+
+    def last_ms(self) -> float:
+        ms = C.c_float()
+        check(_lib.load().nidx_suggest_last_ms(self._h, C.byref(ms)))
+        return ms.value
+
+    def close(self):
+        if self._h is not None:
+            _lib.load().nidx_suggest_dict_close(self._h)
             self._h = None
 
     def __del__(self):

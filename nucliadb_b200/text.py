@@ -252,6 +252,8 @@ class TextDoc:
     created: Optional[int] = None    # IndexMetadata.created / .modified, seconds
     modified: Optional[int] = None
     groups: Sequence[str] = ()       # Resource.security.access_groups; none = public
+    repeated: bool = False           # IndexParagraph.repeated_in_field (paragraph documents): Suggest skips it
+    paragraph: Optional[tuple] = None   # (paragraph id, IndexParagraph) of a paragraph document, for Suggest's results
 
 
 class TextIndexSegment:
@@ -829,10 +831,126 @@ def date_sort_key(seconds: Optional[int], order_type: int):
 
 class ParagraphSearcher(TextSearcher):
     """nidx_paragraph keyword search: OR of TermQuery(Basic) => tf == 1 (keyword_parser.rs:27-67), plus a PhraseQuery per quoted
-    group of two or more words (scored with its real frequency): the body is parsed by parse_paragraph_query."""
+    group of two or more words (scored with its real frequency): the body is parsed by parse_paragraph_query.  suggest() is the
+    paragraph pass of NidxSearcher.Suggest (nucliadb_b200/suggest.py)."""
 
     conjunction = False
     use_tf = False
+    _suggest_dict = None   # the vocabulary in HBM (segment.SuggestDict), built on the first fuzzy pass
+    _repeated = False      # repeated_in_field bits uploaded (on the first suggest)
+
+    def suggest_masks(self, security: Optional[Sequence[str]] = None, paragraph_filter=None, prefilter=None, op_or: bool = False) -> list:
+        """Per segment, on the device, the suggest mask (nidx_txt_suggest_mask): NOT repeated_in_field AND the security bits (when
+        `security` is given) AND op(paragraph_filter's bits, the prefilter's), op OR when op_or, an absent operand dropped.  The
+        paragraph_filter (a nodereader.FilterExpression) runs on the prefilter's evaluator over the paragraphs; the prefilter is a
+        vector.PrefilterResult whose Some is on the device (joined as json_masks joins it), None or All: no operand."""
+        import torch
+
+        if not self._repeated:
+            for s in self.segments:
+                s._gpu.set_repeated(np.asarray([d.repeated for d in s.docs], dtype=bool))
+            self._repeated = True
+        dev = torch.device("cuda", self.segments[0].device)
+        n = len(self.segments)
+        sec = self._security_bits(security) if security is not None else [None] * n
+        pf = [None] * n
+        if paragraph_filter is not None:
+            self._ensure_facets()
+            self._ensure_dates()
+            if self._prefilter is None:
+                self._prefilter = _PrefilterIndex(self)
+            nodes, _keep, phrases = self._prefilter.compile(paragraph_filter)
+            if phrases:
+                self._ensure_positions()
+            pf = []
+            try:
+                for s in self.segments:
+                    pf.append(s._gpu.prefilter(nodes, out=torch.empty(max((s.n_docs + 63) // 64, 1), dtype=torch.int64, device=dev))[0])
+            except _lib.NidxError as e:
+                if e.code == -1:
+                    raise ValueError(str(e)) from e
+                raise
+        joined = self.json_masks(None, prefilter) if prefilter is not None and prefilter.kind == "some" else [None] * n
+        op = _lib.NIDX_F_OR if op_or else _lib.NIDX_F_AND
+        return [s._gpu.suggest_mask(a, b, c, op)[0] for s, a, b, c in zip(self.segments, sec, pf, joined)]
+
+    def suggest(self, body: str, top_k: int, masks: list):
+        """The paragraph pass of Suggest over the segments under `masks` (suggest_masks): the keyword pass (the paragraph search's query,
+        its BM25 bit for bit, TopDocs(top_k)), and when it finds nothing the fuzzy pass (suggest.fuzzy_clauses, nidx_txt_suggest_fuzzy)
+        -> suggest.ParagraphSuggest, hits ordered by (score desc, segment, document), each of the first RESULTS_PER_PAGE fuzzy hits with
+        its matches (the sorted expanded terms of more than 2 bytes that occur in it, one per (fuzzy clause, term))."""
+        from . import suggest as S
+
+        if not 1 <= top_k <= S.MAX_TOP_K:
+            raise ValueError(f"top_k must be in 1..{S.MAX_TOP_K}")
+        tokens = paragraph_query_tokens(body)
+        out = S.ParagraphSuggest([], False, S.ematches(tokens))
+        views = [s._gpu.view(m) for s, m in zip(self.segments, masks)]
+        try:
+            terms, phrases = self._clauses(body)
+            if terms or phrases:
+                qt, qo = np.asarray(terms, dtype=np.uint32), np.asarray([0, len(terms)], dtype=np.uint32)
+                rows = []
+                for ord_, v in enumerate(views):
+                    params = dict(mode=_lib.NIDX_BM25_OR, use_tf=False, docaddr_base=ord_ << 32)
+                    if phrases:
+                        docs, scores, counts, _ = v.search_phrases(qt, qo, [(0, p) for p in phrases], top_k, **params)
+                    else:
+                        docs, scores, counts, _ = v.search(qt, qo, top_k, **params)
+                    rows += [(-float(scores[0, i]), ord_, int(docs[0, i])) for i in range(int(counts[0]))]
+                rows.sort()
+                out.hits = [S.ParagraphHit(-neg, o, d) for neg, o, d in rows[:top_k]]
+            if out.hits:
+                return out
+            clauses = S.fuzzy_clauses(tokens)
+            if not clauses:
+                return out
+            if len(clauses) > _lib.NIDX_SG_MAX_CLAUSES:
+                raise ValueError(f"a suggest body of more than {_lib.NIDX_SG_MAX_CLAUSES} clauses is not supported")
+            out.fuzzy = True
+            out.hits = self._suggest_fuzzy(clauses, top_k, views)
+            return out
+        finally:
+            for v in views:
+                v.close()
+
+    def _suggest_fuzzy(self, clauses: list, top_k: int, views: list) -> list:
+        from . import suggest as S
+        from .segment import SuggestDict
+
+        if self._suggest_dict is None:
+            vocab_terms = [""] * len(self.vocab)
+            for t, i in self.vocab.items():
+                vocab_terms[i] = t
+            self._suggest_dict = SuggestDict(vocab_terms, device=self.segments[0].device)
+            self._vocab_terms = vocab_terms
+        auto = [(v, S.FUZZY_DISTANCE, kind == S.FUZZY_PREFIX) for kind, v in clauses if kind in (S.FUZZY, S.FUZZY_PREFIX)]
+        if sum(len(v) for v, _, _ in auto) > S.MAX_FUZZY_CODE_POINTS:
+            raise ValueError(f"the fuzzy literals of a suggest body hold more than {S.MAX_FUZZY_CODE_POINTS} code points")
+        bits = self._suggest_dict.expand(auto)[0] if auto else None
+        spec, phrases, row = [], [], 0
+        for kind, v in clauses:
+            if kind in (S.FUZZY, S.FUZZY_PREFIX):
+                spec.append((_lib.NIDX_SG_FUZZY, row))
+                row += 1
+            elif kind == S.TERM:
+                spec.append((_lib.NIDX_SG_TERM, self.vocab.get(v, _lib.NIL)))
+            else:
+                spec.append((_lib.NIDX_SG_PHRASE, len(phrases)))
+                phrases.append([self.vocab.get(t, 0xFFFFFFF0) for t in v])
+        if phrases:
+            self._ensure_positions()
+        rows, found = [], {}
+        for ord_, v in enumerate(views):
+            ids, scores, count, trip = v.suggest_fuzzy(spec, bits, len(auto), len(self.vocab), phrases, top_k, min(S.RESULTS_PER_PAGE, top_k))
+            rows += [(-float(scores[i]), ord_, int(ids[i])) for i in range(count)]
+            for h, c, t in trip:
+                found.setdefault((ord_, int(ids[h])), []).append(self._vocab_terms[t])
+        rows.sort()
+        hits = [S.ParagraphHit(-neg, o, d) for neg, o, d in rows[:top_k]]
+        for h in hits[: S.RESULTS_PER_PAGE]:
+            h.matches = sorted(t for t in found.get((h.segment, h.doc), []) if len(t.encode("utf-8")) > 2)
+        return hits
 
     def _clauses(self, body: str):
         words, phrases = parse_paragraph_query(body)
