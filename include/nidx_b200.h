@@ -226,6 +226,10 @@ int nidx_vec_exact_rows(nidx_vec_segment* seg, uint64_t* out);
  * survivors of the filter, [1] queries scanned exactly in full instead (a list that may have overflowed, too many survivors, or
  * a query outside the filter's error bound).  Both are 0 when the scan did not use the filter. */
 int nidx_vec_scan_counters(nidx_vec_segment* seg, uint64_t out[2]);
+/* Queries the last search's dense HNSW walk (NIDX_METHOD_HNSW, or AUTO choosing it) walked a second time because their first
+ * walk overflowed its visited set or dropped a candidate it would have popped.  The second walk cannot overflow and its results
+ * are returned; the counters describe it in place of the first.  0 after any other search, a build, or a walk that needed none. */
+int nidx_vec_walk_reruns(nidx_vec_segment* seg, uint64_t* out);
 
 /* RaBitQ 1-bit codes (vector_types/rabitq.rs; Dot similarity and dimension % 64 == 0 only, config.rs:170-173).
  * nidx_vec_rabitq_encode builds the reference's vectors.quant records ([f32 dot_quant_original][u32 sum_bits][dim/8 sign

@@ -158,6 +158,7 @@ SIGNATURES = {
     "nidx_vec_counters_ex": (i32, [P, P]),
     "nidx_vec_exact_rows": (i32, [P, P]),
     "nidx_vec_scan_counters": (i32, [P, P]),
+    "nidx_vec_walk_reruns": (i32, [P, P]),
     "nidx_vec_rabitq_encode": (i32, [P, P]),
     "nidx_vec_rabitq_codes": (i32, [P, P]),
     "nidx_vec_rabitq_estimate": (i32, [P, P, i32, i32, i32, P, P, P]),

@@ -99,7 +99,7 @@ using DevBuf = DevArray<unsigned char>;
 
 // Per-call scratch; a segment keeps a pool so concurrent searches do not share one.
 struct Workspace {
-    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets, phrases, prefilter;
+    DevBuf queries, qnorms, stage, scores, partial, filter, misc, sched, facets, phrases, prefilter, rerun;
     cudaEvent_t done = nullptr;
     cudaStream_t last_stream = nullptr;
     bool busy = false;
@@ -723,6 +723,17 @@ int nidx_vec_counters_ex(nidx_vec_segment* s, uint64_t out[6]) { return read_cou
 int nidx_vec_counters(nidx_vec_segment* s, uint64_t out[3]) { return read_counters(s, out, {0, 1, -1}); }
 int nidx_vec_exact_rows(nidx_vec_segment* s, uint64_t* out) { return read_counters(s, out, {6}); }
 int nidx_vec_scan_counters(nidx_vec_segment* s, uint64_t out[2]) { return read_counters(s, out, {6, 7}); }
+// The dense walk keeps its flagged-query count in the 64 bytes before the counters (w.sched: [0] the work counter, [2] this count,
+// [3] the re-run's work counter, as unsigned ints), zeroed with them
+int nidx_vec_walk_reruns(nidx_vec_segment* s, uint64_t* out) {
+    if (!s || !out) return fail(NIDX_EINVAL, "null argument");
+    CU(cudaSetDevice(s->cfg.device));
+    unsigned int h = 0;
+    unsigned long long* src = s->last_counters.load();
+    if (src) CU(cudaMemcpy(&h, reinterpret_cast<unsigned int*>(src - 8) + 2, sizeof(h), cudaMemcpyDeviceToHost));
+    *out = h;
+    return 0;
+}
 
 // ---- RaBitQ --------------------------------------------------------------------------------------
 static int rabitq_check(const nidx_vec_segment* s) {
@@ -905,6 +916,10 @@ typedef void (*hs_kernel_t)(VecDev, GraphDev, SearchArgs);
 // defer: closest_up_nodes may settle neighbours on the kept layer-0 set (hnsw_search_kernel's DEFER)
 static hs_kernel_t pick_search_kernel(int ld, bool defer = false) {
     return pick_ng<1, 2, 3, 4, 6, 8>(ld, [defer](auto ng) -> hs_kernel_t { return defer ? hnsw_search_kernel<ng, true> : hnsw_search_kernel<ng>; });
+}
+// the dense walk's re-run of its flagged queries (hnsw_search_kernel's RERUN)
+static hs_kernel_t pick_rerun_kernel(int ld) {
+    return pick_ng<1, 2, 3, 4, 6, 8>(ld, [](auto ng) -> hs_kernel_t { return hnsw_search_kernel<ng, false, true>; });
 }
 
 // w4: the 4-warp CTA shape (quantised_walk)
@@ -1362,6 +1377,10 @@ struct VecCall {
         size_t smem;
         if (!hnsw_search_smem(s, ef0, k, &list_cap, &cu_cap, &hash_bits, &smem))
             return fail(NIDX_EINVAL, "HNSW search needs %zu bytes of shared memory (ef=%d, k=%d, dim=%d): too large", smem, ef0, k, s->d);
+        if (const char* eb = getenv("NIDX_B200_HS_BITS")) {   // tests: a smaller visited table (one that still holds a reseeded list)
+            hash_bits = std::min(hash_bits, std::max(ilog2(next_pow2(4 * ef0)), atoi(eb)));
+            smem = hs_smem_bytes(s->ld, list_cap, hash_bits);
+        }
         VecDev Vh = V;   // with the screening copy attached
         int r = attach_half_copy(s, &Vh);
         // deferral needs the fp16 copy's walk and pops that are never rejected (hs_can_defer)
@@ -1370,7 +1389,34 @@ struct VecCall {
         int grid = 0;
         if (!r) r = walk_grid(kern, HS_THREADS, smem, &grid);
         if (r) return r;
-        return launch_walk(kern, grid, HS_THREADS, smem, Vh, walk_args(ef0, list_cap, cu_cap, hash_bits));
+        // The shared-memory capacities can overflow (a filter that rejects most pops makes closest_up_nodes score thousands of
+        // nodes, where the reference's BitSet and heap are unbounded).  The walk flags the queries that lost something to them, and
+        // a second launch walks those again with lists of n + ef0 entries and a visited table that holds every node, which cannot
+        // overflow.  The second launch is enqueued whatever happened -- no host synchronisation -- and its CTAs exit at once when no
+        // query was flagged.  Its scratch: one slice per CTA, as many CTAs as 1 GiB holds (at least one, at most one per SM).
+        const size_t cap = (size_t)s->n + ef0;
+        const int all_bits = rq_table_bits(s->n);
+        const size_t slice = cap * 16 + ((size_t)4 << all_bits);
+        const int rgrid = (int)std::max<size_t>(1, std::min<size_t>(((size_t)1 << 30) / slice, (size_t)std::min(nq, s->sm_count)));
+        const size_t o_list = ((size_t)nq * 4 + 255) & ~(size_t)255, o_vis = o_list + (size_t)rgrid * cap * 16;
+        ENSURE(w.rerun, o_vis + ((size_t)rgrid << all_bits) * 4);
+        SearchArgs a = walk_args(ef0, list_cap, cu_cap, hash_bits);
+        a.flagged = w.rerun.as<uint32_t>();
+        a.n_flagged = w.sched.as<unsigned int>() + 2;   // zeroed with the counters (nidx_vec_walk_reruns reads it)
+        CU(cudaEventRecord(s->ev_k0, stream));
+        kern<<<grid, HS_THREADS, smem, stream>>>(Vh, s->gdev(), a);
+        LAUNCHED();
+        SearchArgs b = a;
+        b.work_counter = w.sched.as<unsigned int>() + 3;
+        b.list_cap = b.cu_cap = (int)cap;
+        b.hash_bits = 0;
+        b.glist = reinterpret_cast<uint64_t*>(w.rerun.p + o_list);
+        b.gvisited = reinterpret_cast<uint32_t*>(w.rerun.p + o_vis); b.gv_bits = all_bits;
+        pick_rerun_kernel(s->ld)<<<rgrid, HS_THREADS, hs_smem_bytes(s->ld, 0, 0), stream>>>(Vh, s->gdev(), b);
+        LAUNCHED();
+        CU(cudaEventRecord(s->ev_k1, stream));
+        CU(cudaGetLastError());
+        return 0;
     }
 };
 

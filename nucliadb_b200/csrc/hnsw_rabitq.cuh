@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(W * 32, W == HS_WARPS ? 4 : 7) hnsw_rabitq_ker
     const RabitqQueryParams* qparams = reinterpret_cast<const RabitqQueryParams*>(a.qparams);
 
     unsigned q;
-    while (hs_next_query(a, &q)) {
+    while (hs_next_query(a, &q, a.nq)) {
         const float* qsrc = a.queries + (size_t)q * V.ld;
         for (int i = threadIdx.x; i < ng; i += blockDim.x) reinterpret_cast<float4*>(c.qvec)[i] = reinterpret_cast<const float4*>(qsrc)[i];
         for (int i = threadIdx.x; i < 4 * r.nw; i += blockDim.x) planes[i] = a.planes[(size_t)q * 4 * r.nw + i];

@@ -7,7 +7,7 @@
 //   NodeFilter::passes              search.rs:135-171
 //   HnswBuilder::insert (search half) hnsw/build.rs:123-150
 //
-// Data structures per CTA, all in shared memory:
+// Data structures per CTA, all in shared memory (the re-run of hnsw_search_kernel keeps the list and the visited set in global memory):
 //   * ONE sorted list of 64-bit rank keys (score desc, id asc) with an "unexpanded" flag in bit 0.
 //     It is the reference's two BinaryHeaps folded together: a candidate that is not among the best
 //     `ef` results can never be expanded (popping it ends the search, search.rs:268-273), so the
@@ -57,9 +57,14 @@ struct SearchArgs {
     int code_stride;
     const uint32_t* planes;           // [nq][4][d/32] query bit planes
     const void* qparams;              // [nq] RabitqQueryParams
-    uint32_t* gvisited;               // [grid][1 << gv_bits] layer-0 visited table in global memory (L2)
+    uint32_t* gvisited;               // [grid][1 << gv_bits] layer-0 visited table in global memory (L2); the dense re-run's tables
     int gv_bits;
     int last_k;                       // min(k * RERANKING_FACTOR, RERANKING_LIMIT)
+    // dense walk (query mode): the queries whose first pass lost a neighbour or a candidate to a capacity, and their count; the
+    // re-run (hnsw_search_kernel<NG, false, true>) walks them again on its lists in global memory
+    uint32_t* flagged;                // [nq], nullptr: nothing is flagged (the build)
+    unsigned int* n_flagged;
+    uint64_t* glist;                  // re-run: [grid][2][list_cap] the two lists of each CTA
 };
 
 // An exact visited set: open addressing over 1 << bits slots of node ids (NIL = free), linear probing.  Threads insert concurrently.
@@ -180,15 +185,24 @@ __host__ __device__ __forceinline__ size_t hs_smem_bytes(int ld, int list_cap, i
 
 // The CTA's shared state of a walk: the dynamic shared memory laid out as hs_smem_bytes counts it, from `p` on, and the shared
 // scalars.  Returns the end of the layout, where the quantised walk lays out its own arrays.
+// GLOBAL (the dense walk's re-run): the two lists and the visited set are this CTA's slices of a.glist and a.gvisited, and the
+// shared layout has neither (hs_smem_bytes(ld, 0, 0)).
+template <bool GLOBAL = false>
 __device__ inline unsigned char* hs_setup(SearchCtx& c, const SearchArgs& a, unsigned char* p, int ld) {
     __shared__ int s_ints[4];
     __shared__ HopRec s_hops[2];
     __shared__ unsigned long long s_drop;
     c.qvec = reinterpret_cast<float*>(p); p += (size_t)ld * 4;
-    c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
-    c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
+    if (GLOBAL) {
+        c.A = a.glist + (size_t)blockIdx.x * 2 * a.list_cap;
+        c.B = c.A + a.list_cap;
+    } else {
+        c.A = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
+        c.B = reinterpret_cast<uint64_t*>(p); p += (size_t)a.list_cap * 8;
+    }
     c.todo_key = reinterpret_cast<uint64_t*>(p); p += HS_MAX_ROW * 8;
-    c.vis.init(reinterpret_cast<uint32_t*>(p), a.hash_bits); p += (size_t)4 << a.hash_bits;
+    if (GLOBAL) c.vis.init(a.gvisited + ((size_t)blockIdx.x << a.gv_bits), a.gv_bits);
+    else { c.vis.init(reinterpret_cast<uint32_t*>(p), a.hash_bits); p += (size_t)4 << a.hash_bits; }
     c.todo_id = reinterpret_cast<uint32_t*>(p); p += HS_MAX_ROW * 4;
     c.pref_row = reinterpret_cast<uint32_t*>(p); p += 2 * HS_MAX_ROW * 4;
     c.pref_node = reinterpret_cast<uint32_t*>(p); p += 16;
@@ -201,14 +215,14 @@ __device__ inline unsigned char* hs_setup(SearchCtx& c, const SearchArgs& a, uns
     return p;
 }
 
-// The dynamic scheduler: the CTA's next query in *q, false when every query has been taken.
-__device__ inline bool hs_next_query(const SearchArgs& a, unsigned* q) {
+// The dynamic scheduler: the CTA's next item of `n` (a.nq: the next query) in *q, false when every item has been taken.
+__device__ inline bool hs_next_query(const SearchArgs& a, unsigned* q, int n) {
     __shared__ unsigned s_work;
     __syncthreads();
     if (threadIdx.x == 0) s_work = atomicAdd(a.work_counter, 1u);
     __syncthreads();
     *q = s_work;
-    return *q < (unsigned)a.nq;
+    return *q < (unsigned)n;
 }
 
 // counters [0]-[3]: n_dist lives in lane 0 of every warp, the rest in thread 0
@@ -219,6 +233,12 @@ __device__ inline void hs_flush_counters(const SearchCtx& c, unsigned long long*
         if (c.n_overflow & 0xFFFFFFFFull) atomicAdd(&counters[2], c.n_overflow & 0xFFFFFFFFull);
         if (c.n_overflow >> 32) atomicAdd(&counters[3], c.n_overflow >> 32);
     }
+}
+
+// hs_flush_counters and [6] = f32 rows read for a similarity (n_skip lives in lane 0 of every warp, as n_dist)
+__device__ inline void hs_flush_walk_counters(const SearchCtx& c, unsigned long long* counters) {
+    hs_flush_counters(c, counters);
+    if ((threadIdx.x & 31) == 0 && c.n_dist) atomicAdd(&counters[6], c.n_dist - c.n_skip);
 }
 
 // Start a layer search (or closest_up_nodes) on the list in c.A: every entry unexpanded, the visited set `vis` = the list's ids,
@@ -567,16 +587,26 @@ __device__ inline void hs_emit_results(const VecDev& V, const GraphDev& G, Searc
 // DEFER: closest_up_nodes may settle neighbours on the kept layer-0 set (hs_can_defer).  The host launches it only for queries
 // whose pops are all accepted (no filter, duplicates allowed, one vector per paragraph) with the fp16 copy attached; every other
 // walk, and the build, runs the kernel without it.
-template <int NG, bool DEFER = false>
+// A query that loses something to a capacity -- a neighbour the full visited set reports as visited, or a candidate the full
+// closest_up_nodes list dropped and would have popped (both counted in n_overflow) -- is flagged when a.flagged is set: its id goes
+// to a.flagged, and its counts are dropped, so that the counters describe the walks whose results are returned.  Each query's
+// counts are then flushed when it ends (a snapshot of them held through the walk would take registers the hot loop needs).
+// RERUN walks the flagged queries again (the launch after the walk; its CTAs exit at once when none is flagged), with lists of
+// n + ef0 entries and a visited table that holds every node, both in global memory: it cannot overflow, and it overwrites the
+// flagged queries' results.
+template <int NG, bool DEFER = false, bool RERUN = false>
 __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, GraphDev G, SearchArgs a) {
     extern __shared__ __align__(16) unsigned char smem[];
+    const int nwork = RERUN ? (int)*a.n_flagged : a.nq;
+    if (RERUN && nwork == 0) return;
     SearchCtx c;
-    hs_setup(c, a, smem, V.ld);
+    hs_setup<RERUN>(c, a, smem, V.ld);
     int lane = threadIdx.x & 31;
     int ng = V.ld >> 2;
 
     unsigned q;
-    while (hs_next_query(a, &q)) {
+    while (hs_next_query(a, &q, nwork)) {
+        if (RERUN) q = a.flagged[q];
         const float* qsrc;
         uint32_t self = NIL;
         if (a.mode == 0) { qsrc = a.queries + (size_t)q * V.ld; c.qnorm = V.sim != SIM_DOT ? a.qnorms[q] : 0.0f; }
@@ -623,10 +653,17 @@ __global__ void __launch_bounds__(HS_THREADS, 4) hnsw_search_kernel(VecDev V, Gr
             for (int layer = (int)G.entry_layer + 1; layer <= top && layer < HS_MAX_LAYERS; ++layer) a.found_count[(size_t)q * HS_MAX_LAYERS + layer] = 0;
 
         if (a.mode == 0) hs_emit_results<NG, HS_WARPS, DEFER>(V, G, c, a, q);
+        if (!RERUN && a.flagged) {   // the counters hold this query's counts only; thread 0 holds n_overflow
+            if (threadIdx.x == 0) {
+                *c.s_flag = c.n_overflow != 0;
+                if (*c.s_flag) a.flagged[atomicAdd(a.n_flagged, 1u)] = q;
+            }
+            __syncthreads();         // the next hs_next_query's barrier guards s_flag
+            if (!*c.s_flag) hs_flush_walk_counters(c, a.counters);
+            c.n_dist = c.n_expand = c.n_overflow = c.n_skip = 0;
+        }
     }
-    hs_flush_counters(c, a.counters);
-    // [6] = f32 rows read for a similarity (n_skip lives in lane 0 of every warp, as n_dist)
-    if (lane == 0 && c.n_dist) atomicAdd(&a.counters[6], c.n_dist - c.n_skip);
+    hs_flush_walk_counters(c, a.counters);
 }
 
 }  // namespace nidx

@@ -249,6 +249,13 @@ class VectorSegment:
         check(_lib.load().nidx_vec_exact_rows(self._h, C.byref(out)))
         return out.value
 
+    def walk_reruns(self) -> int:
+        """Queries the last dense HNSW walk ran a second time, on capacities that cannot overflow, because their first walk lost a
+        neighbour or a candidate to its visited set or its closest_up_nodes list (0 when nothing overflowed)."""
+        out = C.c_uint64()
+        check(_lib.load().nidx_vec_walk_reruns(self._h, C.byref(out)))
+        return out.value
+
     def scan_counters(self):
         """The last exhaustive scan's tensor-core filter: vectors re-scored as survivors, and queries scanned in full instead
         (both 0 when the scan did not use the filter)."""

@@ -100,6 +100,7 @@ def test_wrappers_agree_with_the_signature_table():
         "VectorSegment.counters_ex": vec.counters_ex,
         "VectorSegment.exact_rows": vec.exact_rows,
         "VectorSegment.scan_counters": vec.scan_counters,
+        "VectorSegment.walk_reruns": vec.walk_reruns,
         "TextSegment.set_stats": lambda: txt.set_stats(4, 10, np.ones(3)),
         "TextSegment.set_alive": lambda: txt.set_alive(np.ones(1, np.uint64)),
         "TextSegment.search": lambda: txt.search(qt, qoff, 3, mode=_lib.NIDX_BM25_AND, use_tf=False, min_score=0.1, after=(1.0, 2, 5), docaddr_base=1 << 32),
