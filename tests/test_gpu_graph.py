@@ -199,6 +199,200 @@ def test_limits_are_einval(knowledge):
     assert ix.search([leaf], G.PATH, 2)
 
 
+def _raw_nodes(ix, t, nodes, terms, keep):
+    """A program tree -> pre-order nidx_graph_node, one node per tree node: ("and", [..]) / ("or", [..]) / ("not", x), and a leaf of
+    graph.py's tree (GraphIndex.compile emits one node for it)."""
+    from nucliadb_b200 import _lib
+
+    if t[0] in ("and", "or", "not"):
+        kind = {"and": _lib.NIDX_G_AND, "or": _lib.NIDX_G_OR, "not": _lib.NIDX_G_NOT}[t[0]]
+        kids = t[1] if t[0] != "not" else [t[1]]
+        nodes.append(_lib.GraphNode(kind, len(kids), 0, 0.0, 0, 0, None))
+        for c in kids:
+            _raw_nodes(ix, c, nodes, terms, keep)
+    else:
+        n0 = len(nodes)
+        ix.compile(t, nodes, terms, keep)
+        assert len(nodes) == n0 + 1
+
+
+def _model_tree(t):
+    """The same program as a graph.py tree for the model: AND -> MUST (a NOT operand -> MUST_NOT: it adds 0 to the sum), OR -> SHOULD."""
+    from nucliadb_b200 import graph as G
+
+    if t[0] == "and":
+        return ("bool", [(G.MUST_NOT, _model_tree(c[1])) if c[0] == "not" else (G.MUST, _model_tree(c)) for c in t[1]])
+    if t[0] == "or":
+        return ("bool", [(G.SHOULD, _model_tree(c)) for c in t[1]])
+    return t
+
+
+def _instructions(t):
+    """graph_eval_kernel's program length: a leaf is 1, an n-operand AND / OR n - 1 more, a NOT 1."""
+    if t[0] in ("and", "or"):
+        return sum(_instructions(c) for c in t[1]) + len(t[1]) - 1
+    if t[0] == "not":
+        return _instructions(t[1]) + 1
+    return 1
+
+
+def _levels(t, lvl=1):
+    """The deepest nesting level of a leaf (the root is level 1)."""
+    if t[0] in ("and", "or"):
+        return max(_levels(c, lvl + 1) for c in t[1])
+    if t[0] == "not":
+        return _levels(t[1], lvl + 1)
+    return lvl
+
+
+def _stack(t):
+    """The deepest the program's bit and score stacks grow (operands are folded left to right)."""
+    if t[0] in ("and", "or"):
+        return max([_stack(t[1][0])] + [1 + _stack(c) for c in t[1][1:]])
+    if t[0] == "not":
+        return _stack(t[1])
+    return 1
+
+
+def _leaf_pool(model, side):
+    """Term leaves over the model's own dictionaries (side "src" / "dst"), each matching some relations."""
+    vals = model.col[f"{side}_norm"][0]
+    labels = model.col["label"][0]
+    subs = [s for s in model.col[f"{side}_sub"][0] if s]
+    toks = model.multi[f"{side}_tok"][0]
+    out = [("term", f"{side}_norm", v) for v in vals[:40]] + [("term", "label", v) for v in labels[:20]]
+    out += [("term", f"{side}_type", i) for i in range(4)] + [("term", f"{side}_sub", s) for s in subs[:4]]
+    out += [("termset", f"{side}_tok", [toks[i], toks[-1 - i]]) for i in range(min(8, len(toks)))]
+    out += [("term", "rel_type", i) for i in range(6)] + [("term", "facet", f) for f in ("/f/a", "/f", "/g")] + [("all",)]
+    return out
+
+
+def _limit_program(model, side, instructions=None, width=2):
+    """AND(l1, AND(l2, ... AND(l62, OR(width leaves)))): the OR's leaves sit at level 64 and the stack reaches 64 levels.  The chain's
+    leaves match all but a few relations (the all query, NOTs of single values); with `instructions` the OR's width makes the program
+    exactly that long."""
+    pool = _leaf_pool(model, side)
+    vals = model.col[f"{side}_norm"][0]
+    left = [("not", ("term", f"{side}_norm", vals[-1 - i % len(vals)])) if i % 5 == 0 else ("all",) for i in range(62)]
+    if instructions is not None:
+        fixed = sum(_instructions(x) for x in left) + len(left)   # the chain's leaves and ANDs; the OR adds 2 * width - 1
+        if (instructions - fixed + 1) % 2:
+            left[1] = ("not", ("term", f"{side}_norm", vals[0]))
+            fixed += 1
+        width = (instructions - fixed + 1) // 2
+    t = ("or", [pool[i % len(pool)] for i in range(width)])
+    for leaf in reversed(left):
+        t = ("and", [leaf, t])
+    if instructions is not None:
+        assert _instructions(t) == instructions
+    return t
+
+
+def _run_raw(ix, model, trees, kind, k):
+    from nucliadb_b200 import _lib
+
+    nodes, terms, keep = [], [], []
+    for t in trees:
+        _raw_nodes(ix, t, nodes, terms, keep)
+    arr = (_lib.GraphNode * len(nodes))(*nodes)
+    tarr = (_lib.GraphTerm * max(len(terms), 1))(*terms)
+    ids, sc, cnt = np.zeros(k, np.uint32), np.zeros(k, np.float32), np.zeros(1, np.int32)
+    rc = _lib.load().nidx_graph_search(ix.graph, arr, len(nodes), tarr, len(terms), kind, k, None, _lib.NIDX_MEM_HOST, _lib.ptr(ids), _lib.ptr(sc),
+                                       _lib.ptr(cnt), None)
+    if rc:
+        return rc, None
+    got = _device_keys(ix, kind, [(int(i), float(s)) for i, s in zip(ids[: cnt[0]], sc[: cnt[0]])])
+    want = model.search([_model_tree(t) for t in trees], kind, k)
+    assert [k_ for k_, _ in got] == [k_ for k_, _ in want]
+    assert [np.float32(s).view(np.uint32) for _, s in got] == [np.float32(s).view(np.uint32) for _, s in want]
+    return rc, got
+
+
+@pytest.fixture(scope="module")
+def synthetic_3000():
+    from nucliadb_b200.graph import GraphIndex
+
+    docs = _synthetic(3000, 7)[0]
+    ix = GraphIndex(docs)
+    yield ix, Model(docs)
+    ix.close()
+
+
+@pytest.mark.parametrize("which", ["knowledge", "synthetic"])
+def test_programs_at_the_depth_and_length_limits(which, knowledge, synthetic_3000):
+    """graph_eval_kernel at its limits, against the model: a right-deep chain whose leaves sit at NIDX_PREFILTER_MAX_DEPTH = 64 levels
+    with a 64-level stack, a program of exactly 4 096 instructions, both at once (4 096 x 32 B of program + 64 x 256 x 4 B of score
+    stack: 192 KiB of shared memory), and a NODES search whose two programs are both that size; one instruction or one level more is
+    NIDX_EINVAL."""
+    from nucliadb_b200 import graph as G
+
+    ix, model = knowledge if which == "knowledge" else synthetic_3000
+    deep = _limit_program(model, "src")
+    assert _levels(deep) == 64 and _stack(deep) == 64 and _instructions(deep) < 4096
+    pool = _leaf_pool(model, "dst")
+    long_ = ("and", [("or", [pool[i % len(pool)] for i in range(2047)]), ("not", ("term", "label", model.col["label"][0][0]))])
+    assert _instructions(long_) == 4096 and _levels(long_) == 3
+    both = _limit_program(model, "src", 4096)
+    both_dst = _limit_program(model, "dst", 4096)
+    assert _instructions(both) == _instructions(both_dst) == 4096 and _levels(both) == _stack(both) == 64
+    assert 4096 * 32 + 64 * 256 * 4 == 192 * 1024
+    for t in (deep, long_, both):
+        for k in (1, 20, 1024):
+            rc, got = _run_raw(ix, model, [t], G.PATH, k)
+            assert rc == 0 and got
+    for k in (1, 100, 1024):
+        rc, got = _run_raw(ix, model, [both, both_dst], G.NODES, k)
+        assert rc == 0 and got
+        rc, got = _run_raw(ix, model, [both], G.RELATIONS, k)
+        assert rc == 0 and got
+    # one past: 4 097 instructions, 65 levels
+    assert _run_raw(ix, model, [_limit_program(model, "src", 4097)], G.PATH, 10)[0] == -1
+    assert _run_raw(ix, model, [both, _limit_program(model, "dst", 4097)], G.NODES, 10)[0] == -1
+    assert _levels(("and", [("all",), deep])) == 65
+    assert _run_raw(ix, model, [("and", [("all",), deep])], G.PATH, 10)[0] == -1
+
+
+@pytest.mark.parametrize("which", ["knowledge", "synthetic"])
+def test_64_automaton_terms_of_4096_code_points(which, knowledge, synthetic_3000):
+    """64 fuzzy leaves (distances 0 - 2, prefix on and off, over both value columns and both token sides, so both dictionaries)
+    whose code points total exactly 4 096: 8 long terms first, so that the matching ones sit at the end of the shared array; one
+    OR of all of them, one AND under a NOT, and a NODES search whose two programs take half each, against the model; one more code
+    point is NIDX_EINVAL."""
+    from nucliadb_b200 import _lib
+    from nucliadb_b200 import graph as G
+
+    ix, model = knowledge if which == "knowledge" else synthetic_3000
+    rng = random.Random(11)
+    fields = ["src_norm", "dst_norm", "src_tok", "dst_tok"]
+    short = []
+    for i in range(56):
+        f = fields[i % 4]
+        src = model.col[f][0] if f.endswith("norm") else model.multi[f][0]
+        v = str(src[rng.randrange(len(src))]) or "a"
+        if i % 3 and len(v) > 1:   # a typo
+            p = rng.randrange(len(v))
+            v = v[:p] + rng.choice("xzé") + v[p + 1:]
+        if i % 7 == 6:
+            v = v[: max(1, len(v) // 2)]
+        short.append(("fuzzy", f, v, i % 3, (i // 3) % 2 == 1))
+    rest = 4096 - sum(len(t[2]) for t in short)
+    assert rest >= 8
+    longs = [("fuzzy", ["src_tok", "dst_tok"][i % 2], ("zq" * 2048)[: rest // 8 + (i < rest % 8)], i % 3, i % 2 == 0) for i in range(8)]
+    leaves = longs + short
+    assert len(leaves) == 64 and sum(len(t[2]) for t in leaves) == 4096
+    assert {t[3] for t in leaves} == {0, 1, 2} and {t[4] for t in leaves} == {False, True}
+    any_of = ("or", leaves)
+    all_but = ("and", [("or", leaves[:32]), ("not", ("or", leaves[32:]))])
+    for k in (1, 50, 1024):
+        rc, got = _run_raw(ix, model, [any_of], G.PATH, k)
+        assert rc == 0 and got
+        assert _run_raw(ix, model, [all_but], G.PATH, k)[0] == 0
+        # NODES: the two programs share the 64 terms (the limit counts the terms of both)
+        assert _run_raw(ix, model, [("or", leaves[:32]), ("or", leaves[32:])], G.NODES, k)[0] == 0
+    over = longs[:7] + [("fuzzy", "src_tok", longs[7][2] + "q", 1, False)] + short
+    assert _run_raw(ix, model, [("or", over)], G.PATH, 10)[0] == -1
+
+
 def test_dict_match_kernel_equals_a_full_dp_over_every_entry():
     """graph_dict_match_kernel's bitsets (read through one automaton leaf over a value column or a token CSR, one document per
     dictionary entry, k = 1024 so every match comes back) against graph_model.fuzzy_match over every entry: d = 0, 1, 2, with and
